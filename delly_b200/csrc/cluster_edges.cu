@@ -176,27 +176,24 @@ __global__ void scan_add_kernel(uint32_t* __restrict__ off, uint32_t n, const un
 }
 
 template <bool SR, typename A>
-int ce_run(dgpu_ctx* ctx, A a, const void* const* host_cols, int ncols, uint64_t n, uint32_t* edge_off, uint32_t* edge_j, uint32_t* edge_w,
+int ce_run(DgpuStage& s, A a, const void* const* host_cols, int ncols, uint64_t n, uint32_t* edge_off, uint32_t* edge_j, uint32_t* edge_w,
            uint64_t edge_cap, uint64_t* n_edges) {
-  DGPU_CUDA(ctx, cudaSetDevice(ctx->device));
-  cudaStream_t st = ctx->stream;
+  dgpu_ctx* ctx = s.ctx;
   int rc;
-  void* p;
+  if ((rc = s.open())) return rc;
+  cudaStream_t st = s.st;
   // record columns: one device arena, ncols x n int32
-  if ((rc = dgpu_reserve(ctx, SLOT_A0, (size_t) ncols * n * 4, &p))) return rc;
-  int32_t* d_cols = (int32_t*) p;
-  for (int k = 0; k < ncols; ++k) DGPU_CUDA(ctx, cudaMemcpyAsync(d_cols + (size_t) k * n, host_cols[k], n * 4, cudaMemcpyHostToDevice, st));
+  int32_t* d_cols = s.alloc<int32_t>((size_t) ncols * n);
+  for (int k = 0; k < ncols; ++k) s.upload(d_cols + (size_t) k * n, host_cols[k], n * 4);
+  const uint32_t tiles = (uint32_t) ((n + SCAN_TILE - 1) / SCAN_TILE);
+  uint32_t* d_cnt = s.alloc<uint32_t>(n + 1);
+  uint32_t* d_off = s.out(edge_off, n + 1);
+  unsigned long long* d_tiles = s.alloc<unsigned long long>((size_t) tiles + 1);
+  if (s.rc) return s.rc;
   const int32_t* col[8];
   for (int k = 0; k < ncols; ++k) col[k] = d_cols + (size_t) k * n;
   if constexpr (SR) { a.chr = col[0]; a.pos = col[1]; a.chr2 = col[2]; a.pos2 = col[3]; a.inslen = col[4]; }
   else { a.pos = col[0]; a.mpos = col[1]; a.mtid = col[2]; a.alen = col[3]; a.median = col[4]; a.maxNormalISize = col[5]; }
-  const uint32_t tiles = (uint32_t) ((n + SCAN_TILE - 1) / SCAN_TILE);
-  if ((rc = dgpu_reserve(ctx, SLOT_A1, (n + 1) * 4, &p))) return rc;
-  uint32_t* d_cnt = (uint32_t*) p;
-  if ((rc = dgpu_reserve(ctx, SLOT_A2, (n + 1) * 4, &p))) return rc;
-  uint32_t* d_off = (uint32_t*) p;
-  if ((rc = dgpu_reserve(ctx, SLOT_A3, ((size_t) tiles + 1) * 8, &p))) return rc;
-  unsigned long long* d_tiles = (unsigned long long*) p;
   unsigned long long* d_total = d_tiles + tiles;
   const unsigned blocks = (unsigned) ((n + CE_THREADS - 1) / CE_THREADS);
   dgpu_prof_begin(ctx, st);
@@ -214,22 +211,14 @@ int ce_run(dgpu_ctx* ctx, A a, const void* const* host_cols, int ncols, uint64_t
   *n_edges = total;
   if (total >= (1ull << 32)) { ctx->last_error = "dgpu_cluster_edges: more than 2^32-1 edges"; return DGPU_ERR_CAPACITY; }
   const uint64_t fillcap = std::min<uint64_t>(total, edge_cap);
-  uint32_t *d_ej = nullptr, *d_ew = nullptr;
-  if (fillcap) {
-    if ((rc = dgpu_reserve(ctx, SLOT_A4, fillcap * 4, &p))) return rc;
-    d_ej = (uint32_t*) p;
-    if ((rc = dgpu_reserve(ctx, SLOT_A5, fillcap * 4, &p))) return rc;
-    d_ew = (uint32_t*) p;
+  if (fillcap) {   // the edge columns are sized by the count pass: staged (and copied back) only now
+    uint32_t *d_ej = s.out(edge_j, fillcap), *d_ew = s.out(edge_w, fillcap);
+    if (s.rc) return s.rc;
     ce_fill_kernel<SR, A><<<blocks, CE_THREADS, 0, st>>>(a, d_off, d_ej, d_ew, fillcap);
     DGPU_LAUNCH_CHECK(ctx, "ce_fill");
   }
   dgpu_prof_end(ctx, st);
-  DGPU_CUDA(ctx, cudaMemcpyAsync(edge_off, d_off, (n + 1) * 4, cudaMemcpyDeviceToHost, st));
-  if (fillcap) {
-    DGPU_CUDA(ctx, cudaMemcpyAsync(edge_j, d_ej, fillcap * 4, cudaMemcpyDeviceToHost, st));
-    DGPU_CUDA(ctx, cudaMemcpyAsync(edge_w, d_ew, fillcap * 4, cudaMemcpyDeviceToHost, st));
-  }
-  DGPU_CUDA(ctx, cudaStreamSynchronize(st));
+  if ((rc = s.finish())) return rc;
   return total > edge_cap ? DGPU_ERR_CAPACITY : DGPU_OK;
 }
 
@@ -240,7 +229,7 @@ extern "C" {
 int dgpu_cluster_edges_sr(dgpu_ctx* ctx, const int32_t* chr, const int32_t* pos, const int32_t* chr2, const int32_t* pos2, const int32_t* inslen,
                           uint64_t n, int svt, uint32_t max_read_sep, uint32_t* edge_off, uint32_t* edge_j, uint32_t* edge_w, uint64_t edge_cap,
                           uint64_t* n_edges) {
-  DgpuCallTrace trace_("dgpu_cluster_edges_sr", n);
+  DgpuStage s(ctx, "dgpu_cluster_edges_sr", n);
   if (!ctx || !edge_off || !n_edges) return DGPU_ERR_ARG;
   *n_edges = 0;
   if (n == 0) { edge_off[0] = 0; return DGPU_OK; }
@@ -248,13 +237,13 @@ int dgpu_cluster_edges_sr(dgpu_ctx* ctx, const int32_t* chr, const int32_t* pos,
   SrArgs a;
   a.n = (uint32_t) n; a.svt = svt; a.maxReadSep = max_read_sep;
   const void* cols[5] = {chr, pos, chr2, pos2, inslen};
-  return ce_run<true>(ctx, a, cols, 5, n, edge_off, edge_j, edge_w, edge_cap, n_edges);
+  return ce_run<true>(s, a, cols, 5, n, edge_off, edge_j, edge_w, edge_cap, n_edges);
 }
 
 int dgpu_cluster_edges_pe(dgpu_ctx* ctx, const int32_t* pos, const int32_t* mpos, const int32_t* mtid, const int32_t* alen, const int32_t* median,
                           const int32_t* max_normal_isize, uint64_t n, int svt, uint32_t varisize, uint32_t* edge_off, uint32_t* edge_j,
                           uint32_t* edge_w, uint64_t edge_cap, uint64_t* n_edges) {
-  DgpuCallTrace trace_("dgpu_cluster_edges_pe", n);
+  DgpuStage s(ctx, "dgpu_cluster_edges_pe", n);
   if (!ctx || !edge_off || !n_edges) return DGPU_ERR_ARG;
   *n_edges = 0;
   if (n == 0) { edge_off[0] = 0; return DGPU_OK; }
@@ -264,7 +253,7 @@ int dgpu_cluster_edges_pe(dgpu_ctx* ctx, const int32_t* pos, const int32_t* mpos
   PeArgs a;
   a.n = (uint32_t) n; a.svt = svt; a.varisize = varisize;
   const void* cols[6] = {pos, mpos, mtid, alen, median, max_normal_isize};
-  return ce_run<false>(ctx, a, cols, 6, n, edge_off, edge_j, edge_w, edge_cap, n_edges);
+  return ce_run<false>(s, a, cols, 6, n, edge_off, edge_j, edge_w, edge_cap, n_edges);
 }
 
 }  // extern "C"

@@ -46,21 +46,30 @@ inline void dgpu_prof_end(dgpu_ctx* ctx, cudaStream_t st) {
   if (ctx->profiling) { cudaEventRecord(ctx->ev1, st); ctx->ev_pending = true; }
 }
 
+// Scratch slots. No slot is both a staging slot and a workspace slot, so a device form may be called from inside a host form (or
+// from another device form) without clobbering what the caller staged.
 enum {
-  SLOT_SEQS = 0, SLOT_QOFF, SLOT_QLEN, SLOT_TOFF, SLOT_TLEN, SLOT_K, SLOT_DIST, SLOT_ENDLOC,
-  SLOT_PERM, SLOT_COUNTS, SLOT_WORK0, SLOT_WORK1, SLOT_WORK2, SLOT_WORK3,
-  SLOT_A0, SLOT_A1, SLOT_A2, SLOT_A3, SLOT_A4, SLOT_A5, SLOT_A6, SLOT_A7, SLOT_A8, SLOT_A9,
-  SLOT_EQTAB,
-  SLOT_EDBAND,  // job lists of the banded NW passes (edit_distance.cu)
+  // Staging slots: only DgpuStage (below) reserves these, for the caller's arrays of one host-pointer call.
+  SLOT_STAGE_ARENA = 0,  // the sequence arena
+  SLOT_STAGE_0,          // every other staged buffer, in the order the host form stages it: its large output buffer (ops / aln / cons,
+                         // the cluster-edge columns) first, so that one slot holds it across all host forms
+  SLOT_STAGE_END = SLOT_STAGE_0 + 11,
+  // Workspace slots: device forms and the functions they call reserve these, each slot only in the files named beside it.
+  // Inside one call a slot is re-reserved only after its previous contents are dead.
+  SLOT_JOB_PERM = SLOT_STAGE_END,  // job permutation by class (edit_distance.cu, long_needle.cu)
+  SLOT_COUNTS,       // class counts (edit_distance.cu, long_needle.cu); rank byte counts (gather.cu); the sink of int_peak.cu
+  SLOT_LN_JOBCLS,    // per-job class bytes of longNeedle (long_needle.cu)
+  SLOT_ED_STRIPES,   // stripe scratch of long edit-distance targets (edit_distance.cu)
+  SLOT_ED_BAND,      // job lists of the banded NW passes (edit_distance.cu)
+  SLOT_WAVEFRONT,    // wavefront workspace of the longNeedle and segment engines; their planners count its capacity as free
+                     // (long_needle.cu, edit_path.cu)
+  SLOT_MSA_SEGJOBS,  // MSA warp workspace (msa.cu); segment job arrays (edit_path.cu)
+  SLOT_EP_MIRROR,    // edit path: the reversed-sequence mirror of the HW start pass, then the traced leaf ops (edit_path.cu)
+  SLOT_EP_TABLE,     // edit path: HW-start target offsets, then the split selection, then the leaf table (edit_path.cu)
+  SLOT_EP_COLS,      // edit path: HW-start target lengths, then the half columns of the split pass (edit_path.cu)
+  SLOT_EP_BOUNDS,    // edit path: HW-start bounds and reverse end locations (edit_path.cu)
+  SLOT_EP_EQTAB,     // edit path: generalised-equality tables (edit_path.cu)
   SLOT_COUNT
-};
-
-// DGPU_TRACE=1: one stderr line per host-form batch call (name, items, wall ms) — where a pipeline stage's time goes, call by call
-struct DgpuCallTrace {
-  const char* name; uint64_t n; double t0; bool on;
-  static double now();
-  DgpuCallTrace(const char* nm, uint64_t items);
-  ~DgpuCallTrace();
 };
 
 #define DGPU_FORK_STREAMS 4
@@ -81,6 +90,74 @@ int dgpu_reserve(dgpu_ctx* ctx, int slot, size_t bytes, void** out);
     cudaError_t _e = cudaGetLastError();                               \
     if (_e != cudaSuccess) return dgpu_set_cuda_error((ctx), _e, name); \
   } while (0)
+
+// Lets `kernel` launch with `smem` bytes of dynamic shared memory (an opt-in above 48 KiB).
+template <typename K>
+int dgpu_smem_optin(dgpu_ctx* ctx, K* kernel, size_t smem, const char* name) {
+  if (smem <= 48 * 1024) return DGPU_OK;
+  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
+  return e == cudaSuccess ? DGPU_OK : dgpu_set_cuda_error(ctx, e, name);
+}
+
+// The device side of one host-pointer call (a host form of the C ABI): the device and stream, the staged copies of the caller's arrays
+// and, with DGPU_TRACE=1, one stderr line per call (name, items, wall ms): where a pipeline stage's time goes, call by call.
+// A host form checks the caller's buffers, open()s, stages, runs its _dev form on `st` and finish()es. Buffers take the staging
+// slots in the order they are staged; a null host array takes its slot and gives nullptr. A failing step leaves its code in `rc`
+// and later steps then do nothing, so one check of `rc` after staging covers them all.
+struct DgpuStage {
+  const char* name; uint64_t items; double t0 = 0; bool traced = false;
+  dgpu_ctx* ctx;
+  cudaStream_t st = nullptr, up = nullptr;  // the call's stream (the context stream); the stream uploads go on (st unless changed)
+  int rc = DGPU_OK, next = SLOT_STAGE_0;
+  struct Back { void* host; const void* dev; size_t bytes; };
+  std::vector<Back> back;  // copies for finish()
+
+  DgpuStage(dgpu_ctx* c, const char* nm, uint64_t n);
+  ~DgpuStage();
+  // every sequence [off[i], off[i] + len[i]), i < n, inside the caller's arena; else DGPU_ERR_ARG, "<name>: a <what> lies outside the arena"
+  int check_arena(uint64_t seqs_bytes, uint64_t n, const uint32_t* off, const uint32_t* len, const char* what = "sequence") {
+    for (uint64_t i = 0; i < n; ++i)
+      if ((uint64_t) off[i] + len[i] > seqs_bytes) { ctx->last_error = std::string(name) + ": a " + what + " lies outside the arena"; return DGPU_ERR_ARG; }
+    return DGPU_OK;
+  }
+  int open() {
+    DGPU_CUDA(ctx, cudaSetDevice(ctx->device));
+    st = up = ctx->stream;
+    return DGPU_OK;
+  }
+  // the arena, reserved as seqs_bytes + 64 so that 16 bytes past every sequence are readable (include/dgpu.h); seqs == nullptr: no upload
+  uint8_t* arena(const uint8_t* seqs, uint64_t seqs_bytes) {
+    void* d = nullptr;
+    if (!rc) rc = dgpu_reserve(ctx, SLOT_STAGE_ARENA, seqs_bytes + 64, &d);
+    if (seqs) upload(d, seqs, seqs_bytes);
+    return rc ? nullptr : (uint8_t*) d;
+  }
+  template <class T> T* alloc(size_t count) {  // the next staging slot
+    void* d = nullptr;
+    if (!rc && next >= SLOT_STAGE_END) { ctx->last_error = "DgpuStage: too many staged buffers"; rc = DGPU_ERR_ARG; }
+    if (!rc) rc = dgpu_reserve(ctx, next++, count * sizeof(T), &d);
+    return rc ? nullptr : (T*) d;
+  }
+  void upload(void* dev, const void* host, size_t bytes) {  // on `up`
+    cudaError_t e = rc ? cudaSuccess : cudaMemcpyAsync(dev, host, bytes, cudaMemcpyHostToDevice, up);
+    if (e != cudaSuccess) rc = dgpu_set_cuda_error(ctx, e, "cudaMemcpyAsync(host to device)");
+  }
+  template <class T> T* in(const T* host, size_t count) {
+    T* d = host ? alloc<T>(count) : (++next, nullptr);
+    if (host) upload(d, host, count * sizeof(T));
+    return d;
+  }
+  template <class T> T* out(T* host, size_t count, size_t pad = 0) {  // copied back into `host` by finish(); `pad` more elements reserved
+    T* d = host ? alloc<T>(count + pad) : (++next, nullptr);
+    if (host && !rc) back.push_back(Back{host, d, count * sizeof(T)});
+    return d;
+  }
+  int finish() {  // the copies back, in the order they were staged, then a synchronise of `st`
+    for (Back const& b : back) DGPU_CUDA(ctx, cudaMemcpyAsync(b.host, b.dev, b.bytes, cudaMemcpyDeviceToHost, st));
+    DGPU_CUDA(ctx, cudaStreamSynchronize(st));
+    return DGPU_OK;
+  }
+};
 
 // ---- unaligned 16-byte chunk reader over a byte arena -------------------------------
 // Reads sequence bytes [16*j, 16*j+16) of the sequence starting at `p` regardless of the

@@ -3,7 +3,6 @@
 #include <chrono>
 #include <cstdio>
 #include <cstdlib>
-#include <cstdio>
 #include <cstring>
 
 int dgpu_set_cuda_error(dgpu_ctx* ctx, cudaError_t e, const char* what) {
@@ -151,10 +150,9 @@ float dgpu_last_kernel_ms(dgpu_ctx* ctx) {
 
 }  // extern "C"
 
-double DgpuCallTrace::now() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
-DgpuCallTrace::DgpuCallTrace(const char* nm, uint64_t items) : name(nm), n(items), t0(0), on(false) {
+static double now_ms() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
+DgpuStage::DgpuStage(dgpu_ctx* c, const char* nm, uint64_t n) : name(nm), items(n), ctx(c) {
   static const bool enabled = getenv("DGPU_TRACE") != nullptr;
-  on = enabled;
-  if (on) t0 = now();
+  if ((traced = enabled)) t0 = now_ms();
 }
-DgpuCallTrace::~DgpuCallTrace() { if (on) fprintf(stderr, "[dgpu] %-22s %10llu items %9.2f ms\n", name, (unsigned long long) n, now() - t0); }
+DgpuStage::~DgpuStage() { if (traced) fprintf(stderr, "[dgpu] %-22s %10llu items %9.2f ms\n", name, (unsigned long long) items, now_ms() - t0); }

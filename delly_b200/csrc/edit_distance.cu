@@ -663,7 +663,7 @@ int launch_mode(dgpu_ctx* ctx, EdArgs& a, const uint32_t* hc, cudaStream_t st) {
     if (hc[24]) {
       a.hbuf_stride = (hc[24] + 255u) & ~255u;
       void* hb;
-      int rc = dgpu_reserve(ctx, SLOT_WORK0, (size_t) g * EDL_WARPS * a.hbuf_stride, &hb);
+      int rc = dgpu_reserve(ctx, SLOT_ED_STRIPES, (size_t) g * EDL_WARPS * a.hbuf_stride, &hb);
       if (rc) return rc;
       a.hbuf = (uint8_t*) hb;
     }
@@ -671,7 +671,7 @@ int launch_mode(dgpu_ctx* ctx, EdArgs& a, const uint32_t* hc, cudaStream_t st) {
       // band passes first (narrowest class first: a pass queues what it could not certify for the next one), the full matrix last
       const uint32_t cap = hc[5];
       void* lp;
-      int rc = dgpu_reserve(ctx, SLOT_EDBAND, (size_t) (EDB_CLASSES + 1) * cap * sizeof(uint32_t), &lp);
+      int rc = dgpu_reserve(ctx, SLOT_ED_BAND, (size_t) (EDB_CLASSES + 1) * cap * sizeof(uint32_t), &lp);
       if (rc) return rc;
       uint32_t* lists = (uint32_t*) lp;
       ed_band_plan_kernel<<<grid_for(hc[5], 8, 8), 256, 0, st>>>(a, lists, cap);
@@ -745,7 +745,7 @@ int dgpu_edit_distance_impl(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_by
   a.eq_f = eq_tabs; a.eq_s = eq_tabs ? eq_tabs + 256 : nullptr; a.eq_cls = eq_tabs ? (const uint8_t*) (eq_tabs + 512) : nullptr;
   a.force_long = eq_tabs ? 1 : 0;
   void* p;
-  int rc = dgpu_reserve(ctx, SLOT_PERM, n * sizeof(uint32_t), &p);
+  int rc = dgpu_reserve(ctx, SLOT_JOB_PERM, n * sizeof(uint32_t), &p);
   if (rc) return rc;
   a.perm = (uint32_t*) p;
   rc = dgpu_reserve(ctx, SLOT_COUNTS, 64 * sizeof(uint32_t), &p);
@@ -788,47 +788,34 @@ int dgpu_edit_distance(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
                        const uint32_t* t_off, const uint32_t* t_len,
                        const int32_t* k, int mode, uint64_t n,
                        int32_t* dist, int32_t* end_loc) {
-  DgpuCallTrace trace_("dgpu_edit_distance", n);
+  DgpuStage s(ctx, "dgpu_edit_distance", n);
   if (!ctx) return DGPU_ERR_ARG;
   if (n == 0) return DGPU_OK;
   if (!seqs || !q_off || !q_len || !t_off || !t_len || !dist) return DGPU_ERR_ARG;
   if (n >= (1ull << 31) || seqs_bytes >= (1ull << 32)) return DGPU_ERR_ARG;
+  const uint64_t njc = std::min<uint64_t>(ED_PIPE_MAX_CHUNKS, n / ED_PIPE_MIN_JOBS);
+  const bool pipelined = njc >= 2 && seqs_bytes >= (32u << 20);
+  int rc;
   // caller buffers: every sequence inside the arena. Small batches are checked here; the pipelined path below checks on the device while it
   // reduces the arena extents (a host loop over 10 M jobs would read 160 MB before the first upload)
-  const uint64_t njc0 = std::min<uint64_t>(ED_PIPE_MAX_CHUNKS, n / ED_PIPE_MIN_JOBS);
-  if (njc0 < 2 || seqs_bytes < (32u << 20))
-    for (uint64_t i = 0; i < n; ++i)
-      if ((uint64_t) q_off[i] + q_len[i] > seqs_bytes || (uint64_t) t_off[i] + t_len[i] > seqs_bytes) { ctx->last_error = "dgpu_edit_distance: a sequence lies outside the arena"; return DGPU_ERR_ARG; }
-  DGPU_CUDA(ctx, cudaSetDevice(ctx->device));
-  cudaStream_t st = ctx->stream;
-  void *d_seqs, *d_qoff, *d_qlen, *d_toff, *d_tlen, *d_k = nullptr, *d_dist, *d_end = nullptr;
-  int rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_SEQS, seqs_bytes + 64, &d_seqs))) return rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_QOFF, n * 4, &d_qoff))) return rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_QLEN, n * 4, &d_qlen))) return rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_TOFF, n * 4, &d_toff))) return rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_TLEN, n * 4, &d_tlen))) return rc;
-  if (k && (rc = dgpu_reserve(ctx, SLOT_K, n * 4, &d_k))) return rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_DIST, n * 4, &d_dist))) return rc;
-  if (end_loc && (rc = dgpu_reserve(ctx, SLOT_ENDLOC, n * 4, &d_end))) return rc;
+  if (!pipelined && ((rc = s.check_arena(seqs_bytes, n, q_off, q_len)) || (rc = s.check_arena(seqs_bytes, n, t_off, t_len)))) return rc;
+  if ((rc = s.open())) return rc;
+  cudaStream_t st = s.st;
+  if (pipelined) {   // the job metadata goes up on the copy stream, the arena piece by piece below
+    if ((rc = dgpu_pipe_init(ctx))) return rc;
+    s.up = ctx->copy_stream;
+  }
+  uint8_t* d_seqs = s.arena(pipelined ? nullptr : seqs, seqs_bytes);
+  uint32_t *d_qoff = s.in(q_off, n), *d_qlen = s.in(q_len, n), *d_toff = s.in(t_off, n), *d_tlen = s.in(t_len, n);
+  int32_t* d_k = s.in(k, n);
+  int32_t *d_dist = s.out(dist, n), *d_end = s.out(end_loc, n);
+  uint32_t* d_ext = pipelined ? s.alloc<uint32_t>(ED_PIPE_MAX_CHUNKS + 1) : nullptr;
+  if (s.rc) { cudaStreamSynchronize(s.up); return s.rc; }   // uploads already queued read the caller's arrays
 
   // Small batches: one copy-in, one pass, one copy-out on the context stream.
-  const uint64_t njc = std::min<uint64_t>(ED_PIPE_MAX_CHUNKS, n / ED_PIPE_MIN_JOBS);
-  if (njc < 2 || seqs_bytes < (32u << 20)) {
-    DGPU_CUDA(ctx, cudaMemcpyAsync(d_seqs, seqs, seqs_bytes, cudaMemcpyHostToDevice, st));
-    DGPU_CUDA(ctx, cudaMemcpyAsync(d_qoff, q_off, n * 4, cudaMemcpyHostToDevice, st));
-    DGPU_CUDA(ctx, cudaMemcpyAsync(d_qlen, q_len, n * 4, cudaMemcpyHostToDevice, st));
-    DGPU_CUDA(ctx, cudaMemcpyAsync(d_toff, t_off, n * 4, cudaMemcpyHostToDevice, st));
-    DGPU_CUDA(ctx, cudaMemcpyAsync(d_tlen, t_len, n * 4, cudaMemcpyHostToDevice, st));
-    if (k) DGPU_CUDA(ctx, cudaMemcpyAsync(d_k, k, n * 4, cudaMemcpyHostToDevice, st));
-    rc = dgpu_edit_distance_dev(ctx, (const uint8_t*) d_seqs, seqs_bytes, (const uint32_t*) d_qoff, (const uint32_t*) d_qlen,
-                                (const uint32_t*) d_toff, (const uint32_t*) d_tlen, (const int32_t*) d_k, mode, n,
-                                (int32_t*) d_dist, (int32_t*) d_end, st);
-    if (rc) return rc;
-    DGPU_CUDA(ctx, cudaMemcpyAsync(dist, d_dist, n * 4, cudaMemcpyDeviceToHost, st));
-    if (end_loc) DGPU_CUDA(ctx, cudaMemcpyAsync(end_loc, d_end, n * 4, cudaMemcpyDeviceToHost, st));
-    DGPU_CUDA(ctx, cudaStreamSynchronize(st));
-    return DGPU_OK;
+  if (!pipelined) {
+    if ((rc = dgpu_edit_distance_dev(ctx, d_seqs, seqs_bytes, d_qoff, d_qlen, d_toff, d_tlen, d_k, mode, n, d_dist, d_end, st))) return rc;
+    return s.finish();
   }
 
   // Large batches (the genotyping batch of src/coverage.h:412-454 is 131072 x threads jobs): the call is PCIe-bound
@@ -836,32 +823,22 @@ int dgpu_edit_distance(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
   // kernels. The job metadata goes first; the arena follows in ED_PIPE_PIECES pieces on a copy stream; the jobs
   // are cut into njc index ranges, and range c is launched as soon as the arena prefix it reads (its largest
   // q_off+q_len / t_off+t_len, reduced on the device from the uploaded metadata) has arrived. Results of a
-  // finished range go back on a third stream. Any job order is correct; arena-ordered jobs (the way batches are
-  // built: reads appended as they are scanned) overlap fully.
-  if ((rc = dgpu_pipe_init(ctx))) return rc;
+  // finished range go back on a third stream, not through s.finish(). Any job order is correct; arena-ordered
+  // jobs (the way batches are built: reads appended as they are scanned) overlap fully.
   cudaStream_t cs = ctx->copy_stream, os = ctx->out_stream;
   cudaEvent_t* ev = ctx->pipe_events.data();  // [0] metadata, [1..PIECES] arena pieces, [1+PIECES..] range done
-  DGPU_CUDA(ctx, cudaMemcpyAsync(d_qoff, q_off, n * 4, cudaMemcpyHostToDevice, cs));
-  DGPU_CUDA(ctx, cudaMemcpyAsync(d_qlen, q_len, n * 4, cudaMemcpyHostToDevice, cs));
-  DGPU_CUDA(ctx, cudaMemcpyAsync(d_toff, t_off, n * 4, cudaMemcpyHostToDevice, cs));
-  DGPU_CUDA(ctx, cudaMemcpyAsync(d_tlen, t_len, n * 4, cudaMemcpyHostToDevice, cs));
-  if (k) DGPU_CUDA(ctx, cudaMemcpyAsync(d_k, k, n * 4, cudaMemcpyHostToDevice, cs));
   DGPU_CUDA(ctx, cudaEventRecord(ev[0], cs));
   const uint64_t piece = (((seqs_bytes + ED_PIPE_PIECES - 1) / ED_PIPE_PIECES) + 0xfffffull) & ~0xfffffull;  // 1 MiB multiple
   int npieces = 0;
   for (uint64_t o = 0; o < seqs_bytes; o += piece, ++npieces) {
     const uint64_t len = std::min<uint64_t>(piece, seqs_bytes - o);
-    DGPU_CUDA(ctx, cudaMemcpyAsync((uint8_t*) d_seqs + o, seqs + o, len, cudaMemcpyHostToDevice, cs));
+    DGPU_CUDA(ctx, cudaMemcpyAsync(d_seqs + o, seqs + o, len, cudaMemcpyHostToDevice, cs));
     DGPU_CUDA(ctx, cudaEventRecord(ev[1 + npieces], cs));
   }
   const uint64_t jobs_per = (n + njc - 1) / njc;
-  void* p;
-  if ((rc = dgpu_reserve(ctx, SLOT_WORK1, (ED_PIPE_MAX_CHUNKS + 1) * sizeof(uint32_t), &p))) return rc;
-  uint32_t* d_ext = (uint32_t*) p;
   DGPU_CUDA(ctx, cudaStreamWaitEvent(st, ev[0], 0));
   DGPU_CUDA(ctx, cudaMemsetAsync(d_ext, 0, (ED_PIPE_MAX_CHUNKS + 1) * sizeof(uint32_t), st));
-  ed_extent_kernel<<<(unsigned) ((n + 255) / 256), 256, 0, st>>>((const uint32_t*) d_qoff, (const uint32_t*) d_qlen, (const uint32_t*) d_toff,
-                                                                 (const uint32_t*) d_tlen, (uint32_t) n, (uint32_t) jobs_per, (uint32_t) seqs_bytes, d_ext);
+  ed_extent_kernel<<<(unsigned) ((n + 255) / 256), 256, 0, st>>>(d_qoff, d_qlen, d_toff, d_tlen, (uint32_t) n, (uint32_t) jobs_per, (uint32_t) seqs_bytes, d_ext);
   DGPU_LAUNCH_CHECK(ctx, "ed_extent");
   uint32_t h_ext[ED_PIPE_MAX_CHUNKS + 1];
   DGPU_CUDA(ctx, cudaMemcpyAsync(h_ext, d_ext, sizeof(h_ext), cudaMemcpyDeviceToHost, st));
@@ -877,15 +854,14 @@ int dgpu_edit_distance(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
     const uint64_t cnt = std::min<uint64_t>(jobs_per, n - j0);
     const int need = h_ext[c] ? (int) ((h_ext[c] - 1) / piece) : 0;   // last arena piece this range reads
     DGPU_CUDA(ctx, cudaStreamWaitEvent(st, ev[1 + std::min(need, npieces - 1)], 0));
-    rc = dgpu_edit_distance_dev(ctx, (const uint8_t*) d_seqs, seqs_bytes, (const uint32_t*) d_qoff + j0, (const uint32_t*) d_qlen + j0,
-                                (const uint32_t*) d_toff + j0, (const uint32_t*) d_tlen + j0, d_k ? (const int32_t*) d_k + j0 : nullptr, mode, cnt,
-                                (int32_t*) d_dist + j0, d_end ? (int32_t*) d_end + j0 : nullptr, st);
+    rc = dgpu_edit_distance_dev(ctx, d_seqs, seqs_bytes, d_qoff + j0, d_qlen + j0, d_toff + j0, d_tlen + j0, d_k ? d_k + j0 : nullptr, mode, cnt,
+                                d_dist + j0, d_end ? d_end + j0 : nullptr, st);
     if (rc) { cudaStreamSynchronize(cs); return rc; }
     cudaEvent_t done = ev[1 + ED_PIPE_PIECES + c];
     DGPU_CUDA(ctx, cudaEventRecord(done, st));
     DGPU_CUDA(ctx, cudaStreamWaitEvent(os, done, 0));
-    DGPU_CUDA(ctx, cudaMemcpyAsync(dist + j0, (int32_t*) d_dist + j0, cnt * 4, cudaMemcpyDeviceToHost, os));
-    if (end_loc) DGPU_CUDA(ctx, cudaMemcpyAsync(end_loc + j0, (int32_t*) d_end + j0, cnt * 4, cudaMemcpyDeviceToHost, os));
+    DGPU_CUDA(ctx, cudaMemcpyAsync(dist + j0, d_dist + j0, cnt * 4, cudaMemcpyDeviceToHost, os));
+    if (end_loc) DGPU_CUDA(ctx, cudaMemcpyAsync(end_loc + j0, d_end + j0, cnt * 4, cudaMemcpyDeviceToHost, os));
   }
   DGPU_CUDA(ctx, cudaStreamSynchronize(cs));
   DGPU_CUDA(ctx, cudaStreamSynchronize(st));

@@ -417,11 +417,12 @@ struct SegRunner {
 
 template <int C, bool MULTI>
 int seg_launch(dgpu_ctx* ctx, SegJobs& a, bool use_eq, unsigned grid, unsigned threads, size_t smem, cudaStream_t st) {
+  int rc;
   if (use_eq) {
-    if (smem > 48 * 1024) cudaFuncSetAttribute(seg_kernel<C, MULTI, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
+    if ((rc = dgpu_smem_optin(ctx, seg_kernel<C, MULTI, true>, smem, "cudaFuncSetAttribute(seg_kernel)"))) return rc;
     seg_kernel<C, MULTI, true><<<grid, threads, smem, st>>>(a);
   } else {
-    if (smem > 48 * 1024) cudaFuncSetAttribute(seg_kernel<C, MULTI, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
+    if ((rc = dgpu_smem_optin(ctx, seg_kernel<C, MULTI, false>, smem, "cudaFuncSetAttribute(seg_kernel)"))) return rc;
     seg_kernel<C, MULTI, false><<<grid, threads, smem, st>>>(a);
   }
   DGPU_LAUNCH_CHECK(ctx, "seg_kernel");
@@ -454,7 +455,7 @@ int SegRunner::run(uint8_t* tmp_ops, int* colbuf) {
   // upload job arrays (one packed scratch buffer)
   const size_t bytes = N * (6 * 4 + 2 + 8 + 4 + 4) + 64 * 16;
   void* p;
-  if ((rc = dgpu_reserve(ctx, SLOT_WORK2, bytes + N * 4, &p))) return rc;
+  if ((rc = dgpu_reserve(ctx, SLOT_MSA_SEGJOBS, bytes + N * 4, &p))) return rc;
   uint8_t* base = (uint8_t*) p;
   auto carve = [&](size_t nbytes) { uint8_t* r = base; base += (nbytes + 15) & ~(size_t) 15; return r; };
   uint32_t* d_qoff = (uint32_t*) carve(N * 4); uint32_t* d_qlen = (uint32_t*) carve(N * 4);
@@ -507,10 +508,10 @@ int SegRunner::run(uint8_t* tmp_ops, int* colbuf) {
     a.work_stride = maxsteps * G * sizeof(uint4);
     size_t grid = std::min<size_t>((L.size() + (size_t) jpw * SEGB_WARPS - 1) / ((size_t) jpw * SEGB_WARPS), (size_t) ctx->num_sms * 8);
     const size_t per_block = (size_t) SEGB_WARPS * jpw * a.work_stride;
-    const size_t budget = (size_t) ((double) free_b * 0.6) + ctx->bufs[SLOT_WORK1].cap;
+    const size_t budget = (size_t) ((double) free_b * 0.6) + ctx->bufs[SLOT_WAVEFRONT].cap;
     if (per_block && grid * per_block > budget) grid = std::max<size_t>(1, budget / per_block);
     void* w;
-    if ((rc = dgpu_reserve(ctx, SLOT_WORK1, std::max<size_t>(grid * per_block, 256), &w))) return rc;
+    if ((rc = dgpu_reserve(ctx, SLOT_WAVEFRONT, std::max<size_t>(grid * per_block, 256), &w))) return rc;
     a.work = (uint8_t*) w;
     a.list = d_list + lo[12 + bc];
     a.count = (uint32_t) L.size();
@@ -539,10 +540,10 @@ int SegRunner::run(uint8_t* tmp_ops, int* colbuf) {
     const size_t smem = (mmax + 15) & ~(size_t) 15;
     const int per_sm = c <= 8 ? 16 : (c == 9 ? 4 : (c == 10 ? 2 : 1));
     size_t grid = std::min<size_t>(lists[c].size(), (size_t) ctx->num_sms * per_sm);
-    size_t budget = (size_t) ((double) free_b * 0.6) + ctx->bufs[SLOT_WORK1].cap;
+    size_t budget = (size_t) ((double) free_b * 0.6) + ctx->bufs[SLOT_WAVEFRONT].cap;
     if (grid * a.work_stride > budget) grid = std::max<size_t>(1, budget / a.work_stride);
     void* w;
-    if ((rc = dgpu_reserve(ctx, SLOT_WORK1, grid * a.work_stride, &w))) return rc;
+    if ((rc = dgpu_reserve(ctx, SLOT_WAVEFRONT, grid * a.work_stride, &w))) return rc;
     a.work = (uint8_t*) w;
     a.list = d_list + lo[c];
     a.count = (uint32_t) lists[c].size();
@@ -605,7 +606,7 @@ int dgpu_edit_path_ex_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_byte
       for (int sy = 0; sy < 5; ++sy)
         if (b == sym[sy] || (tab[b] & tab[256 + sym[sy]]) || (tab[256 + b] & tab[sym[sy]])) cls[b] |= (uint8_t) (1u << sy);
     void* d_tab;
-    if ((rc = dgpu_reserve(ctx, SLOT_EQTAB, sizeof(tab), &d_tab))) return rc;
+    if ((rc = dgpu_reserve(ctx, SLOT_EP_EQTAB, sizeof(tab), &d_tab))) return rc;
     DGPU_CUDA(ctx, cudaMemcpyAsync(d_tab, tab, sizeof(tab), cudaMemcpyHostToDevice, st));
     DGPU_CUDA(ctx, cudaStreamSynchronize(st));  // tab is a stack array
     R.eq.f = (const uint32_t*) d_tab; R.eq.s = (const uint32_t*) d_tab + 256; R.eq_cls = (const uint8_t*) ((const uint32_t*) d_tab + 512);
@@ -619,10 +620,10 @@ int dgpu_edit_path_ex_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_byte
     if (mode == DGPU_MODE_HW) {
       // 2. start location: reversed query vs reversed target prefix, SHW, k = distance, LAST optimal end
       void *d_mirror, *d_t2off, *d_t2len, *d_k2;
-      if ((rc = dgpu_reserve(ctx, SLOT_WORK3, seqs_bytes + 64, &d_mirror))) return rc;
-      if ((rc = dgpu_reserve(ctx, SLOT_A7, n * 4, &d_t2off))) return rc;
-      if ((rc = dgpu_reserve(ctx, SLOT_A8, n * 4, &d_t2len))) return rc;
-      if ((rc = dgpu_reserve(ctx, SLOT_A9, n * 8, &d_k2))) return rc;
+      if ((rc = dgpu_reserve(ctx, SLOT_EP_MIRROR, seqs_bytes + 64, &d_mirror))) return rc;
+      if ((rc = dgpu_reserve(ctx, SLOT_EP_TABLE, n * 4, &d_t2off))) return rc;
+      if ((rc = dgpu_reserve(ctx, SLOT_EP_COLS, n * 4, &d_t2len))) return rc;
+      if ((rc = dgpu_reserve(ctx, SLOT_EP_BOUNDS, n * 8, &d_k2))) return rc;
       d_rev = (uint8_t*) d_k2 + n * 4;
       const uint32_t wb = (uint32_t) ((n * 32 + 255) / 256);
       ep_mirror_kernel<<<wb, 256, 0, st>>>(seqs, (uint8_t*) d_mirror, q_off, q_len, (uint32_t) n);
@@ -675,11 +676,11 @@ int dgpu_edit_path_ex_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_byte
       }
     if (todo.empty()) break;
     void* d_col;
-    if ((rc = dgpu_reserve(ctx, SLOT_A8, (colpos + 16) * sizeof(int), &d_col))) return rc;
+    if ((rc = dgpu_reserve(ctx, SLOT_EP_COLS, (colpos + 16) * sizeof(int), &d_col))) return rc;
     if ((rc = R.run(nullptr, (int*) d_col))) return rc;
     const size_t S = todo.size();
     void* d_sel;
-    if ((rc = dgpu_reserve(ctx, SLOT_A7, S * (8 + 8 + 4 + 4 + 4 + 4 + 12) + 256, &d_sel))) return rc;
+    if ((rc = dgpu_reserve(ctx, SLOT_EP_TABLE, S * (8 + 8 + 4 + 4 + 4 + 4 + 12) + 256, &d_sel))) return rc;
     uint8_t* bp = (uint8_t*) d_sel;
     uint64_t* d_foff = (uint64_t*) bp; bp += S * 8;
     uint64_t* d_boff = (uint64_t*) bp; bp += S * 8;
@@ -737,7 +738,7 @@ int dgpu_edit_path_ex_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_byte
   }
   job_lo[n] = (uint32_t) leaf_kind.size();
   void* d_tmp;
-  if ((rc = dgpu_reserve(ctx, SLOT_WORK3, tmp_bytes + 64, &d_tmp))) return rc;
+  if ((rc = dgpu_reserve(ctx, SLOT_EP_MIRROR, tmp_bytes + 64, &d_tmp))) return rc;
   dgpu_prof_begin(ctx, st);
   if ((rc = R.run((uint8_t*) d_tmp, nullptr))) return rc;
   dgpu_prof_end(ctx, st);
@@ -765,7 +766,7 @@ int dgpu_edit_path_ex_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_byte
     }
   }
   void* d_leaf;
-  if ((rc = dgpu_reserve(ctx, SLOT_A7, (n + 1) * 4 + NL * 16 + 256, &d_leaf))) return rc;
+  if ((rc = dgpu_reserve(ctx, SLOT_EP_TABLE, (n + 1) * 4 + NL * 16 + 256, &d_leaf))) return rc;
   uint8_t* lp = (uint8_t*) d_leaf;
   uint64_t* d_loff = (uint64_t*) lp; lp += NL * 8;
   uint32_t* d_lo = (uint32_t*) lp; lp += (n + 1) * 4;
@@ -796,48 +797,26 @@ int dgpu_edit_path_ex(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
                       const uint32_t* q_off, const uint32_t* q_len, const uint32_t* t_off, const uint32_t* t_len,
                       int mode, const uint8_t* eq_pairs, uint32_t n_eq, uint64_t n, int32_t* dist, int32_t* start_loc, int32_t* end_loc,
                       uint8_t* ops, const uint64_t* ops_off, uint64_t ops_bytes, uint32_t* ops_len, uint32_t* status) {
-  DgpuCallTrace trace_("dgpu_edit_path", n);
+  DgpuStage s(ctx, "dgpu_edit_path", n);
   if (!ctx) return DGPU_ERR_ARG;
   if (n == 0) return DGPU_OK;
   if (!seqs || !q_off || !q_len || !t_off || !t_len || !dist || !start_loc || !end_loc || !ops || !ops_off || !ops_len || !status) return DGPU_ERR_ARG;
-  for (uint64_t i = 0; i < n; ++i) {   // caller buffers: sequences inside the arena, op slots (capacity |q| + |t|) inside ops_bytes
-    if ((uint64_t) q_off[i] + q_len[i] > seqs_bytes || (uint64_t) t_off[i] + t_len[i] > seqs_bytes) { ctx->last_error = "dgpu_edit_path: a sequence lies outside the arena"; return DGPU_ERR_ARG; }
-    if (ops_off[i] + q_len[i] + t_len[i] > ops_bytes) { ctx->last_error = "dgpu_edit_path: op slot beyond ops_bytes"; return DGPU_ERR_CAPACITY; }
-  }
-  DGPU_CUDA(ctx, cudaSetDevice(ctx->device));
-  cudaStream_t st = ctx->stream;
-  void *d_seqs, *d_qoff, *d_qlen, *d_toff, *d_tlen, *d_dist, *d_start, *d_end, *d_ops, *d_opsoff, *d_opslen, *d_status;
   int rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_SEQS, seqs_bytes + 64, &d_seqs))) return rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_QOFF, n * 4, &d_qoff))) return rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_QLEN, n * 4, &d_qlen))) return rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_TOFF, n * 4, &d_toff))) return rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_TLEN, n * 4, &d_tlen))) return rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_DIST, n * 4, &d_dist))) return rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_ENDLOC, n * 4, &d_end))) return rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_K, n * 4, &d_start))) return rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_A0, ops_bytes + 64, &d_ops))) return rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_A1, n * 8, &d_opsoff))) return rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_A2, n * 4, &d_opslen))) return rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_A3, n * 4, &d_status))) return rc;
-  DGPU_CUDA(ctx, cudaMemcpyAsync(d_seqs, seqs, seqs_bytes, cudaMemcpyHostToDevice, st));
-  DGPU_CUDA(ctx, cudaMemcpyAsync(d_qoff, q_off, n * 4, cudaMemcpyHostToDevice, st));
-  DGPU_CUDA(ctx, cudaMemcpyAsync(d_qlen, q_len, n * 4, cudaMemcpyHostToDevice, st));
-  DGPU_CUDA(ctx, cudaMemcpyAsync(d_toff, t_off, n * 4, cudaMemcpyHostToDevice, st));
-  DGPU_CUDA(ctx, cudaMemcpyAsync(d_tlen, t_len, n * 4, cudaMemcpyHostToDevice, st));
-  DGPU_CUDA(ctx, cudaMemcpyAsync(d_opsoff, ops_off, n * 8, cudaMemcpyHostToDevice, st));
-  rc = dgpu_edit_path_ex_dev(ctx, (const uint8_t*) d_seqs, seqs_bytes, (const uint32_t*) d_qoff, (const uint32_t*) d_qlen, (const uint32_t*) d_toff,
-                             (const uint32_t*) d_tlen, mode, eq_pairs, n_eq, n, (int32_t*) d_dist, (int32_t*) d_start, (int32_t*) d_end, (uint8_t*) d_ops,
-                             (const uint64_t*) d_opsoff, (uint32_t*) d_opslen, (uint32_t*) d_status, st);
-  if (rc) return rc;
-  DGPU_CUDA(ctx, cudaMemcpyAsync(dist, d_dist, n * 4, cudaMemcpyDeviceToHost, st));
-  DGPU_CUDA(ctx, cudaMemcpyAsync(start_loc, d_start, n * 4, cudaMemcpyDeviceToHost, st));
-  DGPU_CUDA(ctx, cudaMemcpyAsync(end_loc, d_end, n * 4, cudaMemcpyDeviceToHost, st));
-  DGPU_CUDA(ctx, cudaMemcpyAsync(ops, d_ops, ops_bytes, cudaMemcpyDeviceToHost, st));
-  DGPU_CUDA(ctx, cudaMemcpyAsync(ops_len, d_opslen, n * 4, cudaMemcpyDeviceToHost, st));
-  DGPU_CUDA(ctx, cudaMemcpyAsync(status, d_status, n * 4, cudaMemcpyDeviceToHost, st));
-  DGPU_CUDA(ctx, cudaStreamSynchronize(st));
-  return DGPU_OK;
+  if ((rc = s.check_arena(seqs_bytes, n, q_off, q_len)) || (rc = s.check_arena(seqs_bytes, n, t_off, t_len))) return rc;
+  for (uint64_t i = 0; i < n; ++i)   // op slots (capacity |q| + |t|) inside ops_bytes
+    if (ops_off[i] + q_len[i] + t_len[i] > ops_bytes) { ctx->last_error = "dgpu_edit_path: op slot beyond ops_bytes"; return DGPU_ERR_CAPACITY; }
+  if ((rc = s.open())) return rc;
+  const uint8_t* d_seqs = s.arena(seqs, seqs_bytes);
+  uint8_t* d_ops = s.out(ops, ops_bytes, 64);
+  const uint32_t *d_qoff = s.in(q_off, n), *d_qlen = s.in(q_len, n), *d_toff = s.in(t_off, n), *d_tlen = s.in(t_len, n);
+  const uint64_t* d_opsoff = s.in(ops_off, n);
+  int32_t *d_dist = s.out(dist, n), *d_start = s.out(start_loc, n), *d_end = s.out(end_loc, n);
+  uint32_t *d_opslen = s.out(ops_len, n), *d_status = s.out(status, n);
+  if (s.rc) return s.rc;
+  if ((rc = dgpu_edit_path_ex_dev(ctx, d_seqs, seqs_bytes, d_qoff, d_qlen, d_toff, d_tlen, mode, eq_pairs, n_eq, n, d_dist, d_start, d_end, d_ops,
+                                  d_opsoff, d_opslen, d_status, s.st)))
+    return rc;
+  return s.finish();
 }
 
 int dgpu_edit_path(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,

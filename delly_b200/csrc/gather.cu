@@ -158,13 +158,14 @@ int dgpu_gather_records(dgpu_ctx* ctx, void* comm, const void* local, uint64_t l
   }
   int rc = need_nccl(ctx);
   if (rc) return rc;
-  DGPU_CUDA(ctx, cudaSetDevice(ctx->device));
-  cudaStream_t st = ctx->stream;
+  DgpuStage s(ctx, "dgpu_gather_records", local_bytes);
+  if ((rc = s.open())) return rc;
+  cudaStream_t st = s.st;
   ncclComm_t c = (ncclComm_t) comm;
   int n = 0, me = 0;
   DGPU_NCCL(ctx, nccl().CommCount(c, &n), "ncclCommCount");
   DGPU_NCCL(ctx, nccl().CommUserRank(c, &me), "ncclCommUserRank");
-  void *d_cnt, *d_local, *d_all;
+  void* d_cnt;
   if ((rc = dgpu_reserve(ctx, SLOT_COUNTS, (size_t) (n + 1) * sizeof(uint64_t) + 1024, &d_cnt))) return rc;
   uint64_t* dc = (uint64_t*) d_cnt;   // [0..n-1] gathered counts, [n] this rank's count
   dgpu_prof_begin(ctx, st);
@@ -181,13 +182,14 @@ int dgpu_gather_records(dgpu_ctx* ctx, void* comm, const void* local, uint64_t l
   void* ha = malloc(total ? total : 1);
   if (!ha) { free(hc); return DGPU_ERR_CAPACITY; }
   if (total) {
-    if ((rc = dgpu_reserve(ctx, SLOT_A0, local_bytes + 16, &d_local)) || (rc = dgpu_reserve(ctx, SLOT_A1, total + 16, &d_all))) { free(hc); free(ha); return rc; }
+    uint8_t *d_local = s.alloc<uint8_t>(local_bytes + 16), *d_all = s.alloc<uint8_t>(total + 16);
+    if (s.rc) { free(hc); free(ha); return s.rc; }
     if (local_bytes) e = cudaMemcpyAsync(d_local, local, local_bytes, cudaMemcpyHostToDevice, st);
     if (e != cudaSuccess) { free(hc); free(ha); return dgpu_set_cuda_error(ctx, e, "gather H2D"); }
     ncclResult_t r0 = nccl().GroupStart();
     uint64_t off = 0;
     for (int r = 0; r < n && r0 == 0; ++r) {
-      if (hc[r]) r0 = nccl().Broadcast(d_local, (uint8_t*) d_all + off, (size_t) hc[r], NCCL_UINT8, r, c, st);
+      if (hc[r]) r0 = nccl().Broadcast(d_local, d_all + off, (size_t) hc[r], NCCL_UINT8, r, c, st);
       off += hc[r];
     }
     ncclResult_t r1 = nccl().GroupEnd();

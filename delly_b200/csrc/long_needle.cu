@@ -613,10 +613,8 @@ __global__ void __launch_bounds__(MAXT, (MAXT == 32 ? LN2_OCC : (MAXT == 64 ? LN
 
 template <int C, bool MULTI, int MAXT = 32>
 int ln_launch2(dgpu_ctx* ctx, LnArgs& a, int cls, unsigned grid, unsigned threads, size_t smem, cudaStream_t st) {
-  if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(ln_kernel2<C, MULTI, MAXT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
-    if (e != cudaSuccess) return dgpu_set_cuda_error(ctx, e, "cudaFuncSetAttribute(ln_kernel2)");
-  }
+  int rc = dgpu_smem_optin(ctx, ln_kernel2<C, MULTI, MAXT>, smem, "cudaFuncSetAttribute(ln_kernel2)");
+  if (rc) return rc;
   ln_kernel2<C, MULTI, MAXT><<<grid, threads, smem, st>>>(a, cls);
   DGPU_LAUNCH_CHECK(ctx, "ln_kernel2");
   return DGPU_OK;
@@ -624,10 +622,8 @@ int ln_launch2(dgpu_ctx* ctx, LnArgs& a, int cls, unsigned grid, unsigned thread
 
 template <int C, bool MULTI, int MAXT = 32>
 int ln_launch(dgpu_ctx* ctx, LnArgs& a, int cls, unsigned grid, unsigned threads, size_t smem, cudaStream_t st) {
-  if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(ln_kernel<C, MULTI, MAXT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
-    if (e != cudaSuccess) return dgpu_set_cuda_error(ctx, e, "cudaFuncSetAttribute(ln_kernel)");
-  }
+  int rc = dgpu_smem_optin(ctx, ln_kernel<C, MULTI, MAXT>, smem, "cudaFuncSetAttribute(ln_kernel)");
+  if (rc) return rc;
   ln_kernel<C, MULTI, MAXT><<<grid, threads, smem, st>>>(a, cls);
   DGPU_LAUNCH_CHECK(ctx, "ln_kernel");
   return DGPU_OK;
@@ -653,7 +649,7 @@ int dgpu_long_needle_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes
   a.aln = aln; a.aln_off = aln_off; a.aln_len = aln_len; a.ok = ok; a.info = info;
   void* p;
   int rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_PERM, n * sizeof(uint32_t), &p))) return rc;
+  if ((rc = dgpu_reserve(ctx, SLOT_JOB_PERM, n * sizeof(uint32_t), &p))) return rc;
   a.perm = (uint32_t*) p;
   if ((rc = dgpu_reserve(ctx, SLOT_COUNTS, 2048, &p))) return rc;
   a.counts = (uint32_t*) p;                                   // 96 uint32 = 384 B
@@ -661,7 +657,7 @@ int dgpu_long_needle_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes
   int* d_unsupported = (int*) ((uint8_t*) p + 1280);
   DGPU_CUDA(ctx, cudaMemsetAsync(p, 0, 2048, st));
   void* pc;
-  if ((rc = dgpu_reserve(ctx, SLOT_K, n + 64, &pc))) return rc;
+  if ((rc = dgpu_reserve(ctx, SLOT_LN_JOBCLS, n + 64, &pc))) return rc;
   a.jobcls = (uint8_t*) pc;
   const uint32_t cb = (uint32_t) ((n + 255) / 256);
   ln_count_kernel<<<(uint32_t) ((n * 32 + 255) / 256), 256, 0, st>>>(a, d_unsupported);
@@ -724,13 +720,13 @@ int dgpu_long_needle_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes
     total += pl.grid * pl.a.work_stride;
     plans.push_back(pl);
   }
-  const size_t budget = (size_t) ((double) free_b * 0.6) + ctx->bufs[SLOT_WORK1].cap;
+  const size_t budget = (size_t) ((double) free_b * 0.6) + ctx->bufs[SLOT_WAVEFRONT].cap;
   if (total > budget) {  // shrink every class's grid by the same factor (at least one CTA each)
     const double f = (double) budget / (double) total;
     total = 0;
     for (auto& pl : plans) { pl.grid = std::max<size_t>(1, (size_t) ((double) pl.grid * f)); total += pl.grid * pl.a.work_stride; }
   }
-  if ((rc = dgpu_reserve(ctx, SLOT_WORK1, total, &p))) return rc;
+  if ((rc = dgpu_reserve(ctx, SLOT_WAVEFRONT, total, &p))) return rc;
   { size_t off = 0; for (auto& pl : plans) { pl.a.work = (uint8_t*) p + off; off += pl.grid * pl.a.work_stride; } }
   const bool fork = plans.size() > 1;
   if (fork && (rc = dgpu_fork_init(ctx))) return rc;
@@ -791,44 +787,25 @@ int dgpu_long_needle(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
                      const uint32_t* c_off, const uint32_t* c_len, const uint32_t* r_off, const uint32_t* r_len,
                      uint64_t n, uint8_t* aln, const uint64_t* aln_off, uint64_t aln_bytes, uint32_t* aln_len, uint8_t* ok,
                      int32_t* info) {
-  DgpuCallTrace trace_("dgpu_long_needle", n);
+  DgpuStage s(ctx, "dgpu_long_needle", n);
   if (!ctx) return DGPU_ERR_ARG;
   if (n == 0) return DGPU_OK;
   if (!seqs || !c_off || !c_len || !r_off || !r_len || !aln || !aln_off || !aln_len || !ok) return DGPU_ERR_ARG;
-  for (uint64_t i = 0; i < n; ++i) {   // caller buffers: sequences inside the arena, alignment slots (2 rows of |cons| + |ref|) inside aln_bytes
-    if ((uint64_t) c_off[i] + c_len[i] > seqs_bytes || (uint64_t) r_off[i] + r_len[i] > seqs_bytes) { ctx->last_error = "dgpu_long_needle: a sequence lies outside the arena"; return DGPU_ERR_ARG; }
-    if (aln_off[i] + 2ull * ((uint64_t) c_len[i] + r_len[i]) > aln_bytes) { ctx->last_error = "dgpu_long_needle: alignment slot beyond aln_bytes"; return DGPU_ERR_CAPACITY; }
-  }
-  DGPU_CUDA(ctx, cudaSetDevice(ctx->device));
-  cudaStream_t st = ctx->stream;
-  void *d_seqs, *d_coff, *d_clen, *d_roff, *d_rlen, *d_aln, *d_aoff, *d_alen, *d_ok, *d_info = nullptr;
   int rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_SEQS, seqs_bytes + 64, &d_seqs))) return rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_QOFF, n * 4, &d_coff))) return rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_QLEN, n * 4, &d_clen))) return rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_TOFF, n * 4, &d_roff))) return rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_TLEN, n * 4, &d_rlen))) return rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_A0, aln_bytes + 64, &d_aln))) return rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_A1, n * 8, &d_aoff))) return rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_A2, n * 4, &d_alen))) return rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_A3, n, &d_ok))) return rc;
-  if (info && (rc = dgpu_reserve(ctx, SLOT_A4, n * 16, &d_info))) return rc;
-  DGPU_CUDA(ctx, cudaMemcpyAsync(d_seqs, seqs, seqs_bytes, cudaMemcpyHostToDevice, st));
-  DGPU_CUDA(ctx, cudaMemcpyAsync(d_coff, c_off, n * 4, cudaMemcpyHostToDevice, st));
-  DGPU_CUDA(ctx, cudaMemcpyAsync(d_clen, c_len, n * 4, cudaMemcpyHostToDevice, st));
-  DGPU_CUDA(ctx, cudaMemcpyAsync(d_roff, r_off, n * 4, cudaMemcpyHostToDevice, st));
-  DGPU_CUDA(ctx, cudaMemcpyAsync(d_rlen, r_len, n * 4, cudaMemcpyHostToDevice, st));
-  DGPU_CUDA(ctx, cudaMemcpyAsync(d_aoff, aln_off, n * 8, cudaMemcpyHostToDevice, st));
-  rc = dgpu_long_needle_dev(ctx, (const uint8_t*) d_seqs, seqs_bytes, (const uint32_t*) d_coff, (const uint32_t*) d_clen,
-                            (const uint32_t*) d_roff, (const uint32_t*) d_rlen, n, (uint8_t*) d_aln, (const uint64_t*) d_aoff,
-                            (uint32_t*) d_alen, (uint8_t*) d_ok, (int32_t*) d_info, st);
-  if (rc) return rc;
-  DGPU_CUDA(ctx, cudaMemcpyAsync(aln, d_aln, aln_bytes, cudaMemcpyDeviceToHost, st));
-  DGPU_CUDA(ctx, cudaMemcpyAsync(aln_len, d_alen, n * 4, cudaMemcpyDeviceToHost, st));
-  DGPU_CUDA(ctx, cudaMemcpyAsync(ok, d_ok, n, cudaMemcpyDeviceToHost, st));
-  if (info) DGPU_CUDA(ctx, cudaMemcpyAsync(info, d_info, n * 16, cudaMemcpyDeviceToHost, st));
-  DGPU_CUDA(ctx, cudaStreamSynchronize(st));
-  return DGPU_OK;
+  if ((rc = s.check_arena(seqs_bytes, n, c_off, c_len)) || (rc = s.check_arena(seqs_bytes, n, r_off, r_len))) return rc;
+  for (uint64_t i = 0; i < n; ++i)   // alignment slots (2 rows of |cons| + |ref|) inside aln_bytes
+    if (aln_off[i] + 2ull * ((uint64_t) c_len[i] + r_len[i]) > aln_bytes) { ctx->last_error = "dgpu_long_needle: alignment slot beyond aln_bytes"; return DGPU_ERR_CAPACITY; }
+  if ((rc = s.open())) return rc;
+  const uint8_t* d_seqs = s.arena(seqs, seqs_bytes);
+  uint8_t* d_aln = s.out(aln, aln_bytes, 64);
+  const uint32_t *d_coff = s.in(c_off, n), *d_clen = s.in(c_len, n), *d_roff = s.in(r_off, n), *d_rlen = s.in(r_len, n);
+  const uint64_t* d_aoff = s.in(aln_off, n);
+  uint32_t* d_alen = s.out(aln_len, n);
+  uint8_t* d_ok = s.out(ok, n);
+  int32_t* d_info = s.out(info, n * 4);   // null when the caller wants no info rows
+  if (s.rc) return s.rc;
+  if ((rc = dgpu_long_needle_dev(ctx, d_seqs, seqs_bytes, d_coff, d_clen, d_roff, d_rlen, n, d_aln, d_aoff, d_alen, d_ok, d_info, s.st))) return rc;
+  return s.finish();
 }
 
 }  // extern "C"

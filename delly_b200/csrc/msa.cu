@@ -743,11 +743,11 @@ int dgpu_msa_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
   A.work_stride = A.off_spans + al((size_t) MSA_N * 2 * MSA_MAXR * 2);
   const int per_sm = MSA_PER_SM;  // CTAs of four independent warps
   const size_t smem = sizeof(WarpSm) * MSA_WARPS;
-  DGPU_CUDA(ctx, cudaFuncSetAttribute(msa_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));   // per device and cheap: set on every call
+  int rc = dgpu_smem_optin(ctx, msa_kernel, smem, "cudaFuncSetAttribute(msa_kernel)");   // per device and cheap: set on every call
+  if (rc) return rc;
   size_t grid = std::min<size_t>((nclusters + MSA_WARPS - 1) / MSA_WARPS, (size_t) ctx->num_sms * per_sm);
   void* p;
-  int rc = dgpu_reserve(ctx, SLOT_WORK2, grid * MSA_WARPS * A.work_stride, &p);
-  if (rc) return rc;
+  if ((rc = dgpu_reserve(ctx, SLOT_MSA_SEGJOBS, grid * MSA_WARPS * A.work_stride, &p))) return rc;
   A.work = (uint8_t*) p;
   dgpu_prof_begin(ctx, st);
   msa_kernel<<<(unsigned) grid, MSA_T, smem, st>>>(A);
@@ -762,60 +762,33 @@ int dgpu_msa(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
              int match, int mismatch, int go, int ge, int min_clique,
              uint8_t* cons, const uint64_t* cons_off, uint64_t cons_bytes, uint32_t* cons_len, uint32_t* n_rows,
              uint32_t* status, uint8_t* aln, const uint64_t* aln_off, uint64_t aln_bytes, uint32_t* aln_cols) {
-  DgpuCallTrace trace_("dgpu_msa", nclusters);
+  DgpuStage s(ctx, "dgpu_msa", nclusters);
   if (!ctx) return DGPU_ERR_ARG;
   if (nclusters == 0) return DGPU_OK;
   if (!seqs || !read_off || !read_len || !cluster_off || !cons || !cons_off || !cons_len || !n_rows || !status) return DGPU_ERR_ARG;
-  {   // caller buffers: every read inside the arena, every consensus slot (capacity = the cluster's total read length) inside cons_bytes
-    for (uint32_t r = 0; r < nreads; ++r)
-      if ((uint64_t) read_off[r] + read_len[r] > seqs_bytes) { ctx->last_error = "dgpu_msa: a read lies outside the arena"; return DGPU_ERR_ARG; }
-    for (uint32_t i = 0; i < nclusters; ++i) {
-      if (cluster_off[i] > cluster_off[i + 1] || cluster_off[i + 1] > nreads) { ctx->last_error = "dgpu_msa: cluster_off is not a partition of the reads"; return DGPU_ERR_ARG; }
-      uint64_t cap = 0;
-      for (uint32_t r = cluster_off[i]; r < cluster_off[i + 1]; ++r) cap += read_len[r];
-      if (cons_off[i] + cap > cons_bytes) { ctx->last_error = "dgpu_msa: consensus slot beyond cons_bytes"; return DGPU_ERR_CAPACITY; }
-    }
-  }
-  DGPU_CUDA(ctx, cudaSetDevice(ctx->device));
-  cudaStream_t st = ctx->stream;
-  void *d_seqs, *d_roff, *d_rlen, *d_coff, *d_cons, *d_consoff, *d_conslen, *d_nrows, *d_status, *d_aln = nullptr, *d_alnoff = nullptr, *d_alncols = nullptr;
   int rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_SEQS, seqs_bytes + 64, &d_seqs))) return rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_QOFF, (size_t) nreads * 4, &d_roff))) return rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_QLEN, (size_t) nreads * 4, &d_rlen))) return rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_TOFF, ((size_t) nclusters + 1) * 4, &d_coff))) return rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_A0, cons_bytes + 64, &d_cons))) return rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_A1, (size_t) nclusters * 8, &d_consoff))) return rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_A2, (size_t) nclusters * 4, &d_conslen))) return rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_A3, (size_t) nclusters * 4, &d_nrows))) return rc;
-  if ((rc = dgpu_reserve(ctx, SLOT_A4, (size_t) nclusters * 4, &d_status))) return rc;
-  if (aln) {
-    if (!aln_off || !aln_cols) return DGPU_ERR_ARG;
-    if ((rc = dgpu_reserve(ctx, SLOT_A5, aln_bytes + 64, &d_aln))) return rc;
-    if ((rc = dgpu_reserve(ctx, SLOT_A6, (size_t) nclusters * 8, &d_alnoff))) return rc;
-    if ((rc = dgpu_reserve(ctx, SLOT_A7, (size_t) nclusters * 4, &d_alncols))) return rc;
-    DGPU_CUDA(ctx, cudaMemcpyAsync(d_alnoff, aln_off, (size_t) nclusters * 8, cudaMemcpyHostToDevice, st));
+  if ((rc = s.check_arena(seqs_bytes, nreads, read_off, read_len, "read"))) return rc;
+  for (uint32_t i = 0; i < nclusters; ++i) {   // consensus slots (capacity = the cluster's total read length) inside cons_bytes
+    if (cluster_off[i] > cluster_off[i + 1] || cluster_off[i + 1] > nreads) { ctx->last_error = "dgpu_msa: cluster_off is not a partition of the reads"; return DGPU_ERR_ARG; }
+    uint64_t cap = 0;
+    for (uint32_t r = cluster_off[i]; r < cluster_off[i + 1]; ++r) cap += read_len[r];
+    if (cons_off[i] + cap > cons_bytes) { ctx->last_error = "dgpu_msa: consensus slot beyond cons_bytes"; return DGPU_ERR_CAPACITY; }
   }
-  DGPU_CUDA(ctx, cudaMemcpyAsync(d_seqs, seqs, seqs_bytes, cudaMemcpyHostToDevice, st));
-  DGPU_CUDA(ctx, cudaMemcpyAsync(d_roff, read_off, (size_t) nreads * 4, cudaMemcpyHostToDevice, st));
-  DGPU_CUDA(ctx, cudaMemcpyAsync(d_rlen, read_len, (size_t) nreads * 4, cudaMemcpyHostToDevice, st));
-  DGPU_CUDA(ctx, cudaMemcpyAsync(d_coff, cluster_off, ((size_t) nclusters + 1) * 4, cudaMemcpyHostToDevice, st));
-  DGPU_CUDA(ctx, cudaMemcpyAsync(d_consoff, cons_off, (size_t) nclusters * 8, cudaMemcpyHostToDevice, st));
-  rc = dgpu_msa_dev(ctx, (const uint8_t*) d_seqs, seqs_bytes, (const uint32_t*) d_roff, (const uint32_t*) d_rlen,
-                    (const uint32_t*) d_coff, nclusters, match, mismatch, go, ge, min_clique, (uint8_t*) d_cons,
-                    (const uint64_t*) d_consoff, (uint32_t*) d_conslen, (uint32_t*) d_nrows, (uint32_t*) d_status,
-                    (uint8_t*) d_aln, (const uint64_t*) d_alnoff, (uint32_t*) d_alncols, st);
-  if (rc) return rc;
-  DGPU_CUDA(ctx, cudaMemcpyAsync(cons, d_cons, cons_bytes, cudaMemcpyDeviceToHost, st));
-  DGPU_CUDA(ctx, cudaMemcpyAsync(cons_len, d_conslen, (size_t) nclusters * 4, cudaMemcpyDeviceToHost, st));
-  DGPU_CUDA(ctx, cudaMemcpyAsync(n_rows, d_nrows, (size_t) nclusters * 4, cudaMemcpyDeviceToHost, st));
-  DGPU_CUDA(ctx, cudaMemcpyAsync(status, d_status, (size_t) nclusters * 4, cudaMemcpyDeviceToHost, st));
-  if (aln) {
-    DGPU_CUDA(ctx, cudaMemcpyAsync(aln, d_aln, aln_bytes, cudaMemcpyDeviceToHost, st));
-    DGPU_CUDA(ctx, cudaMemcpyAsync(aln_cols, d_alncols, (size_t) nclusters * 4, cudaMemcpyDeviceToHost, st));
-  }
-  DGPU_CUDA(ctx, cudaStreamSynchronize(st));
-  return DGPU_OK;
+  if (aln && (!aln_off || !aln_cols)) return DGPU_ERR_ARG;
+  if ((rc = s.open())) return rc;
+  const uint8_t* d_seqs = s.arena(seqs, seqs_bytes);
+  uint8_t* d_cons = s.out(cons, cons_bytes, 64);
+  const uint32_t *d_roff = s.in(read_off, nreads), *d_rlen = s.in(read_len, nreads), *d_coff = s.in(cluster_off, (size_t) nclusters + 1);
+  const uint64_t* d_consoff = s.in(cons_off, nclusters);
+  uint32_t *d_conslen = s.out(cons_len, nclusters), *d_nrows = s.out(n_rows, nclusters), *d_status = s.out(status, nclusters);
+  uint8_t* d_aln = s.out(aln, aln_bytes, 64);
+  const uint64_t* d_alnoff = s.in(aln ? aln_off : nullptr, nclusters);
+  uint32_t* d_alncols = s.out(aln ? aln_cols : nullptr, nclusters);
+  if (s.rc) return s.rc;
+  if ((rc = dgpu_msa_dev(ctx, d_seqs, seqs_bytes, d_roff, d_rlen, d_coff, nclusters, match, mismatch, go, ge, min_clique, d_cons, d_consoff, d_conslen,
+                         d_nrows, d_status, d_aln, d_alnoff, d_alncols, s.st)))
+    return rc;
+  return s.finish();
 }
 
 }  // extern "C"

@@ -75,3 +75,14 @@ def test_host_forms_check_caller_buffers(ctx):
     aln = np.zeros(32, np.uint8); ao = np.array([0], np.uint64); al = np.zeros(1, np.uint32); ok = np.zeros(1, np.uint8)
     rc = lib.dgpu_long_needle(ctx.h, p(arena), C.c_uint64(arena.nbytes), p(qo), p(ql), p(to), p(tl), C.c_uint64(1), p(aln), p(ao), C.c_uint64(32), p(al), p(ok), None)
     assert rc == -4
+    # dgpu_msa: two reads in one cluster; a consensus slot needs the cluster's total read length (80 bytes)
+    ro = np.array([0, 40], np.uint32); rl = np.array([40, 40], np.uint32); cons = np.zeros(16, np.uint8); co = np.array([0], np.uint64)
+    cl = np.zeros(1, np.uint32); nr = np.zeros(1, np.uint32); mst = np.zeros(1, np.uint32)
+    msa = lambda coff, cons_bytes: lib.dgpu_msa(ctx.h, p(arena), C.c_uint64(arena.nbytes), p(ro), p(rl), C.c_uint32(2), p(coff), C.c_uint32(1),
+                                                5, -4, -10, -1, 2, p(cons), p(co), C.c_uint64(cons_bytes), p(cl), p(nr), p(mst), None, None,
+                                                C.c_uint64(0), None)
+    rl[1] = 500
+    assert msa(np.array([0, 2], np.uint32), 128) == -2      # the second read runs off the arena
+    rl[1] = 40
+    assert msa(np.array([0, 3], np.uint32), 128) == -2      # cluster_off is not a partition of the two reads
+    assert msa(np.array([0, 2], np.uint32), 16) == -4       # the consensus slot needs 80 bytes, 16 were given
