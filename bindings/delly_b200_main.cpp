@@ -437,7 +437,8 @@ int main(int argc, char** argv) {
   const int r = o.lr ? runLr(o, dev, argv[0]) : runSr(o, dev);
   DeviceLimitLog const& lim = deviceLimitLog();
   if (lim.total())
-    std::cerr << "Warning: " << lim.msaClusters.load() << " read cluster(s), " << lim.pathJobs.load() << " edit-path job(s) and " << lim.needleJobs.load()
+    std::cerr << "Warning: " << lim.msaClusters.load() << " read cluster(s) (over " << DGPU_MSA_LARGE_MAXR << " reads, over 1023 alignment columns or a byte"
+              << " outside ACGTN), " << lim.pathJobs.load() << " edit-path job(s) and " << lim.needleJobs.load()
               << " consensus alignment(s) exceeded a device limit (include/dgpu.h) and were treated as failed alignments of their SV / read; the reference"
                  " has no such limits, so these records may differ from its output." << std::endl;
   // Every output is written and closed at this point. Tearing the CUDA context, the NCCL communicator and a few GB of device scratch down

@@ -14,6 +14,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("DGPU_LIB") or os.path.join(_HERE, "libdelly_b200.so")   # DGPU_LIB: development aid (kernel variants under variants/)
 
 MODE_NW, MODE_SHW, MODE_HW = 0, 1, 2
+MSA_LARGE_MAXR = 1023   # DGPU_MSA_LARGE_MAXR: the largest cluster Context.msa(max_reads=...) can compute
 
 _lib = None
 
@@ -179,8 +180,9 @@ class Context:
 
     # ------------------------------------------------------------------ msa
     def msa(self, seqs, read_off, read_len, cluster_off, sc=(5, -4, -10, -1), min_clique=2, want_alignment=False,
-            check=True):
-        """Host form. Returns (consensus list[bytes], n_rows, status[, alignments list[list[bytes]]])."""
+            check=True, max_reads=32):
+        """Host form. Returns (consensus list[bytes], n_rows, status[, alignments list[list[bytes]]]).
+        Clusters of more than max_reads (at most MSA_LARGE_MAXR) reads get status 1."""
         ncl = len(cluster_off) - 1
         rl = read_len.astype(np.uint64)
         csum = np.concatenate([[0], np.cumsum(rl)])
@@ -198,15 +200,15 @@ class Context:
             aln_bytes = int(acap.sum())
             aln = np.zeros(max(aln_bytes, 1), np.uint8)
             aln_cols = np.zeros(ncl, np.uint32)
-        rc = self._lib.dgpu_msa(self.h, _ptr(seqs), C.c_uint64(_nbytes(seqs)), _ptr(read_off), _ptr(read_len),
-                                C.c_uint32(len(read_off)), _ptr(cluster_off), C.c_uint32(ncl), int(sc[0]), int(sc[1]),
-                                int(sc[2]), int(sc[3]), int(min_clique), _ptr(cons), _ptr(cons_off), C.c_uint64(cons_bytes),
-                                _ptr(cons_len), _ptr(n_rows), _ptr(status), _ptr(aln), _ptr(aln_off), C.c_uint64(aln_bytes),
-                                _ptr(aln_cols))
-        self.check(rc, "dgpu_msa")
+        rc = self._lib.dgpu_msa_ex(self.h, _ptr(seqs), C.c_uint64(_nbytes(seqs)), _ptr(read_off), _ptr(read_len),
+                                   C.c_uint32(len(read_off)), _ptr(cluster_off), C.c_uint32(ncl), int(sc[0]), int(sc[1]),
+                                   int(sc[2]), int(sc[3]), int(min_clique), _ptr(cons), _ptr(cons_off), C.c_uint64(cons_bytes),
+                                   _ptr(cons_len), _ptr(n_rows), _ptr(status), _ptr(aln), _ptr(aln_off), C.c_uint64(aln_bytes),
+                                   _ptr(aln_cols), C.c_uint32(max_reads))
+        self.check(rc, "dgpu_msa_ex")
         if check and status.any():
-            raise DgpuError(f"dgpu_msa: {int((status != 0).sum())} cluster(s) rejected, first status codes "
-                            f"{status[status != 0][:5].tolist()} (1 >32 reads, 2 too long, 3 non-ACGTN byte)")
+            raise DgpuError(f"dgpu_msa_ex: {int((status != 0).sum())} cluster(s) rejected, first status codes "
+                            f"{status[status != 0][:5].tolist()} (1 >{max_reads} reads, 2 too long, 3 non-ACGTN byte)")
         out = [cons[int(o):int(o) + int(l)].tobytes() for o, l in zip(cons_off, cons_len)]
         if not want_alignment:
             return out, n_rows, status
@@ -217,12 +219,12 @@ class Context:
         return out, n_rows, status, alns
 
     def msa_dev(self, seqs, read_off, read_len, cluster_off, ncl, sc, min_clique, cons, cons_off, cons_len, n_rows, status,
-                stream=None):
-        rc = self._lib.dgpu_msa_dev(self.h, _ptr(seqs), C.c_uint64(seqs.numel()), _ptr(read_off), _ptr(read_len),
-                                    _ptr(cluster_off), C.c_uint32(ncl), int(sc[0]), int(sc[1]), int(sc[2]), int(sc[3]),
-                                    int(min_clique), _ptr(cons), _ptr(cons_off), _ptr(cons_len), _ptr(n_rows), _ptr(status),
-                                    _ptr(None), _ptr(None), _ptr(None), C.c_void_p(stream or 0))
-        self.check(rc, "dgpu_msa_dev")
+                stream=None, max_reads=32):
+        rc = self._lib.dgpu_msa_ex_dev(self.h, _ptr(seqs), C.c_uint64(seqs.numel()), _ptr(read_off), _ptr(read_len),
+                                       _ptr(cluster_off), C.c_uint32(ncl), int(sc[0]), int(sc[1]), int(sc[2]), int(sc[3]),
+                                       int(min_clique), _ptr(cons), _ptr(cons_off), _ptr(cons_len), _ptr(n_rows), _ptr(status),
+                                       _ptr(None), _ptr(None), _ptr(None), C.c_uint32(max_reads), C.c_void_p(stream or 0))
+        self.check(rc, "dgpu_msa_ex_dev")
 
 
 def _nbytes(x):

@@ -52,7 +52,7 @@ inline void parallelFor(std::size_t n, F&& fn, std::size_t minPerThread = 1) {
 // computed some other way and never aborts the run: it is treated as a FAILED alignment of that one SV / read (the reference's own
 // behaviour when an alignment fails: the SV stays imprecise or is dropped), counted here, and the binding reports the counts on stderr.
 struct DeviceLimitLog {
-  std::atomic<uint64_t> msaClusters{0};   // dgpu_msa status != 0: > 32 reads, > 1023 alignment columns, a byte outside ACGTN
+  std::atomic<uint64_t> msaClusters{0};   // dgpu_msa_ex status != 0: > DGPU_MSA_LARGE_MAXR reads, > 1023 alignment columns, a byte outside ACGTN
   std::atomic<uint64_t> pathJobs{0};      // dgpu_edit_path status != 0: target slice beyond the path kernel's window
   std::atomic<uint64_t> needleJobs{0};    // dgpu_long_needle: |cons| + |ref| > 32000 or |ref| > 16377
   uint64_t total() const { return msaClusters.load() + pathJobs.load() + needleJobs.load(); }

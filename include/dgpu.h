@@ -186,7 +186,7 @@ int dgpu_long_needle_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes
  * IN THE ORDER THE REFERENCE ITERATES ITS std::unordered_set (the caller preserves that order).
  * Outputs per cluster: consensus bytes at cons + cons_off[i] (reserve sum of the cluster's read
  * lengths), cons_len[i], n_rows[i] (= msa()'s return value), status[i]:
- *   0 ok; 1 more than 32 reads; 2 a read or an intermediate alignment exceeds 1023 columns / the
+ *   0 ok; 1 more than max_reads reads (32 for dgpu_msa / dgpu_msa_dev); 2 a read or an intermediate alignment exceeds 1023 columns / the
  *   per-cluster workspace; 3 a read contains a byte outside ACGTN (the reference's float profile is
  *   NaN there) — such clusters are NOT computed and the caller must treat them as errors.
  * Optional white-box output: the root alignment (n_rows x aln_cols, row-major) at aln + aln_off[i].
@@ -206,6 +206,25 @@ int dgpu_msa_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
                  uint8_t* cons, const uint64_t* cons_off,
                  uint32_t* cons_len, uint32_t* n_rows, uint32_t* status,
                  uint8_t* aln, const uint64_t* aln_off, uint32_t* aln_cols, void* stream);
+/* The _ex forms take max_reads, the largest cluster the caller wants computed (1 .. DGPU_MSA_LARGE_MAXR, else DGPU_ERR_ARG):
+ * clusters of up to 32 reads run one warp each, clusters of 33 .. max_reads one CTA each, larger ones get status 1. max_reads
+ * also sizes the large-cluster workspace (none when it is <= 32; about 17 MB per SM at 1023), so the device form needs no
+ * readback. dgpu_msa / dgpu_msa_dev are the _ex forms with max_reads = 32. */
+#define DGPU_MSA_LARGE_MAXR 1023
+int dgpu_msa_ex(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
+                const uint32_t* read_off, const uint32_t* read_len, uint32_t nreads,
+                const uint32_t* cluster_off, uint32_t nclusters,
+                int match, int mismatch, int go, int ge, int min_clique,
+                uint8_t* cons, const uint64_t* cons_off, uint64_t cons_bytes,
+                uint32_t* cons_len, uint32_t* n_rows, uint32_t* status,
+                uint8_t* aln, const uint64_t* aln_off, uint64_t aln_bytes, uint32_t* aln_cols, uint32_t max_reads);
+int dgpu_msa_ex_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
+                    const uint32_t* read_off, const uint32_t* read_len,
+                    const uint32_t* cluster_off, uint32_t nclusters,
+                    int match, int mismatch, int go, int ge, int min_clique,
+                    uint8_t* cons, const uint64_t* cons_off,
+                    uint32_t* cons_len, uint32_t* n_rows, uint32_t* status,
+                    uint8_t* aln, const uint64_t* aln_off, uint32_t* aln_cols, uint32_t max_reads, void* stream);
 
 /* ---- clustering graphs: candidate edges ------------------------------------------
  * Replaces the windowed pair scans inside cluster() — src/cluster.h:371-431 (SRBamRecord) and :551-623
