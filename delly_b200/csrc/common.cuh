@@ -209,11 +209,6 @@ struct ChunkReader {
   }
 };
 
-__device__ __forceinline__ uint32_t byte_of(const uint4& v, int b) {
-  uint32_t w = (b < 4) ? v.x : (b < 8) ? v.y : (b < 12) ? v.z : v.w;
-  return (w >> ((b & 3) * 8)) & 0xffu;
-}
-
 // DNA byte -> code: A0 C1 G2 T3 N4, anything else 5 (exact byte equality is preserved by
 // routing code 5 through an exact slow path in every kernel).
 __device__ __forceinline__ uint32_t dna_code(uint32_t c) {

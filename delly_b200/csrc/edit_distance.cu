@@ -30,10 +30,15 @@
 namespace {
 
 constexpr int ED_THREADS = 128;
-// grid cap of the one-thread-per-job kernels, in CTAs per SM: twice the 16 CTAs of 128 threads an H100 SM can hold, so that the grid-stride loops end
-// more evenly. On an H100 (10 M configs[1] jobs) 32 ran 3 % faster than 16 and 6 % faster than 8; 64 / 256 threads per CTA instead of
-// 128 changed nothing; a minimal shared-memory carveout (less occupancy) cost 23 %. Results identical in every variant.
-constexpr int ED_CTAS_PER_SM = 32;
+// grid cap of the one-thread-per-job kernels, in CTAs per SM. At 56-72 registers an SM holds 7-9 of these 128-thread CTAs, so the cap
+// launches several waves of CTAs that each take a slice of the grid-stride loop; later waves fill the SMs whose CTAs finished early. On an
+// H100 at 400 W (tools/bench_k1.py, the 10 M configs[1] jobs by class) 32 ran 8 % faster than 7 (one wave) and 3.5 % faster than 14;
+// 64 was 0.8 % faster than 32, too little to tell from run-to-run noise. Results identical in every variant. ED_CTAS_PER_SM_V lets
+// tools/build_variant.sh build such variants.
+#ifndef ED_CTAS_PER_SM_V
+#define ED_CTAS_PER_SM_V 32
+#endif
+constexpr int ED_CTAS_PER_SM = ED_CTAS_PER_SM_V;
 // job classes: 0 trivial, 1..4 = words per thread-job, 5 = warp-per-job
 
 struct EdArgs {
@@ -178,12 +183,20 @@ __device__ __forceinline__ int myers_column(uint32_t (&Pv)[NW], uint32_t (&Mv)[N
     Mh[w] = Pv[w] & Xh;
   }
   int d = (int) ((Ph[NW - 1] >> topbit) & 1u) - (int) ((Mh[NW - 1] >> topbit) & 1u);
+  // shift Ph / Mh up by one row across the words. Every index is a constant after unrolling, so the column stays in registers
+  // (a backward loop with a w == 0 case was left rolled by ptxas and put the arrays on the stack).
+  uint32_t ph[NW], mh[NW];
+  ph[0] = (Ph[0] << 1) | (uint32_t) HIN;
+  mh[0] = Mh[0] << 1;
 #pragma unroll
-  for (int w = NW - 1; w >= 0; --w) {
-    uint32_t ph = (w == 0) ? ((Ph[0] << 1) | (uint32_t) HIN) : __funnelshift_l(Ph[w - 1], Ph[w], 1);
-    uint32_t mh = (w == 0) ? (Mh[0] << 1) : __funnelshift_l(Mh[w - 1], Mh[w], 1);
-    Pv[w] = mh | ~(Xv[w] | ph);
-    Mv[w] = ph & Xv[w];
+  for (int w = 1; w < NW; ++w) {
+    ph[w] = __funnelshift_l(Ph[w - 1], Ph[w], 1);
+    mh[w] = __funnelshift_l(Mh[w - 1], Mh[w], 1);
+  }
+#pragma unroll
+  for (int w = 0; w < NW; ++w) {
+    Pv[w] = mh[w] | ~(Xv[w] | ph[w]);
+    Mv[w] = ph[w] & Xv[w];
   }
   return d;
 }
@@ -192,8 +205,31 @@ __device__ __forceinline__ int myers_column(uint32_t (&Pv)[NW], uint32_t (&Mv)[N
 // can turn four target bytes into four table offsets with packed arithmetic
 __device__ __forceinline__ uint32_t peq_slot(uint32_t code) { return code < 4 ? (code ^ (code >> 1)) : code; }
 
+// match bits of the four bytes of x that equal the byte s (s < 0x80), byte b -> bit b. Exact: a byte of v = x ^ s*0x01010101 is zero iff
+// its low seven bits carry nothing into bit 7 when 0x7f is added and its own bit 7 (that of x) is clear. The multiply moves bits 7, 15, 23,
+// 31 to 28..31 without overlapping any other product term.
+__device__ __forceinline__ uint32_t match4(uint32_t x, uint32_t s) {
+  const uint32_t t = ((x & 0x7f7f7f7fu) ^ (s * 0x01010101u)) + 0x7f7f7f7fu;
+  const uint32_t z = ~(t | x) & 0x80808080u;
+  return (z * 0x00204081u) >> 28;
+}
+
+// exact slow path for a target byte outside ACGTN: byte equality against the query rows q[0..len), len <= 32, bit i = row i. Kept out of
+// line so the column loop holds calls instead of one copy of the loop per column slot; one word per call, so the result comes back in a
+// register rather than through a stack frame.
+__device__ __noinline__ uint32_t eq_word_by_bytes(const uint8_t* q, uint32_t len, uint32_t c) {
+  uint32_t e = 0;
+  for (uint32_t i = 0; i < len; ++i)
+    if (__ldg(q + i) == (uint8_t) c) e |= 1u << i;
+  return e;
+}
+
+// Register budget: no occupancy floor (min 1 CTA), so ptxas keeps the column and the job state of every class in registers (56 / 64 / 72
+// registers for NW = 1 / 2 / 3, 0 spills). On an H100 (400 W) floors of 8 and 9 CTAs per SM (64 and 56 registers, still no spills) ran
+// NW = 1 and 2 at the same speed and NW = 3 1 % slower; floors of 10 and more spill. Without any bound ptxas aims at a higher occupancy
+// and spills in some instantiations.
 template <int NW, int MODE, bool WANT_END>
-__global__ void __launch_bounds__(ED_THREADS) ed_small_kernel(EdArgs a) {
+__global__ void __launch_bounds__(ED_THREADS, 1) ed_small_kernel(EdArgs a) {
   __shared__ uint32_t peq[5 * NW * ED_THREADS];
   constexpr int HIN = (MODE == DGPU_MODE_HW) ? 0 : 1;
   const uint32_t cnt = a.counts[NW];
@@ -205,7 +241,9 @@ __global__ void __launch_bounds__(ED_THREADS) ed_small_kernel(EdArgs a) {
     const uint8_t* q = a.seqs + a.q_off[job];
     const uint8_t* t = a.seqs + a.t_off[job];
 
-    // ---- build Peq (match masks) for A,C,G,T,N -----------------------------------
+    // ---- build Peq (match masks) for A,C,G,T,N, four query bytes at a time ------------
+    // Rows past |q| read whatever follows the query in the arena (the reader stays inside it); the last word is masked to |q|.
+    const uint32_t topbit = (m - 1) & 31u;
     {
       ChunkReader qr;
       qr.init(q, a.seqs_end);
@@ -214,22 +252,22 @@ __global__ void __launch_bounds__(ED_THREADS) ed_small_kernel(EdArgs a) {
         uint32_t pm[5] = {0, 0, 0, 0, 0};
 #pragma unroll
         for (int half = 0; half < 2; ++half) {
-          const uint32_t i0 = w * 32 + half * 16;
-          if (i0 < m) {
-            uint4 v = qr.next();
+          const uint4 v = qr.next();
+          const uint32_t wv[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
-            for (int b = 0; b < 16; ++b) {
-              if (i0 + b < m) {
-                uint32_t code = dna_code(byte_of(v, b));
-                uint32_t bit = 1u << (half * 16 + b);
-#pragma unroll
-                for (int s = 0; s < 5; ++s) pm[s] |= (code == (uint32_t) s) ? bit : 0u;
-              }
-            }
+          for (int k = 0; k < 4; ++k) {
+            const int sh = half * 16 + k * 4;
+            pm[0] |= match4(wv[k], 'A') << sh;
+            pm[1] |= match4(wv[k], 'C') << sh;
+            pm[2] |= match4(wv[k], 'G') << sh;
+            pm[3] |= match4(wv[k], 'T') << sh;
+            pm[4] |= match4(wv[k], 'N') << sh;
           }
         }
+        // jobs of this class have 32 (NW - 1) < |q| <= 32 NW, so only the last word holds rows past |q|
+        const uint32_t keep = (w == NW - 1) ? (2u << topbit) - 1u : 0xffffffffu;
 #pragma unroll
-        for (int s = 0; s < 5; ++s) peq[(peq_slot(s) * NW + w) * ED_THREADS + tid] = pm[s];
+        for (int s = 0; s < 5; ++s) peq[(peq_slot(s) * NW + w) * ED_THREADS + tid] = pm[s] & keep;
       }
     }
 
@@ -240,7 +278,6 @@ __global__ void __launch_bounds__(ED_THREADS) ed_small_kernel(EdArgs a) {
     // candidate end position -1 (score m) exists iff |q| % 64 != 0 (edlib's padding columns)
     int best = (m & 63u) ? (int) m : 0x7fffffff;
     int bpos = -1;
-    const uint32_t topbit = (m - 1) & 31u;
 
     auto step = [&](uint32_t c, uint32_t col) {
       uint32_t Eq[NW];
@@ -249,16 +286,8 @@ __global__ void __launch_bounds__(ED_THREADS) ed_small_kernel(EdArgs a) {
 #pragma unroll
         for (int w = 0; w < NW; ++w) Eq[w] = peq[(peq_slot(code) * NW + w) * ED_THREADS + tid];
       } else {
-        // exact slow path: byte equality against the query
 #pragma unroll
-        for (int w = 0; w < NW; ++w) Eq[w] = 0;
-        for (uint32_t i = 0; i < m; ++i) {
-          if (__ldg(q + i) == (uint8_t) c) {
-#pragma unroll
-            for (int w = 0; w < NW; ++w)
-              if ((int) (i >> 5) == w) Eq[w] |= 1u << (i & 31);
-          }
-        }
+        for (int w = 0; w < NW; ++w) Eq[w] = eq_word_by_bytes(q + w * 32, min(32u, m - w * 32), c);
       }
       score += myers_column<NW, HIN>(Pv, Mv, Eq, topbit);
       if (MODE != DGPU_MODE_NW) {
@@ -300,8 +329,9 @@ __global__ void __launch_bounds__(ED_THREADS) ed_small_kernel(EdArgs a) {
             }
           }
         } else {
-#pragma unroll
-          for (int b = 0; b < 4; ++b) step((wd >> (b * 8)) & 0xffu, c0 + q4 * 4 + b);
+          // a byte outside ACGT among the four: one rolled copy of the general step per word
+#pragma unroll 1
+          for (uint32_t b = 0; b < 4; ++b) step((wd >> (b * 8)) & 0xffu, c0 + q4 * 4 + b);
         }
       }
     }

@@ -1,0 +1,83 @@
+#!/usr/bin/env python
+"""K1 per query-length class: the configs[1] batch of bench.py (10 M HW edit-distance jobs, probes of 26-80 bp against 150 bp reads)
+split by words per thread-job, NW = ceil(|q| / 32), and each class timed on its own with the one-thread-per-job kernel
+ed_small_kernel<NW, HW>.
+
+  kernel_ms           median over the timed calls of the library's CUDA events around the class's kernel (ctx.last_kernel_ms())
+  jobs_per_s          jobs of the class / kernel_ms
+  thread_columns_per_s  DP columns one thread advances (sum of |t| over the class) / kernel_ms
+  window_s            sum of the timed kernel spans: at least --window seconds per class
+
+Every class stays device-resident; the inputs are uploaded once. The card's name, power limit and the SM clock sampled during the timed
+calls are part of the record.
+
+Usage: python tools/bench_k1.py [--jobs 10000000] [--window 1.2] [--out FILE]   (one JSON line on stdout, also written to FILE)
+"""
+import argparse
+import json
+import os
+import sys
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+import delly_b200  # noqa: E402
+from bench import ClockSampler, gpu_info, make_batch  # noqa: E402
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--jobs", type=int, default=10_000_000)
+    ap.add_argument("--window", type=float, default=1.2, help="seconds of timed kernel work per class")
+    ap.add_argument("--out")
+    a = ap.parse_args()
+    import torch
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    ctx = delly_b200.Context(0)
+    ctx.set_profiling(True)
+    b = make_batch(a.jobs, seed=1001)
+    nw = (b["q_len"].astype(np.int64) + 31) // 32
+    seqs = torch.from_numpy(b["seqs"]).to(dev)
+    stream = torch.cuda.current_stream().cuda_stream
+    classes = []
+    sampler = ClockSampler(0)
+    sampler.start()
+    for c in (1, 2, 3):
+        sel = np.nonzero(nw == c)[0]
+        if len(sel) == 0:
+            continue
+        d = {k: torch.from_numpy(np.ascontiguousarray(b[k][sel]).view(np.int32)).to(dev) for k in ("q_off", "q_len", "t_off", "t_len", "k")}
+        dist = torch.empty(len(sel), dtype=torch.int32, device=dev)
+
+        def call():
+            ctx.edit_distance_dev(seqs, d["q_off"], d["q_len"], d["t_off"], d["t_len"], d["k"], delly_b200.MODE_HW, dist, None, stream)
+            torch.cuda.synchronize()
+            return ctx.last_kernel_ms()
+
+        for _ in range(3):
+            est = call()
+        reps = max(10, int(np.ceil(a.window * 1e3 / est)))
+        ks = [call() for _ in range(reps)]
+        kms = float(np.median(ks))
+        cols = int(b["t_len"][sel].astype(np.int64).sum())
+        ql = b["q_len"][sel]
+        classes.append({"nw": c, "q_len": [int(ql.min()), int(ql.max())], "jobs": int(len(sel)), "share": len(sel) / len(nw),
+                        "kernel_ms": kms, "kernel_ms_min_max": [float(min(ks)), float(max(ks))], "reps": reps, "window_s": float(sum(ks)) * 1e-3,
+                        "jobs_per_s": len(sel) / (kms * 1e-3), "thread_columns_per_s": cols / (kms * 1e-3)})
+        del d, dist
+    clocks = sampler.stop()
+    res = {"workload": "configs[1] batch of bench.py split by NW = ceil(|q|/32); ed_small_kernel<NW, HW> per class",
+           "jobs": int(len(nw)), "lib": os.path.relpath(delly_b200.LIB_PATH, ROOT), "gpu": gpu_info(0), "clocks": clocks, "classes": classes}
+    line = json.dumps(res)
+    print(line)
+    if a.out:
+        with open(a.out, "w") as f:
+            f.write(line + "\n")
+    ctx.close()
+
+
+if __name__ == "__main__":
+    main()
