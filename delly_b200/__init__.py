@@ -108,6 +108,12 @@ class Context:
         self.check(self._lib.dgpu_int_peak(self.h, C.byref(t)), "dgpu_int_peak")
         return t.value
 
+    def int_peak_mix(self):
+        """1e12 instructions/s of LOP3 chains alone, with IMAD chains interleaved, and with IMAD.WIDE.U32 chains interleaved."""
+        t = (C.c_double * 3)()
+        self.check(self._lib.dgpu_int_peak_mix(self.h, t), "dgpu_int_peak_mix")
+        return {"lop3": t[0], "lop3_imad": t[1], "lop3_imad_wide": t[2]}
+
     @property
     def launches(self):
         return int(self._lib.dgpu_launch_count(self.h))

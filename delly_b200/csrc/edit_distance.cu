@@ -165,10 +165,16 @@ template <> struct AddChain<4> {
   }
 };
 
-// One DP column of the single-block Myers recurrence over NW 32-bit words.
-// HIN = horizontal delta entering the top row: 0 for HW (free start), +1 for NW/SHW.
-template <int NW, int HIN>
-__device__ __forceinline__ int myers_column(uint32_t (&Pv)[NW], uint32_t (&Mv)[NW], const uint32_t (&Eq)[NW], uint32_t topbit) {
+// One DP column of the single-block Myers recurrence over NW 32-bit words, adding the column's delta of D at the query's last row to
+// `score`. HIN = horizontal delta entering the top row: 0 for HW (free start), +1 for NW/SHW.
+// TOP: the query's last row is bit 31 of the last word (ed_small_kernel's HW layout); otherwise it is bit `topbit` of the last word.
+// The row shift across words is x * 2 + carry-in (an IMAD on the FMA pipe) with carry-out = hi(x * 2), and the bit-31 score update
+// is two mad.hi by 2, which ptxas turns into two LEA.HI instead of the 5 ALU instructions of a read at a variable bit. On an H100
+// (400 W) a multiplier ptxas cannot see, which keeps the mad.hi and the carries on the FMA pipe as IMAD.HI, made the K1 kernels
+// 3-8 % slower than this form: dgpu_int_peak_mix shows IMADs issuing alongside LOP3s at full rate, but IMAD.WIDE.U32 not.
+template <int NW, int HIN, bool TOP>
+__device__ __forceinline__ void myers_column(uint32_t (&Pv)[NW], uint32_t (&Mv)[NW], const uint32_t (&Eq)[NW], uint32_t topbit,
+                                             int& score) {
   uint32_t Xv[NW], t[NW], sum[NW], Ph[NW], Mh[NW];
 #pragma unroll
   for (int w = 0; w < NW; ++w) {
@@ -182,23 +188,28 @@ __device__ __forceinline__ int myers_column(uint32_t (&Pv)[NW], uint32_t (&Mv)[N
     Ph[w] = Mv[w] | ~(Xh | Pv[w]);
     Mh[w] = Pv[w] & Xh;
   }
-  int d = (int) ((Ph[NW - 1] >> topbit) & 1u) - (int) ((Mh[NW - 1] >> topbit) & 1u);
+  if (TOP) {
+    // score += Ph >> 31 (unsigned high word of Ph * 2) - Mh >> 31 (signed high word of Mh * 2: -1 iff bit 31 is set)
+    asm("mad.hi.u32 %0, %1, 2, %0;" : "+r"(score) : "r"(Ph[NW - 1]));
+    asm("mad.hi.s32 %0, %1, 2, %0;" : "+r"(score) : "r"(Mh[NW - 1]));
+  } else {
+    score += (int) ((Ph[NW - 1] >> topbit) & 1u) - (int) ((Mh[NW - 1] >> topbit) & 1u);
+  }
   // shift Ph / Mh up by one row across the words. Every index is a constant after unrolling, so the column stays in registers
   // (a backward loop with a w == 0 case was left rolled by ptxas and put the arrays on the stack).
-  uint32_t ph[NW], mh[NW];
-  ph[0] = (Ph[0] << 1) | (uint32_t) HIN;
-  mh[0] = Mh[0] << 1;
+  uint32_t ph[NW], mh[NW], cp = HIN, cm = 0;
 #pragma unroll
-  for (int w = 1; w < NW; ++w) {
-    ph[w] = __funnelshift_l(Ph[w - 1], Ph[w], 1);
-    mh[w] = __funnelshift_l(Mh[w - 1], Mh[w], 1);
+  for (int w = 0; w < NW; ++w) {
+    ph[w] = Ph[w] * 2u + cp;
+    mh[w] = Mh[w] * 2u + cm;
+    cp = __umulhi(Ph[w], 2u);
+    cm = __umulhi(Mh[w], 2u);
   }
 #pragma unroll
   for (int w = 0; w < NW; ++w) {
     Pv[w] = mh[w] | ~(Xv[w] | ph[w]);
     Mv[w] = ph[w] & Xv[w];
   }
-  return d;
 }
 
 // symbol slot in the shared Peq table: A0 C1 T2 G3 N4 — the order ((c >> 1) & 3) yields for ACGT, so the fast path
@@ -224,6 +235,17 @@ __device__ __noinline__ uint32_t eq_word_by_bytes(const uint8_t* q, uint32_t len
   return e;
 }
 
+// ed_small_kernel's HW layout: the m query rows move up by p = 32 NW - m (0..31) rows, so that the last one is bit 31 of the last word,
+// and the p rows below them become virtual rows that match every target byte (vmask). With HIN = 0 such rows keep Pv = Mv = 0 in every
+// column, compute Ph = Mh = 0 and carry nothing into the add chain, so they shift a 0 into the first query row, as the free top row of
+// HW does: bit 31 reads D[m][c] in every column. Rows past |q| drop out of the top. With HIN = 1 the rows would not be inert.
+template <int NW>
+__device__ __forceinline__ void rows_to_top(uint32_t (&e)[NW], uint32_t p, uint32_t vmask) {
+#pragma unroll
+  for (int w = NW - 1; w > 0; --w) e[w] = __funnelshift_l(e[w - 1], e[w], p);
+  e[0] = (e[0] << p) | vmask;
+}
+
 // Register budget: no occupancy floor (min 1 CTA), so ptxas keeps the column and the job state of every class in registers (56 / 64 / 72
 // registers for NW = 1 / 2 / 3, 0 spills). On an H100 (400 W) floors of 8 and 9 CTAs per SM (64 and 56 registers, still no spills) ran
 // NW = 1 and 2 at the same speed and NW = 3 1 % slower; floors of 10 and more spill. Without any bound ptxas aims at a higher occupancy
@@ -232,6 +254,7 @@ template <int NW, int MODE, bool WANT_END>
 __global__ void __launch_bounds__(ED_THREADS, 1) ed_small_kernel(EdArgs a) {
   __shared__ uint32_t peq[5 * NW * ED_THREADS];
   constexpr int HIN = (MODE == DGPU_MODE_HW) ? 0 : 1;
+  constexpr bool TOP = (MODE == DGPU_MODE_HW);  // query rows at the top of the bit-vector (rows_to_top)
   const uint32_t cnt = a.counts[NW];
   const uint32_t start = a.counts[8 + NW];
   const uint32_t tid = threadIdx.x;
@@ -242,14 +265,18 @@ __global__ void __launch_bounds__(ED_THREADS, 1) ed_small_kernel(EdArgs a) {
     const uint8_t* t = a.seqs + a.t_off[job];
 
     // ---- build Peq (match masks) for A,C,G,T,N, four query bytes at a time ------------
-    // Rows past |q| read whatever follows the query in the arena (the reader stays inside it); the last word is masked to |q|.
+    // Rows past |q| read whatever follows the query in the arena (the reader stays inside it); the last word is masked to |q|, or
+    // in the HW layout those rows are shifted out.
     const uint32_t topbit = (m - 1) & 31u;
+    const uint32_t p = 32u * NW - m, vmask = TOP ? (1u << p) - 1u : 0u;  // jobs of this class have 32 (NW - 1) < |q| <= 32 NW
     {
       ChunkReader qr;
       qr.init(q, a.seqs_end);
+      uint32_t pm[5][NW];
 #pragma unroll
       for (int w = 0; w < NW; ++w) {
-        uint32_t pm[5] = {0, 0, 0, 0, 0};
+#pragma unroll
+        for (int s = 0; s < 5; ++s) pm[s][w] = 0;
 #pragma unroll
         for (int half = 0; half < 2; ++half) {
           const uint4 v = qr.next();
@@ -257,23 +284,27 @@ __global__ void __launch_bounds__(ED_THREADS, 1) ed_small_kernel(EdArgs a) {
 #pragma unroll
           for (int k = 0; k < 4; ++k) {
             const int sh = half * 16 + k * 4;
-            pm[0] |= match4(wv[k], 'A') << sh;
-            pm[1] |= match4(wv[k], 'C') << sh;
-            pm[2] |= match4(wv[k], 'G') << sh;
-            pm[3] |= match4(wv[k], 'T') << sh;
-            pm[4] |= match4(wv[k], 'N') << sh;
+            pm[0][w] |= match4(wv[k], 'A') << sh;
+            pm[1][w] |= match4(wv[k], 'C') << sh;
+            pm[2][w] |= match4(wv[k], 'G') << sh;
+            pm[3][w] |= match4(wv[k], 'T') << sh;
+            pm[4][w] |= match4(wv[k], 'N') << sh;
           }
         }
-        // jobs of this class have 32 (NW - 1) < |q| <= 32 NW, so only the last word holds rows past |q|
-        const uint32_t keep = (w == NW - 1) ? (2u << topbit) - 1u : 0xffffffffu;
+      }
 #pragma unroll
-        for (int s = 0; s < 5; ++s) peq[(peq_slot(s) * NW + w) * ED_THREADS + tid] = pm[s] & keep;
+      for (int s = 0; s < 5; ++s) {
+        if (TOP) rows_to_top<NW>(pm[s], p, vmask);
+        else pm[s][NW - 1] &= (2u << topbit) - 1u;
+#pragma unroll
+        for (int w = 0; w < NW; ++w) peq[(peq_slot(s) * NW + w) * ED_THREADS + tid] = pm[s][w];
       }
     }
 
     uint32_t Pv[NW], Mv[NW];
 #pragma unroll
     for (int w = 0; w < NW; ++w) { Pv[w] = 0xffffffffu; Mv[w] = 0; }
+    Pv[0] = ~vmask;  // virtual rows start at Pv = Mv = 0
     int score = (int) m;
     // candidate end position -1 (score m) exists iff |q| % 64 != 0 (edlib's padding columns)
     int best = (m & 63u) ? (int) m : 0x7fffffff;
@@ -288,8 +319,9 @@ __global__ void __launch_bounds__(ED_THREADS, 1) ed_small_kernel(EdArgs a) {
       } else {
 #pragma unroll
         for (int w = 0; w < NW; ++w) Eq[w] = eq_word_by_bytes(q + w * 32, min(32u, m - w * 32), c);
+        if (TOP) rows_to_top<NW>(Eq, p, vmask);
       }
-      score += myers_column<NW, HIN>(Pv, Mv, Eq, topbit);
+      myers_column<NW, HIN, TOP>(Pv, Mv, Eq, topbit, score);
       if (MODE != DGPU_MODE_NW) {
         if (WANT_END) { if (score < best || (a.last_pos && score == best)) { best = score; bpos = (int) col; } }
         else best = min(best, score);
@@ -315,6 +347,7 @@ __global__ void __launch_bounds__(ED_THREADS, 1) ed_small_kernel(EdArgs a) {
           // byte offsets of the four Peq rows, two per register: slot * (NW*512) + tid*4
           const uint32_t offA = (x & 0x00ff00ffu) * (uint32_t) (NW * 4 * ED_THREADS) + base2;          // columns 0 and 2
           const uint32_t offB = ((x >> 8) & 0x00ff00ffu) * (uint32_t) (NW * 4 * ED_THREADS) + base2;   // columns 1 and 3
+          int prev = 0;
 #pragma unroll
           for (int b = 0; b < 4; ++b) {
             const uint32_t pk = (b & 1) ? offB : offA;
@@ -322,10 +355,11 @@ __global__ void __launch_bounds__(ED_THREADS, 1) ed_small_kernel(EdArgs a) {
             uint32_t Eq[NW];
 #pragma unroll
             for (int w = 0; w < NW; ++w) Eq[w] = *(const uint32_t*) ((const char*) peq + off + w * 4 * ED_THREADS);
-            score += myers_column<NW, HIN>(Pv, Mv, Eq, topbit);
+            myers_column<NW, HIN, TOP>(Pv, Mv, Eq, topbit, score);
             if (MODE != DGPU_MODE_NW) {
               if (WANT_END) { if (score < best || (a.last_pos && score == best)) { best = score; bpos = (int) (c0 + q4 * 4 + b); } }
-              else best = min(best, score);
+              else if (b & 1) best = min(best, min(prev, score));  // two columns per three-input min
+              else prev = score;
             }
           }
         } else {

@@ -82,6 +82,9 @@ float dgpu_last_kernel_ms(dgpu_ctx* ctx);
 /* Measured integer-ALU peak of this device: a LOP3/IADD3 micro-kernel, result in 1e12 int32 op/s.
  * MEASURED_PEAKS.json carries no integer peak, and this path is integer-pipe bound. */
 int dgpu_int_peak(dgpu_ctx* ctx, double* tera_ops_per_s);
+/* Whether IMADs issue to the FMA pipe alongside the integer ALU pipe: 1e12 instructions/s of [0] the LOP3 chains of dgpu_int_peak,
+ * [1] the same LOP3 chains with as many IMAD chains interleaved, [2] the same with IMAD.WIDE.U32 in place of the IMADs. */
+int dgpu_int_peak_mix(dgpu_ctx* ctx, double tera_instr_per_s[3]);
 
 /* ---- Myers bit-vector edit distance (replaces edlibAlign with EDLIB_TASK_DISTANCE) --
  * Call sites: _editDistanceHW, src/coverage.h:107-115 (two per AlignJob in process_batch,

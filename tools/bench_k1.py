@@ -9,7 +9,8 @@ ed_small_kernel<NW, HW>.
   window_s            sum of the timed kernel spans: at least --window seconds per class
 
 Every class stays device-resident; the inputs are uploaded once. The card's name, power limit and the SM clock sampled during the timed
-calls are part of the record.
+calls are part of the record, and so is ctx.int_peak_mix(): the instruction rate of LOP3 chains alone and with IMAD / IMAD.WIDE.U32
+chains interleaved, which shows whether the FMA pipe takes IMADs alongside the integer ALU pipe the kernel is bound by.
 
 Usage: python tools/bench_k1.py [--jobs 10000000] [--window 1.2] [--out FILE]   (one JSON line on stdout, also written to FILE)
 """
@@ -69,8 +70,10 @@ def main():
                         "jobs_per_s": len(sel) / (kms * 1e-3), "thread_columns_per_s": cols / (kms * 1e-3)})
         del d, dist
     clocks = sampler.stop()
+    mix = ctx.int_peak_mix()
     res = {"workload": "configs[1] batch of bench.py split by NW = ceil(|q|/32); ed_small_kernel<NW, HW> per class",
-           "jobs": int(len(nw)), "lib": os.path.relpath(delly_b200.LIB_PATH, ROOT), "gpu": gpu_info(0), "clocks": clocks, "classes": classes}
+           "jobs": int(len(nw)), "lib": os.path.relpath(delly_b200.LIB_PATH, ROOT), "gpu": gpu_info(0), "clocks": clocks,
+           "int_peak_mix_tera_instr_per_s": mix, "classes": classes}
     line = json.dumps(res)
     print(line)
     if a.out:

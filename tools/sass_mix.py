@@ -1,0 +1,121 @@
+#!/usr/bin/env python
+"""Per-column instruction mix of ed_small_kernel's four-column fast block, read from `cuobjdump -sass` of the built library.
+
+For each instantiation ed_small_kernel<NW, MODE, WANT_END> the SASS is split into basic blocks (labels and branches end a block).
+The fast block is the one with the most LDS: the four Myers columns of one target word whose bytes are all ACGT, with their Peq loads
+and the decode of the word. Its counts are divided by four and grouped by the pipe an instruction issues to:
+
+  alu   integer ALU pipe (16 lanes per SMSP: a warp instruction holds it for 2 cycles): LOP3, SHF, IADD3, VIMNMX*, LEA, PRMT, ISETP, SEL, ...
+  fma   FMA pipe: IMAD* (also the IMAD.MOV / IMAD.SHL forms ptxas uses to offload moves and shifts)
+  lds   shared-memory loads
+  vshr  variable-amount right shifts (SHF.R with a register shift amount) among the alu instructions
+
+Usage: python tools/sass_mix.py [LIB] [--json]   (LIB defaults to the in-tree delly_b200/libdelly_b200.so)
+"""
+import json
+import os
+import re
+import shutil
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+MODES = {0: "NW", 1: "SHW", 2: "HW"}
+ALU = ("LOP3", "LOP", "SHF", "IADD3", "VIMNMX", "VIMNMX3", "IMNMX", "LEA", "PRMT", "ISETP", "SEL", "IABS", "BMSK", "SGXT", "FLO", "POPC",
+       "PLOP3", "P2R", "R2P")
+BRANCH = ("BRA", "EXIT", "RET", "CALL", "BRX", "JMP", "JMX")
+INSN = re.compile(r"/\*[0-9a-f]+\*/\s+(@!?U?P\w+\s+)?([A-Z0-9_.]+)\s*([^;]*);")
+KERNEL = re.compile(r"ed_small_kernelILi(\d)ELi(\d)ELb(\d)E")
+
+
+def cuobjdump():
+    exe = shutil.which("cuobjdump")
+    if exe is None and os.path.exists("/usr/local/cuda/bin/cuobjdump"):
+        exe = "/usr/local/cuda/bin/cuobjdump"
+    return exe
+
+
+def functions(sass):
+    """{mangled name: [SASS lines]} of every function in the dump."""
+    out, name = {}, None
+    for line in sass.splitlines():
+        m = re.search(r"Function : (\S+)", line)
+        if m:
+            name = m.group(1)
+            out[name] = []
+        elif name:
+            out[name].append(line)
+    return out
+
+
+def blocks(lines):
+    """Basic blocks as lists of (opcode, operands)."""
+    cur, res = [], []
+    for line in lines:
+        if re.match(r"\s*\.L_\w+:", line):
+            if cur:
+                res.append(cur)
+            cur = []
+            continue
+        m = INSN.search(line)
+        if not m:
+            continue
+        cur.append((m.group(2), m.group(3)))
+        if m.group(2).split(".")[0] in BRANCH:
+            res.append(cur)
+            cur = []
+    if cur:
+        res.append(cur)
+    return res
+
+
+def mix(lines):
+    """Per-column counts of the fast block of one ed_small_kernel instantiation."""
+    fast = max(blocks(lines), key=lambda b: sum(op.startswith("LDS") for op, _ in b))
+    c = {"alu": 0, "fma": 0, "lds": 0, "other": 0, "vshr": 0}
+    ops = {}
+    for op, args in fast:
+        base = op.split(".")[0]
+        ops[base] = ops.get(base, 0) + 1
+        if base == "LDS":
+            c["lds"] += 1
+        elif base == "IMAD":
+            c["fma"] += 1
+        elif base in ALU:
+            c["alu"] += 1
+            # SHF.R.* with a register (not an immediate) shift amount: the third source operand
+            if base == "SHF" and ".R." in op + "." and re.match(r"\S+,\s*\S+,\s*R\d+(\.reuse)?,", args):
+                c["vshr"] += 1
+        elif base not in BRANCH:
+            c["other"] += 1
+    res = {k: v / 4 for k, v in c.items()}
+    res["ops"] = {k: v / 4 for k, v in sorted(ops.items())}
+    return res
+
+
+def report(lib):
+    sass = subprocess.run([cuobjdump(), "-sass", lib], capture_output=True, text=True, check=True).stdout
+    res = {}
+    for name, lines in functions(sass).items():
+        m = KERNEL.search(name)
+        if m:
+            nw, mode, end = int(m.group(1)), int(m.group(2)), int(m.group(3))
+            res[f"NW={nw} {MODES[mode]}{' end' if end else ''}"] = mix(lines)
+    return dict(sorted(res.items()))
+
+
+def main():
+    args = [a for a in sys.argv[1:] if not a.startswith("--")]
+    lib = args[0] if args else os.path.join(ROOT, "delly_b200", "libdelly_b200.so")
+    res = report(lib)
+    if "--json" in sys.argv:
+        print(json.dumps(res))
+        return
+    print(f"{'kernel':<16} {'alu':>6} {'fma':>6} {'lds':>5} {'other':>6} {'vshr':>5}   alu opcodes per column")
+    for k, v in res.items():
+        alu_ops = " ".join(f"{o}:{n:g}" for o, n in v["ops"].items() if o in ALU)
+        print(f"{k:<16} {v['alu']:6.2f} {v['fma']:6.2f} {v['lds']:5.2f} {v['other']:6.2f} {v['vshr']:5.2f}   {alu_ops}")
+
+
+if __name__ == "__main__":
+    main()
