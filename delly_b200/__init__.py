@@ -15,6 +15,7 @@ LIB_PATH = os.environ.get("DGPU_LIB") or os.path.join(_HERE, "libdelly_b200.so")
 
 MODE_NW, MODE_SHW, MODE_HW = 0, 1, 2
 MSA_LARGE_MAXR = 1023   # DGPU_MSA_LARGE_MAXR: the largest cluster Context.msa(max_reads=...) can compute
+LN_MAX_REF = 65535      # DGPU_LN_MAX_REF: the widest reference window Context.long_needle(max_ref=...) can compute
 
 _lib = None
 
@@ -156,8 +157,10 @@ class Context:
         return dist, st, en, [ops[int(o):int(o) + int(l)].tobytes() for o, l in zip(ops_off, ops_len)], status
 
     # ------------------------------------------------------------------ longNeedle
-    def long_needle(self, seqs, c_off, c_len, r_off, r_len, want_info=False):
-        """Host form. Returns (ok[uint8], aln_len[uint32], rows) where rows[i] = (row0 bytes, row1 bytes)."""
+    def long_needle(self, seqs, c_off, c_len, r_off, r_len, want_info=False, max_ref=None):
+        """Host form. Returns (ok[uint8], aln_len[uint32], rows) where rows[i] = (row0 bytes, row1 bytes).
+        max_ref=None: dgpu_long_needle (windows up to 16377 columns); otherwise dgpu_long_needle_ex, which also aligns wider windows
+        up to max_ref (at most LN_MAX_REF) columns. Jobs beyond the limits come back with ok = 0."""
         n = len(c_off)
         cap = (c_len.astype(np.uint64) + r_len.astype(np.uint64))
         aln_off = np.concatenate([[0], np.cumsum(2 * cap)[:-1]]).astype(np.uint64) if n else np.zeros(0, np.uint64)
@@ -166,22 +169,27 @@ class Context:
         aln_len = np.zeros(n, np.uint32)
         ok = np.zeros(n, np.uint8)
         info = np.zeros((n, 4), np.int32) if want_info else None
-        rc = self._lib.dgpu_long_needle(self.h, _ptr(seqs), C.c_uint64(_nbytes(seqs)), _ptr(c_off), _ptr(c_len), _ptr(r_off),
-                                        _ptr(r_len), C.c_uint64(n), _ptr(aln), _ptr(aln_off), C.c_uint64(aln_bytes),
-                                        _ptr(aln_len), _ptr(ok), _ptr(info))
-        self.check(rc, "dgpu_long_needle")
+        args = (self.h, _ptr(seqs), C.c_uint64(_nbytes(seqs)), _ptr(c_off), _ptr(c_len), _ptr(r_off), _ptr(r_len), C.c_uint64(n), _ptr(aln),
+                _ptr(aln_off), C.c_uint64(aln_bytes), _ptr(aln_len), _ptr(ok), _ptr(info))
+        if max_ref is None:
+            self.check(self._lib.dgpu_long_needle(*args), "dgpu_long_needle")
+        else:
+            self.check(self._lib.dgpu_long_needle_ex(*args, C.c_uint32(int(max_ref))), "dgpu_long_needle_ex")
         rows = []
         for i in range(n):
             o, L, c = int(aln_off[i]), int(aln_len[i]), int(cap[i])
             rows.append((aln[o:o + L].tobytes(), aln[o + c:o + c + L].tobytes()))
         return (ok, aln_len, rows, info) if want_info else (ok, aln_len, rows)
 
-    def long_needle_dev(self, seqs, c_off, c_len, r_off, r_len, aln, aln_off, aln_len, ok, info=None, stream=None):
+    def long_needle_dev(self, seqs, c_off, c_len, r_off, r_len, aln, aln_off, aln_len, ok, info=None, stream=None, max_ref=None):
+        """Device form (max_ref as in long_needle)."""
         n = c_off.numel()
-        rc = self._lib.dgpu_long_needle_dev(self.h, _ptr(seqs), C.c_uint64(seqs.numel()), _ptr(c_off), _ptr(c_len), _ptr(r_off),
-                                            _ptr(r_len), C.c_uint64(n), _ptr(aln), _ptr(aln_off), _ptr(aln_len), _ptr(ok),
-                                            _ptr(info), C.c_void_p(stream or 0))
-        self.check(rc, "dgpu_long_needle_dev")
+        args = (self.h, _ptr(seqs), C.c_uint64(seqs.numel()), _ptr(c_off), _ptr(c_len), _ptr(r_off), _ptr(r_len), C.c_uint64(n), _ptr(aln),
+                _ptr(aln_off), _ptr(aln_len), _ptr(ok), _ptr(info))
+        if max_ref is None:
+            self.check(self._lib.dgpu_long_needle_dev(*args, C.c_void_p(stream or 0)), "dgpu_long_needle_dev")
+        else:
+            self.check(self._lib.dgpu_long_needle_ex_dev(*args, C.c_uint32(int(max_ref)), C.c_void_p(stream or 0)), "dgpu_long_needle_ex_dev")
 
 
     # ------------------------------------------------------------------ msa

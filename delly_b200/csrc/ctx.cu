@@ -51,7 +51,7 @@ int dgpu_fork_init(dgpu_ctx* ctx) {
 
 extern "C" {
 
-int dgpu_version(void) { return 1002; }
+int dgpu_version(void) { return 1003; }
 
 const char* dgpu_strerror(int code) {
   switch (code) {

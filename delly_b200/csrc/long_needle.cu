@@ -58,6 +58,8 @@ struct LnArgs {
   uint8_t* work;                 // per-CTA workspace slabs
   size_t work_stride;
   size_t off_dirsR, off_dirsF, off_trace;  // offsets inside a slab (reverse prefix maxima at 0)
+  uint32_t max_ref;              // widest window the wide engine takes (0: none, the dgpu_long_needle forms)
+  unsigned long long wide_budget;  // workspace bytes one wide job may take
 };
 
 // columns per thread of a class
@@ -82,6 +84,47 @@ __host__ __device__ inline int ln_class(uint32_t m, uint32_t n) {
   return -1;
 }
 
+// ---- wide-window engine geometry (lnw_kernel below) --------------------------------------------------------------------------------
+// Jobs beyond ln_class's shapes. One 512-thread CTA per job computes the DP one whole ROW at a time: thread t owns J consecutive chunks
+// of 8 columns, the row's horizontal dependency is resolved by a block-wide max-scan, and the previous row lives in shared memory as int16
+// row-shifted scores U = H + r in [0, 2m]. So |cons| <= 16383 (LNW_MAX_CONS) is what int16 allows, and the window is bounded only by
+// shared memory (DGPU_LN_MAX_REF). Reverse prefix maxima are stored column-mirrored (element x at index n + 7 - x) and the reverse pass's
+// chunks start at column o <= 1 (o = n mod 8), so that both the reverse pass's stores and the forward pass's partner loads are aligned
+// 16-byte vectors. Workspace per job: 2 B (prefix maxima) + 2 x 0.5 B (direction nibbles) per cell.
+constexpr int LN_WIDE = LN_GEN;           // job class of the wide engine (class 0 + LN_GEN is never a class of the wavefront kernels)
+constexpr int LNW_THREADS = 512;
+constexpr int LNW_JMAX = 17;              // chunks per thread at DGPU_LN_MAX_REF: ceil(8193 / 512), odd
+constexpr uint32_t LNW_MAX_CONS = 16383;  // int16 row-shifted scores: U <= 2m <= 32766
+static_assert(((DGPU_LN_MAX_REF + 6) / 8 + 1 + LNW_THREADS - 1) / LNW_THREADS <= LNW_JMAX, "LNW_JMAX below the chunks of the widest window");
+
+struct LnwGeom {
+  int o;                     // first column of the reverse pass's chunk grid (o <= 1, o = n mod 8); the forward grid starts at 1
+  uint32_t nqR, nqF;         // chunks of 8 columns of the reverse / forward pass
+  uint32_t bstride;          // int16 per row of reverse prefix maxima
+  uint32_t dstride;          // nibble words per row of directions
+  unsigned long long off_dirsR, off_dirsF, off_trace, bytes;   // slab layout
+};
+__host__ __device__ inline unsigned long long lnw_al(unsigned long long x) { return (x + 255) & ~255ull; }
+__host__ __device__ inline LnwGeom lnw_geom(uint32_t m, uint32_t n) {
+  LnwGeom g;
+  g.o = 1 - (int) ((1u - n) & 7u);
+  g.nqR = (uint32_t) ((int) n - g.o) / 8 + 1;
+  g.nqF = (n + 7) / 8;
+  g.bstride = (n + 15 + 7) & ~7u;     // mirrored indices reach n + 13 (the grid's columns <= 0)
+  g.dstride = g.nqR;
+  const unsigned long long rows = (unsigned long long) m + 1;
+  g.off_dirsR = lnw_al(rows * g.bstride * 2);
+  g.off_dirsF = g.off_dirsR + lnw_al(rows * g.dstride * 4);
+  g.off_trace = g.off_dirsF + lnw_al(rows * g.dstride * 4);
+  g.bytes = g.off_trace + lnw_al(4ull * (m + n) + 64);
+  return g;
+}
+// dynamic shared memory of lnw_kernel for windows up to max_ref and consensus up to mmax
+inline size_t lnw_smem(uint32_t max_ref, size_t mmax) {
+  const size_t nq = (max_ref + 6) / 8 + 1;
+  return ((2 * (8 * nq + 8) + 15) & ~(size_t) 15) + 8 * nq + ((mmax + 15) & ~(size_t) 15);
+}
+
 // one WARP per job: class by shape, and whether every byte of both sequences is one of ACGTN (then the packed engine applies)
 __global__ void ln_count_kernel(LnArgs a, int* unsupported) {
   const uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -89,6 +132,7 @@ __global__ void ln_count_kernel(LnArgs a, int* unsupported) {
   if (i >= a.n) return;
   const uint32_t m = a.c_len[i], n = a.r_len[i];
   int c = ln_class(m, n);
+  if (c < 0 && n <= a.max_ref && m <= LNW_MAX_CONS && lnw_geom(m, n).bytes <= a.wide_budget) c = LN_WIDE;
   if (c < 0) {   // beyond the kernel's shapes: this ONE job is reported as not aligned (ok = 0, info[2] = -1) and counted; the batch goes on
     if (lane == 0) {
       atomicAdd(unsupported, 1);
@@ -98,7 +142,7 @@ __global__ void ln_count_kernel(LnArgs a, int* unsupported) {
     }
     return;
   }
-  if (c > 0) {
+  if (c > 0 && c != LN_WIDE) {   // (the wide engine compares bytes)
     bool bad = false;
     const uint8_t* s1 = a.seqs + a.c_off[i];
     const uint8_t* s2 = a.seqs + a.r_off[i];
@@ -110,6 +154,11 @@ __global__ void ln_count_kernel(LnArgs a, int* unsupported) {
   a.jobcls[i] = (uint8_t) c;
   atomicAdd(&a.counts[c], 1u);
   if (c == 0) { a.ok[i] = 0; a.aln_len[i] = 0; return; }
+  if (c == LN_WIDE) {   // slab bytes, not cells: the wide kernel lays its slab out per job (lnw_geom)
+    atomicMax(&a.maxcells[c], lnw_geom(m, n).bytes);
+    atomicMax(&a.maxcells[64 + c], (unsigned long long) m);
+    return;
+  }
   const int g = c & (LN_GEN - 1);
   atomicMax(&a.maxcells[c], (unsigned long long) (m + 1) * ln_bstride(n, ln_cols(g)));
   atomicMax(&a.maxcells[32 + c], (unsigned long long) (m + n));
@@ -611,6 +660,286 @@ __global__ void __launch_bounds__(MAXT, (MAXT == 32 ? LN2_OCC : (MAXT == 64 ? LN
   }
 }
 
+// ---- wide-window kernel (geometry and layout: lnw_geom) -------------------------------------------------------------------------------
+// Block-wide exclusive max-scan over the (at most 32) warps of the CTA: max(init, v of every lower thread). One block barrier; sm_w = 32 ints.
+__device__ __forceinline__ int lnw_excl_max(int v, int init, int* sm_w) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  int incl = v;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) { const int o = __shfl_up_sync(0xffffffffu, incl, d); if (lane >= d) incl = max(incl, o); }
+  int excl = __shfl_up_sync(0xffffffffu, incl, 1);
+  if (lane == 0) excl = init;
+  if (lane == 31) sm_w[w] = incl;
+  __syncthreads();
+  int pw = (lane < w) ? sm_w[lane] : init;
+#pragma unroll
+  for (int d = 16; d >= 1; d >>= 1) pw = max(pw, __shfl_xor_sync(0xffffffffu, pw, d));
+  return max(max(excl, pw), init);
+}
+
+// One DP pass of the wide engine over rows 1..m. Shared rows prepared by the caller: sm_rows[r-1] = row byte, sm_col[k] = byte of column
+// o + k (0 outside 1..n), sm_u[8 + k] = U of column o + k in the previous row (row 0: all 0), sm_u[7] = column o - 1.
+// Thread t owns chunks q = t*J .. t*J+J-1 (columns o + 8q .. o + 8q + 7); J is odd, so the 16-byte shared accesses of a warp are free of
+// bank conflicts. Per row, three sweeps over the thread's chunks:
+//   1. D = max(U_diag + (match ? 2 : 0), U_up), X = D + g*c; block max-scan of X: U[c] = max_{k<=c} X[k] - g*c (column 0: X = U = 0);
+//   2. U and its direction (vertical > horizontal > diagonal, as wavefront.cuh), U written over the previous row in place; block max-scan of U;
+//   3. the row's prefix maxima: REV stores them mirrored with the "equals the row maximum" bit, FWD evaluates the join of needle.h:104-115
+//      against the stored reverse row m - r, keeping the first maximum in row-major order.
+// Grid columns <= 0 (only the reverse grid has them) are pinned to the column-0 value U = 0. *corner receives H[m][n].
+template <bool REVP>
+__device__ __forceinline__ void lnw_pass(const uint8_t* sm_rows, const uint8_t* sm_col, int16_t* sm_u, int* sm_w, const int m, const int n, const int o,
+                                         const int nq, const int J, int16_t* __restrict__ brev, const uint32_t bstride, uint32_t* __restrict__ dirs,
+                                         const uint32_t dstride, wf::Best& best, int* corner) {
+  const int tid = threadIdx.x;
+  const int qa = tid * J;
+  for (int r = 1; r <= m; ++r) {
+    const int g = (r == m) ? 0 : 1;   // AlignConfig<true,false>: horizontal moves in the last row are free
+    const uint32_t a = sm_rows[r - 1];
+    const int u0 = (qa < nq) ? (int) sm_u[8 * qa + 7] : 0;   // previous row, column left of the first chunk (read before anyone overwrites it)
+    // ---- sweep 1: the row maximum of X per thread
+    int xmax = wf::NEG;
+    {
+      int pd = u0;
+#pragma unroll
+      for (int j = 0; j < LNW_JMAX; ++j) {
+        const int q = qa + j;
+        if (j < J && q < nq) {
+          const int cb = o + 8 * q;
+          const uint4 pv = *(const uint4*) (sm_u + 8 * q + 8);
+          const uint2 cv = *(const uint2*) (sm_col + 8 * q);
+          const uint32_t pw[4] = {pv.x, pv.y, pv.z, pv.w};
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            const int up = (int) ((pw[i >> 1] >> ((i & 1) * 16)) & 0xffffu);
+            const uint32_t b = (((i < 4) ? cv.x : cv.y) >> ((i & 3) * 8)) & 0xffu;
+            const int c = cb + i;
+            const int x = max(pd + (a == b ? 2 : 0), up) + g * c;
+            pd = up;
+            if (c >= 1) xmax = max(xmax, x);
+          }
+        }
+      }
+    }
+    const int carry = lnw_excl_max(xmax, 0, sm_w);
+    // ---- sweep 2: scores, directions, the row maximum of U per thread
+    int rmax = wf::NEG;
+    uint32_t dc[(LNW_JMAX + 1) / 2];   // 2-bit directions, two chunks per word (expanded to nibbles in sweep 3)
+#pragma unroll
+    for (int j = 0; j < (LNW_JMAX + 1) / 2; ++j) dc[j] = 0;
+    {
+      int pd = u0, pm = carry;
+      int ul = carry - g * (o + 8 * qa - 1);   // U of the column left of the first chunk, this row
+#pragma unroll
+      for (int j = 0; j < LNW_JMAX; ++j) {
+        const int q = qa + j;
+        if (j < J && q < nq) {
+          const int cb = o + 8 * q;
+          const uint4 pv = *(const uint4*) (sm_u + 8 * q + 8);
+          const uint2 cv = *(const uint2*) (sm_col + 8 * q);
+          const uint32_t pw[4] = {pv.x, pv.y, pv.z, pv.w};
+          uint32_t uw[4] = {0, 0, 0, 0};
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            const int up = (int) ((pw[i >> 1] >> ((i & 1) * 16)) & 0xffffu);
+            const uint32_t b = (((i < 4) ? cv.x : cv.y) >> ((i & 3) * 8)) & 0xffu;
+            const int c = cb + i;
+            const int x = max(pd + (a == b ? 2 : 0), up) + g * c;
+            pd = up;
+            int U = 0;
+            if (c >= 1) { pm = max(pm, x); U = pm - g * c; }
+            const uint32_t code = (U == up) ? 1u : ((U == ul - g) ? 2u : 0u);
+            ul = U;
+            rmax = max(rmax, U);
+            dc[j >> 1] |= code << ((j & 1) * 16 + i * 2);
+            uw[i >> 1] |= (uint32_t) U << ((i & 1) * 16);
+            if (r == m && c == n) *corner = U - m;
+          }
+          *(uint4*) (sm_u + 8 * q + 8) = make_uint4(uw[0], uw[1], uw[2], uw[3]);
+        }
+      }
+    }
+    const int carry2 = lnw_excl_max(rmax, 0, sm_w + 32);
+    // ---- sweep 3: prefix maxima
+    int rm = carry2;
+    if (!REVP && tid == 0) {   // column 0 (H = -r, shifted 0) against reverse row m - r at x = n (index 7)
+      const int v = (int) __ldcg(brev + (size_t) (m - r) * bstride + 7) - m;
+      if (v > best.val) { best.val = v; best.row = r; best.col = 0; best.bm = -r; }
+    }
+#pragma unroll
+    for (int j = 0; j < LNW_JMAX; ++j) {
+      const int q = qa + j;
+      if (j < J && q < nq) {
+        const int cb = o + 8 * q;
+        const uint4 uv = *(const uint4*) (sm_u + 8 * q + 8);
+        const uint32_t uw[4] = {uv.x, uv.y, uv.z, uv.w};
+        uint32_t dw = 0;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) dw |= ((dc[j >> 1] >> ((j & 1) * 16 + i * 2)) & 3u) << (i * 4);
+        if (REVP) {
+          uint32_t sw[4] = {0, 0, 0, 0};
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            const int U = (int) ((uw[i >> 1] >> ((i & 1) * 16)) & 0xffffu);
+            rm = max(rm, U);
+            if (U == rm) dw |= 4u << (i * 4);
+            const int h = 7 - i;   // column cb + i is element x = cb + i at index n + 7 - x = (n - cb) + h
+            sw[h >> 1] |= (uint32_t) rm << ((h & 1) * 16);
+          }
+          *(uint4*) (brev + (size_t) r * bstride + (n - cb)) = make_uint4(sw[0], sw[1], sw[2], sw[3]);
+        } else {
+          const uint4 pv = __ldcg((const uint4*) (brev + (size_t) (m - r) * bstride + cb + 7));   // partners x = n - c of columns cb ..
+          const uint32_t pw[4] = {pv.x, pv.y, pv.z, pv.w};
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            const int U = (int) ((uw[i >> 1] >> ((i & 1) * 16)) & 0xffffu);
+            rm = max(rm, U);
+            const int c = cb + i;
+            const int v = rm + (int) (int16_t) ((pw[i >> 1] >> ((i & 1) * 16)) & 0xffffu) - m;
+            if (c <= n && v > best.val) { best.val = v; best.row = r; best.col = c; best.bm = rm - r; }
+          }
+        }
+        dirs[(size_t) r * dstride + q] = dw;
+      }
+    }
+    if (REVP && tid == 0) brev[(size_t) r * bstride + n + 7] = 0;   // x = 0: H = -r, shifted 0
+  }
+}
+
+// One CTA per wide job: reverse pass, forward pass with the join, refRight, the two warp tracebacks and the stitched output, with the
+// semantics of ln_kernel (see the head of this file).
+__global__ void __launch_bounds__(LNW_THREADS, 1) lnw_kernel(LnArgs a) {
+  extern __shared__ uint8_t sm_dyn[];
+  const uint32_t nqmax = (a.max_ref + 6) / 8 + 1;
+  int16_t* sm_u = (int16_t*) sm_dyn;                                        // [8 * nqmax + 8]
+  uint8_t* sm_col = sm_dyn + ((2 * (8 * (size_t) nqmax + 8) + 15) & ~(size_t) 15);   // [8 * nqmax]
+  uint8_t* sm_rows = sm_col + 8 * (size_t) nqmax;                            // [m]
+  __shared__ int sm_w[64];
+  __shared__ int sm_pub[8];
+  __shared__ uint32_t sm_win[128];
+  __shared__ wf::Best sm_best[LNW_THREADS / 32];
+  const int tid = threadIdx.x;
+  const int lane = tid & 31;
+  const uint32_t cnt = a.counts[LN_WIDE], start = a.counts[32 + LN_WIDE];
+  uint8_t* slab = a.work + (size_t) blockIdx.x * a.work_stride;
+
+  for (uint32_t idx = blockIdx.x; idx < cnt; idx += gridDim.x) {
+    const uint32_t job = a.perm[start + idx];
+    const uint32_t m = a.c_len[job], n = a.r_len[job];
+    const uint8_t* s1 = a.seqs + a.c_off[job];
+    const uint8_t* s2 = a.seqs + a.r_off[job];
+    const LnwGeom G = lnw_geom(m, n);
+    int16_t* brev = (int16_t*) slab;
+    uint32_t* dirsR = (uint32_t*) (slab + G.off_dirsR);
+    uint32_t* dirsF = (uint32_t*) (slab + G.off_dirsF);
+    uint8_t* trace = slab + G.off_trace;
+    const int J = (int) (((G.nqR + LNW_THREADS - 1) / LNW_THREADS) | 1u);
+    __syncthreads();
+    // ---- reverse pass on (revcomp s1, revcomp s2) ----
+    for (uint32_t i = tid; i < m; i += LNW_THREADS) sm_rows[i] = revcomp_at(s1, m, i);
+    for (uint32_t k = tid; k < 8 * G.nqR; k += LNW_THREADS) {
+      const int c = G.o + (int) k;
+      sm_col[k] = (c >= 1 && c <= (int) n) ? revcomp_at(s2, n, (uint32_t) (c - 1)) : 0;
+    }
+    for (uint32_t k = tid; k < 8 * G.nqR + 8; k += LNW_THREADS) sm_u[k] = 0;
+    for (uint32_t k = tid; k < G.bstride; k += LNW_THREADS) brev[k] = 0;              // row 0: prefix maxima 0
+    for (uint32_t k = tid; k < G.dstride; k += LNW_THREADS) dirsR[k] = 0x44444444u;   // row 0: every cell equals its row maximum
+    __syncthreads();
+    wf::Best dummy;
+    lnw_pass<true>(sm_rows, sm_col, sm_u, sm_w, (int) m, (int) n, G.o, (int) G.nqR, J, brev, G.bstride, dirsR, G.dstride, dummy, &sm_pub[0]);
+    __syncthreads();
+    // ---- forward pass with the fused join ----
+    for (uint32_t i = tid; i < m; i += LNW_THREADS) sm_rows[i] = s1[i];
+    for (uint32_t k = tid; k < 8 * G.nqF; k += LNW_THREADS) sm_col[k] = (k < n) ? s2[k] : 0;   // grid origin 1: column k + 1
+    for (uint32_t k = tid; k < 8 * G.nqF + 8; k += LNW_THREADS) sm_u[k] = 0;
+    wf::Best best;
+    best.val = wf::NEG; best.row = 0; best.col = 0; best.bm = 0;
+    {  // join candidates of row 0: bestMat[0][c] = 0 against reverse row m at x = n - c (index c + 7)
+      const int16_t* prow = brev + (size_t) m * G.bstride;
+      for (uint32_t c = tid; c <= n; c += LNW_THREADS) {
+        const int v = (int) __ldcg(prow + c + 7) - (int) m;
+        if (v > best.val) { best.val = v; best.row = 0; best.col = (int) c; best.bm = 0; }
+      }
+    }
+    __syncthreads();
+    lnw_pass<false>(sm_rows, sm_col, sm_u, sm_w, (int) m, (int) n, 1, (int) G.nqF, J, brev, G.bstride, dirsF, G.dstride, best, &sm_pub[1]);
+#pragma unroll
+    for (int d = 16; d >= 1; d >>= 1) {
+      wf::Best o;
+      o.val = __shfl_xor_sync(0xffffffffu, best.val, d);
+      o.row = __shfl_xor_sync(0xffffffffu, best.row, d);
+      o.col = __shfl_xor_sync(0xffffffffu, best.col, d);
+      o.bm = __shfl_xor_sync(0xffffffffu, best.bm, d);
+      if (wf::best_before(o, best)) best = o;
+    }
+    if (lane == 0) sm_best[tid >> 5] = best;
+    __syncthreads();
+    best = sm_best[0];
+    for (int w = 1; w < LNW_THREADS / 32; ++w)
+      if (wf::best_before(sm_best[w], best)) best = sm_best[w];
+    const int revCorner = sm_pub[0], matCorner = sm_pub[1];
+    __syncthreads();
+    const int gbest = best.val, consLeft = best.row, refLeft = best.col, matv = best.bm;
+    const bool ok = (matCorner == revCorner) && (gbest != matCorner);  // needle.h:83-86, :152
+    if (!ok) {
+      if (tid == 0) {
+        a.ok[job] = 0; a.aln_len[job] = 0;
+        if (a.info) { a.info[4 * job] = consLeft; a.info[4 * job + 1] = refLeft; a.info[4 * job + 2] = 0; a.info[4 * job + 3] = gbest; }
+      }
+      continue;
+    }
+    // refRight (needle.h:116-123) from the stored prefix maxima and "equals maximum" bits, as in ln_kernel
+    const uint32_t consRight = m - (uint32_t) consLeft;
+    {
+      const int16_t* brow = brev + (size_t) consRight * G.bstride;
+      const uint32_t* drow = dirsR + (size_t) consRight * G.dstride;
+      const int target = gbest - matv + (int) consRight;
+      int bestRight = 0;
+      for (uint32_t x = tid; x <= n - (uint32_t) refLeft; x += LNW_THREADS) {
+        if ((int) __ldcg(brow + (n + 7 - x)) != target) continue;
+        bool eq = true;
+        if (x > 0) { const uint32_t k = (uint32_t) ((int) x - G.o); eq = ((__ldcg(drow + (k >> 3)) >> ((k & 7) * 4)) & 4u) != 0; }
+        if (eq) bestRight = max(bestRight, (int) x);
+      }
+#pragma unroll
+      for (int d = 16; d >= 1; d >>= 1) bestRight = max(bestRight, __shfl_xor_sync(0xffffffffu, bestRight, d));
+      if (lane == 0) sm_w[tid >> 5] = bestRight;
+      __syncthreads();
+      for (int w = 0; w < LNW_THREADS / 32; ++w) bestRight = max(bestRight, sm_w[w]);
+      if (tid == 0) sm_pub[2] = bestRight;
+      __syncthreads();
+    }
+    const uint32_t refRight = (uint32_t) sm_pub[2];
+    uint8_t* tFA = trace;
+    uint8_t* tFB = trace + (m + n);
+    uint8_t* tRA = trace + 2 * (size_t) (m + n);
+    uint8_t* tRB = trace + 3 * (size_t) (m + n);
+    if (tid < 32) {
+      const uint32_t v = ln_traceback_warp<false>(dirsF, G.dstride, 1, s1, m, s2, n, (uint32_t) consLeft, (uint32_t) refLeft, tFA, tFB, sm_win, lane);
+      if (lane == 0) sm_pub[3] = (int) v;
+    } else if (tid < 64) {
+      const uint32_t v = ln_traceback_warp<true>(dirsR, G.dstride, G.o, s1, m, s2, n, consRight, refRight, tRA, tRB, sm_win + 64, lane);
+      if (lane == 0) sm_pub[4] = (int) v;
+    }
+    __syncthreads();
+    const uint32_t Lf = (uint32_t) sm_pub[3], Lr = (uint32_t) sm_pub[4];
+    const uint32_t gapref = (n - refRight) - (uint32_t) refLeft;
+    const uint32_t L = Lf + gapref + Lr;
+    uint8_t* o0 = a.aln + a.aln_off[job];
+    uint8_t* o1 = o0 + (m + n);
+    for (uint32_t i = tid; i < L; i += LNW_THREADS) {
+      uint8_t x, y;
+      if (i < Lf) { x = tFA[Lf - 1 - i]; y = tFB[Lf - 1 - i]; }
+      else if (i < Lf + gapref) { x = '-'; y = s2[refLeft + (i - Lf)]; }
+      else { x = tRA[i - Lf - gapref]; y = tRB[i - Lf - gapref]; }
+      o0[i] = x; o1[i] = y;
+    }
+    if (tid == 0) {
+      a.ok[job] = 1; a.aln_len[job] = L;
+      if (a.info) { a.info[4 * job] = consLeft; a.info[4 * job + 1] = refLeft; a.info[4 * job + 2] = (int) refRight; a.info[4 * job + 3] = gbest; }
+    }
+  }
+}
+
 template <int C, bool MULTI, int MAXT = 32>
 int ln_launch2(dgpu_ctx* ctx, LnArgs& a, int cls, unsigned grid, unsigned threads, size_t smem, cudaStream_t st) {
   int rc = dgpu_smem_optin(ctx, ln_kernel2<C, MULTI, MAXT>, smem, "cudaFuncSetAttribute(ln_kernel2)");
@@ -629,15 +958,16 @@ int ln_launch(dgpu_ctx* ctx, LnArgs& a, int cls, unsigned grid, unsigned threads
   return DGPU_OK;
 }
 
-}  // namespace
+int check_max_ref(dgpu_ctx* ctx, uint32_t max_ref) {
+  if (max_ref >= 1 && max_ref <= DGPU_LN_MAX_REF) return DGPU_OK;
+  ctx->last_error = "dgpu_long_needle_ex: max_ref must be 1 .. " + std::to_string(DGPU_LN_MAX_REF);
+  return DGPU_ERR_ARG;
+}
 
-extern "C" {
-
-int dgpu_long_needle_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
-                         const uint32_t* c_off, const uint32_t* c_len, const uint32_t* r_off, const uint32_t* r_len,
-                         uint64_t n, uint8_t* aln, const uint64_t* aln_off, uint32_t* aln_len, uint8_t* ok,
-                         int32_t* info, void* stream) {
-  if (!ctx) return DGPU_ERR_ARG;
+// the device form of both entry points; max_ref = 0: no wide engine (dgpu_long_needle_dev)
+int ln_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes, const uint32_t* c_off, const uint32_t* c_len, const uint32_t* r_off,
+           const uint32_t* r_len, uint64_t n, uint8_t* aln, const uint64_t* aln_off, uint32_t* aln_len, uint8_t* ok, int32_t* info,
+           uint32_t max_ref, void* stream) {
   if (n == 0) return DGPU_OK;
   if (n >= (1ull << 31) || seqs_bytes >= (1ull << 32)) return DGPU_ERR_ARG;
   if (!seqs || !c_off || !c_len || !r_off || !r_len || !aln || !aln_off || !aln_len || !ok) return DGPU_ERR_ARG;
@@ -647,8 +977,14 @@ int dgpu_long_needle_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes
   a.seqs = seqs;
   a.c_off = c_off; a.c_len = c_len; a.r_off = r_off; a.r_len = r_len; a.n = (uint32_t) n;
   a.aln = aln; a.aln_off = aln_off; a.aln_len = aln_len; a.ok = ok; a.info = info;
+  a.max_ref = max_ref; a.wide_budget = 0;
   void* p;
   int rc;
+  if (max_ref) {   // a wide job may take half of the workspace budget below; one that needs more is refused alone
+    size_t free0 = 0, total0 = 0;
+    cudaMemGetInfo(&free0, &total0);
+    a.wide_budget = (unsigned long long) (((double) free0 * 0.6 + (double) ctx->bufs[SLOT_WAVEFRONT].cap) * 0.5);
+  }
   if ((rc = dgpu_reserve(ctx, SLOT_JOB_PERM, n * sizeof(uint32_t), &p))) return rc;
   a.perm = (uint32_t*) p;
   if ((rc = dgpu_reserve(ctx, SLOT_COUNTS, 2048, &p))) return rc;
@@ -671,7 +1007,10 @@ int dgpu_long_needle_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes
   DGPU_CUDA(ctx, cudaStreamSynchronize(st));
   if (h.unsupported) {   // per-item refusal: those jobs come back with ok = 0 (and info[2] = -1); never a silent approximation, never a failed batch
     ctx->unsupported += (uint64_t) h.unsupported;
-    ctx->last_error = "dgpu_long_needle: " + std::to_string(h.unsupported) + " job(s) with |cons|+|ref| > 32000 or |ref| > 16377 were not aligned (ok = 0)";
+    ctx->last_error = max_ref
+        ? "dgpu_long_needle_ex: " + std::to_string(h.unsupported) + " job(s) with |ref| > max_ref (" + std::to_string(max_ref) + "), |cons| > " +
+              std::to_string(LNW_MAX_CONS) + " or a workspace beyond the device budget were not aligned (ok = 0)"
+        : "dgpu_long_needle: " + std::to_string(h.unsupported) + " job(s) with |cons|+|ref| > 32000 or |ref| > 16377 were not aligned (ok = 0)";
   }
   size_t free_b = 0, total_b = 0;
   cudaMemGetInfo(&free_b, &total_b);
@@ -683,11 +1022,21 @@ int dgpu_long_needle_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes
   std::vector<Plan> plans;
   size_t total = 0;
   for (int c = 1; c < 2 * LN_NCLS; ++c) {
-    if (c == LN_GEN || !h.counts[c]) continue;
-    const int g = c & (LN_GEN - 1);
-    const bool packed = c < LN_GEN;
+    if (!h.counts[c]) continue;
     Plan pl;
     pl.c = c; pl.a = a;
+    if (c == LN_WIDE) {   // one 512-thread CTA per SM; the slab is the largest job's (lnw_geom), laid out per job by the kernel
+      pl.a.work_stride = (size_t) h.maxc[c];
+      pl.threads = LNW_THREADS;
+      pl.smem = lnw_smem(max_ref, (size_t) h.maxc[64 + c]);
+      pl.grid = std::min<size_t>(h.counts[c], (size_t) ctx->num_sms);
+      pl.off = 0;
+      total += pl.grid * pl.a.work_stride;
+      plans.push_back(pl);
+      continue;
+    }
+    const int g = c & (LN_GEN - 1);
+    const bool packed = c < LN_GEN;
     const size_t cells = (size_t) h.maxc[c];
     const size_t mn = (size_t) h.maxc[32 + c];
     const size_t mmax = (size_t) h.maxc[64 + c];
@@ -721,11 +1070,24 @@ int dgpu_long_needle_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes
     plans.push_back(pl);
   }
   const size_t budget = (size_t) ((double) free_b * 0.6) + ctx->bufs[SLOT_WAVEFRONT].cap;
-  if (total > budget) {  // shrink every class's grid by the same factor (at least one CTA each)
-    const double f = (double) budget / (double) total;
+  // The wide class's slabs are hundreds of MB: left in the common shrink, a few wide jobs would cut the grids of every ordinary class. So
+  // the ordinary classes keep what they ask for, up to half of the budget, and the wide class is sized within the rest (all of it when
+  // the batch has only wide jobs).
+  size_t wide_total = 0;
+  for (auto& pl : plans)
+    if (pl.c == LN_WIDE) {
+      total -= pl.grid * pl.a.work_stride;
+      const size_t wide_cap = budget - std::min(total, budget / 2);
+      pl.grid = std::max<size_t>(1, std::min<size_t>(pl.grid, wide_cap / pl.a.work_stride));
+      wide_total = pl.grid * pl.a.work_stride;
+    }
+  if (total + wide_total > budget) {  // shrink every ordinary class's grid by the same factor (at least one CTA each)
+    const double f = (double) (budget > wide_total ? budget - wide_total : 0) / (double) total;
     total = 0;
-    for (auto& pl : plans) { pl.grid = std::max<size_t>(1, (size_t) ((double) pl.grid * f)); total += pl.grid * pl.a.work_stride; }
+    for (auto& pl : plans)
+      if (pl.c != LN_WIDE) { pl.grid = std::max<size_t>(1, (size_t) ((double) pl.grid * f)); total += pl.grid * pl.a.work_stride; }
   }
+  total += wide_total;
   if ((rc = dgpu_reserve(ctx, SLOT_WAVEFRONT, total, &p))) return rc;
   { size_t off = 0; for (auto& pl : plans) { pl.a.work = (uint8_t*) p + off; off += pl.grid * pl.a.work_stride; } }
   const bool fork = plans.size() > 1;
@@ -756,6 +1118,11 @@ int dgpu_long_needle_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes
       case 13: rc = ln_launch2<48, true, 256>(ctx, pl.a, c, grid, threads, smem, cs); break;
       case 14: rc = ln_launch2<56, true, 256>(ctx, pl.a, c, grid, threads, smem, cs); break;
       case 15: rc = ln_launch2<64, true, 256>(ctx, pl.a, c, grid, threads, smem, cs); break;
+      case LN_WIDE:
+        if ((rc = dgpu_smem_optin(ctx, lnw_kernel, smem, "cudaFuncSetAttribute(lnw_kernel)"))) break;
+        lnw_kernel<<<grid, threads, smem, cs>>>(pl.a);
+        DGPU_LAUNCH_CHECK(ctx, "lnw_kernel");
+        break;
       case 17: rc = ln_launch<8, false>(ctx, pl.a, c, grid, threads, smem, cs); break;
       case 18: rc = ln_launch<16, false>(ctx, pl.a, c, grid, threads, smem, cs); break;
       case 19: rc = ln_launch<24, false>(ctx, pl.a, c, grid, threads, smem, cs); break;
@@ -783,18 +1150,18 @@ int dgpu_long_needle_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes
   return DGPU_OK;
 }
 
-int dgpu_long_needle(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
-                     const uint32_t* c_off, const uint32_t* c_len, const uint32_t* r_off, const uint32_t* r_len,
-                     uint64_t n, uint8_t* aln, const uint64_t* aln_off, uint64_t aln_bytes, uint32_t* aln_len, uint8_t* ok,
-                     int32_t* info) {
-  DgpuStage s(ctx, "dgpu_long_needle", n);
+// the host form of both entry points (max_ref = 0: dgpu_long_needle)
+int ln_host(dgpu_ctx* ctx, const char* name, const uint8_t* seqs, uint64_t seqs_bytes, const uint32_t* c_off, const uint32_t* c_len,
+            const uint32_t* r_off, const uint32_t* r_len, uint64_t n, uint8_t* aln, const uint64_t* aln_off, uint64_t aln_bytes, uint32_t* aln_len,
+            uint8_t* ok, int32_t* info, uint32_t max_ref) {
+  DgpuStage s(ctx, name, n);
   if (!ctx) return DGPU_ERR_ARG;
   if (n == 0) return DGPU_OK;
   if (!seqs || !c_off || !c_len || !r_off || !r_len || !aln || !aln_off || !aln_len || !ok) return DGPU_ERR_ARG;
   int rc;
   if ((rc = s.check_arena(seqs_bytes, n, c_off, c_len)) || (rc = s.check_arena(seqs_bytes, n, r_off, r_len))) return rc;
   for (uint64_t i = 0; i < n; ++i)   // alignment slots (2 rows of |cons| + |ref|) inside aln_bytes
-    if (aln_off[i] + 2ull * ((uint64_t) c_len[i] + r_len[i]) > aln_bytes) { ctx->last_error = "dgpu_long_needle: alignment slot beyond aln_bytes"; return DGPU_ERR_CAPACITY; }
+    if (aln_off[i] + 2ull * ((uint64_t) c_len[i] + r_len[i]) > aln_bytes) { ctx->last_error = std::string(name) + ": alignment slot beyond aln_bytes"; return DGPU_ERR_CAPACITY; }
   if ((rc = s.open())) return rc;
   const uint8_t* d_seqs = s.arena(seqs, seqs_bytes);
   uint8_t* d_aln = s.out(aln, aln_bytes, 64);
@@ -804,8 +1171,47 @@ int dgpu_long_needle(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
   uint8_t* d_ok = s.out(ok, n);
   int32_t* d_info = s.out(info, n * 4);   // null when the caller wants no info rows
   if (s.rc) return s.rc;
-  if ((rc = dgpu_long_needle_dev(ctx, d_seqs, seqs_bytes, d_coff, d_clen, d_roff, d_rlen, n, d_aln, d_aoff, d_alen, d_ok, d_info, s.st))) return rc;
+  if ((rc = ln_dev(ctx, d_seqs, seqs_bytes, d_coff, d_clen, d_roff, d_rlen, n, d_aln, d_aoff, d_alen, d_ok, d_info, max_ref, s.st))) return rc;
   return s.finish();
+}
+
+}  // namespace
+
+extern "C" {
+
+int dgpu_long_needle_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
+                         const uint32_t* c_off, const uint32_t* c_len, const uint32_t* r_off, const uint32_t* r_len,
+                         uint64_t n, uint8_t* aln, const uint64_t* aln_off, uint32_t* aln_len, uint8_t* ok,
+                         int32_t* info, void* stream) {
+  if (!ctx) return DGPU_ERR_ARG;
+  return ln_dev(ctx, seqs, seqs_bytes, c_off, c_len, r_off, r_len, n, aln, aln_off, aln_len, ok, info, 0, stream);
+}
+
+int dgpu_long_needle_ex_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
+                            const uint32_t* c_off, const uint32_t* c_len, const uint32_t* r_off, const uint32_t* r_len,
+                            uint64_t n, uint8_t* aln, const uint64_t* aln_off, uint32_t* aln_len, uint8_t* ok,
+                            int32_t* info, uint32_t max_ref, void* stream) {
+  if (!ctx) return DGPU_ERR_ARG;
+  int rc;
+  if ((rc = check_max_ref(ctx, max_ref))) return rc;
+  return ln_dev(ctx, seqs, seqs_bytes, c_off, c_len, r_off, r_len, n, aln, aln_off, aln_len, ok, info, max_ref, stream);
+}
+
+int dgpu_long_needle(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
+                     const uint32_t* c_off, const uint32_t* c_len, const uint32_t* r_off, const uint32_t* r_len,
+                     uint64_t n, uint8_t* aln, const uint64_t* aln_off, uint64_t aln_bytes, uint32_t* aln_len, uint8_t* ok,
+                     int32_t* info) {
+  return ln_host(ctx, "dgpu_long_needle", seqs, seqs_bytes, c_off, c_len, r_off, r_len, n, aln, aln_off, aln_bytes, aln_len, ok, info, 0);
+}
+
+int dgpu_long_needle_ex(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
+                        const uint32_t* c_off, const uint32_t* c_len, const uint32_t* r_off, const uint32_t* r_len,
+                        uint64_t n, uint8_t* aln, const uint64_t* aln_off, uint64_t aln_bytes, uint32_t* aln_len, uint8_t* ok,
+                        int32_t* info, uint32_t max_ref) {
+  if (!ctx) return DGPU_ERR_ARG;
+  int rc;
+  if ((rc = check_max_ref(ctx, max_ref))) return rc;
+  return ln_host(ctx, "dgpu_long_needle_ex", seqs, seqs_bytes, c_off, c_len, r_off, r_len, n, aln, aln_off, aln_bytes, aln_len, ok, info, max_ref);
 }
 
 }  // extern "C"

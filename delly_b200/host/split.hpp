@@ -282,7 +282,8 @@ inline int splitAlignBatch(dgpu_ctx* ctx, std::vector<std::string> const& cons, 
 
 // Batched _consRefAlignment (src/split.h:540-558): align[0] = consensus row, align[1] = reference row.
 // Insertions (svt 4) go through splitAlignBatch (three dgpu_edit_path rounds; rows swapped afterwards, :548-552),
-// everything else through ONE dgpu_long_needle call. ok[k] = the reference function's return value.
+// everything else through ONE dgpu_long_needle (or, with windows beyond its shapes, dgpu_long_needle_ex) call. ok[k] = the reference
+// function's return value.
 inline int consRefAlignmentBatch(dgpu_ctx* ctx, std::vector<int32_t> const& svt, std::vector<const std::string*> const& cons,
                                  std::vector<const std::string*> const& refs, std::vector<uint8_t>& ok, std::vector<TAlign>& aligns) {
   const std::size_t N = svt.size();
@@ -322,9 +323,20 @@ inline int consRefAlignmentBatch(dgpu_ctx* ctx, std::vector<int32_t> const& svt,
   }
   std::vector<uint8_t> aln(abytes + 1), okk(idx.size());
   std::vector<uint32_t> alen(idx.size());
+  // Windows beyond the wavefront kernels' shapes (|ref| > 16377 or |cons| + |ref| > 32000) need dgpu_long_needle_ex, with max_ref = the
+  // batch's widest window. Every other batch goes through dgpu_long_needle, the entry point every binding of the ABI provides, including
+  // the CPU suite's stand-in of it (tests/standin/host_standin.cpp forwards dgpu_long_needle to the reference's longNeedle).
+  bool wide = false;
+  uint32_t widest = 0;
+  for (std::size_t k = 0; k < idx.size(); ++k) {
+    widest = std::max(widest, rl[k]);
+    wide |= rl[k] > 16377 || (uint64_t) cl[k] + rl[k] > 32000;
+  }
   const uint64_t refusedBefore = dgpu_unsupported_count(ctx);
-  rc = dgpu_long_needle(ctx, (const uint8_t*) arena.data(), arena.size(), co.data(), cl.data(), ro.data(), rl.data(), idx.size(), aln.data(),
-                        ao.data(), abytes, alen.data(), okk.data(), nullptr);
+  rc = wide ? dgpu_long_needle_ex(ctx, (const uint8_t*) arena.data(), arena.size(), co.data(), cl.data(), ro.data(), rl.data(), idx.size(), aln.data(),
+                                  ao.data(), abytes, alen.data(), okk.data(), nullptr, std::max<uint32_t>(1, std::min<uint32_t>(widest, DGPU_LN_MAX_REF)))
+            : dgpu_long_needle(ctx, (const uint8_t*) arena.data(), arena.size(), co.data(), cl.data(), ro.data(), rl.data(), idx.size(), aln.data(),
+                               ao.data(), abytes, alen.data(), okk.data(), nullptr);
   if (rc) return rc;
   deviceLimitLog().needleJobs += dgpu_unsupported_count(ctx) - refusedBefore;   // jobs beyond the kernel's shapes come back as failed alignments (ok = 0)
   for (std::size_t k = 0; k < idx.size(); ++k) {

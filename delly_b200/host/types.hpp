@@ -54,7 +54,7 @@ inline void parallelFor(std::size_t n, F&& fn, std::size_t minPerThread = 1) {
 struct DeviceLimitLog {
   std::atomic<uint64_t> msaClusters{0};   // dgpu_msa_ex status != 0: > DGPU_MSA_LARGE_MAXR reads, > 1023 alignment columns, a byte outside ACGTN
   std::atomic<uint64_t> pathJobs{0};      // dgpu_edit_path status != 0: target slice beyond the path kernel's window
-  std::atomic<uint64_t> needleJobs{0};    // dgpu_long_needle: |cons| + |ref| > 32000 or |ref| > 16377
+  std::atomic<uint64_t> needleJobs{0};    // dgpu_long_needle[_ex]: |cons| > 16383, |ref| > DGPU_LN_MAX_REF, or a workspace beyond the device budget
   uint64_t total() const { return msaClusters.load() + pathJobs.load() + needleJobs.load(); }
 };
 inline DeviceLimitLog& deviceLimitLog() { static DeviceLimitLog log; return log; }

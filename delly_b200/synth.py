@@ -147,6 +147,37 @@ def sub_noise(rng, a, rate):
     return a
 
 
+def _revcomp(a):
+    """reverse complement of an ACGT array"""
+    a = np.asarray(a, np.uint8)
+    out = a[::-1].copy()
+    for x, y in zip(b"ACGT", b"TGCA"):
+        out[a[::-1] == x] = y
+    return out
+
+
+def wide_consref_job(rng, kind, m, n, bp=None, noise=0.02):
+    """One consensus / window pair shaped like _getSVRef's output (src/split.h:114-160) for a window of n columns and a consensus of about
+    m bases. 'del': one window, flank + deleted segment + flank, the consensus joins the two flanks (breakpoint at column bp of the window);
+    'dup' / 'inv': two flanks of n/2 columns cut around the two breakpoints, taken from distant places of the genome (the second one
+    reverse-complemented for 'inv'); the consensus joins the first flank's left part to the second flank's right part."""
+    g = _ACGT[rng.integers(0, 4, size=2 * n + 100, dtype=np.uint8)]
+    h = m // 2
+    if kind == "del":
+        ref = g[:n]
+        a = bp if bp is not None else m
+        b = n - (m - h) - int(rng.integers(0, max(1, (n - a - m) // 4)))
+        cons = np.concatenate([ref[a - h:a], ref[b:b + (m - h)]])
+    else:
+        half = n // 2
+        second = g[n + 50:n + 50 + (n - half)]
+        ref = np.concatenate([g[:half], _revcomp(second) if kind == "inv" else second])
+        p = bp if bp is not None else half // 2 + int(rng.integers(0, half // 4))
+        q = half + (n - half) // 2
+        cons = np.concatenate([ref[p - h:p], ref[q:q + (m - h)]])
+    return sub_noise(rng, cons, noise), ref
+
+
 def k3_consref_batch(n_jobs, seed=1003, cons_range=(150, 300), err=0.01, kinds=(0, 1, 2, 3), ref_cap=None, genome_len=2_000_000,
                      fast=False):
     """K3/K5: consensus vs SV-reference-window jobs shaped like _getSVRef's output (src/split.h:70-163).

@@ -166,7 +166,8 @@ int dgpu_edit_path_ex_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_byte
  *   aln         row 0 (consensus) at aln + aln_off[i], row 1 (reference) at aln + aln_off[i] +
  *               (c_len[i] + r_len[i]); the caller reserves 2*(c_len+r_len) bytes per job.
  *   info        optional [consLeft, refLeft, refRight, bestScore] per job (white-box tests)
- * Limits: c_len + r_len <= 32000 (scores are stored as int16); otherwise DGPU_ERR_UNSUPPORTED.
+ * Limits of dgpu_long_needle / dgpu_long_needle_dev: r_len <= 16377 and c_len + r_len <= 32000 (the wavefront kernels' shapes). A job
+ * beyond them is refused alone: ok = 0, aln_len = 0, info[2] = -1, dgpu_unsupported_count + 1; the call succeeds.
  */
 int dgpu_long_needle(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
                      const uint32_t* c_off, const uint32_t* c_len,
@@ -178,6 +179,23 @@ int dgpu_long_needle_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes
                          const uint32_t* r_off, const uint32_t* r_len, uint64_t n,
                          uint8_t* aln, const uint64_t* aln_off,
                          uint32_t* aln_len, uint8_t* ok, int32_t* info, void* stream);
+/* The _ex forms take max_ref, the widest reference window the caller wants computed (1 .. DGPU_LN_MAX_REF, else DGPU_ERR_ARG).
+ * Jobs inside the wavefront kernels' shapes run exactly as in dgpu_long_needle; jobs beyond them with r_len <= max_ref and
+ * c_len <= 16383 run on the wide-window engine (one CTA per job computing whole DP rows, ~3 B of workspace per cell). Any other job,
+ * and a job whose workspace alone exceeds half of the device budget (0.6 x free memory), is refused alone as above.
+ * Caps: c_len <= 16383 because the wide engine keeps row-shifted scores U = H + r in [0, 2 c_len] as int16; DGPU_LN_MAX_REF because it
+ * keeps the previous DP row (int16) and both sequences of a job in shared memory, about 213 KB at 65535 columns (227 KB per CTA on sm_90). */
+#define DGPU_LN_MAX_REF 65535
+int dgpu_long_needle_ex(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
+                        const uint32_t* c_off, const uint32_t* c_len,
+                        const uint32_t* r_off, const uint32_t* r_len, uint64_t n,
+                        uint8_t* aln, const uint64_t* aln_off, uint64_t aln_bytes,
+                        uint32_t* aln_len, uint8_t* ok, int32_t* info, uint32_t max_ref);
+int dgpu_long_needle_ex_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
+                            const uint32_t* c_off, const uint32_t* c_len,
+                            const uint32_t* r_off, const uint32_t* r_len, uint64_t n,
+                            uint8_t* aln, const uint64_t* aln_off,
+                            uint32_t* aln_len, uint8_t* ok, int32_t* info, uint32_t max_ref, void* stream);
 
 /* ---- per-cluster MSA + consensus (replaces msa) -----------------------------------------
  * Call sites: msa(c, seqStore[svid], consensus), src/shortpe.h:185 and :252 (one call per SV
