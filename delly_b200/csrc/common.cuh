@@ -66,7 +66,7 @@ enum {
   SLOT_MSA_SEGJOBS,  // MSA warp workspace (msa.cu); segment job arrays (edit_path.cu)
   SLOT_MSA_LARGE,    // msa_large_kernel's per-CTA workspace, sized from max_reads (msa.cu)
   SLOT_EP_MIRROR,    // edit path: the reversed-sequence mirror of the HW start pass, then the traced leaf ops (edit_path.cu)
-  SLOT_EP_TABLE,     // edit path: HW-start target offsets, then the split selection, then the leaf table (edit_path.cu)
+  SLOT_EP_TABLE,     // edit path: HW-start target offsets and mirror offsets, then the split selection, then the leaf table (edit_path.cu)
   SLOT_EP_COLS,      // edit path: HW-start target lengths, then the half columns of the split pass (edit_path.cu)
   SLOT_EP_BOUNDS,    // edit path: HW-start bounds and reverse end locations (edit_path.cu)
   SLOT_EP_EQTAB,     // edit path: generalised-equality tables (edit_path.cu)

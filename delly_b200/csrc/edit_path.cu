@@ -31,20 +31,23 @@ namespace {
 
 // ------------------------------------------------------------------------------------------------------------
 // Device side of stages 1-2 (distance, end, HW start) — unchanged semantics, see header comment.
-__global__ void ep_mirror_kernel(const uint8_t* seqs, uint8_t* mirror, const uint32_t* off, const uint32_t* len, uint32_t n) {
+// Job w's sequence seqs[off[w] .. +len[w]) reversed into mirror[dst[w] ..]. Every job has its own mirror bytes: sequences may share arena
+// bytes (a query inside its target, overlapping windows of one contig), and a reversal written back at the arena address would overwrite them.
+__global__ void ep_mirror_kernel(const uint8_t* seqs, uint8_t* mirror, const uint32_t* off, const uint32_t* len, const uint32_t* dst, uint32_t n) {
   const uint32_t w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (w >= n) return;
-  const uint32_t o = off[w], L = len[w];
-  for (uint32_t i = lane; i < L; i += 32) mirror[o + i] = seqs[o + L - 1 - i];
+  const uint32_t o = off[w], L = len[w], d = dst[w];
+  for (uint32_t i = lane; i < L; i += 32) mirror[d + i] = seqs[o + L - 1 - i];
 }
 
-__global__ void ep_hwstart_jobs_kernel(const uint32_t* t_off, const uint32_t* t_len, const int32_t* dist, const int32_t* end_loc, uint32_t n,
+// mt_off: where the reversed target starts in the mirror
+__global__ void ep_hwstart_jobs_kernel(const uint32_t* mt_off, const uint32_t* t_len, const int32_t* dist, const int32_t* end_loc, uint32_t n,
                                        uint32_t* t2_off, uint32_t* t2_len, int32_t* k2) {
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const int e = end_loc[i], d = dist[i];
-  if (d < 0 || e < 0) { t2_off[i] = t_off[i]; t2_len[i] = 0; k2[i] = 0; return; }
-  t2_off[i] = t_off[i] + (t_len[i] - (uint32_t) e - 1);
+  if (d < 0 || e < 0) { t2_off[i] = mt_off[i]; t2_len[i] = 0; k2[i] = 0; return; }
+  t2_off[i] = mt_off[i] + (t_len[i] - (uint32_t) e - 1);
   t2_len[i] = (uint32_t) e + 1;
   k2[i] = d;
 }
@@ -568,6 +571,10 @@ inline bool seg_needs_split(uint32_t m, uint32_t n) {  // src/edlib.cpp:1189-119
   return est >= 1024 * 1024;
 }
 
+// Bytes of one run of the HW start-pass mirror. The mirror holds a private copy of every job's query and target, so jobs that share a
+// sequence (many reads against one window) need more than the arena; runs bound that and keep offsets 32-bit.
+constexpr uint64_t EP_MIRROR_RUN = 1ull << 30;
+
 }  // namespace
 
 extern "C" {
@@ -617,23 +624,50 @@ int dgpu_edit_path_ex_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_byte
     // 1. distance + first end location (k = -1 at every PATH call site of the reference); generalised equalities ride along as tables
     if ((rc = dgpu_edit_distance_impl(ctx, seqs, seqs_bytes, q_off, q_len, t_off, t_len, nullptr, mode, n, dist, end_loc, st, 0, d_eqtabs))) return rc;
     void* d_rev = nullptr;
+    // mirror layout of the HW start pass: job i's reversed query at mq[i], its reversed target right after it, jobs back to back in runs
+    // of at most EP_MIRROR_RUN bytes; each run is mirrored and searched in one SHW pass (offsets relative to the run)
+    std::vector<uint32_t> h_moff;
+    std::vector<uint64_t> run_lo, run_bytes;
     if (mode == DGPU_MODE_HW) {
+      h_moff.resize(2 * n);
+      uint64_t pos = 0;
+      for (uint64_t i = 0; i < n; ++i) {
+        const uint64_t need = (uint64_t) h_qlen[i] + h_tlen[i];
+        if (need > EP_MIRROR_RUN) { ctx->last_error = "dgpu_edit_path: a HW job's query and target exceed the start-pass mirror"; return DGPU_ERR_CAPACITY; }
+        if (i == 0 || pos + need > EP_MIRROR_RUN) {
+          if (i) run_bytes.push_back(pos);
+          run_lo.push_back(i);
+          pos = 0;
+        }
+        h_moff[i] = (uint32_t) pos; h_moff[n + i] = (uint32_t) (pos + h_qlen[i]);
+        pos += need;
+      }
+      run_bytes.push_back(pos);
+      run_lo.push_back(n);
+      const uint64_t run_max = *std::max_element(run_bytes.begin(), run_bytes.end());
       // 2. start location: reversed query vs reversed target prefix, SHW, k = distance, LAST optimal end
       void *d_mirror, *d_t2off, *d_t2len, *d_k2;
-      if ((rc = dgpu_reserve(ctx, SLOT_EP_MIRROR, seqs_bytes + 64, &d_mirror))) return rc;
-      if ((rc = dgpu_reserve(ctx, SLOT_EP_TABLE, n * 4, &d_t2off))) return rc;
+      if ((rc = dgpu_reserve(ctx, SLOT_EP_MIRROR, run_max + 64, &d_mirror))) return rc;
+      if ((rc = dgpu_reserve(ctx, SLOT_EP_TABLE, n * 12, &d_t2off))) return rc;
       if ((rc = dgpu_reserve(ctx, SLOT_EP_COLS, n * 4, &d_t2len))) return rc;
       if ((rc = dgpu_reserve(ctx, SLOT_EP_BOUNDS, n * 8, &d_k2))) return rc;
       d_rev = (uint8_t*) d_k2 + n * 4;
-      const uint32_t wb = (uint32_t) ((n * 32 + 255) / 256);
-      ep_mirror_kernel<<<wb, 256, 0, st>>>(seqs, (uint8_t*) d_mirror, q_off, q_len, (uint32_t) n);
-      DGPU_LAUNCH_CHECK(ctx, "ep_mirror(q)");
-      ep_mirror_kernel<<<wb, 256, 0, st>>>(seqs, (uint8_t*) d_mirror, t_off, t_len, (uint32_t) n);
-      DGPU_LAUNCH_CHECK(ctx, "ep_mirror(t)");
-      ep_hwstart_jobs_kernel<<<nb, 256, 0, st>>>(t_off, t_len, dist, end_loc, (uint32_t) n, (uint32_t*) d_t2off, (uint32_t*) d_t2len, (int32_t*) d_k2);
+      uint32_t* d_mq = (uint32_t*) d_t2off + n;
+      uint32_t* d_mt = d_mq + n;
+      DGPU_CUDA(ctx, cudaMemcpyAsync(d_mq, h_moff.data(), 2 * n * 4, cudaMemcpyHostToDevice, st));
+      ep_hwstart_jobs_kernel<<<nb, 256, 0, st>>>(d_mt, t_len, dist, end_loc, (uint32_t) n, (uint32_t*) d_t2off, (uint32_t*) d_t2len, (int32_t*) d_k2);
       DGPU_LAUNCH_CHECK(ctx, "ep_hwstart_jobs");
-      if ((rc = dgpu_edit_distance_impl(ctx, (const uint8_t*) d_mirror, seqs_bytes, q_off, q_len, (const uint32_t*) d_t2off, (const uint32_t*) d_t2len,
-                                        (const int32_t*) d_k2, DGPU_MODE_SHW, n, start_loc, (int32_t*) d_rev, st, 1, d_eqtabs))) return rc;
+      for (size_t r = 0; r + 1 < run_lo.size(); ++r) {   // a run reuses the mirror after the previous run's pass on the same stream
+        const uint64_t j0 = run_lo[r], cnt = run_lo[r + 1] - j0;
+        const uint32_t wb = (uint32_t) ((cnt * 32 + 255) / 256);
+        ep_mirror_kernel<<<wb, 256, 0, st>>>(seqs, (uint8_t*) d_mirror, q_off + j0, q_len + j0, d_mq + j0, (uint32_t) cnt);
+        DGPU_LAUNCH_CHECK(ctx, "ep_mirror(q)");
+        ep_mirror_kernel<<<wb, 256, 0, st>>>(seqs, (uint8_t*) d_mirror, t_off + j0, t_len + j0, d_mt + j0, (uint32_t) cnt);
+        DGPU_LAUNCH_CHECK(ctx, "ep_mirror(t)");
+        if ((rc = dgpu_edit_distance_impl(ctx, (const uint8_t*) d_mirror, run_bytes[r], d_mq + j0, q_len + j0, (const uint32_t*) d_t2off + j0,
+                                          (const uint32_t*) d_t2len + j0, (const int32_t*) d_k2 + j0, DGPU_MODE_SHW, cnt, start_loc + j0,
+                                          (int32_t*) d_rev + j0, st, 1, d_eqtabs))) return rc;
+      }
     }
     ep_start_kernel<<<nb, 256, 0, st>>>(mode, q_len, t_len, dist, end_loc, (const int32_t*) d_rev, (uint32_t) n, start_loc);
     DGPU_LAUNCH_CHECK(ctx, "ep_start");

@@ -12,7 +12,8 @@
  *    DGPU_ERR_* code; no exceptions cross the boundary.
  *  - Sequences are 1 byte per base in one packed arena (`seqs`); equality is byte
  *    equality exactly like edlib / the reference's char compares (so IUPAC codes,
- *    'N' and lower case keep the reference's semantics).
+ *    'N' and lower case keep the reference's semantics). Sequences may share or overlap
+ *    bytes anywhere in the arena (a query inside its target, windows of one contig).
  *  - Every batch call exists in two forms:
  *      dgpu_<op>        host pointers in/out; the call stages H2D, launches, copies the
  *                       results D2H and returns when they are in the caller's buffers.
