@@ -16,6 +16,8 @@
 //     |q|-1 so no padding/wildcard columns are needed. The per-job match masks Peq[5][NW] live in a
 //     per-thread-private, bank-conflict-free slice of shared memory; the target is streamed with
 //     aligned LDG.128 + PRMT realignment (ChunkReader).
+//   * HW jobs 2i and 2i+1 on the same target (a read's ALT and REF probes) with queries of one class
+//     run as a pair in one thread (ed_pair_kernel): one target stream and decode, two Myers columns.
 //   * |q| > 128: ONE WARP PER JOB, anti-diagonal wavefront: lane l owns a 64-row block and processes
 //     column t-l at step t; the horizontal delta (hout) crosses lanes by shuffle. Queries longer
 //     than 2048 rows are processed in 2048-row stripes, the stripe's bottom hout per column being
@@ -39,7 +41,12 @@ constexpr int ED_THREADS = 128;
 #define ED_CTAS_PER_SM_V 32
 #endif
 constexpr int ED_CTAS_PER_SM = ED_CTAS_PER_SM_V;
-// job classes: 0 trivial, 1..4 = words per thread-job, 5 = warp-per-job
+// job classes: 0 trivial, 1..4 = words per thread-job, 5 = warp-per-job, ED_PAIR + 1..4 = target-sharing pairs of class 1..4 (ed_pair_kernel)
+constexpr int ED_PAIR = 5;
+constexpr int ED_NCLS = ED_PAIR + 5;
+// counts layout (SLOT_COUNTS): [0, 16) jobs per class, [ED_START, +16) class starts in perm, [ED_CUR, +16) scatter cursors, [ED_TMAX] max t_len
+// of multi-stripe jobs, [ED_BANDQ, +EDB_CLASSES + 1) band pass queues
+constexpr int ED_START = 16, ED_CUR = 32, ED_TMAX = 48, ED_BANDQ = 64, ED_COUNTS_WORDS = 128;
 
 struct EdArgs {
   const uint8_t* seqs;
@@ -53,8 +60,9 @@ struct EdArgs {
   int32_t* dist;
   int32_t* end_loc;
   uint32_t* perm;
-  uint32_t* counts;  // [0..7] class counts, [8..15] class starts, [16..23] scatter cursors, [24] max t_len of multi-stripe jobs, [32..36] band pass queues
-  int last_pos;      // HW/SHW: report the LAST optimal end position instead of the first (edlib's positionsSHW.back(), src/edlib.cpp:250)
+  uint32_t* counts;  // ED_START / ED_CUR / ED_TMAX / ED_BANDQ layout above
+  int pair;          // HW distances without end locations or equality tables: target-sharing job pairs take ed_pair_kernel (ed_slot)
+  int last_pos;     // HW/SHW: report the LAST optimal end position instead of the first (edlib's positionsSHW.back(), src/edlib.cpp:250)
   uint8_t* hbuf;     // per-warp scratch rows for multi-stripe jobs
   uint32_t hbuf_stride;
   // generalised equality (edlib's additionalEqualities, src/edlib.cpp:58-79); all jobs then take the warp-per-job kernel
@@ -87,17 +95,29 @@ __device__ __forceinline__ int apply_k(int d, int k, int mode, int m, int n) {
   }
 }
 
+// Count slot of job i: its class, or, for the even member i of a pair (i, i + 1) of one-thread jobs of the same class on the same target
+// (equal t_off and t_len: the ALT and REF probes of one genotyping read), the pair class ED_PAIR + class; -1 for the odd member of a pair.
+// Indices are relative to the call.
+__device__ __forceinline__ int ed_slot(const EdArgs& a, uint32_t i) {
+  const uint32_t tl = a.t_len[i];
+  const int c = ed_class(a.q_len[i], tl, a.force_long);
+  if (!a.pair || c < 1 || c > 4) return c;
+  const uint32_t o = i ^ 1u;
+  if (o >= a.n || a.t_off[o] != a.t_off[i] || a.t_len[o] != tl || ed_class(a.q_len[o], tl, 0) != c) return c;
+  return (i & 1u) ? -1 : ED_PAIR + c;
+}
+
 __global__ void ed_count_kernel(EdArgs a, int mode) {
-  __shared__ uint32_t h[8];
+  __shared__ uint32_t h[ED_NCLS];
   __shared__ uint32_t hmax;
-  if (threadIdx.x < 8) h[threadIdx.x] = 0;
+  if (threadIdx.x < ED_NCLS) h[threadIdx.x] = 0;
   if (threadIdx.x == 0) hmax = 0;
   __syncthreads();
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < a.n) {
     uint32_t ql = a.q_len[i], tl = a.t_len[i];
-    int c = ed_class(ql, tl, a.force_long);
-    atomicAdd(&h[c], 1u);
+    int c = ed_slot(a, i);
+    if (c >= 0) atomicAdd(&h[c], 1u);
     if (c == 5 && ql > 2048) atomicMax(&hmax, tl);
     if (c == 0) {
       // src/edlib.cpp:158-177: NW -> max(len), endLocations[0] = n-1; HW/SHW -> |q|, endLocations[0] = -1.
@@ -108,33 +128,33 @@ __global__ void ed_count_kernel(EdArgs a, int mode) {
     }
   }
   __syncthreads();
-  if (threadIdx.x < 8 && h[threadIdx.x]) atomicAdd(&a.counts[threadIdx.x], h[threadIdx.x]);
-  if (threadIdx.x == 0 && hmax) atomicMax(&a.counts[24], hmax);
+  if (threadIdx.x < ED_NCLS && h[threadIdx.x]) atomicAdd(&a.counts[threadIdx.x], h[threadIdx.x]);
+  if (threadIdx.x == 0 && hmax) atomicMax(&a.counts[ED_TMAX], hmax);
 }
 
 __global__ void ed_offsets_kernel(uint32_t* counts) {
   uint32_t s = 0;
-  for (int c = 0; c < 8; ++c) {
-    counts[8 + c] = s;
-    counts[16 + c] = s;
+  for (int c = 0; c < ED_NCLS; ++c) {
+    counts[ED_START + c] = s;
+    counts[ED_CUR + c] = s;
     s += counts[c];
   }
 }
 
 __global__ void ed_scatter_kernel(EdArgs a) {
-  __shared__ uint32_t h[8];
-  __shared__ uint32_t base[8];
-  if (threadIdx.x < 8) h[threadIdx.x] = 0;
+  __shared__ uint32_t h[ED_NCLS];
+  __shared__ uint32_t base[ED_NCLS];
+  if (threadIdx.x < ED_NCLS) h[threadIdx.x] = 0;
   __syncthreads();
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   int c = -1;
   uint32_t r = 0;
   if (i < a.n) {
-    c = ed_class(a.q_len[i], a.t_len[i], a.force_long);
-    r = atomicAdd(&h[c], 1u);
+    c = ed_slot(a, i);
+    if (c >= 0) r = atomicAdd(&h[c], 1u);
   }
   __syncthreads();
-  if (threadIdx.x < 8) base[threadIdx.x] = h[threadIdx.x] ? atomicAdd(&a.counts[16 + threadIdx.x], h[threadIdx.x]) : 0;
+  if (threadIdx.x < ED_NCLS) base[threadIdx.x] = h[threadIdx.x] ? atomicAdd(&a.counts[ED_CUR + threadIdx.x], h[threadIdx.x]) : 0;
   __syncthreads();
   if (c >= 0) a.perm[base[c] + r] = i;
 }
@@ -225,6 +245,23 @@ __device__ __forceinline__ uint32_t match4(uint32_t x, uint32_t s) {
   return (z * 0x00204081u) >> 28;
 }
 
+// x = the slots ((c >> 1) & 3) of four bytes; returns the four bytes ACGT would have at those slots. The byte of slot x is
+// 0x41 + 2 x + 15 [x == 2] ('A' 'C' 'T' 'G'), two multiply-adds, so a word is all ACGT iff it equals acgt_bytes((w >> 1) & 0x03030303).
+__device__ __forceinline__ uint32_t acgt_bytes(uint32_t x) {
+  const uint32_t is_t = (x >> 1) & ~x & 0x01010101u;
+  return x * 2u + 0x41414141u + is_t * 15u;
+}
+
+// match bits of 32 bytes against the byte s, byte b -> bit b: the exact Peq word of a query word holding a byte outside ACGT. Out of line,
+// since such words are rare and the Peq build stays one straight block without them.
+__device__ __noinline__ uint32_t match32(uint4 lo, uint4 hi, uint32_t s) {
+  const uint32_t wv[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
+  uint32_t e = 0;
+#pragma unroll
+  for (int k = 0; k < 8; ++k) e |= match4(wv[k], s) << (k * 4);
+  return e;
+}
+
 // exact slow path for a target byte outside ACGTN: byte equality against the query rows q[0..len), len <= 32, bit i = row i. Kept out of
 // line so the column loop holds calls instead of one copy of the loop per column slot; one word per call, so the result comes back in a
 // register rather than through a stack frame.
@@ -246,6 +283,182 @@ __device__ __forceinline__ void rows_to_top(uint32_t (&e)[NW], uint32_t p, uint3
   e[0] = (e[0] << p) | vmask;
 }
 
+// Match masks of one query for the Peq table, in slot order A0 C1 T2 G3 N4; word w of slot s goes to pq[(s * SW + w) * ED_THREADS].
+// Per query word: bits 1 and 2 of the 32 bytes are gathered into two 32-row planes (one multiply per plane and 4-byte group moves bit
+// 8i + k of the group to bit 28 + i, as match4 does; a funnel shift appends the group below the later ones), and each of A C T G is one
+// LOP3 of the planes, with no N row. A word with any byte outside ACGT is built exactly by match32 instead (N rows get the N mask, other
+// bytes no bit). Rows past |q| read whatever follows the query in the arena (the reader stays inside it); the last word is masked to |q|, or
+// in the HW layout those rows are shifted out.
+template <int NW, bool TOP>
+__device__ __forceinline__ void build_peq(uint32_t* pq, int SW, const uint8_t* q, const uint8_t* seqs_end, uint32_t topbit, uint32_t p,
+                                          uint32_t vmask) {
+  ChunkReader qr;
+  qr.init(q, seqs_end);
+  uint32_t pm[5][NW];
+#pragma unroll
+  for (int w = 0; w < NW; ++w) {
+    const uint4 lo = qr.next(), hi = qr.next();
+    const uint32_t wv[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
+    uint32_t p1 = 0, p2 = 0, bad = 0;
+#pragma unroll
+    for (int g = 7; g >= 0; --g) {
+      const uint32_t x = (wv[g] >> 1) & 0x03030303u;
+      bad |= wv[g] ^ acgt_bytes(x);
+      p1 = __funnelshift_l((x & 0x01010101u) * 0x10204080u, p1, 4);
+      p2 = __funnelshift_l((x & 0x02020202u) * 0x08102040u, p2, 4);
+    }
+    if (bad == 0) {
+      pm[0][w] = ~(p1 | p2);
+      pm[1][w] = p1 & ~p2;
+      pm[2][w] = p2 & ~p1;
+      pm[3][w] = p1 & p2;
+      pm[4][w] = 0;
+    } else {
+      pm[0][w] = match32(lo, hi, 'A');
+      pm[1][w] = match32(lo, hi, 'C');
+      pm[2][w] = match32(lo, hi, 'T');
+      pm[3][w] = match32(lo, hi, 'G');
+      pm[4][w] = match32(lo, hi, 'N');
+    }
+  }
+#pragma unroll
+  for (int s = 0; s < 5; ++s) {
+    if (TOP) rows_to_top<NW>(pm[s], p, vmask);
+    else pm[s][NW - 1] &= (2u << topbit) - 1u;
+#pragma unroll
+    for (int w = 0; w < NW; ++w) pq[(s * SW + w) * ED_THREADS] = pm[s][w];
+  }
+}
+
+// NJ (1 or 2) jobs of one thread that share a target: jobs perm[i], ..., perm[i] + NJ - 1 of the class `cls` segment of perm. One target stream,
+// one byte decode and one Peq address per column feed NJ independent Myers columns. The Peq table of the thread holds, per symbol slot,
+// the NW words of each job's query: peq[(slot * NJ NW + j NW + w) * ED_THREADS + tid].
+template <int NW, int MODE, bool WANT_END, int NJ>
+__device__ __forceinline__ void ed_small_jobs(const EdArgs& a, uint32_t* peq, int cls) {
+  constexpr int HIN = (MODE == DGPU_MODE_HW) ? 0 : 1;
+  constexpr bool TOP = (MODE == DGPU_MODE_HW);  // query rows at the top of the bit-vector (rows_to_top)
+  constexpr int SW = NJ * NW;                    // Peq words per symbol slot
+  const uint32_t cnt = a.counts[cls];
+  const uint32_t start = a.counts[ED_START + cls];
+  const uint32_t tid = threadIdx.x;
+  for (uint32_t idx = blockIdx.x * ED_THREADS + tid; idx < cnt; idx += gridDim.x * ED_THREADS) {
+    const uint32_t job0 = a.perm[start + idx];
+    const uint32_t n = a.t_len[job0];
+    const uint8_t* t = a.seqs + a.t_off[job0];
+    uint32_t m[NJ], topbit[NJ], p[NJ], vmask[NJ];
+    const uint8_t* q[NJ];
+    uint32_t Pv[NJ][NW], Mv[NJ][NW];
+    int score[NJ], best[NJ], bpos[NJ], prev[NJ];
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) {
+      m[j] = a.q_len[job0 + j];
+      q[j] = a.seqs + a.q_off[job0 + j];
+      topbit[j] = (m[j] - 1) & 31u;
+      p[j] = 32u * NW - m[j];  // jobs of this class have 32 (NW - 1) < |q| <= 32 NW
+      vmask[j] = TOP ? (1u << p[j]) - 1u : 0u;
+      build_peq<NW, TOP>(peq + j * NW * ED_THREADS + tid, SW, q[j], a.seqs_end, topbit[j], p[j], vmask[j]);
+#pragma unroll
+      for (int w = 0; w < NW; ++w) { Pv[j][w] = 0xffffffffu; Mv[j][w] = 0; }
+      Pv[j][0] = ~vmask[j];  // virtual rows start at Pv = Mv = 0
+      score[j] = (int) m[j];
+      // candidate end position -1 (score m) exists iff |q| % 64 != 0 (edlib's padding columns)
+      best[j] = (m[j] & 63u) ? (int) m[j] : 0x7fffffff;
+      bpos[j] = -1;
+      prev[j] = 0;
+    }
+
+    auto track = [&](int j, uint32_t col) {
+      if (MODE != DGPU_MODE_NW) {
+        if (WANT_END) { if (score[j] < best[j] || (a.last_pos && score[j] == best[j])) { best[j] = score[j]; bpos[j] = (int) col; } }
+        else best[j] = min(best[j], score[j]);
+      }
+    };
+    // one column through the table (ACGTN) or the exact slow path (any other byte)
+    auto step = [&](uint32_t c, uint32_t col) {
+      const uint32_t code = dna_code(c);
+#pragma unroll
+      for (int j = 0; j < NJ; ++j) {
+        uint32_t Eq[NW];
+        if (code < 5) {
+#pragma unroll
+          for (int w = 0; w < NW; ++w) Eq[w] = peq[(peq_slot(code) * SW + j * NW + w) * ED_THREADS + tid];
+        } else {
+#pragma unroll
+          for (int w = 0; w < NW; ++w) Eq[w] = eq_word_by_bytes(q[j] + w * 32, min(32u, m[j] - w * 32), c);
+          if (TOP) rows_to_top<NW>(Eq, p[j], vmask[j]);
+        }
+        myers_column<NW, HIN, TOP>(Pv[j], Mv[j], Eq, topbit[j], score[j]);
+        track(j, col);
+      }
+    };
+    const uint32_t base2 = (tid * 4u) * 0x00010001u;  // this thread's slot offset in both 16-bit halves
+    // the four columns of target bytes wd, the first being column col
+    auto group4 = [&](uint32_t wd, uint32_t col) {
+      // four bytes at once: x = slot of each byte if it is one of ACGT
+      const uint32_t x = (wd >> 1) & 0x03030303u;
+      if (wd == acgt_bytes(x)) {
+        // byte offsets of the four Peq rows, two per register: slot * (SW*512) + tid*4
+        const uint32_t offA = (x & 0x00ff00ffu) * (uint32_t) (SW * 4 * ED_THREADS) + base2;          // columns 0 and 2
+        const uint32_t offB = ((x >> 8) & 0x00ff00ffu) * (uint32_t) (SW * 4 * ED_THREADS) + base2;   // columns 1 and 3
+#pragma unroll
+        for (int b = 0; b < 4; ++b) {
+          const uint32_t pk = (b & 1) ? offB : offA;
+          const uint32_t off = (b & 2) ? (pk >> 16) : (pk & 0xffffu);
+#pragma unroll
+          for (int j = 0; j < NJ; ++j) {
+            uint32_t Eq[NW];
+#pragma unroll
+            for (int w = 0; w < NW; ++w) Eq[w] = *(const uint32_t*) ((const char*) peq + off + (j * NW + w) * 4 * ED_THREADS);
+            myers_column<NW, HIN, TOP>(Pv[j], Mv[j], Eq, topbit[j], score[j]);
+            if (MODE != DGPU_MODE_NW) {
+              if (WANT_END) track(j, col + b);
+              else if (b & 1) best[j] = min(best[j], min(prev[j], score[j]));  // two columns per three-input min
+              else prev[j] = score[j];
+            }
+          }
+        }
+      } else {
+        // a byte outside ACGT among the four: one rolled copy of the general step per word
+#pragma unroll 1
+        for (uint32_t b = 0; b < 4; ++b) step((wd >> (b * 8)) & 0xffu, col + b);
+      }
+    };
+
+    ChunkReader tr;
+    tr.init(t, a.seqs_end);
+    uint32_t c0 = 0;
+    for (; c0 + 16 <= n; c0 += 16) {
+      const uint4 v = tr.next();
+      const uint32_t wv[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+      for (int q4 = 0; q4 < 4; ++q4) group4(wv[q4], c0 + q4 * 4);
+    }
+    if (c0 < n) {
+      // the last 1..15 columns: whole words of four through the same fast block, then 0..3 single columns. No column past |t| is run.
+      const uint4 v = tr.next();
+      uint32_t w0 = v.x, w1 = v.y, w2 = v.z;
+#pragma unroll 1
+      for (; c0 + 4 <= n; c0 += 4) {
+        group4(w0, c0);
+        w0 = w1; w1 = w2; w2 = v.w;
+      }
+#pragma unroll 1
+      for (; c0 < n; ++c0, w0 >>= 8) step(w0 & 0xffu, c0);
+    }
+
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) {
+      int d, e;
+      if (MODE == DGPU_MODE_NW) { d = score[j]; e = (int) n - 1; }
+      else { d = best[j]; e = bpos[j]; }
+      const int kk = a.k ? a.k[job0 + j] : -1;
+      d = apply_k(d, kk, MODE, (int) m[j], (int) n);
+      a.dist[job0 + j] = d;
+      if (a.end_loc) a.end_loc[job0 + j] = (d < 0) ? -1 : e;
+    }
+  }
+}
+
 // Register budget: no occupancy floor (min 1 CTA), so ptxas keeps the column and the job state of every class in registers (56 / 64 / 72
 // registers for NW = 1 / 2 / 3, 0 spills). On an H100 (400 W) floors of 8 and 9 CTAs per SM (64 and 56 registers, still no spills) ran
 // NW = 1 and 2 at the same speed and NW = 3 1 % slower; floors of 10 and more spill. Without any bound ptxas aims at a higher occupancy
@@ -253,142 +466,15 @@ __device__ __forceinline__ void rows_to_top(uint32_t (&e)[NW], uint32_t p, uint3
 template <int NW, int MODE, bool WANT_END>
 __global__ void __launch_bounds__(ED_THREADS, 1) ed_small_kernel(EdArgs a) {
   __shared__ uint32_t peq[5 * NW * ED_THREADS];
-  constexpr int HIN = (MODE == DGPU_MODE_HW) ? 0 : 1;
-  constexpr bool TOP = (MODE == DGPU_MODE_HW);  // query rows at the top of the bit-vector (rows_to_top)
-  const uint32_t cnt = a.counts[NW];
-  const uint32_t start = a.counts[8 + NW];
-  const uint32_t tid = threadIdx.x;
-  for (uint32_t idx = blockIdx.x * ED_THREADS + tid; idx < cnt; idx += gridDim.x * ED_THREADS) {
-    const uint32_t job = a.perm[start + idx];
-    const uint32_t m = a.q_len[job], n = a.t_len[job];
-    const uint8_t* q = a.seqs + a.q_off[job];
-    const uint8_t* t = a.seqs + a.t_off[job];
+  ed_small_jobs<NW, MODE, WANT_END, 1>(a, peq, NW);
+}
 
-    // ---- build Peq (match masks) for A,C,G,T,N, four query bytes at a time ------------
-    // Rows past |q| read whatever follows the query in the arena (the reader stays inside it); the last word is masked to |q|, or
-    // in the HW layout those rows are shifted out.
-    const uint32_t topbit = (m - 1) & 31u;
-    const uint32_t p = 32u * NW - m, vmask = TOP ? (1u << p) - 1u : 0u;  // jobs of this class have 32 (NW - 1) < |q| <= 32 NW
-    {
-      ChunkReader qr;
-      qr.init(q, a.seqs_end);
-      uint32_t pm[5][NW];
-#pragma unroll
-      for (int w = 0; w < NW; ++w) {
-#pragma unroll
-        for (int s = 0; s < 5; ++s) pm[s][w] = 0;
-#pragma unroll
-        for (int half = 0; half < 2; ++half) {
-          const uint4 v = qr.next();
-          const uint32_t wv[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const int sh = half * 16 + k * 4;
-            pm[0][w] |= match4(wv[k], 'A') << sh;
-            pm[1][w] |= match4(wv[k], 'C') << sh;
-            pm[2][w] |= match4(wv[k], 'G') << sh;
-            pm[3][w] |= match4(wv[k], 'T') << sh;
-            pm[4][w] |= match4(wv[k], 'N') << sh;
-          }
-        }
-      }
-#pragma unroll
-      for (int s = 0; s < 5; ++s) {
-        if (TOP) rows_to_top<NW>(pm[s], p, vmask);
-        else pm[s][NW - 1] &= (2u << topbit) - 1u;
-#pragma unroll
-        for (int w = 0; w < NW; ++w) peq[(peq_slot(s) * NW + w) * ED_THREADS + tid] = pm[s][w];
-      }
-    }
-
-    uint32_t Pv[NW], Mv[NW];
-#pragma unroll
-    for (int w = 0; w < NW; ++w) { Pv[w] = 0xffffffffu; Mv[w] = 0; }
-    Pv[0] = ~vmask;  // virtual rows start at Pv = Mv = 0
-    int score = (int) m;
-    // candidate end position -1 (score m) exists iff |q| % 64 != 0 (edlib's padding columns)
-    int best = (m & 63u) ? (int) m : 0x7fffffff;
-    int bpos = -1;
-
-    auto step = [&](uint32_t c, uint32_t col) {
-      uint32_t Eq[NW];
-      uint32_t code = dna_code(c);
-      if (code < 5) {
-#pragma unroll
-        for (int w = 0; w < NW; ++w) Eq[w] = peq[(peq_slot(code) * NW + w) * ED_THREADS + tid];
-      } else {
-#pragma unroll
-        for (int w = 0; w < NW; ++w) Eq[w] = eq_word_by_bytes(q + w * 32, min(32u, m - w * 32), c);
-        if (TOP) rows_to_top<NW>(Eq, p, vmask);
-      }
-      myers_column<NW, HIN, TOP>(Pv, Mv, Eq, topbit, score);
-      if (MODE != DGPU_MODE_NW) {
-        if (WANT_END) { if (score < best || (a.last_pos && score == best)) { best = score; bpos = (int) col; } }
-        else best = min(best, score);
-      }
-    };
-
-    ChunkReader tr;
-    tr.init(t, a.seqs_end);
-    uint32_t c0 = 0;
-    const uint32_t base2 = (tid * 4u) * 0x00010001u;  // this thread's slot offset in both 16-bit halves
-    for (; c0 + 16 <= n; c0 += 16) {
-      uint4 v = tr.next();
-      const uint32_t wv[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-      for (int q4 = 0; q4 < 4; ++q4) {
-        const uint32_t wd = wv[q4];
-        // four bytes at once: x = slot of each byte if it is one of ACGT; `expected` rebuilds the bytes from the slots
-        const uint32_t x = (wd >> 1) & 0x03030303u;
-        uint32_t sel = x | (x >> 4);
-        sel = (sel & 0xffu) | ((sel >> 8) & 0xff00u);
-        const uint32_t expected = __byte_perm(0x47544341u, 0u, sel);
-        if (wd == expected) {
-          // byte offsets of the four Peq rows, two per register: slot * (NW*512) + tid*4
-          const uint32_t offA = (x & 0x00ff00ffu) * (uint32_t) (NW * 4 * ED_THREADS) + base2;          // columns 0 and 2
-          const uint32_t offB = ((x >> 8) & 0x00ff00ffu) * (uint32_t) (NW * 4 * ED_THREADS) + base2;   // columns 1 and 3
-          int prev = 0;
-#pragma unroll
-          for (int b = 0; b < 4; ++b) {
-            const uint32_t pk = (b & 1) ? offB : offA;
-            const uint32_t off = (b & 2) ? (pk >> 16) : (pk & 0xffffu);
-            uint32_t Eq[NW];
-#pragma unroll
-            for (int w = 0; w < NW; ++w) Eq[w] = *(const uint32_t*) ((const char*) peq + off + w * 4 * ED_THREADS);
-            myers_column<NW, HIN, TOP>(Pv, Mv, Eq, topbit, score);
-            if (MODE != DGPU_MODE_NW) {
-              if (WANT_END) { if (score < best || (a.last_pos && score == best)) { best = score; bpos = (int) (c0 + q4 * 4 + b); } }
-              else if (b & 1) best = min(best, min(prev, score));  // two columns per three-input min
-              else prev = score;
-            }
-          }
-        } else {
-          // a byte outside ACGT among the four: one rolled copy of the general step per word
-#pragma unroll 1
-          for (uint32_t b = 0; b < 4; ++b) step((wd >> (b * 8)) & 0xffu, c0 + q4 * 4 + b);
-        }
-      }
-    }
-    if (c0 < n) {
-      uint4 v = tr.next();
-      uint32_t wv[4] = {v.x, v.y, v.z, v.w};
-      for (uint32_t b = 0; c0 + b < n; ++b) {
-        uint32_t w = wv[0];
-        w = (b >> 2) == 1 ? wv[1] : w;
-        w = (b >> 2) == 2 ? wv[2] : w;
-        w = (b >> 2) == 3 ? wv[3] : w;
-        step((w >> ((b & 3) * 8)) & 0xffu, c0 + b);
-      }
-    }
-
-    int d, e;
-    if (MODE == DGPU_MODE_NW) { d = score; e = (int) n - 1; }
-    else { d = best; e = bpos; }
-    const int kk = a.k ? a.k[job] : -1;
-    d = apply_k(d, kk, MODE, (int) m, (int) n);
-    a.dist[job] = d;
-    if (a.end_loc) a.end_loc[job] = (d < 0) ? -1 : e;
-  }
+// One thread per pair of HW jobs on one target (ed_slot): the ALT and REF probes of a genotyping read are realigned in one pass over the
+// read, so the target load, its decode, the Peq addresses, the job setup and the tail are paid once for two jobs.
+template <int NW>
+__global__ void __launch_bounds__(ED_THREADS, 1) ed_pair_kernel(EdArgs a) {
+  __shared__ uint32_t peq[5 * 2 * NW * ED_THREADS];
+  ed_small_jobs<NW, DGPU_MODE_HW, false, 2>(a, peq, ED_PAIR + NW);
 }
 
 // ---- warp-per-job wavefront for |q| > 128 -------------------------------------------
@@ -400,7 +486,7 @@ __global__ void __launch_bounds__(EDL_WARPS * 32) ed_long_kernel(EdArgs a, const
   constexpr int HIN0 = (MODE == DGPU_MODE_HW) ? 0 : 1;
   // job list: the class-5 segment of perm, or (NW with band passes in front) what the band passes left over
   const uint32_t cnt = list ? *list_cnt : a.counts[5];
-  if (!list) list = a.perm + a.counts[8 + 5];
+  if (!list) list = a.perm + a.counts[ED_START + 5];
   const int lane = threadIdx.x & 31;
   const int wib = threadIdx.x >> 5;
   const uint32_t gwarp = blockIdx.x * EDL_WARPS + wib;
@@ -527,9 +613,9 @@ __global__ void __launch_bounds__(EDL_WARPS * 32) ed_long_kernel(EdArgs a, const
 //     staircase covers the whole matrix. Otherwise the job goes to the next class (band twice as wide), finally to ed_long_kernel.
 //   * the first class of a job comes from a cheap upper bound (mismatches on the main diagonal + |d|, ed_band_plan_kernel): when it
 //     fits a class that class is certain to succeed; otherwise classes are tried from kvalid >= 64 upwards like the reference does.
-// counts[32 + c] = jobs queued for band class c (c < EDB_CLASSES), counts[32 + EDB_CLASSES] = jobs left to ed_long_kernel
+// counts[ED_BANDQ + c] = jobs queued for band class c (c < EDB_CLASSES), counts[ED_BANDQ + EDB_CLASSES] = jobs left to ed_long_kernel
 __device__ __forceinline__ void band_queue(const EdArgs& a, uint32_t* lists, uint32_t cap, int c, uint32_t job) {
-  lists[(size_t) c * cap + atomicAdd(&a.counts[32 + c], 1u)] = job;
+  lists[(size_t) c * cap + atomicAdd(&a.counts[ED_BANDQ + c], 1u)] = job;
 }
 
 // first class, from c0 on, that can hold the job and (need >= 0) certifies distances up to `need`, or covers the whole matrix
@@ -544,7 +630,7 @@ __device__ __forceinline__ int band_first_class(int c0, int m, int n, int need) 
 }
 
 __global__ void __launch_bounds__(256) ed_band_plan_kernel(EdArgs a, uint32_t* lists, uint32_t cap) {
-  const uint32_t cnt = a.counts[5], start = a.counts[8 + 5];
+  const uint32_t cnt = a.counts[5], start = a.counts[ED_START + 5];
   const int lane = threadIdx.x & 31;
   const uint32_t gwarp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
   for (uint32_t idx = gwarp; idx < cnt; idx += nwarps) {
@@ -580,7 +666,7 @@ __global__ void __launch_bounds__(EDB_WARPS * 32) ed_band_kernel(EdArgs a, uint3
   __shared__ uint64_t peq_s[EDB_WARPS][EDB_PEQ_WORDS];
   __shared__ uint64_t hoP[EDB_WARPS][32], hoM[EDB_WARPS][32];
   __shared__ int hoS[EDB_WARPS][32];
-  const uint32_t cnt = a.counts[32 + CLS];
+  const uint32_t cnt = a.counts[ED_BANDQ + CLS];
   const uint32_t* list = lists + (size_t) CLS * cap;
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
   const int p = lane & (G - 1), grp = lane / G;
@@ -720,12 +806,22 @@ int launch_mode(dgpu_ctx* ctx, EdArgs& a, const uint32_t* hc, cudaStream_t st) {
   ED_LAUNCH_SMALL(3)
   ED_LAUNCH_SMALL(4)
 #undef ED_LAUNCH_SMALL
+#define ED_LAUNCH_PAIR(NWV)                                                                                 \
+  if (hc[ED_PAIR + NWV]) {                                                                                  \
+    ed_pair_kernel<NWV><<<grid_for(hc[ED_PAIR + NWV], ED_THREADS, ED_CTAS_PER_SM), ED_THREADS, 0, st>>>(a); \
+    DGPU_LAUNCH_CHECK(ctx, "ed_pair");                                                                      \
+  }
+  ED_LAUNCH_PAIR(1)
+  ED_LAUNCH_PAIR(2)
+  ED_LAUNCH_PAIR(3)
+  ED_LAUNCH_PAIR(4)
+#undef ED_LAUNCH_PAIR
   if (hc[5]) {
     uint32_t g = grid_for(hc[5], EDL_WARPS, 8);
     a.hbuf = nullptr;
     a.hbuf_stride = 0;
-    if (hc[24]) {
-      a.hbuf_stride = (hc[24] + 255u) & ~255u;
+    if (hc[ED_TMAX]) {
+      a.hbuf_stride = (hc[ED_TMAX] + 255u) & ~255u;
       void* hb;
       int rc = dgpu_reserve(ctx, SLOT_ED_STRIPES, (size_t) g * EDL_WARPS * a.hbuf_stride, &hb);
       if (rc) return rc;
@@ -750,8 +846,8 @@ int launch_mode(dgpu_ctx* ctx, EdArgs& a, const uint32_t* hc, cudaStream_t st) {
       ED_LAUNCH_BAND(16)
       ED_LAUNCH_BAND(32)
 #undef ED_LAUNCH_BAND
-      if (a.eq_cls) ed_long_kernel<MODE, true><<<g, EDL_WARPS * 32, 0, st>>>(a, lists + (size_t) EDB_CLASSES * cap, a.counts + 32 + EDB_CLASSES);
-      else ed_long_kernel<MODE, false><<<g, EDL_WARPS * 32, 0, st>>>(a, lists + (size_t) EDB_CLASSES * cap, a.counts + 32 + EDB_CLASSES);
+      if (a.eq_cls) ed_long_kernel<MODE, true><<<g, EDL_WARPS * 32, 0, st>>>(a, lists + (size_t) EDB_CLASSES * cap, a.counts + ED_BANDQ + EDB_CLASSES);
+      else ed_long_kernel<MODE, false><<<g, EDL_WARPS * 32, 0, st>>>(a, lists + (size_t) EDB_CLASSES * cap, a.counts + ED_BANDQ + EDB_CLASSES);
       DGPU_LAUNCH_CHECK(ctx, "ed_long");
     } else if (a.eq_cls) {
       ed_long_kernel<MODE, true><<<g, EDL_WARPS * 32, 0, st>>>(a, nullptr, nullptr);
@@ -805,6 +901,7 @@ int dgpu_edit_distance_impl(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_by
   a.n = (uint32_t) n; a.dist = dist; a.end_loc = end_loc;
   a.hbuf = nullptr; a.hbuf_stride = 0;
   a.last_pos = last_pos;
+  a.pair = (mode == DGPU_MODE_HW && !end_loc && !eq_tabs) ? 1 : 0;
   // eq_tabs (device): uint32 f[256], uint32 s[256], then uint8 cls[256]
   a.eq_f = eq_tabs; a.eq_s = eq_tabs ? eq_tabs + 256 : nullptr; a.eq_cls = eq_tabs ? (const uint8_t*) (eq_tabs + 512) : nullptr;
   a.force_long = eq_tabs ? 1 : 0;
@@ -812,11 +909,11 @@ int dgpu_edit_distance_impl(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_by
   int rc = dgpu_reserve(ctx, SLOT_JOB_PERM, n * sizeof(uint32_t), &p);
   if (rc) return rc;
   a.perm = (uint32_t*) p;
-  rc = dgpu_reserve(ctx, SLOT_COUNTS, 64 * sizeof(uint32_t), &p);
+  rc = dgpu_reserve(ctx, SLOT_COUNTS, ED_COUNTS_WORDS * sizeof(uint32_t), &p);
   if (rc) return rc;
   a.counts = (uint32_t*) p;
 
-  DGPU_CUDA(ctx, cudaMemsetAsync(a.counts, 0, 64 * sizeof(uint32_t), st));
+  DGPU_CUDA(ctx, cudaMemsetAsync(a.counts, 0, ED_COUNTS_WORDS * sizeof(uint32_t), st));
   const uint32_t cb = (uint32_t) ((n + 255) / 256);
   ed_count_kernel<<<cb, 256, 0, st>>>(a, mode);
   DGPU_LAUNCH_CHECK(ctx, "ed_count");
@@ -824,16 +921,21 @@ int dgpu_edit_distance_impl(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_by
   DGPU_LAUNCH_CHECK(ctx, "ed_offsets");
   ed_scatter_kernel<<<cb, 256, 0, st>>>(a);
   DGPU_LAUNCH_CHECK(ctx, "ed_scatter");
-  uint32_t hc[32];
+  uint32_t hc[ED_TMAX + 1];
   if (ctx->async_bound) {
     // Asynchronous form (dgpu_set_async_bound): no host round trip. Every class is launched with a grid sized from the job count (the kernels
     // read their own class counts on the device and an empty class returns at once), the stripe scratch of long targets from the caller's bound.
-    for (int c = 0; c < 32; ++c) hc[c] = 0;
+    for (uint32_t& c : hc) c = 0;
     const uint32_t bound = ctx->async_bound;
     hc[1] = hc[2] = (uint32_t) n;
     if (bound > 64) hc[3] = (uint32_t) n;
     if (bound > 96) hc[4] = (uint32_t) n;
-    if (bound > 128 || a.force_long) { hc[5] = (uint32_t) n; if (bound > 2048) hc[24] = bound; }
+    if (bound > 128 || a.force_long) { hc[5] = (uint32_t) n; if (bound > 2048) hc[ED_TMAX] = bound; }
+    if (a.pair) {   // a pair takes two jobs
+      hc[ED_PAIR + 1] = hc[ED_PAIR + 2] = (uint32_t) (n / 2);
+      if (bound > 64) hc[ED_PAIR + 3] = (uint32_t) (n / 2);
+      if (bound > 96) hc[ED_PAIR + 4] = (uint32_t) (n / 2);
+    }
   } else {
     // One small D2H so that launches are sized exactly and empty classes cost nothing.
     DGPU_CUDA(ctx, cudaMemcpyAsync(hc, a.counts, sizeof(hc), cudaMemcpyDeviceToHost, st));
@@ -899,7 +1001,8 @@ int dgpu_edit_distance(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
     DGPU_CUDA(ctx, cudaMemcpyAsync(d_seqs + o, seqs + o, len, cudaMemcpyHostToDevice, cs));
     DGPU_CUDA(ctx, cudaEventRecord(ev[1 + npieces], cs));
   }
-  const uint64_t jobs_per = (n + njc - 1) / njc;
+  // an even range size, so that no range starts on the odd member of a target-sharing pair (ed_slot pairs jobs 2i and 2i + 1 of a call)
+  const uint64_t jobs_per = (((n + njc - 1) / njc) + 1) & ~1ull;
   DGPU_CUDA(ctx, cudaStreamWaitEvent(st, ev[0], 0));
   DGPU_CUDA(ctx, cudaMemsetAsync(d_ext, 0, (ED_PIPE_MAX_CHUNKS + 1) * sizeof(uint32_t), st));
   ed_extent_kernel<<<(unsigned) ((n + 255) / 256), 256, 0, st>>>(d_qoff, d_qlen, d_toff, d_tlen, (uint32_t) n, (uint32_t) jobs_per, (uint32_t) seqs_bytes, d_ext);

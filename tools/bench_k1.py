@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """K1 per query-length class: the configs[1] batch of bench.py (10 M HW edit-distance jobs, probes of 26-80 bp against 150 bp reads)
-split by words per thread-job, NW = ceil(|q| / 32), and each class timed on its own with the one-thread-per-job kernel
-ed_small_kernel<NW, HW>.
+split by words per thread-job, NW = ceil(|q| / 32), and each class timed on its own with the one-thread kernels: ed_pair_kernel<NW> for
+the ALT / REF probe pairs of one read (jobs 2i and 2i + 1 on one target, both of the class), ed_small_kernel<NW, HW> for the probes whose
+partner is in another class. A class's jobs are its pairs first, in batch order (so each pair stays at an even index), then its lone probes.
 
   kernel_ms           median over the timed calls of the library's CUDA events around the class's kernel (ctx.last_kernel_ms())
   jobs_per_s          jobs of the class / kernel_ms
@@ -47,7 +48,10 @@ def main():
     sampler = ClockSampler(0)
     sampler.start()
     for c in (1, 2, 3):
-        sel = np.nonzero(nw == c)[0]
+        both = (nw[0::2] == c) & (nw[1::2] == c) & (b["t_off"][0::2] == b["t_off"][1::2])
+        pairs = np.stack([np.nonzero(both)[0] * 2, np.nonzero(both)[0] * 2 + 1], axis=1).reshape(-1)
+        lone = np.nonzero(nw == c)[0]
+        sel = np.concatenate([pairs, np.setdiff1d(lone, pairs)])
         if len(sel) == 0:
             continue
         d = {k: torch.from_numpy(np.ascontiguousarray(b[k][sel]).view(np.int32)).to(dev) for k in ("q_off", "q_len", "t_off", "t_len", "k")}
@@ -65,13 +69,13 @@ def main():
         kms = float(np.median(ks))
         cols = int(b["t_len"][sel].astype(np.int64).sum())
         ql = b["q_len"][sel]
-        classes.append({"nw": c, "q_len": [int(ql.min()), int(ql.max())], "jobs": int(len(sel)), "share": len(sel) / len(nw),
+        classes.append({"nw": c, "q_len": [int(ql.min()), int(ql.max())], "jobs": int(len(sel)), "paired_jobs": int(len(pairs)), "share": len(sel) / len(nw),
                         "kernel_ms": kms, "kernel_ms_min_max": [float(min(ks)), float(max(ks))], "reps": reps, "window_s": float(sum(ks)) * 1e-3,
                         "jobs_per_s": len(sel) / (kms * 1e-3), "thread_columns_per_s": cols / (kms * 1e-3)})
         del d, dist
     clocks = sampler.stop()
     mix = ctx.int_peak_mix()
-    res = {"workload": "configs[1] batch of bench.py split by NW = ceil(|q|/32); ed_small_kernel<NW, HW> per class",
+    res = {"workload": "configs[1] batch of bench.py split by NW = ceil(|q|/32); ed_pair_kernel<NW> + ed_small_kernel<NW, HW> per class",
            "jobs": int(len(nw)), "lib": os.path.relpath(delly_b200.LIB_PATH, ROOT), "gpu": gpu_info(0), "clocks": clocks,
            "int_peak_mix_tera_instr_per_s": mix, "classes": classes}
     line = json.dumps(res)

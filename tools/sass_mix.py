@@ -10,6 +10,9 @@ and the decode of the word. Its counts are divided by four and grouped by the pi
   lds   shared-memory loads
   vshr  variable-amount right shifts (SHF.R with a register shift amount) among the alu instructions
 
+pair_report() gives the same mix for ed_pair_kernel<NW> per job-column (its fast block runs four columns of two jobs), and
+small_prologues() / prologue_alu() count the ALU instructions of the job load and Peq build (up to the function's last STS).
+
 Usage: python tools/sass_mix.py [LIB] [--json]   (LIB defaults to the in-tree delly_b200/libdelly_b200.so)
 """
 import json
@@ -26,6 +29,7 @@ ALU = ("LOP3", "LOP", "SHF", "IADD3", "VIMNMX", "VIMNMX3", "IMNMX", "LEA", "PRMT
 BRANCH = ("BRA", "EXIT", "RET", "CALL", "BRX", "JMP", "JMX")
 INSN = re.compile(r"/\*[0-9a-f]+\*/\s+(@!?U?P\w+\s+)?([A-Z0-9_.]+)\s*([^;]*);")
 KERNEL = re.compile(r"ed_small_kernelILi(\d)ELi(\d)ELb(\d)E")
+PAIR_KERNEL = re.compile(r"ed_pair_kernelILi(\d)E")
 
 
 def cuobjdump():
@@ -93,8 +97,44 @@ def mix(lines):
     return res
 
 
+def prologue_alu(lines):
+    """Integer-ALU instructions from the start of a function through its last shared-memory store: for ed_small_kernel and ed_pair_kernel
+    the job load and the Peq build (with the set-up of the out-of-line calls that build words holding a byte outside ACGT)."""
+    ops = [m.group(2) for m in map(INSN.search, lines) if m]
+    last = max(i for i, op in enumerate(ops) if op.startswith("STS"))
+    return sum(op.split(".")[0] in ALU for op in ops[:last + 1])
+
+
+def pair_report(lib):
+    """{"NW=n": mix} of the fast block of ed_pair_kernel<n>, per job-column (the block runs four columns of two jobs), with "prologue_alu"."""
+    res = {}
+    for name, lines in functions(_sass(lib)).items():
+        m = PAIR_KERNEL.search(name)
+        if m:
+            r = mix(lines)
+            r = {k: (v / 2 if k != "ops" else {o: n / 2 for o, n in v.items()}) for k, v in r.items()}
+            r["prologue_alu"] = prologue_alu(lines)
+            res[f"NW={m.group(1)}"] = r
+    return dict(sorted(res.items()))
+
+
+def small_prologues(lib):
+    """{"NW=n MODE[ end]": prologue_alu} of every ed_small_kernel instantiation."""
+    res = {}
+    for name, lines in functions(_sass(lib)).items():
+        m = KERNEL.search(name)
+        if m:
+            nw, mode, end = int(m.group(1)), int(m.group(2)), int(m.group(3))
+            res[f"NW={nw} {MODES[mode]}{' end' if end else ''}"] = prologue_alu(lines)
+    return dict(sorted(res.items()))
+
+
+def _sass(lib):
+    return subprocess.run([cuobjdump(), "-sass", lib], capture_output=True, text=True, check=True).stdout
+
+
 def report(lib):
-    sass = subprocess.run([cuobjdump(), "-sass", lib], capture_output=True, text=True, check=True).stdout
+    sass = _sass(lib)
     res = {}
     for name, lines in functions(sass).items():
         m = KERNEL.search(name)
