@@ -17,7 +17,8 @@
 //     per-thread-private, bank-conflict-free slice of shared memory; the target is streamed with
 //     aligned LDG.128 + PRMT realignment (ChunkReader).
 //   * HW jobs 2i and 2i+1 on the same target (a read's ALT and REF probes) with queries of one class
-//     run as a pair in one thread (ed_pair_kernel): one target stream and decode, two Myers columns.
+//     run as a pair in one thread (ed_pair_kernel): one target stream and decode, two Myers columns. Pairs whose two queries fit one
+//     column of 3 or 5 words with a separator row between them (33-47 bp or 65-79 bp probe pairs) share that column (ed_pack_kernel).
 //   * |q| > 128: ONE WARP PER JOB, anti-diagonal wavefront: lane l owns a 64-row block and processes
 //     column t-l at step t; the horizontal delta (hout) crosses lanes by shuffle. Queries longer
 //     than 2048 rows are processed in 2048-row stripes, the stripe's bottom hout per column being
@@ -41,9 +42,11 @@ constexpr int ED_THREADS = 128;
 #define ED_CTAS_PER_SM_V 32
 #endif
 constexpr int ED_CTAS_PER_SM = ED_CTAS_PER_SM_V;
-// job classes: 0 trivial, 1..4 = words per thread-job, 5 = warp-per-job, ED_PAIR + 1..4 = target-sharing pairs of class 1..4 (ed_pair_kernel)
+// job classes: 0 trivial, 1..4 = words per thread-job, 5 = warp-per-job, ED_PAIR + 1..4 = target-sharing pairs of class 1..4 (ed_pair_kernel),
+// ED_PACK + 0 / + 1 = target-sharing pairs packed into one column of 3 / 5 words (ed_pack_kernel<3, 1> / <5, 2>)
 constexpr int ED_PAIR = 5;
-constexpr int ED_NCLS = ED_PAIR + 5;
+constexpr int ED_PACK = ED_PAIR + 5;
+constexpr int ED_NCLS = ED_PACK + 2;
 // counts layout (SLOT_COUNTS): [0, 16) jobs per class, [ED_START, +16) class starts in perm, [ED_CUR, +16) scatter cursors, [ED_TMAX] max t_len
 // of multi-stripe jobs, [ED_BANDQ, +EDB_CLASSES + 1) band pass queues
 constexpr int ED_START = 16, ED_CUR = 32, ED_TMAX = 48, ED_BANDQ = 64, ED_COUNTS_WORDS = 128;
@@ -95,15 +98,33 @@ __device__ __forceinline__ int apply_k(int d, int k, int mode, int m, int n) {
   }
 }
 
-// Count slot of job i: its class, or, for the even member i of a pair (i, i + 1) of one-thread jobs of the same class on the same target
-// (equal t_off and t_len: the ALT and REF probes of one genotyping read), the pair class ED_PAIR + class; -1 for the odd member of a pair.
-// Indices are relative to the call.
+// Whether two HW queries of a target fit one column of W words (ed_pack_kernel<W, WA>) in the order A = ma at the bottom, B = mb at the
+// top: A's last row lies in word WA (32 WA < ma <= 32 WA + 31, so that the row above it, the first separator row, is in the same word),
+// and at least one separator row is left between A and B (ma + mb + 1 <= 32 W).
+__device__ __forceinline__ bool pack_fits(uint32_t ma, uint32_t mb, int W, int WA) {
+  return ma > 32u * WA && ma <= 32u * WA + 31u && mb >= 1u && ma + mb < 32u * W;
+}
+
+// Pack class of the pair of query lengths (m0, m1) of jobs 2i and 2i + 1, in the order (m0, m1) or else (m1, m0); -1 if neither fits.
+__device__ __forceinline__ int pack_class(uint32_t m0, uint32_t m1) {
+  if (pack_fits(m0, m1, 3, 1) || pack_fits(m1, m0, 3, 1)) return ED_PACK;
+  if (pack_fits(m0, m1, 5, 2) || pack_fits(m1, m0, 5, 2)) return ED_PACK + 1;
+  return -1;
+}
+
+// Count slot of job i: its class, or, for the even member i of a pair (i, i + 1) of one-thread jobs on the same target (equal t_off and
+// t_len: the ALT and REF probes of one genotyping read), the pack class if the two queries fit one (pack_class), else the pair class
+// ED_PAIR + class if both are of the same class; -1 for the odd member of a pair. Indices are relative to the call.
 __device__ __forceinline__ int ed_slot(const EdArgs& a, uint32_t i) {
   const uint32_t tl = a.t_len[i];
   const int c = ed_class(a.q_len[i], tl, a.force_long);
   if (!a.pair || c < 1 || c > 4) return c;
   const uint32_t o = i ^ 1u;
-  if (o >= a.n || a.t_off[o] != a.t_off[i] || a.t_len[o] != tl || ed_class(a.q_len[o], tl, 0) != c) return c;
+  if (o >= a.n || a.t_off[o] != a.t_off[i] || a.t_len[o] != tl) return c;
+  const uint32_t mi = a.q_len[i], mo = a.q_len[o];
+  const int pk = (i & 1u) ? pack_class(mo, mi) : pack_class(mi, mo);
+  if (pk >= 0) return (i & 1u) ? -1 : pk;
+  if (ed_class(mo, tl, 0) != c) return c;
   return (i & 1u) ? -1 : ED_PAIR + c;
 }
 
@@ -184,6 +205,13 @@ template <> struct AddChain<4> {
         : "r"(x[0]), "r"(x[1]), "r"(x[2]), "r"(x[3]), "r"(y[0]), "r"(y[1]), "r"(y[2]), "r"(y[3]));
   }
 };
+template <> struct AddChain<5> {
+  static __device__ __forceinline__ void run(uint32_t* s, const uint32_t* x, const uint32_t* y) {
+    asm("add.cc.u32 %0, %5, %10;\n\taddc.cc.u32 %1, %6, %11;\n\taddc.cc.u32 %2, %7, %12;\n\taddc.cc.u32 %3, %8, %13;\n\taddc.u32 %4, %9, %14;"
+        : "=r"(s[0]), "=r"(s[1]), "=r"(s[2]), "=r"(s[3]), "=r"(s[4])
+        : "r"(x[0]), "r"(x[1]), "r"(x[2]), "r"(x[3]), "r"(x[4]), "r"(y[0]), "r"(y[1]), "r"(y[2]), "r"(y[3]), "r"(y[4]));
+  }
+};
 
 // One DP column of the single-block Myers recurrence over NW 32-bit words, adding the column's delta of D at the query's last row to
 // `score`. HIN = horizontal delta entering the top row: 0 for HW (free start), +1 for NW/SHW.
@@ -192,9 +220,13 @@ template <> struct AddChain<4> {
 // is two mad.hi by 2, which ptxas turns into two LEA.HI instead of the 5 ALU instructions of a read at a variable bit. On an H100
 // (400 W) a multiplier ptxas cannot see, which keeps the mad.hi and the carries on the FMA pipe as IMAD.HI, made the K1 kernels
 // 3-8 % slower than this form: dgpu_int_peak_mix shows IMADs issuing alongside LOP3s at full rate, but IMAD.WIDE.U32 not.
-template <int NW, int HIN, bool TOP>
+// SEPW >= 0: the packed layout of ed_pack_kernel, a second query A in the rows below the first separator row, bit `sep` of word SEPW.
+// The shift carries A's last-row Ph / Mh into that row; clearing the bit in the new Pv and Mv keeps it at Pv = Mv = 0, so the separator
+// stays inert (ed_pack_kernel). A's delta is added to score_a: A's last row, bit s of word SEPW, moves to bit 31 with a plain IMAD by
+// mula = 2^(31 - s) on the FMA pipe, then read as above.
+template <int NW, int HIN, bool TOP, int SEPW = -1>
 __device__ __forceinline__ void myers_column(uint32_t (&Pv)[NW], uint32_t (&Mv)[NW], const uint32_t (&Eq)[NW], uint32_t topbit,
-                                             int& score) {
+                                             int& score, uint32_t sep = 0, uint32_t mula = 0, int* score_a = nullptr) {
   uint32_t Xv[NW], t[NW], sum[NW], Ph[NW], Mh[NW];
 #pragma unroll
   for (int w = 0; w < NW; ++w) {
@@ -215,6 +247,11 @@ __device__ __forceinline__ void myers_column(uint32_t (&Pv)[NW], uint32_t (&Mv)[
   } else {
     score += (int) ((Ph[NW - 1] >> topbit) & 1u) - (int) ((Mh[NW - 1] >> topbit) & 1u);
   }
+  if constexpr (SEPW >= 0) {
+    const uint32_t pa = Ph[SEPW] * mula, ma = Mh[SEPW] * mula;
+    asm("mad.hi.u32 %0, %1, 2, %0;" : "+r"(*score_a) : "r"(pa));
+    asm("mad.hi.s32 %0, %1, 2, %0;" : "+r"(*score_a) : "r"(ma));
+  }
   // shift Ph / Mh up by one row across the words. Every index is a constant after unrolling, so the column stays in registers
   // (a backward loop with a w == 0 case was left rolled by ptxas and put the arrays on the stack).
   uint32_t ph[NW], mh[NW], cp = HIN, cm = 0;
@@ -229,6 +266,10 @@ __device__ __forceinline__ void myers_column(uint32_t (&Pv)[NW], uint32_t (&Mv)[
   for (int w = 0; w < NW; ++w) {
     Pv[w] = mh[w] | ~(Xv[w] | ph[w]);
     Mv[w] = ph[w] & Xv[w];
+    if (w == SEPW) {
+      Pv[w] &= ~sep;
+      Mv[w] &= ~sep;
+    }
   }
 }
 
@@ -289,12 +330,10 @@ __device__ __forceinline__ void rows_to_top(uint32_t (&e)[NW], uint32_t p, uint3
 // LOP3 of the planes, with no N row. A word with any byte outside ACGT is built exactly by match32 instead (N rows get the N mask, other
 // bytes no bit). Rows past |q| read whatever follows the query in the arena (the reader stays inside it); the last word is masked to |q|, or
 // in the HW layout those rows are shifted out.
-template <int NW, bool TOP>
-__device__ __forceinline__ void build_peq(uint32_t* pq, int SW, const uint8_t* q, const uint8_t* seqs_end, uint32_t topbit, uint32_t p,
-                                          uint32_t vmask) {
+template <int NW>
+__device__ __forceinline__ void peq_words(uint32_t (&pm)[5][NW], const uint8_t* q, const uint8_t* seqs_end) {
   ChunkReader qr;
   qr.init(q, seqs_end);
-  uint32_t pm[5][NW];
 #pragma unroll
   for (int w = 0; w < NW; ++w) {
     const uint4 lo = qr.next(), hi = qr.next();
@@ -321,6 +360,13 @@ __device__ __forceinline__ void build_peq(uint32_t* pq, int SW, const uint8_t* q
       pm[4][w] = match32(lo, hi, 'N');
     }
   }
+}
+
+template <int NW, bool TOP>
+__device__ __forceinline__ void build_peq(uint32_t* pq, int SW, const uint8_t* q, const uint8_t* seqs_end, uint32_t topbit, uint32_t p,
+                                          uint32_t vmask) {
+  uint32_t pm[5][NW];
+  peq_words<NW>(pm, q, seqs_end);
 #pragma unroll
   for (int s = 0; s < 5; ++s) {
     if (TOP) rows_to_top<NW>(pm[s], p, vmask);
@@ -330,14 +376,81 @@ __device__ __forceinline__ void build_peq(uint32_t* pq, int SW, const uint8_t* q
   }
 }
 
+// ---- ed_pack_kernel's layout: two HW queries of one target in one column of R = 32 W rows ----------------------------------------------
+// A in rows 0 .. mA-1 (its last row in word WA), B in rows R-mB .. R-1 (its last row bit 31 of word W-1, as in ed_small_kernel's HW
+// layout), and between them at least one separator row. Separator rows are virtual rows like those below a query in the HW layout: Eq = 1
+// for every byte, Pv = Mv = 0 at the start. The first one (bit mA & 31 of word WA) would take A's last-row Ph / Mh through the shift, so
+// myers_column clears it in Pv and Mv (SEPW); every other separator row computes Ph = Mh = 0, carries nothing, and shifts a 0 into the
+// row above it, so B's first row sees HW's free top row just as A's row 0 does at the bottom of the column.
+
+// bits of word w that are rows in [lo, hi)
+__device__ __forceinline__ uint32_t rows_in(uint32_t w, uint32_t lo, uint32_t hi) {
+  auto below = [](int x) { return x <= 0 ? 0u : x >= 32 ? 0xffffffffu : (1u << x) - 1u; };
+  return below((int) hi - (int) (32u * w)) & ~below((int) lo - (int) (32u * w));
+}
+
+// B's Peq words in the HW layout of its own class, NB = ceil(mB / 32) words, stored as the top NB words of the W-word column (NBMAX >= NB)
+template <int W, int NBMAX>
+__device__ __forceinline__ void build_peq_top(uint32_t* pq, const uint8_t* q, uint32_t m, const uint8_t* seqs_end) {
+  if constexpr (NBMAX > 1) {
+    if (m <= 32u * (NBMAX - 1)) {
+      build_peq_top<W, NBMAX - 1>(pq, q, m, seqs_end);
+      return;
+    }
+  }
+  const uint32_t p = 32u * NBMAX - m;
+  build_peq<NBMAX, true>(pq + (W - NBMAX) * ED_THREADS, W, q, seqs_end, 0, p, (1u << p) - 1u);
+}
+
+// The packed Peq table of one thread (pq = peq + tid, W words per symbol slot): B's words at the top, words of separator rows only all
+// ones, then A's words from the bottom, A's last word WA taking the separator and B rows above mA from what is stored there.
+template <int W, int WA>
+__device__ __forceinline__ void build_pack_peq(uint32_t* pq, const uint8_t* qa, uint32_t ma, const uint8_t* qb, uint32_t mb,
+                                               const uint8_t* seqs_end) {
+  build_peq_top<W, W - WA>(pq, qb, mb, seqs_end);
+  const uint32_t nb = (mb + 31u) >> 5;
+#pragma unroll 1
+  for (uint32_t w = WA; w < W - nb; ++w)
+#pragma unroll
+    for (int s = 0; s < 5; ++s) pq[(s * W + w) * ED_THREADS] = 0xffffffffu;
+  uint32_t pm[5][WA + 1];
+  peq_words<WA + 1>(pm, qa, seqs_end);
+  const uint32_t low = (2u << ((ma - 1u) & 31u)) - 1u;
+#pragma unroll
+  for (int s = 0; s < 5; ++s) {
+#pragma unroll
+    for (int w = 0; w < WA; ++w) pq[(s * W + w) * ED_THREADS] = pm[s][w];
+    uint32_t& top = pq[(s * W + WA) * ED_THREADS];
+    top = (pm[s][WA] & low) | (top & ~low);
+  }
+}
+
+// word w of the packed column's match mask for a target byte c outside ACGTN (the exact slow path): byte equality in A's and B's rows,
+// 1 in the separator rows. Out of line, like eq_word_by_bytes.
+__device__ __noinline__ uint32_t pack_eq_word(const uint8_t* qa, uint32_t ma, const uint8_t* qb, uint32_t b0, uint32_t w, uint32_t c) {
+  uint32_t e = 0;
+  for (uint32_t i = 0; i < 32; ++i) {
+    const uint32_t r = 32u * w + i;
+    const bool eq = r < ma ? __ldg(qa + r) == (uint8_t) c : r < b0 ? true : __ldg(qb + (r - b0)) == (uint8_t) c;
+    e |= (uint32_t) eq << i;
+  }
+  return e;
+}
+
 // NJ (1 or 2) jobs of one thread that share a target: jobs perm[i], ..., perm[i] + NJ - 1 of the class `cls` segment of perm. One target stream,
 // one byte decode and one Peq address per column feed NJ independent Myers columns. The Peq table of the thread holds, per symbol slot,
 // the NW words of each job's query: peq[(slot * NJ NW + j NW + w) * ED_THREADS + tid].
-template <int NW, int MODE, bool WANT_END, int NJ>
+// WA >= 0 (ed_pack_kernel, NJ = 2, HW): the two queries share ONE column of NW words (the packed layout above build_pack_peq), A = job 0 in
+// the bottom rows with its last row in word WA, B = job 1 at the top; job 0 is the call's job perm[i] if the pair fits in that order
+// (pack_fits), else perm[i] + 1. The Peq table then holds NW words per slot.
+template <int NW, int MODE, bool WANT_END, int NJ, int WA = -1>
 __device__ __forceinline__ void ed_small_jobs(const EdArgs& a, uint32_t* peq, int cls) {
   constexpr int HIN = (MODE == DGPU_MODE_HW) ? 0 : 1;
   constexpr bool TOP = (MODE == DGPU_MODE_HW);  // query rows at the top of the bit-vector (rows_to_top)
-  constexpr int SW = NJ * NW;                    // Peq words per symbol slot
+  constexpr bool PACK = WA >= 0;
+  constexpr int NC = PACK ? 1 : NJ;              // Myers columns per thread
+  constexpr int SW = NC * NW;                    // Peq words per symbol slot
+  static_assert(!PACK || (NJ == 2 && MODE == DGPU_MODE_HW && !WANT_END), "a packed column holds two HW distances");
   const uint32_t cnt = a.counts[cls];
   const uint32_t start = a.counts[ED_START + cls];
   const uint32_t tid = threadIdx.x;
@@ -345,21 +458,45 @@ __device__ __forceinline__ void ed_small_jobs(const EdArgs& a, uint32_t* peq, in
     const uint32_t job0 = a.perm[start + idx];
     const uint32_t n = a.t_len[job0];
     const uint8_t* t = a.seqs + a.t_off[job0];
-    uint32_t m[NJ], topbit[NJ], p[NJ], vmask[NJ];
+    uint32_t m[NJ], jid[NJ], topbit[NC], p[NC], vmask[NC];
     const uint8_t* q[NJ];
-    uint32_t Pv[NJ][NW], Mv[NJ][NW];
+    uint32_t Pv[NC][NW], Mv[NC][NW];
+    uint32_t sep = 0, mula = 0;
     int score[NJ], best[NJ], bpos[NJ], prev[NJ];
+    if constexpr (PACK) {
+      const uint32_t m0 = a.q_len[job0], m1 = a.q_len[job0 + 1];
+      const uint32_t sw = pack_fits(m0, m1, NW, WA) ? 0u : 1u;
+      jid[0] = job0 + sw;
+      jid[1] = job0 + (sw ^ 1u);
+      m[0] = sw ? m1 : m0;
+      m[1] = sw ? m0 : m1;
+      q[0] = a.seqs + a.q_off[jid[0]];
+      q[1] = a.seqs + a.q_off[jid[1]];
+      build_pack_peq<NW, WA>(peq + tid, q[0], m[0], q[1], m[1], a.seqs_end);
+      p[0] = 32u * NW - m[1];  // first row of B; the separator is rows m[0] .. p[0] - 1
+#pragma unroll
+      for (int w = 0; w < NW; ++w) { Pv[0][w] = ~rows_in(w, m[0], p[0]); Mv[0][w] = 0; }
+      // both through a mov that ptxas cannot see into: a multiplier it knows to be 1 << x becomes a variable SHF.L on the ALU pipe again,
+      // and a mask it can rebuild from m[0] is recomputed in the column loop (two ALU instructions per four columns)
+      asm("mov.b32 %0, %1;" : "=r"(sep) : "r"(1u << (m[0] & 31u)));
+      asm("mov.b32 %0, %1;" : "=r"(mula) : "r"(1u << (31u - ((m[0] - 1u) & 31u))));
+      topbit[0] = 0;
+      vmask[0] = 0;
+    }
 #pragma unroll
     for (int j = 0; j < NJ; ++j) {
-      m[j] = a.q_len[job0 + j];
-      q[j] = a.seqs + a.q_off[job0 + j];
-      topbit[j] = (m[j] - 1) & 31u;
-      p[j] = 32u * NW - m[j];  // jobs of this class have 32 (NW - 1) < |q| <= 32 NW
-      vmask[j] = TOP ? (1u << p[j]) - 1u : 0u;
-      build_peq<NW, TOP>(peq + j * NW * ED_THREADS + tid, SW, q[j], a.seqs_end, topbit[j], p[j], vmask[j]);
+      if constexpr (!PACK) {
+        jid[j] = job0 + j;
+        m[j] = a.q_len[job0 + j];
+        q[j] = a.seqs + a.q_off[job0 + j];
+        topbit[j] = (m[j] - 1) & 31u;
+        p[j] = 32u * NW - m[j];  // jobs of this class have 32 (NW - 1) < |q| <= 32 NW
+        vmask[j] = TOP ? (1u << p[j]) - 1u : 0u;
+        build_peq<NW, TOP>(peq + j * NW * ED_THREADS + tid, SW, q[j], a.seqs_end, topbit[j], p[j], vmask[j]);
 #pragma unroll
-      for (int w = 0; w < NW; ++w) { Pv[j][w] = 0xffffffffu; Mv[j][w] = 0; }
-      Pv[j][0] = ~vmask[j];  // virtual rows start at Pv = Mv = 0
+        for (int w = 0; w < NW; ++w) { Pv[j][w] = 0xffffffffu; Mv[j][w] = 0; }
+        Pv[j][0] = ~vmask[j];  // virtual rows start at Pv = Mv = 0
+      }
       score[j] = (int) m[j];
       // candidate end position -1 (score m) exists iff |q| % 64 != 0 (edlib's padding columns)
       best[j] = (m[j] & 63u) ? (int) m[j] : 0x7fffffff;
@@ -374,21 +511,30 @@ __device__ __forceinline__ void ed_small_jobs(const EdArgs& a, uint32_t* peq, in
       }
     };
     // one column through the table (ACGTN) or the exact slow path (any other byte)
+    // column j's Myers step; it updates the score of job j, or in the packed layout those of both jobs (B through the top row, A through
+    // word WA)
+    auto column = [&](int j, const uint32_t (&Eq)[NW]) {
+      myers_column<NW, HIN, TOP, WA>(Pv[j], Mv[j], Eq, topbit[j], score[PACK ? 1 : j], sep, mula, &score[0]);
+    };
     auto step = [&](uint32_t c, uint32_t col) {
       const uint32_t code = dna_code(c);
 #pragma unroll
-      for (int j = 0; j < NJ; ++j) {
+      for (int j = 0; j < NC; ++j) {
         uint32_t Eq[NW];
         if (code < 5) {
 #pragma unroll
           for (int w = 0; w < NW; ++w) Eq[w] = peq[(peq_slot(code) * SW + j * NW + w) * ED_THREADS + tid];
+        } else if (PACK) {
+#pragma unroll
+          for (int w = 0; w < NW; ++w) Eq[w] = pack_eq_word(q[0], m[0], q[1], p[0], w, c);
         } else {
 #pragma unroll
           for (int w = 0; w < NW; ++w) Eq[w] = eq_word_by_bytes(q[j] + w * 32, min(32u, m[j] - w * 32), c);
           if (TOP) rows_to_top<NW>(Eq, p[j], vmask[j]);
         }
-        myers_column<NW, HIN, TOP>(Pv[j], Mv[j], Eq, topbit[j], score[j]);
-        track(j, col);
+        column(j, Eq);
+#pragma unroll
+        for (int s = PACK ? 0 : j; s < (PACK ? NJ : j + 1); ++s) track(s, col);
       }
     };
     const uint32_t base2 = (tid * 4u) * 0x00010001u;  // this thread's slot offset in both 16-bit halves
@@ -405,15 +551,18 @@ __device__ __forceinline__ void ed_small_jobs(const EdArgs& a, uint32_t* peq, in
           const uint32_t pk = (b & 1) ? offB : offA;
           const uint32_t off = (b & 2) ? (pk >> 16) : (pk & 0xffffu);
 #pragma unroll
-          for (int j = 0; j < NJ; ++j) {
+          for (int j = 0; j < NC; ++j) {
             uint32_t Eq[NW];
 #pragma unroll
             for (int w = 0; w < NW; ++w) Eq[w] = *(const uint32_t*) ((const char*) peq + off + (j * NW + w) * 4 * ED_THREADS);
-            myers_column<NW, HIN, TOP>(Pv[j], Mv[j], Eq, topbit[j], score[j]);
-            if (MODE != DGPU_MODE_NW) {
-              if (WANT_END) track(j, col + b);
-              else if (b & 1) best[j] = min(best[j], min(prev[j], score[j]));  // two columns per three-input min
-              else prev[j] = score[j];
+            column(j, Eq);
+#pragma unroll
+            for (int s = PACK ? 0 : j; s < (PACK ? NJ : j + 1); ++s) {
+              if (MODE != DGPU_MODE_NW) {
+                if (WANT_END) track(s, col + b);
+                else if (b & 1) best[s] = min(best[s], min(prev[s], score[s]));  // two columns per three-input min
+                else prev[s] = score[s];
+              }
             }
           }
         }
@@ -451,10 +600,10 @@ __device__ __forceinline__ void ed_small_jobs(const EdArgs& a, uint32_t* peq, in
       int d, e;
       if (MODE == DGPU_MODE_NW) { d = score[j]; e = (int) n - 1; }
       else { d = best[j]; e = bpos[j]; }
-      const int kk = a.k ? a.k[job0 + j] : -1;
+      const int kk = a.k ? a.k[jid[j]] : -1;
       d = apply_k(d, kk, MODE, (int) m[j], (int) n);
-      a.dist[job0 + j] = d;
-      if (a.end_loc) a.end_loc[job0 + j] = (d < 0) ? -1 : e;
+      a.dist[jid[j]] = d;
+      if (a.end_loc) a.end_loc[jid[j]] = (d < 0) ? -1 : e;
     }
   }
 }
@@ -475,6 +624,15 @@ template <int NW>
 __global__ void __launch_bounds__(ED_THREADS, 1) ed_pair_kernel(EdArgs a) {
   __shared__ uint32_t peq[5 * 2 * NW * ED_THREADS];
   ed_small_jobs<NW, DGPU_MODE_HW, false, 2>(a, peq, ED_PAIR + NW);
+}
+
+// One thread per pair of HW jobs on one target whose two queries fit one column of W words (pack_fits): W = 3 for a 33-63 bp query with a
+// partner of up to 95 - |q| bp, W = 5 for 65-95 bp with up to 159 - |q|. Two 33-47 bp probes then take 3 words instead of 2 x 2, two
+// 65-79 bp probes 5 instead of 2 x 3, and every word of the column needs one Peq load per target column for both jobs.
+template <int W, int WA>
+__global__ void __launch_bounds__(ED_THREADS, 1) ed_pack_kernel(EdArgs a) {
+  __shared__ uint32_t peq[5 * W * ED_THREADS];
+  ed_small_jobs<W, DGPU_MODE_HW, false, 2, WA>(a, peq, W == 3 ? ED_PACK : ED_PACK + 1);
 }
 
 // ---- warp-per-job wavefront for |q| > 128 -------------------------------------------
@@ -816,6 +974,14 @@ int launch_mode(dgpu_ctx* ctx, EdArgs& a, const uint32_t* hc, cudaStream_t st) {
   ED_LAUNCH_PAIR(3)
   ED_LAUNCH_PAIR(4)
 #undef ED_LAUNCH_PAIR
+  if (hc[ED_PACK]) {
+    ed_pack_kernel<3, 1><<<grid_for(hc[ED_PACK], ED_THREADS, ED_CTAS_PER_SM), ED_THREADS, 0, st>>>(a);
+    DGPU_LAUNCH_CHECK(ctx, "ed_pack");
+  }
+  if (hc[ED_PACK + 1]) {
+    ed_pack_kernel<5, 2><<<grid_for(hc[ED_PACK + 1], ED_THREADS, ED_CTAS_PER_SM), ED_THREADS, 0, st>>>(a);
+    DGPU_LAUNCH_CHECK(ctx, "ed_pack");
+  }
   if (hc[5]) {
     uint32_t g = grid_for(hc[5], EDL_WARPS, 8);
     a.hbuf = nullptr;
@@ -935,6 +1101,8 @@ int dgpu_edit_distance_impl(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_by
       hc[ED_PAIR + 1] = hc[ED_PAIR + 2] = (uint32_t) (n / 2);
       if (bound > 64) hc[ED_PAIR + 3] = (uint32_t) (n / 2);
       if (bound > 96) hc[ED_PAIR + 4] = (uint32_t) (n / 2);
+      hc[ED_PACK] = (uint32_t) (n / 2);
+      if (bound > 64) hc[ED_PACK + 1] = (uint32_t) (n / 2);
     }
   } else {
     // One small D2H so that launches are sized exactly and empty classes cost nothing.

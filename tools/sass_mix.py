@@ -10,8 +10,9 @@ and the decode of the word. Its counts are divided by four and grouped by the pi
   lds   shared-memory loads
   vshr  variable-amount right shifts (SHF.R with a register shift amount) among the alu instructions
 
-pair_report() gives the same mix for ed_pair_kernel<NW> per job-column (its fast block runs four columns of two jobs), and
-small_prologues() / prologue_alu() count the ALU instructions of the job load and Peq build (up to the function's last STS).
+pair_report() gives the same mix for ed_pair_kernel<NW> per job-column (its fast block runs four columns of two jobs), pack_report() for
+ed_pack_kernel<W, WA> (four columns of one W-word column that holds two jobs), and small_prologues() / prologue_alu() count the ALU
+instructions of the job load and Peq build (up to the function's last STS).
 
 Usage: python tools/sass_mix.py [LIB] [--json]   (LIB defaults to the in-tree delly_b200/libdelly_b200.so)
 """
@@ -30,6 +31,7 @@ BRANCH = ("BRA", "EXIT", "RET", "CALL", "BRX", "JMP", "JMX")
 INSN = re.compile(r"/\*[0-9a-f]+\*/\s+(@!?U?P\w+\s+)?([A-Z0-9_.]+)\s*([^;]*);")
 KERNEL = re.compile(r"ed_small_kernelILi(\d)ELi(\d)ELb(\d)E")
 PAIR_KERNEL = re.compile(r"ed_pair_kernelILi(\d)E")
+PACK_KERNEL = re.compile(r"ed_pack_kernelILi(\d)ELi(\d)E")
 
 
 def cuobjdump():
@@ -105,16 +107,32 @@ def prologue_alu(lines):
     return sum(op.split(".")[0] in ALU for op in ops[:last + 1])
 
 
+def _per_job(lines):
+    """mix() of a kernel whose column steps advance two jobs, per job-column, with "prologue_alu"."""
+    r = mix(lines)
+    r = {k: (v / 2 if k != "ops" else {o: n / 2 for o, n in v.items()}) for k, v in r.items()}
+    r["prologue_alu"] = prologue_alu(lines)
+    return r
+
+
 def pair_report(lib):
     """{"NW=n": mix} of the fast block of ed_pair_kernel<n>, per job-column (the block runs four columns of two jobs), with "prologue_alu"."""
     res = {}
     for name, lines in functions(_sass(lib)).items():
         m = PAIR_KERNEL.search(name)
         if m:
-            r = mix(lines)
-            r = {k: (v / 2 if k != "ops" else {o: n / 2 for o, n in v.items()}) for k, v in r.items()}
-            r["prologue_alu"] = prologue_alu(lines)
-            res[f"NW={m.group(1)}"] = r
+            res[f"NW={m.group(1)}"] = _per_job(lines)
+    return dict(sorted(res.items()))
+
+
+def pack_report(lib):
+    """{"W=w WA=a": mix} of the fast block of ed_pack_kernel<w, a>, per job-column (the block runs four columns of one packed column that
+    holds two jobs), with "prologue_alu"."""
+    res = {}
+    for name, lines in functions(_sass(lib)).items():
+        m = PACK_KERNEL.search(name)
+        if m:
+            res[f"W={m.group(1)} WA={m.group(2)}"] = _per_job(lines)
     return dict(sorted(res.items()))
 
 
@@ -148,13 +166,19 @@ def main():
     args = [a for a in sys.argv[1:] if not a.startswith("--")]
     lib = args[0] if args else os.path.join(ROOT, "delly_b200", "libdelly_b200.so")
     res = report(lib)
+    pairs = {f"pair {k}": v for k, v in pair_report(lib).items()}
+    packs = {f"pack {k}": v for k, v in pack_report(lib).items()}
     if "--json" in sys.argv:
-        print(json.dumps(res))
+        print(json.dumps({**res, **pairs, **packs}))
         return
     print(f"{'kernel':<16} {'alu':>6} {'fma':>6} {'lds':>5} {'other':>6} {'vshr':>5}   alu opcodes per column")
     for k, v in res.items():
         alu_ops = " ".join(f"{o}:{n:g}" for o, n in v["ops"].items() if o in ALU)
         print(f"{k:<16} {v['alu']:6.2f} {v['fma']:6.2f} {v['lds']:5.2f} {v['other']:6.2f} {v['vshr']:5.2f}   {alu_ops}")
+    print(f"\n{'two-job kernel':<16} {'alu':>6} {'fma':>6} {'lds':>5} {'other':>6} {'vshr':>5} {'prologue':>8}   alu opcodes per job-column")
+    for k, v in {**pairs, **packs}.items():
+        alu_ops = " ".join(f"{o}:{n:g}" for o, n in v["ops"].items() if o in ALU)
+        print(f"{k:<16} {v['alu']:6.2f} {v['fma']:6.2f} {v['lds']:5.2f} {v['other']:6.2f} {v['vshr']:5.2f} {v['prologue_alu']:8d}   {alu_ops}")
 
 
 if __name__ == "__main__":
