@@ -20,7 +20,8 @@ struct dgpu_ctx {
   // pipelined host-pointer calls: upload stream, download stream and their events (created on first use)
   cudaStream_t copy_stream = nullptr, out_stream = nullptr;
   std::vector<cudaEvent_t> pipe_events;
-  // fork/join pool for independent launches of one batch call (job classes): [0] fork event, [1..] join events
+  // fork/join pool for independent launches of one batch call (the job classes of longNeedle and of the edit distance): [0] fork event,
+  // [1..] join events
   std::vector<cudaStream_t> fork_streams;
   std::vector<cudaEvent_t> fork_events;
   std::string last_error;
@@ -61,6 +62,7 @@ enum {
   SLOT_LN_JOBCLS,    // per-job class bytes of longNeedle (long_needle.cu)
   SLOT_ED_STRIPES,   // stripe scratch of long edit-distance targets (edit_distance.cu)
   SLOT_ED_BAND,      // job lists of the banded NW passes (edit_distance.cu)
+  SLOT_ED_SLOTS,     // per-job count slot bytes of the edit-distance classification (edit_distance.cu)
   SLOT_WAVEFRONT,    // wavefront workspace of the longNeedle and segment engines; their planners count its capacity as free
                      // (long_needle.cu, edit_path.cu)
   SLOT_MSA_SEGJOBS,  // MSA warp workspace (msa.cu); segment job arrays (edit_path.cu)

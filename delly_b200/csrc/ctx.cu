@@ -18,6 +18,8 @@ int dgpu_set_cuda_error(dgpu_ctx* ctx, cudaError_t e, const char* what) {
 int dgpu_reserve(dgpu_ctx* ctx, int slot, size_t bytes, void** out) {
   DevBuf& b = ctx->bufs[slot];
   if (bytes > b.cap) {
+    // cudaFree synchronises the device. Callers rely on that: the edit distance's class kernels of an earlier call may still read a slot
+    // from the fork/join streams, and a stream-ordered free would release the buffer under them.
     if (b.p) DGPU_CUDA(ctx, cudaFree(b.p));
     b.p = nullptr;
     b.cap = 0;

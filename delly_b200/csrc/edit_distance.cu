@@ -10,7 +10,9 @@
 //   src/edlib.cpp:728-929  NW: -1 if k < |n-m|, k=min(k,max(m,n)), D[m][n] if <= k
 //
 // Device design (H100, integer-ALU bound; HBM traffic is ~(|q|+|t|)/2..1 byte per 30+ int ops):
-//   * jobs are binned on the device by ceil(|q|/32) (counting sort: count -> offsets -> scatter),
+//   * jobs are binned on the device by ceil(|q|/32) (counting sort: ed_count_kernel classifies each job once, keeps its slot byte and, in its
+//     last block, turns the counts into class starts; ed_scatter_kernel places the jobs from the slot bytes). The class kernels then run
+//     side by side on the context's fork/join streams, costliest class first (launch_mode),
 //   * |q| <= 128: ONE THREAD PER JOB. The whole DP column is one multi-word bit-vector held in
 //     registers (NW = 1..4 x 32 bit, add-with-carry chain, funnel shifts), the score is read at bit
 //     |q|-1 so no padding/wildcard columns are needed. The per-job match masks Peq[5][NW] live in a
@@ -48,8 +50,9 @@ constexpr int ED_PAIR = 5;
 constexpr int ED_PACK = ED_PAIR + 5;
 constexpr int ED_NCLS = ED_PACK + 2;
 // counts layout (SLOT_COUNTS): [0, 16) jobs per class, [ED_START, +16) class starts in perm, [ED_CUR, +16) scatter cursors, [ED_TMAX] max t_len
-// of multi-stripe jobs, [ED_BANDQ, +EDB_CLASSES + 1) band pass queues
-constexpr int ED_START = 16, ED_CUR = 32, ED_TMAX = 48, ED_BANDQ = 64, ED_COUNTS_WORDS = 128;
+// of multi-stripe jobs, [ED_TICKET] blocks of ed_count_kernel done, [ED_BANDQ, +EDB_CLASSES + 1) band pass queues
+constexpr int ED_START = 16, ED_CUR = 32, ED_TMAX = 48, ED_TICKET = 49, ED_BANDQ = 64, ED_COUNTS_WORDS = 128;
+constexpr uint8_t ED_NO_SLOT = 0xff;  // slot byte of the odd member of a pair (ed_slot's -1)
 
 struct EdArgs {
   const uint8_t* seqs;
@@ -63,7 +66,8 @@ struct EdArgs {
   int32_t* dist;
   int32_t* end_loc;
   uint32_t* perm;
-  uint32_t* counts;  // ED_START / ED_CUR / ED_TMAX / ED_BANDQ layout above
+  uint32_t* counts;  // ED_START / ED_CUR / ED_TMAX / ED_TICKET / ED_BANDQ layout above
+  uint8_t* slots;    // per job: its count slot (ed_slot) or ED_NO_SLOT, written by ed_count_kernel, read by ed_scatter_kernel
   int pair;          // HW distances without end locations or equality tables: target-sharing job pairs take ed_pair_kernel (ed_slot)
   int last_pos;     // HW/SHW: report the LAST optimal end position instead of the first (edlib's positionsSHW.back(), src/edlib.cpp:250)
   uint8_t* hbuf;     // per-warp scratch rows for multi-stripe jobs
@@ -115,69 +119,141 @@ __device__ __forceinline__ int pack_class(uint32_t m0, uint32_t m1) {
 // Count slot of job i: its class, or, for the even member i of a pair (i, i + 1) of one-thread jobs on the same target (equal t_off and
 // t_len: the ALT and REF probes of one genotyping read), the pack class if the two queries fit one (pack_class), else the pair class
 // ED_PAIR + class if both are of the same class; -1 for the odd member of a pair. Indices are relative to the call.
-__device__ __forceinline__ int ed_slot(const EdArgs& a, uint32_t i) {
-  const uint32_t tl = a.t_len[i];
-  const int c = ed_class(a.q_len[i], tl, a.force_long);
-  if (!a.pair || c < 1 || c > 4) return c;
+// The words of job i and its partner o = i ^ 1 (in the same cache lines) are loaded by slot_words, separately from ed_slot, so that a
+// thread can have the loads of several jobs in flight before it branches on any of them.
+struct SlotWords {
+  uint32_t mi, tl, to, mo, tlo, too;  // q_len, t_len, t_off of job i, then of its partner (0 if there is none)
+};
+
+__device__ __forceinline__ SlotWords slot_words(const EdArgs& a, uint32_t i) {
   const uint32_t o = i ^ 1u;
-  if (o >= a.n || a.t_off[o] != a.t_off[i] || a.t_len[o] != tl) return c;
-  const uint32_t mi = a.q_len[i], mo = a.q_len[o];
+  const bool has_o = o < a.n;
+  return SlotWords{a.q_len[i], a.t_len[i], a.t_off[i], has_o ? a.q_len[o] : 0u, has_o ? a.t_len[o] : 0u, has_o ? a.t_off[o] : 0u};
+}
+
+__device__ __forceinline__ int ed_slot(const EdArgs& a, uint32_t i, const SlotWords& v) {
+  const uint32_t mi = v.mi, tl = v.tl, mo = v.mo;
+  const int c = ed_class(mi, tl, a.force_long);
+  if (!a.pair || c < 1 || c > 4) return c;
+  if ((i ^ 1u) >= a.n || v.too != v.to || v.tlo != tl) return c;
   const int pk = (i & 1u) ? pack_class(mo, mi) : pack_class(mi, mo);
   if (pk >= 0) return (i & 1u) ? -1 : pk;
   if (ed_class(mo, tl, 0) != c) return c;
   return (i & 1u) ? -1 : ED_PAIR + c;
 }
 
-__global__ void ed_count_kernel(EdArgs a, int mode) {
+// Both binning kernels run ED_BIN_CTAS_PER_SM blocks of ED_BIN_THREADS per SM (one wave) and loop over their jobs, so that each block's
+// global atomics on the counts line (per class, plus the ticket) are paid once per block rather than once per 256 jobs. Each thread keeps
+// several jobs' loads in flight at once (ED_COUNT_UNROLL jobs in ed_count_kernel, one 4-byte word of slots in ed_scatter_kernel): with one
+// job per thread the loads of a wave were too few to keep HBM busy.
+constexpr int ED_BIN_THREADS = 256, ED_BIN_CTAS_PER_SM = 8, ED_COUNT_UNROLL = 2;
+
+// The one classification of a call: each job's count slot (ed_slot) goes to a.slots, so that ed_scatter_kernel reads one byte per job instead
+// of the lengths and target offsets of the job and its partner. Trivial jobs get their result here. Counts are summed per warp (one shared
+// atomic per distinct slot, from the lowest lane holding it), then per block; the last block to finish (a ticket taken after a fence) turns
+// the class counts into the class starts and scatter cursors.
+__global__ void __launch_bounds__(ED_BIN_THREADS) ed_count_kernel(EdArgs a, int mode) {
   __shared__ uint32_t h[ED_NCLS];
   __shared__ uint32_t hmax;
   if (threadIdx.x < ED_NCLS) h[threadIdx.x] = 0;
   if (threadIdx.x == 0) hmax = 0;
   __syncthreads();
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < a.n) {
-    uint32_t ql = a.q_len[i], tl = a.t_len[i];
-    int c = ed_slot(a, i);
-    if (c >= 0) atomicAdd(&h[c], 1u);
-    if (c == 5 && ql > 2048) atomicMax(&hmax, tl);
-    if (c == 0) {
-      // src/edlib.cpp:158-177: NW -> max(len), endLocations[0] = n-1; HW/SHW -> |q|, endLocations[0] = -1.
-      // (this special case is taken before k is looked at)
-      int d = (mode == DGPU_MODE_NW) ? (int) max(ql, tl) : (int) ql;
-      a.dist[i] = d;
-      if (a.end_loc) a.end_loc[i] = (mode == DGPU_MODE_NW) ? (int) tl - 1 : -1;
+  // the loop bound is the block's first job, so every lane of a warp runs every iteration (__match_any_sync over the full warp)
+  constexpr uint32_t STEP = ED_COUNT_UNROLL * ED_BIN_THREADS;
+  for (uint32_t i0 = blockIdx.x * STEP; i0 < a.n; i0 += gridDim.x * STEP) {
+    SlotWords v[ED_COUNT_UNROLL];
+#pragma unroll
+    for (int u = 0; u < ED_COUNT_UNROLL; ++u) {  // every job's loads before any branch or store
+      const uint32_t i = i0 + u * ED_BIN_THREADS + threadIdx.x;
+      if (i < a.n) v[u] = slot_words(a, i);
+    }
+#pragma unroll
+    for (int u = 0; u < ED_COUNT_UNROLL; ++u) {
+      const uint32_t i = i0 + u * ED_BIN_THREADS + threadIdx.x;
+      const int c = i < a.n ? ed_slot(a, i, v[u]) : -1;
+      if (i < a.n) {
+        a.slots[i] = c >= 0 ? (uint8_t) c : ED_NO_SLOT;
+        if (c == 5 && a.q_len[i] > 2048) atomicMax(&hmax, a.t_len[i]);
+        if (c == 0) {
+          // src/edlib.cpp:158-177: NW -> max(len), endLocations[0] = n-1; HW/SHW -> |q|, endLocations[0] = -1.
+          // (this special case is taken before k is looked at)
+          const uint32_t ql = a.q_len[i], tl = a.t_len[i];
+          int d = (mode == DGPU_MODE_NW) ? (int) max(ql, tl) : (int) ql;
+          a.dist[i] = d;
+          if (a.end_loc) a.end_loc[i] = (mode == DGPU_MODE_NW) ? (int) tl - 1 : -1;
+        }
+      }
+      const uint32_t peers = __match_any_sync(0xffffffffu, c);
+      if (c >= 0 && (threadIdx.x & 31u) == (uint32_t) (__ffs(peers) - 1)) atomicAdd(&h[c], (uint32_t) __popc(peers));
     }
   }
   __syncthreads();
-  if (threadIdx.x < ED_NCLS && h[threadIdx.x]) atomicAdd(&a.counts[threadIdx.x], h[threadIdx.x]);
-  if (threadIdx.x == 0 && hmax) atomicMax(&a.counts[ED_TMAX], hmax);
-}
-
-__global__ void ed_offsets_kernel(uint32_t* counts) {
-  uint32_t s = 0;
-  for (int c = 0; c < ED_NCLS; ++c) {
-    counts[ED_START + c] = s;
-    counts[ED_CUR + c] = s;
-    s += counts[c];
+  if (threadIdx.x < 32) {  // warp 0 makes every global update of the block
+    if (threadIdx.x < ED_NCLS && h[threadIdx.x]) atomicAdd(&a.counts[threadIdx.x], h[threadIdx.x]);
+    if (threadIdx.x == 0 && hmax) atomicMax(&a.counts[ED_TMAX], hmax);
+    __threadfence();
+    __syncwarp();
+    if (threadIdx.x == 0 && atomicAdd(&a.counts[ED_TICKET], 1u) == gridDim.x - 1) {
+      // every other block's counts are in: class starts in perm, and the scatter cursors at the same place
+      __threadfence();
+      const volatile uint32_t* cnt = a.counts;
+      uint32_t s = 0;
+      for (int k = 0; k < ED_NCLS; ++k) {
+        a.counts[ED_START + k] = s;
+        a.counts[ED_CUR + k] = s;
+        s += cnt[k];
+      }
+    }
   }
 }
 
-__global__ void ed_scatter_kernel(EdArgs a) {
+// perm entries from the slot bytes. Each block takes one contiguous range of jobs and passes over its slot bytes twice: the first pass counts
+// the range's jobs per class, one global atomic per class on its scatter cursor reserves their places, and the second pass hands the places
+// out. A thread reads the slots of four consecutive jobs as one word (a.slots has 16 bytes of slack past n) and takes them one at a time;
+// per warp and job, one shared atomic per distinct slot (the lowest lane holding it takes room for all its peers). Any order of the jobs
+// within a class segment gives the same results.
+__global__ void __launch_bounds__(ED_BIN_THREADS) ed_scatter_kernel(EdArgs a) {
+  constexpr uint32_t STEP = 4 * ED_BIN_THREADS;
   __shared__ uint32_t h[ED_NCLS];
-  __shared__ uint32_t base[ED_NCLS];
   if (threadIdx.x < ED_NCLS) h[threadIdx.x] = 0;
   __syncthreads();
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  int c = -1;
-  uint32_t r = 0;
-  if (i < a.n) {
-    c = ed_slot(a, i);
-    if (c >= 0) r = atomicAdd(&h[c], 1u);
+  const uint32_t per = ((a.n + gridDim.x - 1) / gridDim.x + STEP - 1) / STEP * STEP;
+  const uint32_t lo = blockIdx.x * per, hi = min(a.n, lo + per);
+  const uint32_t lane = threadIdx.x & 31u;
+  // the slots of jobs i0 + 4 threadIdx.x + 0..3, byte b = job b; past the range ED_NO_SLOT
+  auto word = [&](uint32_t i0) {
+    const uint32_t i = i0 + 4u * threadIdx.x;
+    if (i >= hi) return 0xffffffffu;
+    const uint32_t w = *(const uint32_t*) (a.slots + i);
+    return hi - i >= 4u ? w : w | (0xffffffffu << (8u * (hi - i)));
+  };
+  for (uint32_t i0 = lo; i0 < hi; i0 += STEP) {
+    const uint32_t w = word(i0);
+#pragma unroll
+    for (int b = 0; b < 4; ++b) {
+      const uint32_t s = (w >> (8 * b)) & 0xffu;
+      const int c = s == ED_NO_SLOT ? -1 : (int) s;
+      const uint32_t peers = __match_any_sync(0xffffffffu, c);
+      if (c >= 0 && (int) lane == __ffs(peers) - 1) atomicAdd(&h[c], (uint32_t) __popc(peers));
+    }
   }
   __syncthreads();
-  if (threadIdx.x < ED_NCLS) base[threadIdx.x] = h[threadIdx.x] ? atomicAdd(&a.counts[ED_CUR + threadIdx.x], h[threadIdx.x]) : 0;
+  if (threadIdx.x < ED_NCLS && h[threadIdx.x]) h[threadIdx.x] = atomicAdd(&a.counts[ED_CUR + threadIdx.x], h[threadIdx.x]);
   __syncthreads();
-  if (c >= 0) a.perm[base[c] + r] = i;
+  for (uint32_t i0 = lo; i0 < hi; i0 += STEP) {
+    const uint32_t w = word(i0);
+#pragma unroll
+    for (int b = 0; b < 4; ++b) {
+      const uint32_t s = (w >> (8 * b)) & 0xffu;
+      const int c = s == ED_NO_SLOT ? -1 : (int) s;
+      const uint32_t peers = __match_any_sync(0xffffffffu, c);
+      const int lead = __ffs(peers) - 1;
+      uint32_t r = 0;
+      if (c >= 0 && (int) lane == lead) r = atomicAdd(&h[c], (uint32_t) __popc(peers));
+      r = __shfl_sync(0xffffffffu, r, lead) + (uint32_t) __popc(peers & ((1u << lane) - 1u));
+      if (c >= 0) a.perm[r] = i0 + 4u * threadIdx.x + (uint32_t) b;
+    }
+  }
 }
 
 // ---- multi-word add with carry ---------------------------------------------------------
@@ -951,60 +1027,71 @@ int launch_mode(dgpu_ctx* ctx, EdArgs& a, const uint32_t* hc, cudaStream_t st) {
     uint32_t cap = (uint32_t) (sms * max_per_sm);
     return need < cap ? need : cap;
   };
-  dgpu_prof_begin(ctx, st);
   const bool want_end = (a.end_loc != nullptr);
-#define ED_LAUNCH_SMALL(NWV)                                                                                              \
-  if (hc[NWV]) {                                                                                                          \
-    if (want_end) ed_small_kernel<NWV, MODE, true><<<grid_for(hc[NWV], ED_THREADS, ED_CTAS_PER_SM), ED_THREADS, 0, st>>>(a); \
-    else ed_small_kernel<NWV, MODE, false><<<grid_for(hc[NWV], ED_THREADS, ED_CTAS_PER_SM), ED_THREADS, 0, st>>>(a);         \
-    DGPU_LAUNCH_CHECK(ctx, "ed_small");                                                                                   \
+  // Scratch of class 5, reserved before any class kernel of this call is launched (see the note on dgpu_reserve where perm is reserved).
+  const bool band = MODE == DGPU_MODE_NW && !ctx->no_band;
+  const uint32_t g5 = grid_for(hc[5], EDL_WARPS, 8);
+  uint32_t* lists = nullptr;
+  a.hbuf = nullptr;
+  a.hbuf_stride = 0;
+  if (hc[5] && hc[ED_TMAX]) {
+    a.hbuf_stride = (hc[ED_TMAX] + 255u) & ~255u;
+    void* hb;
+    int rc = dgpu_reserve(ctx, SLOT_ED_STRIPES, (size_t) g5 * EDL_WARPS * a.hbuf_stride, &hb);
+    if (rc) return rc;
+    a.hbuf = (uint8_t*) hb;
   }
-  ED_LAUNCH_SMALL(1)
-  ED_LAUNCH_SMALL(2)
-  ED_LAUNCH_SMALL(3)
-  ED_LAUNCH_SMALL(4)
-#undef ED_LAUNCH_SMALL
-#define ED_LAUNCH_PAIR(NWV)                                                                                 \
-  if (hc[ED_PAIR + NWV]) {                                                                                  \
-    ed_pair_kernel<NWV><<<grid_for(hc[ED_PAIR + NWV], ED_THREADS, ED_CTAS_PER_SM), ED_THREADS, 0, st>>>(a); \
-    DGPU_LAUNCH_CHECK(ctx, "ed_pair");                                                                      \
+  if (hc[5] && band) {
+    void* lp;
+    int rc = dgpu_reserve(ctx, SLOT_ED_BAND, (size_t) (EDB_CLASSES + 1) * hc[5] * sizeof(uint32_t), &lp);
+    if (rc) return rc;
+    lists = (uint32_t*) lp;
   }
-  ED_LAUNCH_PAIR(1)
-  ED_LAUNCH_PAIR(2)
-  ED_LAUNCH_PAIR(3)
-  ED_LAUNCH_PAIR(4)
-#undef ED_LAUNCH_PAIR
-  if (hc[ED_PACK]) {
-    ed_pack_kernel<3, 1><<<grid_for(hc[ED_PACK], ED_THREADS, ED_CTAS_PER_SM), ED_THREADS, 0, st>>>(a);
-    DGPU_LAUNCH_CHECK(ctx, "ed_pack");
-  }
-  if (hc[ED_PACK + 1]) {
-    ed_pack_kernel<5, 2><<<grid_for(hc[ED_PACK + 1], ED_THREADS, ED_CTAS_PER_SM), ED_THREADS, 0, st>>>(a);
-    DGPU_LAUNCH_CHECK(ctx, "ed_pack");
-  }
-  if (hc[5]) {
-    uint32_t g = grid_for(hc[5], EDL_WARPS, 8);
-    a.hbuf = nullptr;
-    a.hbuf_stride = 0;
-    if (hc[ED_TMAX]) {
-      a.hbuf_stride = (hc[ED_TMAX] + 255u) & ~255u;
-      void* hb;
-      int rc = dgpu_reserve(ctx, SLOT_ED_STRIPES, (size_t) g * EDL_WARPS * a.hbuf_stride, &hb);
-      if (rc) return rc;
-      a.hbuf = (uint8_t*) hb;
+
+  // one class on stream cs: ed_small / ed_pair / ed_pack, or class 5's chain in order on one stream (band passes narrowest first, as a
+  // pass queues what it could not certify for the next one, then the full matrix; without band passes the full matrix alone)
+  auto launch = [&](int c, cudaStream_t cs) -> int {
+    const uint32_t g = grid_for(hc[c], ED_THREADS, ED_CTAS_PER_SM);
+    switch (c) {
+#define ED_CASE_SMALL(NWV)                                                                  \
+      case NWV:                                                                             \
+        if (want_end) ed_small_kernel<NWV, MODE, true><<<g, ED_THREADS, 0, cs>>>(a);        \
+        else ed_small_kernel<NWV, MODE, false><<<g, ED_THREADS, 0, cs>>>(a);                \
+        DGPU_LAUNCH_CHECK(ctx, "ed_small");                                                 \
+        return DGPU_OK;
+      ED_CASE_SMALL(1)
+      ED_CASE_SMALL(2)
+      ED_CASE_SMALL(3)
+      ED_CASE_SMALL(4)
+#undef ED_CASE_SMALL
+#define ED_CASE_PAIR(NWV)                                                                   \
+      case ED_PAIR + NWV:                                                                   \
+        ed_pair_kernel<NWV><<<g, ED_THREADS, 0, cs>>>(a);                                   \
+        DGPU_LAUNCH_CHECK(ctx, "ed_pair");                                                  \
+        return DGPU_OK;
+      ED_CASE_PAIR(1)
+      ED_CASE_PAIR(2)
+      ED_CASE_PAIR(3)
+      ED_CASE_PAIR(4)
+#undef ED_CASE_PAIR
+      case ED_PACK:
+        ed_pack_kernel<3, 1><<<g, ED_THREADS, 0, cs>>>(a);
+        DGPU_LAUNCH_CHECK(ctx, "ed_pack");
+        return DGPU_OK;
+      case ED_PACK + 1:
+        ed_pack_kernel<5, 2><<<g, ED_THREADS, 0, cs>>>(a);
+        DGPU_LAUNCH_CHECK(ctx, "ed_pack");
+        return DGPU_OK;
+      default:
+        break;
     }
-    if (MODE == DGPU_MODE_NW && !ctx->no_band) {
-      // band passes first (narrowest class first: a pass queues what it could not certify for the next one), the full matrix last
+    if (band) {
       const uint32_t cap = hc[5];
-      void* lp;
-      int rc = dgpu_reserve(ctx, SLOT_ED_BAND, (size_t) (EDB_CLASSES + 1) * cap * sizeof(uint32_t), &lp);
-      if (rc) return rc;
-      uint32_t* lists = (uint32_t*) lp;
-      ed_band_plan_kernel<<<grid_for(hc[5], 8, 8), 256, 0, st>>>(a, lists, cap);
+      ed_band_plan_kernel<<<grid_for(hc[5], 8, 8), 256, 0, cs>>>(a, lists, cap);
       DGPU_LAUNCH_CHECK(ctx, "ed_band_plan");
 #define ED_LAUNCH_BAND(GV)                                                                                                    \
-      if (a.eq_cls) ed_band_kernel<GV, true><<<grid_for(hc[5], EDB_WARPS * (32 / GV), 5), EDB_WARPS * 32, 0, st>>>(a, lists, cap);  \
-      else ed_band_kernel<GV, false><<<grid_for(hc[5], EDB_WARPS * (32 / GV), 5), EDB_WARPS * 32, 0, st>>>(a, lists, cap);         \
+      if (a.eq_cls) ed_band_kernel<GV, true><<<grid_for(hc[5], EDB_WARPS * (32 / GV), 5), EDB_WARPS * 32, 0, cs>>>(a, lists, cap);  \
+      else ed_band_kernel<GV, false><<<grid_for(hc[5], EDB_WARPS * (32 / GV), 5), EDB_WARPS * 32, 0, cs>>>(a, lists, cap);         \
       DGPU_LAUNCH_CHECK(ctx, "ed_band");
       ED_LAUNCH_BAND(2)
       ED_LAUNCH_BAND(4)
@@ -1012,15 +1099,45 @@ int launch_mode(dgpu_ctx* ctx, EdArgs& a, const uint32_t* hc, cudaStream_t st) {
       ED_LAUNCH_BAND(16)
       ED_LAUNCH_BAND(32)
 #undef ED_LAUNCH_BAND
-      if (a.eq_cls) ed_long_kernel<MODE, true><<<g, EDL_WARPS * 32, 0, st>>>(a, lists + (size_t) EDB_CLASSES * cap, a.counts + ED_BANDQ + EDB_CLASSES);
-      else ed_long_kernel<MODE, false><<<g, EDL_WARPS * 32, 0, st>>>(a, lists + (size_t) EDB_CLASSES * cap, a.counts + ED_BANDQ + EDB_CLASSES);
-      DGPU_LAUNCH_CHECK(ctx, "ed_long");
+      if (a.eq_cls) ed_long_kernel<MODE, true><<<g5, EDL_WARPS * 32, 0, cs>>>(a, lists + (size_t) EDB_CLASSES * cap, a.counts + ED_BANDQ + EDB_CLASSES);
+      else ed_long_kernel<MODE, false><<<g5, EDL_WARPS * 32, 0, cs>>>(a, lists + (size_t) EDB_CLASSES * cap, a.counts + ED_BANDQ + EDB_CLASSES);
     } else if (a.eq_cls) {
-      ed_long_kernel<MODE, true><<<g, EDL_WARPS * 32, 0, st>>>(a, nullptr, nullptr);
-      DGPU_LAUNCH_CHECK(ctx, "ed_long");
+      ed_long_kernel<MODE, true><<<g5, EDL_WARPS * 32, 0, cs>>>(a, nullptr, nullptr);
     } else {
-      ed_long_kernel<MODE, false><<<g, EDL_WARPS * 32, 0, st>>>(a, nullptr, nullptr);
-      DGPU_LAUNCH_CHECK(ctx, "ed_long");
+      ed_long_kernel<MODE, false><<<g5, EDL_WARPS * 32, 0, cs>>>(a, nullptr, nullptr);
+    }
+    DGPU_LAUNCH_CHECK(ctx, "ed_long");
+    return DGPU_OK;
+  };
+
+  // The classes are independent once perm is scattered, so they run side by side: the k-th class launched goes to pool stream
+  // k % DGPU_FORK_STREAMS, each stream's first class waits for the fork event recorded on st, and st waits for every pool stream used
+  // before the profiling bracket closes. A caller that synchronises st therefore sees every result, and last_kernel_ms spans all classes.
+  // Costliest class per job first: the block scheduler starts the CTAs of earlier launches first, so the classes launched last fill the
+  // SMs while the long ones drain, where one stream let every class drain the GPU alone.
+  static constexpr int order[] = {ED_PACK + 1, ED_PAIR + 2, ED_PAIR + 3, ED_PAIR + 4, ED_PACK, ED_PAIR + 1, 4, 3, 2, 1, 5};
+  int nl = 0;
+  for (int c : order) nl += hc[c] != 0;
+  const bool fork = nl > 1;
+  int rc;
+  if (fork && (rc = dgpu_fork_init(ctx))) return rc;
+  dgpu_prof_begin(ctx, st);
+  if (fork) DGPU_CUDA(ctx, cudaEventRecord(ctx->fork_events[0], st));
+  int k = 0;
+  for (int c : order) {
+    if (!hc[c]) continue;
+    cudaStream_t cs = st;
+    if (fork) {
+      cs = ctx->fork_streams[k % DGPU_FORK_STREAMS];
+      if (k < DGPU_FORK_STREAMS) DGPU_CUDA(ctx, cudaStreamWaitEvent(cs, ctx->fork_events[0], 0));
+    }
+    ++k;
+    if ((rc = launch(c, cs))) return rc;
+  }
+  if (fork) {  // join
+    for (int s = 0; s < std::min(k, DGPU_FORK_STREAMS); ++s) {
+      DGPU_CUDA(ctx, cudaEventRecord(ctx->fork_events[1 + s], ctx->fork_streams[s]));
+      DGPU_CUDA(ctx, cudaStreamWaitEvent(st, ctx->fork_events[1 + s], 0));
     }
   }
   dgpu_prof_end(ctx, st);
@@ -1071,6 +1188,9 @@ int dgpu_edit_distance_impl(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_by
   // eq_tabs (device): uint32 f[256], uint32 s[256], then uint8 cls[256]
   a.eq_f = eq_tabs; a.eq_s = eq_tabs ? eq_tabs + 256 : nullptr; a.eq_cls = eq_tabs ? (const uint8_t*) (eq_tabs + 512) : nullptr;
   a.force_long = eq_tabs ? 1 : 0;
+  // The class kernels of an earlier call may still run on the pool streams (launch_mode) and read this scratch. A call on the same stream
+  // is ordered after them by the join. A slot that has to grow is freed with cudaFree, which synchronises the whole device, so the old
+  // buffer is idle whichever stream the earlier call used. dgpu_reserve must keep freeing that way.
   void* p;
   int rc = dgpu_reserve(ctx, SLOT_JOB_PERM, n * sizeof(uint32_t), &p);
   if (rc) return rc;
@@ -1078,14 +1198,15 @@ int dgpu_edit_distance_impl(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_by
   rc = dgpu_reserve(ctx, SLOT_COUNTS, ED_COUNTS_WORDS * sizeof(uint32_t), &p);
   if (rc) return rc;
   a.counts = (uint32_t*) p;
+  rc = dgpu_reserve(ctx, SLOT_ED_SLOTS, n + 16, &p);   // ed_scatter_kernel reads whole words
+  if (rc) return rc;
+  a.slots = (uint8_t*) p;
 
   DGPU_CUDA(ctx, cudaMemsetAsync(a.counts, 0, ED_COUNTS_WORDS * sizeof(uint32_t), st));
-  const uint32_t cb = (uint32_t) ((n + 255) / 256);
-  ed_count_kernel<<<cb, 256, 0, st>>>(a, mode);
+  const uint32_t cb = (uint32_t) std::min<uint64_t>((n + ED_BIN_THREADS - 1) / ED_BIN_THREADS, (uint64_t) ctx->num_sms * ED_BIN_CTAS_PER_SM);
+  ed_count_kernel<<<cb, ED_BIN_THREADS, 0, st>>>(a, mode);
   DGPU_LAUNCH_CHECK(ctx, "ed_count");
-  ed_offsets_kernel<<<1, 1, 0, st>>>(a.counts);
-  DGPU_LAUNCH_CHECK(ctx, "ed_offsets");
-  ed_scatter_kernel<<<cb, 256, 0, st>>>(a);
+  ed_scatter_kernel<<<cb, ED_BIN_THREADS, 0, st>>>(a);
   DGPU_LAUNCH_CHECK(ctx, "ed_scatter");
   uint32_t hc[ED_TMAX + 1];
   if (ctx->async_bound) {
