@@ -438,7 +438,8 @@ int main(int argc, char** argv) {
   DeviceLimitLog const& lim = deviceLimitLog();
   if (lim.total())
     std::cerr << "Warning: " << lim.msaClusters.load() << " read cluster(s) (over " << DGPU_MSA_LARGE_MAXR << " reads, over 1023 alignment columns or a byte"
-              << " outside ACGTN), " << lim.pathJobs.load() << " edit-path job(s) and " << lim.needleJobs.load()
+              << " outside ACGTN), " << lim.pathJobs.load() << " edit-path job(s) (an aligned target slice over " << DGPU_EP_MAX_SLICE
+              << " bases) and " << lim.needleJobs.load()
               << " consensus alignment(s) (a consensus over 16383 bases or a reference window over " << DGPU_LN_MAX_REF << " bases) exceeded a device limit (include/dgpu.h) and were treated as failed alignments of their SV / read; the reference"
                  " has no such limits, so these records may differ from its output." << std::endl;
   // Every output is written and closed at this point. Tearing the CUDA context, the NCCL communicator and a few GB of device scratch down

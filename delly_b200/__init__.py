@@ -16,6 +16,7 @@ LIB_PATH = os.environ.get("DGPU_LIB") or os.path.join(_HERE, "libdelly_b200.so")
 MODE_NW, MODE_SHW, MODE_HW = 0, 1, 2
 MSA_LARGE_MAXR = 1023   # DGPU_MSA_LARGE_MAXR: the largest cluster Context.msa(max_reads=...) can compute
 LN_MAX_REF = 65535      # DGPU_LN_MAX_REF: the widest reference window Context.long_needle(max_ref=...) can compute
+EP_MAX_SLICE = 262144   # DGPU_EP_MAX_SLICE: the widest aligned target slice Context.edit_path(max_slice=...) can trace
 
 _lib = None
 
@@ -141,8 +142,10 @@ class Context:
 
 
     # ------------------------------------------------------------------ edit path
-    def edit_path(self, seqs, q_off, q_len, t_off, t_len, mode, eq=b""):
-        """Host form. eq = additional equality pairs as bytes (first,second,...). Returns (dist, start, end, ops list[bytes], status)."""
+    def edit_path(self, seqs, q_off, q_len, t_off, t_len, mode, eq=b"", max_slice=None):
+        """Host form. eq = additional equality pairs as bytes (first,second,...). Returns (dist, start, end, ops list[bytes], status).
+        max_slice=None: dgpu_edit_path_ex (aligned target slices up to 16384 columns); otherwise dgpu_edit_path_wide, which traces slices
+        up to max_slice (at most EP_MAX_SLICE) columns. Jobs with a wider slice come back with status 2."""
         n = len(q_off)
         cap = q_len.astype(np.uint64) + t_len.astype(np.uint64)
         ops_off = np.concatenate([[0], np.cumsum(cap)[:-1]]).astype(np.uint64) if n else np.zeros(0, np.uint64)
@@ -150,11 +153,27 @@ class Context:
         ops = np.zeros(max(ops_bytes, 1), np.uint8)
         dist = np.zeros(n, np.int32); st = np.zeros(n, np.int32); en = np.zeros(n, np.int32)
         ops_len = np.zeros(n, np.uint32); status = np.zeros(n, np.uint32)
-        rc = self._lib.dgpu_edit_path_ex(self.h, _ptr(seqs), C.c_uint64(_nbytes(seqs)), _ptr(q_off), _ptr(q_len), _ptr(t_off), _ptr(t_len), int(mode),
-                                         C.c_char_p(eq) if eq else None, C.c_uint32(len(eq) // 2 if eq else 0), C.c_uint64(n), _ptr(dist), _ptr(st), _ptr(en),
-                                         _ptr(ops), _ptr(ops_off), C.c_uint64(ops_bytes), _ptr(ops_len), _ptr(status))
-        self.check(rc, "dgpu_edit_path_ex")
+        args = (self.h, _ptr(seqs), C.c_uint64(_nbytes(seqs)), _ptr(q_off), _ptr(q_len), _ptr(t_off), _ptr(t_len), int(mode),
+                C.c_char_p(eq) if eq else None, C.c_uint32(len(eq) // 2 if eq else 0), C.c_uint64(n), _ptr(dist), _ptr(st), _ptr(en),
+                _ptr(ops), _ptr(ops_off), C.c_uint64(ops_bytes), _ptr(ops_len), _ptr(status))
+        if max_slice is None:
+            self.check(self._lib.dgpu_edit_path_ex(*args), "dgpu_edit_path_ex")
+        else:
+            self.check(self._lib.dgpu_edit_path_wide(*args, C.c_uint32(int(max_slice))), "dgpu_edit_path_wide")
         return dist, st, en, [ops[int(o):int(o) + int(l)].tobytes() for o, l in zip(ops_off, ops_len)], status
+
+    def edit_path_dev(self, seqs, q_off, q_len, t_off, t_len, mode, dist, start, end, ops, ops_off, ops_len, status, eq=b"", stream=None,
+                      max_slice=None):
+        """Device form: CUDA tensors in, results written in place (ops at ops_off, |q| + |t| bytes reserved per job); max_slice as in
+        edit_path."""
+        n = q_off.numel()
+        args = (self.h, _ptr(seqs), C.c_uint64(seqs.numel()), _ptr(q_off), _ptr(q_len), _ptr(t_off), _ptr(t_len), int(mode),
+                C.c_char_p(eq) if eq else None, C.c_uint32(len(eq) // 2 if eq else 0), C.c_uint64(n), _ptr(dist), _ptr(start), _ptr(end),
+                _ptr(ops), _ptr(ops_off), _ptr(ops_len), _ptr(status))
+        if max_slice is None:
+            self.check(self._lib.dgpu_edit_path_ex_dev(*args, C.c_void_p(stream or 0)), "dgpu_edit_path_ex_dev")
+        else:
+            self.check(self._lib.dgpu_edit_path_wide_dev(*args, C.c_uint32(int(max_slice)), C.c_void_p(stream or 0)), "dgpu_edit_path_wide_dev")
 
     # ------------------------------------------------------------------ longNeedle
     def long_needle(self, seqs, c_off, c_len, r_off, r_len, want_info=False, max_ref=None):

@@ -72,6 +72,7 @@ enum {
   SLOT_EP_COLS,      // edit path: HW-start target lengths, then the half columns of the split pass (edit_path.cu)
   SLOT_EP_BOUNDS,    // edit path: HW-start bounds and reverse end locations (edit_path.cu)
   SLOT_EP_EQTAB,     // edit path: generalised-equality tables (edit_path.cu)
+  SLOT_EP_HROW,      // edit path: per-warp scratch rows of the half columns wider than the wavefront classes (edit_path.cu)
   SLOT_COUNT
 };
 

@@ -53,7 +53,7 @@ int dgpu_fork_init(dgpu_ctx* ctx) {
 
 extern "C" {
 
-int dgpu_version(void) { return 1003; }
+int dgpu_version(void) { return 1004; }
 
 const char* dgpu_strerror(int code) {
   switch (code) {

@@ -335,6 +335,223 @@ __global__ void __launch_bounds__(SEGB_WARPS * 32) seg_band_kernel(SegJobs a) {
   }
 }
 
+// ---- segments wider than the wavefront classes (n > 16384 columns) that no band class certifies ---------------------------------------
+// Hirschberg only produces these from slices wider than 16384 columns: half columns of any height and width, and leaves of at most two
+// 64-row blocks (20 ceil(m/64) n + 8 n < 2^20 with n > 16384 forces m <= 128).
+constexpr int EPW_WARPS = 4;     // warps per CTA of seg_half_wide_kernel
+constexpr int EPL_WARPS = 2;     // warps per CTA of seg_leaf_wide_kernel
+constexpr int EPL_G = 2;         // lanes per leaf: one per 64-row block
+constexpr int EPL_WCOLS = 32;    // traceback window, columns
+
+// Half column (kind 1) of an unbanded segment: one warp per segment, one 64-row Myers block per lane, an anti-diagonal wavefront over
+// 2048-row stripes whose bottom horizontal deltas are parked in the warp's scratch row (n bytes), as ed_long_kernel computes edit distances.
+// NW top boundary (D[0][j] = j), rows / columns read back to front when rev. After each stripe the lanes' final Pv / Mv are the vertical
+// deltas of column n, which give colbuf[out_off + i] = -D[i][n] for every row of the stripe, run on from the stripe above; the column is
+// exact on every row.
+template <bool EQ>
+__global__ void __launch_bounds__(EPW_WARPS * 32) seg_half_wide_kernel(SegJobs a, size_t hrow_stride) {
+  __shared__ uint64_t peq_s[EPW_WARPS][5][32];
+  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+  const uint32_t gwarp = blockIdx.x * EPW_WARPS + wib, nwarps = gridDim.x * EPW_WARPS;
+  volatile int8_t* hrow = (volatile int8_t*) (a.work + (size_t) gwarp * hrow_stride);
+  for (uint32_t idx = gwarp; idx < a.count; idx += nwarps) {
+    const uint32_t job = a.list[idx];
+    const uint32_t m = a.q_len[job], n = a.t_len[job];
+    const uint8_t* q = a.seqs + a.q_off[job];
+    const uint8_t* t = a.seqs + a.t_off[job];
+    const bool rev = a.rev[job] != 0;
+    int* colv = a.colbuf + a.out_off[job];
+    if (lane == 0) colv[0] = -(int) n;
+    int top = (int) n;   // D[s * 2048][n]: the column value above the current stripe
+    const uint32_t nstripes = (m + 2047) / 2048;
+    for (uint32_t s = 0; s < nstripes; ++s) {
+      const uint32_t row0 = s * 2048 + (uint32_t) lane * 64;
+      const int nb = (int) min(32u, (m - s * 2048 + 63) / 64);
+      const bool last_stripe = (s + 1 == nstripes), active = lane < nb;
+      const int rows = active ? (int) min(64u, m - row0) : 0;
+      uint64_t other = 0;   // rows holding a byte outside ACGTN: compared byte by byte (pair tables included under EQ)
+      {
+        uint64_t pm[5] = {0, 0, 0, 0, 0};
+        for (int i = 0; i < rows; ++i) {
+          const uint32_t code = dna_code(__ldg(rev ? q + (m - 1 - row0 - i) : q + row0 + i));
+#pragma unroll
+          for (int sy = 0; sy < 5; ++sy) pm[sy] |= (code == (uint32_t) sy) ? (1ull << i) : 0ull;
+          if (code == 5u) other |= 1ull << i;
+        }
+        __syncwarp();
+#pragma unroll
+        for (int sy = 0; sy < 5; ++sy) peq_s[wib][sy][lane] = pm[sy];
+        __syncwarp();
+      }
+      uint64_t Pv = ~0ull, Mv = 0;
+      int hout = 0;
+      uint32_t cbuf = 0, cchar = 0;
+      const uint32_t nsteps = n + (uint32_t) nb - 1;
+      for (uint32_t st = 0; st < nsteps; ++st) {
+        if ((st & 31u) == 0) {
+          const uint32_t p = st + (uint32_t) lane;
+          cbuf = (p < n) ? (uint32_t) __ldg(rev ? t + (n - 1 - p) : t + p) : 0u;
+        }
+        const uint32_t newc = __shfl_sync(0xffffffffu, cbuf, (int) (st & 31u));
+        const uint32_t upc = __shfl_up_sync(0xffffffffu, cchar, 1);
+        cchar = (lane == 0) ? newc : upc;
+        const int hin_sh = __shfl_up_sync(0xffffffffu, hout, 1);
+        const int col = (int) st - lane;
+        if (active && col >= 0 && col < (int) n) {
+          const int hin = lane ? hin_sh : (s == 0 ? 1 : (int) hrow[col]);
+          uint64_t Eq, rest = other;
+          if (EQ) {
+            const uint32_t cm = a.eq_cls[cchar & 0xffu];
+            Eq = 0;
+#pragma unroll
+            for (int sy = 0; sy < 5; ++sy)
+              if ((cm >> sy) & 1u) Eq |= peq_s[wib][sy][lane];
+          } else {
+            const uint32_t code = dna_code(cchar);
+            Eq = code < 5 ? peq_s[wib][code][lane] : 0ull;
+            if (code < 5) rest = 0;   // an ACGTN column byte equals no row outside ACGTN
+          }
+          if (rest) {
+            const uint32_t cf = EQ ? a.eq.f[cchar & 0xffu] : 0u, cs = EQ ? a.eq.s[cchar & 0xffu] : 0u;
+            while (rest) {
+              const int i = __ffsll((long long) rest) - 1;
+              rest &= rest - 1;
+              const uint32_t qb = __ldg(rev ? q + (m - 1 - row0 - i) : q + row0 + i);
+              if (qb == (cchar & 0xffu) || (EQ && ((a.eq.f[qb] & cs) || (a.eq.s[qb] & cf)))) Eq |= 1ull << i;
+            }
+          }
+          uint64_t Ph, Mh;
+          hout = block64(Pv, Mv, Eq, hin, Ph, Mh);
+          if (lane == nb - 1 && !last_stripe) hrow[col] = (int8_t) hout;
+        }
+      }
+      __syncwarp();
+      __threadfence_block();
+      // this stripe's rows of column n: exclusive prefix of the lanes' delta sums, then each lane writes its own rows
+      const uint64_t valid = rows == 64 ? ~0ull : ((1ull << rows) - 1);
+      const int sum = __popcll(Pv & valid) - __popcll(Mv & valid);
+      int incl = sum;
+      for (int o = 1; o < 32; o <<= 1) {
+        const int v = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += v;
+      }
+      int v = top + incl - sum;
+      for (int j = 0; j < rows; ++j) {
+        v += (int) ((Pv >> j) & 1ull) - (int) ((Mv >> j) & 1ull);
+        colv[row0 + j + 1] = -v;
+      }
+      top += __shfl_sync(0xffffffffu, incl, 31);
+    }
+    if (lane == 0) a.corner[job] = -top;
+  }
+}
+
+// Leaf (kind 0) of at most two 64-row blocks and any width: EPL_G = 2 lanes per leaf, 16 leaves per warp. Lane p holds block p over the
+// whole column (lane 1 one step behind lane 0, its horizontal delta arriving by shuffle) and stores (Pv after the column, Ph into the
+// column) for every column, 16 B per lane-column. The traceback is the one of seg_band_kernel (up > left > diagonal through a window of
+// EPL_WCOLS columns of the current block in shared memory); ops are written from the END of the job's slot backwards.
+template <bool EQ>
+__global__ void __launch_bounds__(EPL_WARPS * 32) seg_leaf_wide_kernel(SegJobs a) {
+  constexpr int G = EPL_G, JPW = 32 / G;
+  __shared__ uint64_t peq_s[EPL_WARPS][JPW * G * EDB_BLOCK_WORDS];
+  __shared__ uint4 win_s[EPL_WARPS][JPW * EPL_WCOLS];
+  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+  const int p = lane & (G - 1), grp = lane / G;
+  const uint32_t gwarp = blockIdx.x * EPL_WARPS + wib, nwarps = gridDim.x * EPL_WARPS;
+  uint64_t* peq = &peq_s[wib][grp * G * EDB_BLOCK_WORDS];
+  uint4* win = &win_s[wib][grp * EPL_WCOLS];
+  uint4* store = (uint4*) (a.work + ((size_t) gwarp * JPW + grp) * a.work_stride);
+  const EqTabs tabs = {a.eq.f, a.eq.s, a.eq_cls};
+
+  for (uint32_t base = gwarp * JPW; base < a.count; base += nwarps * JPW) {
+    const bool have = base + grp < a.count;
+    const uint32_t job = have ? a.list[base + grp] : 0;
+    const int m = have ? (int) a.q_len[job] : 0, n = have ? (int) a.t_len[job] : 0;
+    const uint8_t* q = a.seqs + (have ? a.q_off[job] : 0);
+    const uint8_t* t = a.seqs + (have ? a.t_off[job] : 0);
+    const bool rev = have && a.rev[job] != 0;
+    const int nblk = (m + 63) >> 6;
+    const bool mine = p < nblk;   // this lane holds a block of the leaf
+
+    __syncwarp();
+    band_build_peq<G>(peq, q, m, rev, p);
+    __syncwarp();
+
+    int steps = have ? n + G - 1 : 0;
+    for (int o = 16; o; o >>= 1) steps = max(steps, __shfl_xor_sync(0xffffffffu, steps, o));
+    uint64_t Pv = ~0ull, Mv = 0;
+    int hout = 1, sc = m;   // sc: D[m][col + 1] on the lane of the last block
+    const int tb = (m - 1) & 63;
+    uint32_t chn = (have && n > 0) ? __ldg(rev ? t + (n - 1) : t) : 0u;
+    for (int st = 0; st < steps; ++st) {
+      const int hin_sh = __shfl_up_sync(0xffffffffu, hout, 1, G);
+      const int col = st - p;
+      if (mine && col >= 0 && col < n) {
+        const uint32_t ch = chn;
+        if (col + 1 < n) chn = __ldg(rev ? t + (n - 2 - col) : t + col + 1);
+        const uint64_t Eq = band_eq<EQ>(peq, p, ch, q, m, rev, tabs);
+        uint64_t Ph, Mh;
+        hout = block64(Pv, Mv, Eq, p == 0 ? 1 : hin_sh, Ph, Mh);
+        if (p == nblk - 1) sc += (int) ((Ph >> tb) & 1ull) - (int) ((Mh >> tb) & 1ull);
+        store[(size_t) col * nblk + p] = make_uint4((uint32_t) Pv, (uint32_t) (Pv >> 32), (uint32_t) Ph, (uint32_t) (Ph >> 32));
+      }
+    }
+    __threadfence_block();
+    __syncwarp();
+    {
+      const int s = __shfl_sync(0xffffffffu, sc, grp * G + ((nblk - 1) & (G - 1)));
+      if (have && p == 0) a.corner[job] = -s;
+    }
+
+    // traceback (src/edlib.cpp:1021-1131: up = insert 1, left = delete 2, diagonal = match 0 / mismatch 3)
+    int r = m - 1, cc = n - 1;
+    uint32_t k = 0;
+    const uint32_t cap = (uint32_t) (m + n);
+    uint8_t* out = a.tmp_ops + (have ? a.out_off[job] : 0);
+    int wb = -1, wc0 = -1;
+    while (__any_sync(0xffffffffu, have && r >= 0 && cc >= 0)) {
+      const bool go = have && r >= 0 && cc >= 0;
+      const int b = r >> 6;
+      const bool need = go && (b != wb || cc > wc0 || cc <= wc0 - EPL_WCOLS);
+      if (__any_sync(0xffffffffu, need)) {
+        if (need) {
+          for (int x = p; x < EPL_WCOLS; x += G) {
+            const int col = cc - x;
+            win[x] = col >= 0 ? __ldcg(store + (size_t) col * nblk + b) : make_uint4(0, 0, 0, 0);
+          }
+          wb = b; wc0 = cc;
+        }
+        __syncwarp();
+      }
+      if (go) {
+        const uint4 w = win[wc0 - cc];
+        const int bit = r & 63;
+        const uint32_t pv = ((bit < 32 ? w.x : w.y) >> (bit & 31)) & 1u;
+        const uint32_t ph = ((bit < 32 ? w.z : w.w) >> (bit & 31)) & 1u;
+        uint8_t op;
+        if (pv) { op = 1; --r; }
+        else if (ph) { op = 2; --cc; }
+        else {
+          const uint32_t x = __ldg(rev ? q + (m - 1 - r) : q + r), y = __ldg(rev ? t + (n - 1 - cc) : t + cc);
+          op = (EQ ? a.eq.equal(x, y) : (x == y)) ? 0 : 3;
+          --r; --cc;
+        }
+        if (p == 0) out[cap - 1 - k] = op;
+        ++k;
+      }
+      __syncwarp();
+    }
+    if (have) {
+      for (int i = p; i <= r; i += G) out[cap - 1 - (k + (uint32_t) i)] = 1;    // column 0 reached: the remaining rows are inserts
+      if (r >= 0) k += (uint32_t) (r + 1);
+      for (int i = p; i <= cc; i += G) out[cap - 1 - (k + (uint32_t) i)] = 2;   // row 0 reached: the remaining columns are deletes
+      if (cc >= 0) k += (uint32_t) (cc + 1);
+      if (p == 0) a.out_len[job] = k;
+    }
+    __syncwarp();
+  }
+}
+
 // Hirschberg split row (src/edlib.cpp:1303-1338): F = forward half column (F[i] = -fcol[i]), B = reverse half column
 // (B[i] = -bcol[m-i]); interior rows i = 1..m-1 ascending, then i = 0, then i = m. One warp per segment.
 __global__ void hb_select_kernel(const int* colbuf, const uint64_t* f_off, const uint64_t* b_off, const uint32_t* m_arr, const uint32_t* h_arr,
@@ -404,9 +621,10 @@ struct SegRunner {
   std::vector<uint64_t> out_off;
   std::vector<uint32_t> plan_m, plan_n;  // problem whose band the segment lives in (seg_band_kernel)
   std::vector<int32_t> bound;            // optimum of that problem
-  std::vector<uint8_t> banded;           // set by run(): the segment went through seg_band_kernel (a leaf's ops then end at the end of its slot)
+  std::vector<uint8_t> tail_ops;         // set by run(): the segment went through seg_band_kernel or seg_leaf_wide_kernel (a leaf's ops then end at
+                                         // the end of its slot)
   const uint8_t* eq_cls = nullptr;
-  void clear() { qoff.clear(); qlen.clear(); toff.clear(); tlen.clear(); rev.clear(); kind.clear(); out_off.clear(); plan_m.clear(); plan_n.clear(); bound.clear(); banded.clear(); }
+  void clear() { qoff.clear(); qlen.clear(); toff.clear(); tlen.clear(); rev.clear(); kind.clear(); out_off.clear(); plan_m.clear(); plan_n.clear(); bound.clear(); tail_ops.clear(); }
   size_t add(uint32_t qo, uint32_t ql, uint32_t to, uint32_t tl, bool r, int kd, uint64_t oo, uint32_t pm, uint32_t pn, int32_t k) {
     qoff.push_back(qo); qlen.push_back(ql); toff.push_back(to); tlen.push_back(tl); rev.push_back(r); kind.push_back((uint8_t) kd); out_off.push_back(oo);
     plan_m.push_back(pm); plan_n.push_back(pn); bound.push_back(k);
@@ -451,6 +669,24 @@ inline int seg_band_class(uint32_t m, uint32_t pm, uint32_t pn, int32_t k) {
   return -1;
 }
 
+// Whether seg_kernel cannot stage m query rows in shared memory: the launch's opt-in of (m + 15) & ~15 dynamic bytes would exceed the
+// device's per-block maximum less the kernel's static shared memory, and the whole call would fail. Such half columns (Hirschberg over a
+// query of more than ~230 kb) run on seg_half_wide_kernel instead; every segment seg_kernel can launch still runs there.
+bool seg_rows_exceed(dgpu_ctx* ctx, uint32_t m, bool multi, bool eq) {
+  static size_t room[2][2] = {{0, 0}, {0, 0}};   // [multi][eq]: dynamic shared memory seg_kernel may opt in to
+  size_t& r = room[multi][eq];
+  if (!r) {
+    int optin = 0;
+    cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device);
+    cudaFuncAttributes fa{};
+    if (multi) cudaFuncGetAttributes(&fa, eq ? (const void*) seg_kernel<32, true, true> : (const void*) seg_kernel<32, true, false>);
+    else cudaFuncGetAttributes(&fa, eq ? (const void*) seg_kernel<8, false, true> : (const void*) seg_kernel<8, false, false>);
+    r = (size_t) optin - fa.sharedSizeBytes;
+  }
+  const size_t smem = ((size_t) m + 15) & ~(size_t) 15;
+  return smem > 48 * 1024 && smem > r;
+}
+
 int SegRunner::run(uint8_t* tmp_ops, int* colbuf) {
   const size_t N = qoff.size();
   if (!N) return DGPU_OK;
@@ -479,20 +715,29 @@ int SegRunner::run(uint8_t* tmp_ops, int* colbuf) {
   DGPU_CUDA(ctx, cudaMemcpyAsync(d_kind, kind.data(), N, cudaMemcpyHostToDevice, st));
   // class lists
   // lists[1..11]: wavefront classes by target length; lists[12..16]: band classes G = 2, 4, 8, 16, 32
+  // wide_half / wide_leaf: unbanded segments wider than the wavefront classes (seg_half_wide_kernel, seg_leaf_wide_kernel)
   std::vector<std::vector<uint32_t> > lists(12 + EDB_CLASSES);
-  banded.assign(N, 0);
-  static const bool no_band = getenv("DGPU_EP_NO_BAND") != nullptr;   // development switch: everything through the wavefront kernels
+  std::vector<uint32_t> wide_half, wide_leaf;
+  tail_ops.assign(N, 0);
+  static const bool no_band = getenv("DGPU_EP_NO_BAND") != nullptr;   // development switch: no band classes (wavefront and wide kernels only)
   for (size_t i = 0; i < N; ++i) {
     const int bc = no_band ? -1 : seg_band_class(qlen[i], plan_m[i], plan_n[i], bound[i]);
-    if (bc >= 0) { lists[12 + bc].push_back((uint32_t) i); banded[i] = 1; continue; }
+    if (bc >= 0) { lists[12 + bc].push_back((uint32_t) i); tail_ops[i] = 1; continue; }
     const int c = seg_class(tlen[i]);
-    if (c <= 0) return DGPU_ERR_UNSUPPORTED;
-    lists[c].push_back((uint32_t) i);
+    if (c > 0 && !(kind[i] == 1 && seg_rows_exceed(ctx, qlen[i], c > 8, use_eq))) { lists[c].push_back((uint32_t) i); continue; }
+    if (kind[i] == 1) { wide_half.push_back((uint32_t) i); continue; }
+    if (qlen[i] > 64 * EPL_G) return DGPU_ERR_UNSUPPORTED;   // Hirschberg's split rule leaves no such leaf
+    wide_leaf.push_back((uint32_t) i);
+    tail_ops[i] = 1;
   }
   std::vector<uint32_t> flat;
   std::vector<size_t> lo(13 + EDB_CLASSES, 0);
   for (int c = 1; c < 12 + EDB_CLASSES; ++c) { lo[c] = flat.size(); flat.insert(flat.end(), lists[c].begin(), lists[c].end()); }
   lo[12 + EDB_CLASSES] = flat.size();
+  const size_t lo_half = flat.size();
+  flat.insert(flat.end(), wide_half.begin(), wide_half.end());
+  const size_t lo_leaf = flat.size();
+  flat.insert(flat.end(), wide_leaf.begin(), wide_leaf.end());
   DGPU_CUDA(ctx, cudaMemcpyAsync(d_list, flat.data(), flat.size() * 4, cudaMemcpyHostToDevice, st));
   SegJobs a;
   a.seqs = seqs; a.q_off = d_qoff; a.q_len = d_qlen; a.t_off = d_toff; a.t_len = d_tlen; a.rev = d_rev; a.kind = d_kind; a.out_off = d_oo;
@@ -527,12 +772,47 @@ int SegRunner::run(uint8_t* tmp_ops, int* colbuf) {
     }
     if (rc) return rc;
   }
+  if (!wide_half.empty()) {   // one warp per half column, a scratch row of n bytes per warp (SLOT_EP_HROW)
+    size_t nmax = 0;
+    for (uint32_t i : wide_half) nmax = std::max<size_t>(nmax, tlen[i]);
+    const size_t stride = (nmax + 255) & ~(size_t) 255;
+    size_t grid = std::min<size_t>((wide_half.size() + EPW_WARPS - 1) / EPW_WARPS, (size_t) ctx->num_sms * 4);
+    const size_t budget = (size_t) ((double) free_b * 0.6) + ctx->bufs[SLOT_EP_HROW].cap;
+    if (grid * EPW_WARPS * stride > budget) grid = std::max<size_t>(1, budget / (EPW_WARPS * stride));
+    void* w;
+    if ((rc = dgpu_reserve(ctx, SLOT_EP_HROW, grid * EPW_WARPS * stride, &w))) return rc;
+    a.work = (uint8_t*) w;
+    a.list = d_list + lo_half;
+    a.count = (uint32_t) wide_half.size();
+    if (use_eq) seg_half_wide_kernel<true><<<(unsigned) grid, EPW_WARPS * 32, 0, st>>>(a, stride);
+    else seg_half_wide_kernel<false><<<(unsigned) grid, EPW_WARPS * 32, 0, st>>>(a, stride);
+    DGPU_LAUNCH_CHECK(ctx, "seg_half_wide_kernel");
+  }
+  if (!wide_leaf.empty()) {   // trace storage of a leaf: one uint4 per block and column
+    constexpr int jpw = 32 / EPL_G;
+    size_t maxcells = 0;
+    for (uint32_t i : wide_leaf) maxcells = std::max<size_t>(maxcells, (size_t) tlen[i] * ((qlen[i] + 63) >> 6));
+    a.off_trace = 0;
+    a.work_stride = maxcells * sizeof(uint4);
+    size_t grid = std::min<size_t>((wide_leaf.size() + (size_t) jpw * EPL_WARPS - 1) / ((size_t) jpw * EPL_WARPS), (size_t) ctx->num_sms * 8);
+    const size_t per_block = (size_t) EPL_WARPS * jpw * a.work_stride;
+    const size_t budget = (size_t) ((double) free_b * 0.6) + ctx->bufs[SLOT_WAVEFRONT].cap;
+    if (grid * per_block > budget) grid = std::max<size_t>(1, budget / per_block);
+    void* w;
+    if ((rc = dgpu_reserve(ctx, SLOT_WAVEFRONT, grid * per_block, &w))) return rc;
+    a.work = (uint8_t*) w;
+    a.list = d_list + lo_leaf;
+    a.count = (uint32_t) wide_leaf.size();
+    if (use_eq) seg_leaf_wide_kernel<true><<<(unsigned) grid, EPL_WARPS * 32, 0, st>>>(a);
+    else seg_leaf_wide_kernel<false><<<(unsigned) grid, EPL_WARPS * 32, 0, st>>>(a);
+    DGPU_LAUNCH_CHECK(ctx, "seg_leaf_wide_kernel");
+  }
   for (int c = 1; c < 12; ++c) {
     if (lists[c].empty()) continue;
     const int C = seg_cols(c);
     size_t maxwords = 0, mmax = 0, mnmax = 0;
     for (uint32_t i : lists[c]) {
-      maxwords = std::max(maxwords, (size_t) (qlen[i] + 1) * seg_dstride(tlen[i], C));
+      if (kind[i] == 0) maxwords = std::max(maxwords, (size_t) (qlen[i] + 1) * seg_dstride(tlen[i], C));   // half columns store no directions
       mmax = std::max<size_t>(mmax, qlen[i]);
       mnmax = std::max<size_t>(mnmax, (size_t) qlen[i] + tlen[i]);
     }
@@ -575,14 +855,17 @@ inline bool seg_needs_split(uint32_t m, uint32_t n) {  // src/edlib.cpp:1189-119
 // sequence (many reads against one window) need more than the arena; runs bound that and keep offsets 32-bit.
 constexpr uint64_t EP_MIRROR_RUN = 1ull << 30;
 
-}  // namespace
+int check_max_slice(dgpu_ctx* ctx, uint32_t max_slice) {
+  if (max_slice >= 1 && max_slice <= DGPU_EP_MAX_SLICE) return DGPU_OK;
+  if (ctx) ctx->last_error = "dgpu_edit_path_wide: max_slice must be 1 .. " + std::to_string(DGPU_EP_MAX_SLICE);
+  return DGPU_ERR_ARG;
+}
 
-extern "C" {
-
-int dgpu_edit_path_ex_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
-                          const uint32_t* q_off, const uint32_t* q_len, const uint32_t* t_off, const uint32_t* t_len,
-                          int mode, const uint8_t* eq_pairs, uint32_t n_eq, uint64_t n, int32_t* dist, int32_t* start_loc, int32_t* end_loc,
-                          uint8_t* ops, const uint64_t* ops_off, uint32_t* ops_len, uint32_t* status, void* stream) {
+// The device form of every entry point: a job whose aligned target slice is wider than max_slice gets status 2 alone.
+int ep_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
+           const uint32_t* q_off, const uint32_t* q_len, const uint32_t* t_off, const uint32_t* t_len,
+           int mode, const uint8_t* eq_pairs, uint32_t n_eq, uint64_t n, int32_t* dist, int32_t* start_loc, int32_t* end_loc,
+           uint8_t* ops, const uint64_t* ops_off, uint32_t* ops_len, uint32_t* status, uint32_t max_slice, void* stream) {
   if (!ctx) return DGPU_ERR_ARG;
   if (n == 0) return DGPU_OK;
   if (n >= (1ull << 31) || seqs_bytes >= (1ull << 32)) return DGPU_ERR_ARG;
@@ -684,7 +967,7 @@ int dgpu_edit_path_ex_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_byte
     if (h_qlen[i] == 0 || h_tlen[i] == 0 || h_dist[i] < 0) continue;  // no path at all (edlib returns early)
     const int s = h_start[i], e = h_end[i];
     Seg sg; sg.job = (uint32_t) i; sg.qoff = h_qoff[i]; sg.qlen = h_qlen[i]; sg.toff = h_toff[i] + (uint32_t) s; sg.tlen = (uint32_t) (e - s + 1); sg.score = h_dist[i];
-    if (sg.tlen > 16384) { h_status[i] = 2; continue; }
+    if (sg.tlen > max_slice) { h_status[i] = 2; continue; }
     perjob[i].push_back(sg);
     if (sg.qlen && sg.tlen && seg_needs_split(sg.qlen, sg.tlen)) any_split = true;
   }
@@ -793,7 +1076,7 @@ int dgpu_edit_path_ex_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_byte
         if (leaf_slot[li] != (size_t) -1) {
           leaf_len_h[li] = traced_len[leaf_slot[li]];
           if (-traced_corner[leaf_slot[li]] != g.score) h_status[i] = 3;
-          else if (R.banded[leaf_slot[li]]) leaf_off[li] += (uint64_t) g.qlen + g.tlen - traced_len[leaf_slot[li]];   // seg_band_kernel writes from the end of the slot
+          else if (R.tail_ops[leaf_slot[li]]) leaf_off[li] += (uint64_t) g.qlen + g.tlen - traced_len[leaf_slot[li]];   // seg_band_kernel / seg_leaf_wide_kernel write from the end of the slot
         }
         ++li;
       }
@@ -819,26 +1102,19 @@ int dgpu_edit_path_ex_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_byte
   return DGPU_OK;
 }
 
-int dgpu_edit_path_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
-                       const uint32_t* q_off, const uint32_t* q_len, const uint32_t* t_off, const uint32_t* t_len,
-                       int mode, uint64_t n, int32_t* dist, int32_t* start_loc, int32_t* end_loc,
-                       uint8_t* ops, const uint64_t* ops_off, uint32_t* ops_len, uint32_t* status, void* stream) {
-  return dgpu_edit_path_ex_dev(ctx, seqs, seqs_bytes, q_off, q_len, t_off, t_len, mode, nullptr, 0, n, dist, start_loc, end_loc, ops, ops_off, ops_len,
-                               status, stream);
-}
-
-int dgpu_edit_path_ex(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
-                      const uint32_t* q_off, const uint32_t* q_len, const uint32_t* t_off, const uint32_t* t_len,
-                      int mode, const uint8_t* eq_pairs, uint32_t n_eq, uint64_t n, int32_t* dist, int32_t* start_loc, int32_t* end_loc,
-                      uint8_t* ops, const uint64_t* ops_off, uint64_t ops_bytes, uint32_t* ops_len, uint32_t* status) {
-  DgpuStage s(ctx, "dgpu_edit_path", n);
+// The host form of every entry point.
+int ep_host(dgpu_ctx* ctx, const char* name, const uint8_t* seqs, uint64_t seqs_bytes,
+            const uint32_t* q_off, const uint32_t* q_len, const uint32_t* t_off, const uint32_t* t_len,
+            int mode, const uint8_t* eq_pairs, uint32_t n_eq, uint64_t n, int32_t* dist, int32_t* start_loc, int32_t* end_loc,
+            uint8_t* ops, const uint64_t* ops_off, uint64_t ops_bytes, uint32_t* ops_len, uint32_t* status, uint32_t max_slice) {
+  DgpuStage s(ctx, name, n);
   if (!ctx) return DGPU_ERR_ARG;
   if (n == 0) return DGPU_OK;
   if (!seqs || !q_off || !q_len || !t_off || !t_len || !dist || !start_loc || !end_loc || !ops || !ops_off || !ops_len || !status) return DGPU_ERR_ARG;
   int rc;
   if ((rc = s.check_arena(seqs_bytes, n, q_off, q_len)) || (rc = s.check_arena(seqs_bytes, n, t_off, t_len))) return rc;
   for (uint64_t i = 0; i < n; ++i)   // op slots (capacity |q| + |t|) inside ops_bytes
-    if (ops_off[i] + q_len[i] + t_len[i] > ops_bytes) { ctx->last_error = "dgpu_edit_path: op slot beyond ops_bytes"; return DGPU_ERR_CAPACITY; }
+    if (ops_off[i] + q_len[i] + t_len[i] > ops_bytes) { ctx->last_error = std::string(name) + ": op slot beyond ops_bytes"; return DGPU_ERR_CAPACITY; }
   if ((rc = s.open())) return rc;
   const uint8_t* d_seqs = s.arena(seqs, seqs_bytes);
   uint8_t* d_ops = s.out(ops, ops_bytes, 64);
@@ -847,18 +1123,66 @@ int dgpu_edit_path_ex(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
   int32_t *d_dist = s.out(dist, n), *d_start = s.out(start_loc, n), *d_end = s.out(end_loc, n);
   uint32_t *d_opslen = s.out(ops_len, n), *d_status = s.out(status, n);
   if (s.rc) return s.rc;
-  if ((rc = dgpu_edit_path_ex_dev(ctx, d_seqs, seqs_bytes, d_qoff, d_qlen, d_toff, d_tlen, mode, eq_pairs, n_eq, n, d_dist, d_start, d_end, d_ops,
-                                  d_opsoff, d_opslen, d_status, s.st)))
+  if ((rc = ep_dev(ctx, d_seqs, seqs_bytes, d_qoff, d_qlen, d_toff, d_tlen, mode, eq_pairs, n_eq, n, d_dist, d_start, d_end, d_ops, d_opsoff, d_opslen,
+                   d_status, max_slice, s.st)))
     return rc;
   return s.finish();
+}
+
+}  // namespace
+
+extern "C" {
+
+int dgpu_edit_path_wide_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
+                            const uint32_t* q_off, const uint32_t* q_len, const uint32_t* t_off, const uint32_t* t_len,
+                            int mode, const uint8_t* eq_pairs, uint32_t n_eq, uint64_t n, int32_t* dist, int32_t* start_loc, int32_t* end_loc,
+                            uint8_t* ops, const uint64_t* ops_off, uint32_t* ops_len, uint32_t* status, uint32_t max_slice, void* stream) {
+  int rc;
+  if ((rc = check_max_slice(ctx, max_slice))) return rc;
+  return ep_dev(ctx, seqs, seqs_bytes, q_off, q_len, t_off, t_len, mode, eq_pairs, n_eq, n, dist, start_loc, end_loc, ops, ops_off, ops_len, status,
+                max_slice, stream);
+}
+
+int dgpu_edit_path_ex_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
+                          const uint32_t* q_off, const uint32_t* q_len, const uint32_t* t_off, const uint32_t* t_len,
+                          int mode, const uint8_t* eq_pairs, uint32_t n_eq, uint64_t n, int32_t* dist, int32_t* start_loc, int32_t* end_loc,
+                          uint8_t* ops, const uint64_t* ops_off, uint32_t* ops_len, uint32_t* status, void* stream) {
+  return ep_dev(ctx, seqs, seqs_bytes, q_off, q_len, t_off, t_len, mode, eq_pairs, n_eq, n, dist, start_loc, end_loc, ops, ops_off, ops_len, status,
+                DGPU_EP_CLASSIC_SLICE, stream);
+}
+
+int dgpu_edit_path_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
+                       const uint32_t* q_off, const uint32_t* q_len, const uint32_t* t_off, const uint32_t* t_len,
+                       int mode, uint64_t n, int32_t* dist, int32_t* start_loc, int32_t* end_loc,
+                       uint8_t* ops, const uint64_t* ops_off, uint32_t* ops_len, uint32_t* status, void* stream) {
+  return ep_dev(ctx, seqs, seqs_bytes, q_off, q_len, t_off, t_len, mode, nullptr, 0, n, dist, start_loc, end_loc, ops, ops_off, ops_len, status,
+                DGPU_EP_CLASSIC_SLICE, stream);
+}
+
+int dgpu_edit_path_wide(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
+                        const uint32_t* q_off, const uint32_t* q_len, const uint32_t* t_off, const uint32_t* t_len,
+                        int mode, const uint8_t* eq_pairs, uint32_t n_eq, uint64_t n, int32_t* dist, int32_t* start_loc, int32_t* end_loc,
+                        uint8_t* ops, const uint64_t* ops_off, uint64_t ops_bytes, uint32_t* ops_len, uint32_t* status, uint32_t max_slice) {
+  int rc;
+  if ((rc = check_max_slice(ctx, max_slice))) return rc;
+  return ep_host(ctx, "dgpu_edit_path_wide", seqs, seqs_bytes, q_off, q_len, t_off, t_len, mode, eq_pairs, n_eq, n, dist, start_loc, end_loc, ops, ops_off,
+                 ops_bytes, ops_len, status, max_slice);
+}
+
+int dgpu_edit_path_ex(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
+                      const uint32_t* q_off, const uint32_t* q_len, const uint32_t* t_off, const uint32_t* t_len,
+                      int mode, const uint8_t* eq_pairs, uint32_t n_eq, uint64_t n, int32_t* dist, int32_t* start_loc, int32_t* end_loc,
+                      uint8_t* ops, const uint64_t* ops_off, uint64_t ops_bytes, uint32_t* ops_len, uint32_t* status) {
+  return ep_host(ctx, "dgpu_edit_path", seqs, seqs_bytes, q_off, q_len, t_off, t_len, mode, eq_pairs, n_eq, n, dist, start_loc, end_loc, ops, ops_off,
+                 ops_bytes, ops_len, status, DGPU_EP_CLASSIC_SLICE);
 }
 
 int dgpu_edit_path(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
                    const uint32_t* q_off, const uint32_t* q_len, const uint32_t* t_off, const uint32_t* t_len,
                    int mode, uint64_t n, int32_t* dist, int32_t* start_loc, int32_t* end_loc,
                    uint8_t* ops, const uint64_t* ops_off, uint64_t ops_bytes, uint32_t* ops_len, uint32_t* status) {
-  return dgpu_edit_path_ex(ctx, seqs, seqs_bytes, q_off, q_len, t_off, t_len, mode, nullptr, 0, n, dist, start_loc, end_loc, ops, ops_off, ops_bytes,
-                           ops_len, status);
+  return ep_host(ctx, "dgpu_edit_path", seqs, seqs_bytes, q_off, q_len, t_off, t_len, mode, nullptr, 0, n, dist, start_loc, end_loc, ops, ops_off,
+                 ops_bytes, ops_len, status, DGPU_EP_CLASSIC_SLICE);
 }
 
 }  // extern "C"

@@ -1306,4 +1306,7 @@ int dh_detect_tandem_repeat(const char* s, int n, int maxPeriod, float minFracti
 
 #include "capi_sharded.inc"
 
+// edit-path jobs refused so far by a device limit (DeviceLimitLog::pathJobs; the binding reports it on stderr)
+uint64_t dh_path_jobs_refused(void) { return deviceLimitLog().pathJobs.load(); }
+
 }  // extern "C"

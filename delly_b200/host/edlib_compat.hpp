@@ -7,6 +7,7 @@
 #include <vector>
 
 #include "../../include/dgpu.h"
+#include "editpath.hpp"
 #define DGPU_EDLIB_NO_ALIASES
 #include "../../include/dgpu_edlib.h"
 
@@ -79,8 +80,8 @@ EdlibAlignResult dgpu_edlibAlign(const char* query, int queryLength, const char*
   uint32_t opsLen = 0, status = 0;
   std::vector<uint8_t> eq;
   for (int i = 0; i < config.additionalEqualitiesLength; ++i) { eq.push_back((uint8_t) config.additionalEqualities[i].first); eq.push_back((uint8_t) config.additionalEqualities[i].second); }
-  rc = dgpu_edit_path_ex(ctx, (const uint8_t*) arena.data(), arena.size(), &qo, &ql, &to, &tl, (int) config.mode, eq.empty() ? nullptr : eq.data(),
-                         (uint32_t) (eq.size() / 2), 1, &dist, &start, &end, ops.data(), &opsOff, ops.size(), &opsLen, &status);
+  rc = dellyb200::editPathCall(ctx, (const uint8_t*) arena.data(), arena.size(), &qo, &ql, &to, &tl, (int) config.mode, eq.empty() ? nullptr : eq.data(),
+                               (uint32_t) (eq.size() / 2), 1, &dist, &start, &end, ops.data(), &opsOff, ops.size(), &opsLen, &status);
   if (rc || status) { r.status = EDLIB_STATUS_ERROR; return r; }
   if (k >= 0 && dist > k) dist = -1;   // the path entry points are unbounded; edlib reports -1 (and no locations) beyond k
   r.editDistance = dist;

@@ -290,11 +290,11 @@ inline int flushInsertionJobs(dgpu_ctx* ctx, MethylConfig const& mc, std::vector
   }
   std::vector<int32_t> dist(J), startLoc(J), endLoc(J);
   std::vector<uint8_t> ops(opsBytes + 1);
-  int rc = dgpu_edit_path(ctx, (const uint8_t*) arena.data(), arena.size(), qo.data(), ql.data(), to.data(), tl.data(), DGPU_MODE_HW, J, dist.data(),
-                          startLoc.data(), endLoc.data(), ops.data(), opsOff.data(), opsBytes, opsLen.data(), status.data());
+  int rc = editPathCall(ctx, (const uint8_t*) arena.data(), arena.size(), qo.data(), ql.data(), to.data(), tl.data(), DGPU_MODE_HW, nullptr, 0, J,
+                        dist.data(), startLoc.data(), endLoc.data(), ops.data(), opsOff.data(), opsBytes, opsLen.data(), status.data());
   if (rc) return rc;
   for (std::size_t j = 0; j < J; ++j)
-    if (status[j] != 0) ++deviceLimitLog().pathJobs;   // e.g. a consensus insertion above the path kernel's 16384-column slice: no calls from this read
+    if (status[j] != 0) ++deviceLimitLog().pathJobs;   // e.g. a consensus insertion above DGPU_EP_MAX_SLICE columns: no calls from this read
   static const int32_t CPGTOL = 8;
   for (std::size_t j = 0; j < J; ++j) {
     InsertionJob const& jb = queue[j];

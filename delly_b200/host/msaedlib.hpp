@@ -240,8 +240,8 @@ inline int msaEdlibBatch(dgpu_ctx* ctx, Config const& c, std::vector<std::vector
     std::vector<int32_t> dist(J), st(J), en(J);
     std::vector<uint32_t> olen(J), status(J);
     std::vector<uint8_t> ops(obytes + 1);
-    rc = dgpu_edit_path_ex(ctx, (const uint8_t*) arena.data(), arena.size(), qo.data(), ql.data(), to.data(), tl.data(), DGPU_MODE_NW, iupac, 20, J, dist.data(),
-                           st.data(), en.data(), ops.data(), oo.data(), obytes, olen.data(), status.data());
+    rc = editPathCall(ctx, (const uint8_t*) arena.data(), arena.size(), qo.data(), ql.data(), to.data(), tl.data(), DGPU_MODE_NW, iupac, 20, J, dist.data(),
+                      st.data(), en.data(), ops.data(), oo.data(), obytes, olen.data(), status.data());
     if (rc) return rc;
     lap(tPath);
     for (std::size_t k = 0; k < J; ++k)

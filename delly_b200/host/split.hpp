@@ -19,6 +19,7 @@
 #include <vector>
 
 #include "../../include/dgpu.h"
+#include "editpath.hpp"
 #include "types.hpp"
 
 namespace dellyb200 {

@@ -37,8 +37,8 @@ inline int editPathBatch(dgpu_ctx* ctx, std::vector<std::pair<std::string, std::
   std::vector<int32_t> dist(N), st(N), en(N);
   std::vector<uint32_t> olen(N), status(N);
   std::vector<uint8_t> ops(obytes + 1);
-  int rc = dgpu_edit_path_ex(ctx, (const uint8_t*) arena.data(), arena.size(), qo.data(), ql.data(), to.data(), tl.data(), mode, eq_pairs, n_eq, N, dist.data(),
-                             st.data(), en.data(), ops.data(), oo.data(), obytes, olen.data(), status.data());
+  int rc = editPathCall(ctx, (const uint8_t*) arena.data(), arena.size(), qo.data(), ql.data(), to.data(), tl.data(), mode, eq_pairs, n_eq, N, dist.data(),
+                        st.data(), en.data(), ops.data(), oo.data(), obytes, olen.data(), status.data());
   if (rc) return rc;
   for (std::size_t i = 0; i < N; ++i) {
     if (status[i]) { ++deviceLimitLog().pathJobs; out[i].failed = true; out[i].end = 0; out[i].start = 0; continue; }   // never approximated: failed, counted

@@ -53,7 +53,7 @@ inline void parallelFor(std::size_t n, F&& fn, std::size_t minPerThread = 1) {
 // behaviour when an alignment fails: the SV stays imprecise or is dropped), counted here, and the binding reports the counts on stderr.
 struct DeviceLimitLog {
   std::atomic<uint64_t> msaClusters{0};   // dgpu_msa_ex status != 0: > DGPU_MSA_LARGE_MAXR reads, > 1023 alignment columns, a byte outside ACGTN
-  std::atomic<uint64_t> pathJobs{0};      // dgpu_edit_path status != 0: target slice beyond the path kernel's window
+  std::atomic<uint64_t> pathJobs{0};      // dgpu_edit_path[_wide] status != 0: target slice beyond DGPU_EP_MAX_SLICE columns
   std::atomic<uint64_t> needleJobs{0};    // dgpu_long_needle[_ex]: |cons| > 16383, |ref| > DGPU_LN_MAX_REF, or a workspace beyond the device budget
   uint64_t total() const { return msaClusters.load() + pathJobs.load() + needleJobs.load(); }
 };

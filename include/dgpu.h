@@ -118,8 +118,8 @@ int dgpu_edit_distance_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_byt
  * ops = the alignment array (0 match, 1 insert, 2 delete, 3 mismatch; src/edlib.h:84-87) at ops + ops_off[i]
  * (reserve q_len + t_len bytes), ops_len (alignmentLength). Problems above edlib's 1 MiB switch are split with
  * Hirschberg's recursion exactly like the reference (src/edlib.cpp:1189-1212, :1232-1397), so paths are identical
- * at every size. status: 0 ok; 2 = aligned target slice longer than 16384 (not supported, path NOT produced);
- * 3 = internal consistency failure.
+ * at every size. status: 0 ok; 2 = aligned target slice t[start..end] wider than DGPU_EP_CLASSIC_SLICE = 16384 columns (_wide forms: wider than
+ * max_slice); the job keeps the reference's distance and locations, its path is NOT produced; 3 = internal consistency failure.
  * The _ex forms take edlib's additionalEqualities (src/edlib.h:100-106) as 2*n_eq bytes (first,second pairs,
  * n_eq <= 32) in every mode — the reference's call sites are src/assemble.h:425-447 (NW, msaEdlib) and
  * src/assemble.h:663-693 (HW, msaWfa).
@@ -152,6 +152,33 @@ int dgpu_edit_path_ex_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_byte
                           int32_t* dist, int32_t* start_loc, int32_t* end_loc,
                           uint8_t* ops, const uint64_t* ops_off,
                           uint32_t* ops_len, uint32_t* status, void* stream);
+/* The _wide forms take the _ex arguments plus max_slice, the widest aligned target slice the caller wants traced (1 .. DGPU_EP_MAX_SLICE,
+ * else DGPU_ERR_ARG); a job with a wider slice gets status 2 alone. The other forms are the _wide forms with max_slice =
+ * DGPU_EP_CLASSIC_SLICE. Hirschberg segments of up to 16384 columns run on the band and wavefront engines as they always did; unbanded
+ * segments wider than that run on a warp-per-segment half-column engine (a scratch row of one byte per column) and a two-lanes-per-leaf
+ * traceback engine (leaves of at most 128 rows, 16 B per block and column). In every form, a half column with more query rows than the
+ * wavefront engine can stage in shared memory (about 230 k; such a call used to fail with DGPU_ERR_CUDA) also runs on the half-column engine.
+ * Cap: no buffer of these engines is sized by the slice width beyond O(m + n) scratch per segment, and their 32-bit arithmetic (int32 end
+ * locations and step counts, the -(1<<28) over-estimate of banded half columns) would hold up to 2^27 columns. What bounds the cap is time:
+ * an unbanded half column takes one warp for (m / 2048) x n steps, so a path's time grows with the square of the width. One 8 %-divergent NW
+ * pair at 2^18 columns takes 15.7 s on an H100 80GB HBM3 at 700 W (profiles/h100_bench_epw.json); 2^19 would take about four times that
+ * per path. DGPU_EP_MAX_SLICE is the widest slice the test suite checks against the reference. */
+#define DGPU_EP_CLASSIC_SLICE 16384   /* the slice limit of dgpu_edit_path[_ex][_dev] */
+#define DGPU_EP_MAX_SLICE 262144
+int dgpu_edit_path_wide(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
+                        const uint32_t* q_off, const uint32_t* q_len,
+                        const uint32_t* t_off, const uint32_t* t_len, int mode,
+                        const uint8_t* eq_pairs, uint32_t n_eq, uint64_t n,
+                        int32_t* dist, int32_t* start_loc, int32_t* end_loc,
+                        uint8_t* ops, const uint64_t* ops_off, uint64_t ops_bytes,
+                        uint32_t* ops_len, uint32_t* status, uint32_t max_slice);
+int dgpu_edit_path_wide_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
+                            const uint32_t* q_off, const uint32_t* q_len,
+                            const uint32_t* t_off, const uint32_t* t_len, int mode,
+                            const uint8_t* eq_pairs, uint32_t n_eq, uint64_t n,
+                            int32_t* dist, int32_t* start_loc, int32_t* end_loc,
+                            uint8_t* ops, const uint64_t* ops_off,
+                            uint32_t* ops_len, uint32_t* status, uint32_t max_slice, void* stream);
 
 /* ---- consensus vs SV-reference split alignment (replaces longNeedle) --------------------
  * Call sites: _consRefAlignment for svt != 4, src/split.h:555 (reached from alignConsensus,
