@@ -63,6 +63,7 @@ enum {
   SLOT_ED_STRIPES,   // stripe scratch of long edit-distance targets (edit_distance.cu)
   SLOT_ED_BAND,      // job lists of the banded NW passes (edit_distance.cu)
   SLOT_ED_SLOTS,     // per-job count slot bytes of the edit-distance classification (edit_distance.cu)
+  SLOT_ED_PEQ,       // shared Peq tables of target-sharing HW job pairs: hash slots, then one entry per slot (edit_distance.cu)
   SLOT_WAVEFRONT,    // wavefront workspace of the longNeedle and segment engines; their planners count its capacity as free
                      // (long_needle.cu, edit_path.cu)
   SLOT_MSA_SEGJOBS,  // MSA warp workspace (msa.cu); segment job arrays (edit_path.cu)

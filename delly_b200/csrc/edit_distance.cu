@@ -21,6 +21,8 @@
 //   * HW jobs 2i and 2i+1 on the same target (a read's ALT and REF probes) with queries of one class
 //     run as a pair in one thread (ed_pair_kernel): one target stream and decode, two Myers columns. Pairs whose two queries fit one
 //     column of 3 or 5 words with a separator row between them (33-47 bp or 65-79 bp probe pairs) share that column (ed_pack_kernel).
+//     Every read over one breakpoint has the same two probes, so the first such pair to run publishes its Peq table in a per-call hash
+//     table keyed by the probes' offsets, and later pairs of that key copy it instead of building it (peq_find / peq_publish).
 //   * |q| > 128: ONE WARP PER JOB, anti-diagonal wavefront: lane l owns a 64-row block and processes
 //     column t-l at step t; the horizontal delta (hout) crosses lanes by shuffle. Queries longer
 //     than 2048 rows are processed in 2048-row stripes, the stripe's bottom hout per column being
@@ -77,7 +79,83 @@ struct EdArgs {
   const uint32_t* eq_s;  // [256] ... the second member
   const uint8_t* eq_cls; // [256] bitmask over {A,C,G,T,N} of the class symbols the byte is equal to
   int force_long;
+  uint4* peq_slots;      // shared Peq tables of pairs (ED_PEQ_SLOTS_V below): hash slots, null unless pair
+  uint4* peq_pool;       // one entry of ED_PEQ_WORDS words per slot
+  uint32_t peq_mask;     // hash slots - 1
 };
+
+// Shared Peq tables (SLOT_ED_PEQ, calls with a.pair only). Every read over one SV breakpoint is realigned against the same ALT and REF
+// probes, and the Peq table of a pair or pack slot depends only on the two probes' offsets and lengths. So the first thread of a pair that
+// finds no table for it builds the table in its shared slice as before and publishes it: it claims an empty hash slot for the key
+// (q_off[2i], q_off[2i + 1]) with a CAS, writes the entry of that slot, fences, and then stores the slot's tag. A later pair of the same
+// key and lengths copies the entry instead of building it. Until the tag is stored, pairs of that key build their own table. Hash slots
+// are uint4 {q_off[2i], q_off[2i + 1], tag, unused}, all ones when empty (no q_off is 0xffffffff: the arena is shorter than 4 GiB and a
+// probe in a pair is not empty). The tag is 0x80000000 | q_len[2i] | q_len[2i + 1] << 16, so one word carries readiness and lengths. The
+// call sizes the table as the power of two >= n jobs, capped at ED_PEQ_SLOTS_V, and clears it on its stream, so no entry outlives it.
+#ifndef ED_PEQ_SLOTS_V
+#define ED_PEQ_SLOTS_V (1u << 18)
+#endif
+constexpr uint32_t ED_PEQ_SLOTS_MAX = ED_PEQ_SLOTS_V, ED_PEQ_SLOTS_MIN = 256;
+constexpr int ED_PEQ_PROBE = 4;                  // slots a lookup probes
+constexpr int ED_PEQ_WORDS = 40;                 // words per entry: 5 symbol slots x 8 words (ed_pair_kernel<4>)
+constexpr uint32_t ED_PEQ_NONE = 0xffffffffu;
+
+__device__ __forceinline__ uint32_t peq_hash(uint32_t o0, uint32_t o1, uint32_t mask) {
+  const uint32_t h = ((o0 * 0x9e3779b1u) ^ o1) * 0x85ebca6bu;
+  return (h ^ (h >> 16)) & mask;
+}
+
+// The published entry of the key (o0, o1) with tag `tag`, or null. On a miss, `claim` is the first empty slot met (the one the caller
+// may publish into), else ED_PEQ_NONE. Slots are read with plain loads, cached in L1: a stale slot is only an older state of it (empty, or
+// claimed and not tagged yet), which sends the pair to the in-thread build. On an H100 at 700 W, reading every slot from L2 instead (ld.cg)
+// made the class kernels 2.6x slower. Entries are read from L2 (copy_peq), where peq_publish's fence puts an entry before its tag, and an
+// entry is read only after its tag has been seen; entries share cache lines, so an L1 copy of one could be older than the entry.
+__device__ __forceinline__ const uint4* peq_find(const EdArgs& a, uint32_t o0, uint32_t o1, uint32_t tag, uint32_t& claim) {
+  claim = ED_PEQ_NONE;
+  uint32_t h = peq_hash(o0, o1, a.peq_mask);
+#pragma unroll 1
+  for (int k = 0; k < ED_PEQ_PROBE; ++k, h = (h + 1u) & a.peq_mask) {
+    const uint4 s = a.peq_slots[h];
+    if (s.x == o0 && s.y == o1) {
+      if (s.z != tag) return nullptr;   // not published yet, or other lengths
+      return a.peq_pool + (size_t) h * (ED_PEQ_WORDS / 4);
+    }
+    if ((s.x & s.y) == 0xffffffffu) { claim = h; return nullptr; }
+  }
+  return nullptr;
+}
+
+// Publishes the N words of the thread's slice pq (word e at pq[e * ED_THREADS]) as the entry of slot h for the key (o0, o1), unless
+// another thread claims the slot first.
+template <int N>
+__device__ __forceinline__ void peq_publish(const EdArgs& a, uint32_t h, uint32_t o0, uint32_t o1, uint32_t tag, const uint32_t* pq) {
+  const unsigned long long key = (unsigned long long) o0 | (unsigned long long) o1 << 32;
+  if (atomicCAS((unsigned long long*) (a.peq_slots + h), ~0ull, key) != ~0ull) return;
+  uint4* e = a.peq_pool + (size_t) h * (ED_PEQ_WORDS / 4);
+  // rolled: once per distinct pair, and it keeps the column loop the block of the kernel with the most shared loads
+#pragma unroll 1
+  for (int i = 0; i < (N + 3) / 4; ++i) {
+    uint32_t w[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) w[k] = 4 * i + k < N ? pq[(4 * i + k) * ED_THREADS] : 0u;
+    __stcg(e + i, make_uint4(w[0], w[1], w[2], w[3]));
+  }
+  __threadfence();
+  atomicExch(&a.peq_slots[h].z, tag);
+}
+
+// An entry's first N words into the thread's slice (word e to pq[e * ED_THREADS]), 16 bytes per load.
+template <int N>
+__device__ __forceinline__ void copy_peq(uint32_t* pq, const uint4* e) {
+#pragma unroll
+  for (int i = 0; i < (N + 3) / 4; ++i) {
+    const uint4 v = __ldcg(e + i);
+    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      if (4 * i + k < N) pq[(4 * i + k) * ED_THREADS] = w[k];
+  }
+}
 
 __device__ __forceinline__ int ed_class(uint32_t ql, uint32_t tl, int force_long) {
   if (ql == 0 || tl == 0) return 0;
@@ -527,6 +605,7 @@ __device__ __forceinline__ void ed_small_jobs(const EdArgs& a, uint32_t* peq, in
   constexpr int NC = PACK ? 1 : NJ;              // Myers columns per thread
   constexpr int SW = NC * NW;                    // Peq words per symbol slot
   static_assert(!PACK || (NJ == 2 && MODE == DGPU_MODE_HW && !WANT_END), "a packed column holds two HW distances");
+  static_assert(NJ == 1 || (MODE == DGPU_MODE_HW && !WANT_END), "target-sharing pairs are HW distances");
   const uint32_t cnt = a.counts[cls];
   const uint32_t start = a.counts[ED_START + cls];
   const uint32_t tid = threadIdx.x;
@@ -539,16 +618,36 @@ __device__ __forceinline__ void ed_small_jobs(const EdArgs& a, uint32_t* peq, in
     uint32_t Pv[NC][NW], Mv[NC][NW];
     uint32_t sep = 0, mula = 0;
     int score[NJ], best[NJ], bpos[NJ], prev[NJ];
-    if constexpr (PACK) {
+    if constexpr (NJ == 2) {
+      // a pair or pack slot (HW): the shared Peq table of its two probes if one is published (peq_find), else built here and published
       const uint32_t m0 = a.q_len[job0], m1 = a.q_len[job0 + 1];
-      const uint32_t sw = pack_fits(m0, m1, NW, WA) ? 0u : 1u;
+      const uint32_t o0 = a.q_off[job0], o1 = a.q_off[job0 + 1];
+      const uint32_t sw = PACK && !pack_fits(m0, m1, NW, WA) ? 1u : 0u;
       jid[0] = job0 + sw;
       jid[1] = job0 + (sw ^ 1u);
       m[0] = sw ? m1 : m0;
       m[1] = sw ? m0 : m1;
-      q[0] = a.seqs + a.q_off[jid[0]];
-      q[1] = a.seqs + a.q_off[jid[1]];
-      build_pack_peq<NW, WA>(peq + tid, q[0], m[0], q[1], m[1], a.seqs_end);
+      q[0] = a.seqs + (sw ? o1 : o0);
+      q[1] = a.seqs + (sw ? o0 : o1);
+      const uint32_t tag = 0x80000000u | m0 | m1 << 16;
+      uint32_t claim;
+      const uint4* ent = peq_find(a, o0, o1, tag, claim);
+      if (ent) {
+        copy_peq<5 * SW>(peq + tid, ent);
+      } else {
+        if constexpr (PACK) {
+          build_pack_peq<NW, WA>(peq + tid, q[0], m[0], q[1], m[1], a.seqs_end);
+        } else {
+#pragma unroll
+          for (int j = 0; j < 2; ++j) {
+            const uint32_t pj = 32u * NW - m[j];
+            build_peq<NW, true>(peq + j * NW * ED_THREADS + tid, SW, q[j], a.seqs_end, 0, pj, (1u << pj) - 1u);
+          }
+        }
+        if (claim != ED_PEQ_NONE) peq_publish<5 * SW>(a, claim, o0, o1, tag, peq + tid);
+      }
+    }
+    if constexpr (PACK) {
       p[0] = 32u * NW - m[1];  // first row of B; the separator is rows m[0] .. p[0] - 1
 #pragma unroll
       for (int w = 0; w < NW; ++w) { Pv[0][w] = ~rows_in(w, m[0], p[0]); Mv[0][w] = 0; }
@@ -562,13 +661,15 @@ __device__ __forceinline__ void ed_small_jobs(const EdArgs& a, uint32_t* peq, in
 #pragma unroll
     for (int j = 0; j < NJ; ++j) {
       if constexpr (!PACK) {
-        jid[j] = job0 + j;
-        m[j] = a.q_len[job0 + j];
-        q[j] = a.seqs + a.q_off[job0 + j];
+        if constexpr (NJ == 1) {
+          jid[j] = job0 + j;
+          m[j] = a.q_len[job0 + j];
+          q[j] = a.seqs + a.q_off[job0 + j];
+        }
         topbit[j] = (m[j] - 1) & 31u;
         p[j] = 32u * NW - m[j];  // jobs of this class have 32 (NW - 1) < |q| <= 32 NW
         vmask[j] = TOP ? (1u << p[j]) - 1u : 0u;
-        build_peq<NW, TOP>(peq + j * NW * ED_THREADS + tid, SW, q[j], a.seqs_end, topbit[j], p[j], vmask[j]);
+        if constexpr (NJ == 1) build_peq<NW, TOP>(peq + j * NW * ED_THREADS + tid, SW, q[j], a.seqs_end, topbit[j], p[j], vmask[j]);
 #pragma unroll
         for (int w = 0; w < NW; ++w) { Pv[j][w] = 0xffffffffu; Mv[j][w] = 0; }
         Pv[j][0] = ~vmask[j];  // virtual rows start at Pv = Mv = 0
@@ -1203,6 +1304,18 @@ int dgpu_edit_distance_impl(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_by
   a.slots = (uint8_t*) p;
 
   DGPU_CUDA(ctx, cudaMemsetAsync(a.counts, 0, ED_COUNTS_WORDS * sizeof(uint32_t), st));
+  a.peq_slots = a.peq_pool = nullptr;
+  a.peq_mask = 0;
+  if (a.pair) {   // the shared Peq tables of pairs (ED_PEQ_SLOTS_V), cleared on st: no entry outlives the call
+    uint32_t hs = ED_PEQ_SLOTS_MIN;
+    while (hs < n && hs < ED_PEQ_SLOTS_MAX) hs <<= 1;
+    rc = dgpu_reserve(ctx, SLOT_ED_PEQ, (size_t) hs * (sizeof(uint4) + ED_PEQ_WORDS * sizeof(uint32_t)), &p);
+    if (rc) return rc;
+    a.peq_slots = (uint4*) p;
+    a.peq_pool = a.peq_slots + hs;
+    a.peq_mask = hs - 1;
+    DGPU_CUDA(ctx, cudaMemsetAsync(a.peq_slots, 0xff, (size_t) hs * sizeof(uint4), st));
+  }
   const uint32_t cb = (uint32_t) std::min<uint64_t>((n + ED_BIN_THREADS - 1) / ED_BIN_THREADS, (uint64_t) ctx->num_sms * ED_BIN_CTAS_PER_SM);
   ed_count_kernel<<<cb, ED_BIN_THREADS, 0, st>>>(a, mode);
   DGPU_LAUNCH_CHECK(ctx, "ed_count");
