@@ -252,11 +252,12 @@ class Context:
         return out, n_rows, status, alns
 
     def msa_dev(self, seqs, read_off, read_len, cluster_off, ncl, sc, min_clique, cons, cons_off, cons_len, n_rows, status,
-                stream=None, max_reads=32):
+                stream=None, max_reads=32, aln=None, aln_off=None, aln_cols=None):
+        """Device form: CUDA tensors in, results written in place; aln / aln_off / aln_cols (optional) receive the root alignments."""
         rc = self._lib.dgpu_msa_ex_dev(self.h, _ptr(seqs), C.c_uint64(seqs.numel()), _ptr(read_off), _ptr(read_len),
                                        _ptr(cluster_off), C.c_uint32(ncl), int(sc[0]), int(sc[1]), int(sc[2]), int(sc[3]),
                                        int(min_clique), _ptr(cons), _ptr(cons_off), _ptr(cons_len), _ptr(n_rows), _ptr(status),
-                                       _ptr(None), _ptr(None), _ptr(None), C.c_uint32(max_reads), C.c_void_p(stream or 0))
+                                       _ptr(aln), _ptr(aln_off), _ptr(aln_cols), C.c_uint32(max_reads), C.c_void_p(stream or 0))
         self.check(rc, "dgpu_msa_ex_dev")
 
 

@@ -737,7 +737,7 @@ __global__ void __launch_bounds__(MSA_T, MSA_PER_SM) msa_kernel(MsaArgs A) {
       gotoh_dp(m, n, A, tr, rowwords, ids1, ids2, Sptr, sstride, Sptr != w.u.g.t.S, bnd, lane);
       const int L = msa_traceback(tr, rowwords, m, n, w.win, src1, src2, lane);
       const int R = a1.R + a2.R;
-      if (L > MSA_LCAP || bump + (size_t) R * L > A.aln_cap) { status = ST_TOO_LONG; break; }
+      if (L > MSA_LCAP) { status = ST_TOO_LONG; break; }   // every node of at most MSA_LCAP columns fits A.aln_cap
       uint8_t* out = alnbuf + bump;
       bump += ((size_t) R * L + 15) & ~(size_t) 15;
       // _createAlignment (src/align.h:202-229): rows of a1, then rows of a2
@@ -1067,7 +1067,9 @@ int dgpu_msa_ex_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
   A.cons = cons; A.cons_off = cons_off; A.cons_len = cons_len; A.n_rows = n_rows; A.status = status;
   A.aln = aln; A.aln_off = aln_off; A.aln_cols = aln_cols;
   auto al = [](size_t x) { return (x + 255) & ~(size_t) 255; };
-  A.aln_cap = al((size_t) (MSA_MAXR * (MSA_MAXR + 1) / 2) * 384);  // node alignments of one cluster
+  // node alignments of one cluster, never freed: a node takes R x L bytes rounded up to 16, at most R x (MSA_LCAP + 1). The R of all
+  // nodes sum to the leaves' depths, at most 2 + 3 + .. + MSA_MAXR for a chain-shaped guide tree.
+  A.aln_cap = al((size_t) (MSA_MAXR * (MSA_MAXR + 1) / 2 - 1) * (MSA_LCAP + 1));
   A.off_prof = A.aln_cap;
   const size_t b_prof = al((size_t) (MSA_LCAP + 1) * 5);  // gapped consensus + the two column-kind arrays
   A.off_trace = A.off_prof + b_prof;

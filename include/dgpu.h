@@ -235,8 +235,8 @@ int dgpu_long_needle_ex_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_by
  * IN THE ORDER THE REFERENCE ITERATES ITS std::unordered_set (the caller preserves that order).
  * Outputs per cluster: consensus bytes at cons + cons_off[i] (reserve sum of the cluster's read
  * lengths), cons_len[i], n_rows[i] (= msa()'s return value), status[i]:
- *   0 ok; 1 more than max_reads reads (32 for dgpu_msa / dgpu_msa_dev); 2 a read or an intermediate alignment exceeds 1023 columns / the
- *   per-cluster workspace; 3 a read contains a byte outside ACGTN (the reference's float profile is
+ *   0 ok; 1 more than max_reads reads (32 for dgpu_msa / dgpu_msa_dev); 2 a read is empty or a read or an intermediate alignment
+ *   exceeds 1023 columns; 3 a read contains a byte outside ACGTN (the reference's float profile is
  *   NaN there) — such clusters are NOT computed and the caller must treat them as errors.
  * Optional white-box output: the root alignment (n_rows x aln_cols, row-major) at aln + aln_off[i].
  * Scoring: (match, mismatch, go, ge) = DnaScore, e.g. (5,-4,-10,-1); requires go <= 0 and ge <= 0.

@@ -13,6 +13,7 @@
 // Each function is written from the algorithm's definition (plain full-matrix DP, no banding, no
 // bit-vectors) and cites the reference lines whose observable behaviour it restates.
 #include <algorithm>
+#include <array>
 #include <atomic>
 #include <climits>
 #include <cstdint>
@@ -334,9 +335,43 @@ void consensus(Rows const& a, int minClique, std::string& gapped, std::string& c
   for (char c : gapped) if (c != '-') cs.push_back(c);
 }
 
+// Number of distinct column profiles of an alignment, counted on the integers profile() divides (the A,C,G,T,N counts and the number
+// of covering rows): columns with equal integers have bit-identical float profiles.
+int distinct_profiles(Rows const& a) {
+  size_t R = a.size(), L = a[0].size();
+  std::vector<long> first(R, -1), last(R, (long) L);
+  for (size_t i = 0; i < R; ++i)
+    for (size_t j = 0; j < L; ++j)
+      if (a[i][j] != '-') { if (first[i] == -1) first[i] = (long) j; last[i] = (long) j; }
+  std::vector<std::array<int, 6>> keys(L);
+  for (size_t j = 0; j < L; ++j) {
+    std::array<int, 6> k{};
+    for (size_t i = 0; i < R; ++i) {
+      if (first[i] <= (long) j && (long) j <= last[i]) {
+        ++k[5];
+        char c = a[i][j];
+        if (c == 'A' || c == 'a') ++k[0];
+        else if (c == 'C' || c == 'c') ++k[1];
+        else if (c == 'G' || c == 'g') ++k[2];
+        else if (c == 'T' || c == 't') ++k[3];
+        else if (c == 'N' || c == 'n') ++k[4];
+        else if (c != '-') --k[5];
+      }
+    }
+    keys[j] = k;
+  }
+  std::sort(keys.begin(), keys.end());
+  return (int) (std::unique(keys.begin(), keys.end()) - keys.begin());
+}
+
+// One inner node of the guide tree: its rows and columns, the columns of its two children (the DP's rows and columns) and their
+// distinct column profiles (0 when both children are single reads, which gotoh compares character by character).
+struct NodeInfo { int R, L, L1, L2, U1, U2; };
+
 // msa (src/msa.h:185-239): LCS similarity matrix, UPGMA guide tree, progressive gotoh, consensus.
+// nodes (optional): every inner node in creation order.
 int msa(std::vector<std::string> const& reads, int minClique, int match, int mismatch, int go, int ge,
-        std::string& cs, Rows* alnOut) {
+        std::string& cs, Rows* alnOut, std::vector<NodeInfo>* nodes = nullptr) {
   int num = (int) reads.size(), N = 2 * num + 1;
   std::vector<int> d((size_t) N * N, -1);
   for (int i = 0; i < num; ++i)
@@ -363,16 +398,23 @@ int msa(std::vector<std::string> const& reads, int minClique, int match, int mis
   // post-order progressive alignment (msa.h:91-109)
   struct Rec {
     static void run(int node, std::vector<int> const& lc, std::vector<int> const& rc, std::vector<std::string> const& reads,
-                    int match, int mismatch, int go, int ge, Rows& out) {
+                    int match, int mismatch, int go, int ge, Rows& out, std::vector<NodeInfo>* info) {
       if (lc[node] == -1 && rc[node] == -1) { out.assign(1, reads[node]); return; }
       Rows a, b;
-      run(lc[node], lc, rc, reads, match, mismatch, go, ge, a);
-      run(rc[node], lc, rc, reads, match, mismatch, go, ge, b);
+      run(lc[node], lc, rc, reads, match, mismatch, go, ge, a, info);
+      run(rc[node], lc, rc, reads, match, mismatch, go, ge, b, info);
       gotoh(a, b, match, mismatch, go, ge, out);
+      if (info) {
+        const bool prof = a.size() > 1 || b.size() > 1;
+        (*info)[node] = NodeInfo{(int) out.size(), (int) out[0].size(), (int) a[0].size(), (int) b[0].size(),
+                                 prof ? distinct_profiles(a) : 0, prof ? distinct_profiles(b) : 0};
+      }
     }
   };
   Rows aln;
-  Rec::run(root, lc, rc, reads, match, mismatch, go, ge, aln);
+  std::vector<NodeInfo> info(nodes ? N : 0);
+  Rec::run(root, lc, rc, reads, match, mismatch, go, ge, aln, nodes ? &info : nullptr);
+  if (nodes) nodes->assign(info.begin() + num, info.begin() + std::max(num, root + 1));
   std::string gapped;
   consensus(aln, minClique, gapped, cs);
   if (alnOut) *alnOut = aln;
@@ -466,6 +508,24 @@ int ora_msa(const char* arena, const uint32_t* off, const uint32_t* len, int nre
     for (size_t i = 0; i < aln.size(); ++i) memcpy(aln_out + i * aln[0].size(), aln[i].data(), aln[0].size());
   }
   return rows;
+}
+
+// The guide tree's inner nodes of ora_msa's cluster in creation order: (R, L, L1, L2, U1, U2) per node at nodes[6 * k], see NodeInfo.
+// Returns the number of nodes, or -1 if there are more than cap.
+int ora_msa_nodes(const char* arena, const uint32_t* off, const uint32_t* len, int nreads, int match, int mismatch, int go, int ge,
+                  int* nodes, int cap) {
+  std::vector<std::string> reads;
+  for (int i = 0; i < nreads; ++i) reads.push_back(std::string(arena + off[i], len[i]));
+  std::string cs;
+  std::vector<NodeInfo> info;
+  msa(reads, 2, match, mismatch, go, ge, cs, nullptr, &info);
+  if ((int) info.size() > cap) return -1;
+  for (size_t k = 0; k < info.size(); ++k) {
+    const NodeInfo& x = info[k];
+    int* o = nodes + 6 * k;
+    o[0] = x.R; o[1] = x.L; o[2] = x.L1; o[3] = x.L2; o[4] = x.U1; o[5] = x.U2;
+  }
+  return (int) info.size();
 }
 
 int ora_hardware_threads() { return (int) std::thread::hardware_concurrency(); }

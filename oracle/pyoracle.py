@@ -335,5 +335,19 @@ def msa(lib, reads, min_clique=2, sc=(5, -4, -10, -1), want_alignment=False):
     return rows, cons.raw[: clen.value], al
 
 
+def msa_nodes(lib, reads, sc=(5, -4, -10, -1)):
+    """The guide tree's inner nodes of msa(reads) in creation order, as an int array of rows (R, L, L1, L2, U1, U2): the node's rows and
+    alignment columns, its two children's columns (gotoh's DP rows and columns) and their distinct column profiles (0, 0 when both
+    children are single reads). Oracle only."""
+    reads = [_b(r) for r in reads]
+    arena = b"".join(reads)
+    lens = np.array([len(r) for r in reads], np.uint32)
+    offs = np.concatenate([[0], np.cumsum(lens)[:-1]]).astype(np.uint32)
+    out = np.zeros((max(len(reads), 1), 6), np.int32)
+    n = lib.ora_msa_nodes(arena, _p(offs, u32p), _p(lens, u32p), len(reads), sc[0], sc[1], sc[2], sc[3], _p(out, i32p), len(out))
+    assert n >= 0
+    return out[:n]
+
+
 def hardware_threads():
     return os.cpu_count() or 1
