@@ -818,7 +818,6 @@ constexpr int EDL_WARPS = 4;  // warps per CTA in the long kernel
 template <int MODE, bool EQ>
 __global__ void __launch_bounds__(EDL_WARPS * 32) ed_long_kernel(EdArgs a, const uint32_t* list, const uint32_t* list_cnt) {
   __shared__ uint64_t peq_s[EDL_WARPS][5][32];
-  constexpr int HIN0 = (MODE == DGPU_MODE_HW) ? 0 : 1;
   // job list: the class-5 segment of perm, or (NW with band passes in front) what the band passes left over
   const uint32_t cnt = list ? *list_cnt : a.counts[5];
   if (!list) list = a.perm + a.counts[ED_START + 5];
@@ -826,100 +825,21 @@ __global__ void __launch_bounds__(EDL_WARPS * 32) ed_long_kernel(EdArgs a, const
   const int wib = threadIdx.x >> 5;
   const uint32_t gwarp = blockIdx.x * EDL_WARPS + wib;
   const uint32_t nwarps = gridDim.x * EDL_WARPS;
-  volatile uint8_t* hrow = a.hbuf ? a.hbuf + (size_t) gwarp * a.hbuf_stride : nullptr;
+  volatile int8_t* hrow = a.hbuf ? (volatile int8_t*) a.hbuf + (size_t) gwarp * a.hbuf_stride : nullptr;
+  const EqTabs tabs = {a.eq_f, a.eq_s, a.eq_cls};
 
   for (uint32_t idx = gwarp; idx < cnt; idx += nwarps) {
     const uint32_t job = list[idx];
     const uint32_t m = a.q_len[job], n = a.t_len[job];
-    const uint8_t* q = a.seqs + a.q_off[job];
-    const uint8_t* t = a.seqs + a.t_off[job];
-    const uint32_t nstripes = (m + 2047) / 2048;
+    const int topbit = (int) ((m - 1) & 63u);
     int score = (int) m;  // D[m][0]; only meaningful on the lane that owns row m-1
     int best = (m & 63u) ? (int) m : 0x7fffffff, bpos = -1;  // end position -1 exists iff |q| % 64 != 0
-
-    for (uint32_t s = 0; s < nstripes; ++s) {
-      const uint32_t row0 = s * 2048 + (uint32_t) lane * 64;  // first query row of this lane's block
-      const uint32_t rows_left = m - s * 2048;
-      const int nb = (int) min(32u, (rows_left + 63) / 64);   // active lanes in this stripe
-      const bool last_stripe = (s + 1 == nstripes);
-      const bool active = lane < nb;
-      const int topbit = (int) ((m - 1) & 63u);
-
-      // Peq for this lane's 64 rows
-      uint64_t pm_other = 0;  // EQ: rows holding a byte outside ACGTN (compared exactly, pair tables included)
-      {
-        uint64_t pm[5] = {0, 0, 0, 0, 0};
-        pm_other = 0;
-        if (active) {
-          for (uint32_t i = 0; i < 64 && row0 + i < m; ++i) {
-            uint32_t code = dna_code(__ldg(q + row0 + i));
-#pragma unroll
-            for (int sy = 0; sy < 5; ++sy) pm[sy] |= (code == (uint32_t) sy) ? (1ull << i) : 0ull;
-            if (EQ && code == 5u) pm_other |= 1ull << i;
-          }
-        }
-        __syncwarp();
-#pragma unroll
-        for (int sy = 0; sy < 5; ++sy) peq_s[wib][sy][lane] = pm[sy];
-        __syncwarp();
-      }
-
-      uint64_t Pv = ~0ull, Mv = 0;
-      int hout = 0;
-      uint32_t cbuf = 0;   // 32 target bytes, one per lane, refreshed every 32 steps
-      uint32_t cchar = 0;  // this lane's current column byte
-      const uint32_t nsteps = n + (uint32_t) nb - 1;
-      for (uint32_t st = 0; st < nsteps; ++st) {
-        if ((st & 31u) == 0) {
-          uint32_t p = st + (uint32_t) lane;
-          cbuf = (p < n) ? (uint32_t) __ldg(t + p) : 0u;
-        }
-        uint32_t newc = __shfl_sync(0xffffffffu, cbuf, (int) (st & 31u));
-        uint32_t upc = __shfl_up_sync(0xffffffffu, cchar, 1);
-        cchar = (lane == 0) ? newc : upc;
-        int hin_sh = __shfl_up_sync(0xffffffffu, hout, 1);
-        const int col = (int) st - lane;
-        if (active && col >= 0 && col < (int) n) {
-          int hin;
-          if (lane == 0) hin = (s == 0) ? HIN0 : (int) (int8_t) hrow[col];
-          else hin = hin_sh;
-          uint32_t code = dna_code(cchar);
-          uint64_t Eq;
-          if (EQ) {
-            const uint32_t cm = a.eq_cls[cchar & 0xffu];
-            Eq = 0;
-#pragma unroll
-            for (int sy = 0; sy < 5; ++sy)
-              if ((cm >> sy) & 1u) Eq |= peq_s[wib][sy][lane];
-            uint64_t rest = pm_other;
-            const uint32_t cf = a.eq_f[cchar & 0xffu], cs = a.eq_s[cchar & 0xffu];
-            while (rest) {
-              const int i = __ffsll((long long) rest) - 1;
-              rest &= rest - 1;
-              const uint32_t qb = __ldg(q + row0 + i);
-              if (qb == (cchar & 0xffu) || (a.eq_f[qb] & cs) || (a.eq_s[qb] & cf)) Eq |= 1ull << i;
-            }
-          } else if (code < 5) Eq = peq_s[wib][code][lane];
-          else {
-            Eq = 0;
-            for (uint32_t i = 0; i < 64 && row0 + i < m; ++i)
-              if (__ldg(q + row0 + i) == (uint8_t) cchar) Eq |= 1ull << i;
-          }
-          uint64_t Ph, Mh;
-          hout = block64(Pv, Mv, Eq, hin, Ph, Mh);
-          if (lane == nb - 1 && last_stripe) {
-            // delta of row m-1 (inside this block)
-            score += (int) ((Ph >> topbit) & 1ull) - (int) ((Mh >> topbit) & 1ull);
-            if (MODE != DGPU_MODE_NW) {
-              if (score < best || (a.last_pos && score == best)) { best = score; bpos = col; }
-            }
-          }
-          if (lane == nb - 1 && !last_stripe) hrow[col] = (uint8_t) (int8_t) hout;
-        }
-      }
-      __syncwarp();
-      __threadfence_block();
-    }
+    stripes<EQ>(peq_s[wib], hrow, a.seqs + a.q_off[job], a.seqs + a.t_off[job], m, n, false, MODE == DGPU_MODE_HW ? 0 : 1, tabs,
+                [&](int col, uint64_t Ph, uint64_t Mh) {
+                  score += (int) ((Ph >> topbit) & 1ull) - (int) ((Mh >> topbit) & 1ull);   // delta of row m-1
+                  if (MODE != DGPU_MODE_NW && (score < best || (a.last_pos && score == best))) { best = score; bpos = col; }
+                },
+                [](uint32_t, int, uint64_t, uint64_t) {});
     // broadcast the result from the lane that owns row m-1
     const int owner = (int) (((m - 1) & 2047u) >> 6);
     int d = (MODE == DGPU_MODE_NW) ? score : best;
@@ -1015,58 +935,16 @@ __global__ void __launch_bounds__(EDB_WARPS * 32) ed_band_kernel(EdArgs a, uint3
     const int m = have ? (int) a.q_len[job] : 0, n = have ? (int) a.t_len[job] : 0;
     const uint8_t* q = a.seqs + (have ? a.q_off[job] : 0);
     const uint8_t* t = a.seqs + (have ? a.t_off[job] : 0);
-    const int nblk = (m + 63) >> 6;
     const BandPlan bp = band_plan(G, max(m, 1), max(n, 1));
 
     __syncwarp();
     band_build_peq<G>(peq, q, m, false, p);
     __syncwarp();
 
-    const int Jend = (n - 1) >> 6;
-    int steps = have ? 65 * Jend + ((n - 1) & 63) + G : 0;
-    for (int o = 16; o; o >>= 1) steps = max(steps, __shfl_xor_sync(0xffffffffu, steps, o));
-
-    uint64_t Pv = ~0ull, Mv = 0;
-    int blk = p - bp.A, J = 0, c = -p;             // c < 0: waiting for the skew; 0..63: column 64J + c; 64: hand-over slot
-    int sc = 64 * (blk + 1);                        // D[last row of the block][column before the current one]
-    int hout = 1;
-    uint32_t chn = (have && n > 0) ? __ldg(t) : 0u;
-    for (int st = 0; st < steps; ++st) {
-      const int hin_sh = __shfl_up_sync(0xffffffffu, hout, 1, G);
-      if (c >= 0 && c < 64) {
-        const int col = (J << 6) + c;
-        if (col < n) {
-          const uint32_t ch = chn;
-          if (col + 1 < n) chn = __ldg(t + col + 1);
-          if (blk >= 0 && blk < nblk) {
-            const uint64_t Eq = band_eq<EQ>(peq, blk, ch, q, m, false, tabs);
-            const int hin = (p == 0 || blk == 0) ? 1 : hin_sh;   // above: the matrix border or a cell outside the band
-            uint64_t Ph, Mh;
-            hout = block64(Pv, Mv, Eq, hin, Ph, Mh);
-            sc += hout;
-          }
-        }
-      }
-      const bool give = (c == 63), take = (c == 64) && (((J + 1) << 6) < n);
-      if (__any_sync(0xffffffffu, give || take)) {
-        if (give) { hoP[wib][lane] = Pv; hoM[wib][lane] = Mv; hoS[wib][lane] = sc; }
-        __syncwarp();
-        if (take) {
-          if (p < G - 1) { Pv = hoP[wib][lane + 1]; Mv = hoM[wib][lane + 1]; sc = hoS[wib][lane + 1]; }
-          else { Pv = ~0ull; Mv = 0; sc += 64; }
-          ++blk; ++J; c = -1;
-        }
-        __syncwarp();
-      }
-      ++c;
-    }
-
-    // D[m][n]: the block holding row m-1, corrected by the vertical deltas of the rows below it inside the block
-    const int tb = (m - 1) & 63;
-    const uint64_t below = tb == 63 ? 0ull : (~0ull << (tb + 1));
-    int s = sc - __popcll(Pv & below) + __popcll(Mv & below);
-    const int plast = (nblk - 1) - (Jend - bp.A);
-    s = __shfl_sync(0xffffffffu, s, (grp * G) + (plast & (G - 1)));
+    uint64_t Pv, Mv;
+    int sc, blk, plast;
+    band_pass<G, EQ>(peq, q, t, m, n, false, bp, hoP[wib], hoM[wib], hoS[wib], tabs, Pv, Mv, sc, blk, [](int, uint64_t, uint64_t) {});
+    const int s = band_corner<G>(Pv, Mv, sc, m, n, bp, plast);
     if (have && p == 0) {
       const int kk = a.k ? a.k[job] : -1;
       if (plast >= 0 && plast < G && (bp.whole || s <= bp.kvalid)) {

@@ -171,9 +171,8 @@ __global__ void __launch_bounds__(MULTI ? 512 : 32) seg_kernel(SegJobs a) {
 //     elsewhere — hb_select_kernel only ever tests l + r == optimum, which over-estimates cannot satisfy. Both halves of a parent use the
 //     parent's band (the reversed problem maps it onto itself).
 //   kind 0 (leaf): every lane stores, per column, its block's vertical deltas after the column (Pv) and the horizontal deltas into the
-//     column (Ph): 2 bits per cell. The traceback of src/edlib.cpp:1021-1131 needs nothing else: up iff Pv bit, else left iff Ph bit,
-//     else diagonal. The lane group walks the path together through a 32-column window of its current block staged in shared memory.
-//     Ops are written from the END of the job's slot backwards (out_len says how many); the host shifts the leaf offset.
+//     column (Ph): 2 bits per cell, all leaf_trace needs. Ops are written from the END of the job's slot backwards (out_len says how
+//     many); the host shifts the leaf offset.
 constexpr int SEGB_WARPS = 2;
 
 template <int G, bool EQ>
@@ -208,57 +207,17 @@ __global__ void __launch_bounds__(SEGB_WARPS * 32) seg_band_kernel(SegJobs a) {
     band_build_peq<G>(peq, q, m, rev, p);
     __syncwarp();
 
-    const int Jend = (n - 1) >> 6;
-    int steps = have ? 65 * Jend + ((n - 1) & 63) + G : 0;
-    for (int o = 16; o; o >>= 1) steps = max(steps, __shfl_xor_sync(0xffffffffu, steps, o));
-
-    uint64_t Pv = ~0ull, Mv = 0;
-    int blk = p - bp.A, J = 0, c = -p;
-    int sc = 64 * (blk + 1);
-    int hout = 1;
-    uint32_t chn = (have && n > 0) ? __ldg(rev ? t + (n - 1) : t) : 0u;
-    for (int st = 0; st < steps; ++st) {
-      const int hin_sh = __shfl_up_sync(0xffffffffu, hout, 1, G);
-      if (c >= 0 && c < 64) {
-        const int col = (J << 6) + c;
-        if (col < n) {
-          const uint32_t ch = chn;
-          if (col + 1 < n) chn = __ldg(rev ? t + (n - 2 - col) : t + col + 1);
-          if (blk >= 0 && blk < nblk) {
-            const uint64_t Eq = band_eq<EQ>(peq, blk, ch, q, m, rev, tabs);
-            const int hin = (p == 0 || blk == 0) ? 1 : hin_sh;
-            uint64_t Ph, Mh;
-            hout = block64(Pv, Mv, Eq, hin, Ph, Mh);
-            sc += hout;
-            if (kind == 0) store[(size_t) st * G + p] = make_uint4((uint32_t) Pv, (uint32_t) (Pv >> 32), (uint32_t) Ph, (uint32_t) (Ph >> 32));
-          }
-        }
-      }
-      const bool give = (c == 63), take = (c == 64) && (((J + 1) << 6) < n);
-      if (__any_sync(0xffffffffu, give || take)) {
-        if (give) { hoP[wib][lane] = Pv; hoM[wib][lane] = Mv; hoS[wib][lane] = sc; }
-        __syncwarp();
-        if (take) {
-          if (p < G - 1) { Pv = hoP[wib][lane + 1]; Mv = hoM[wib][lane + 1]; sc = hoS[wib][lane + 1]; }
-          else { Pv = ~0ull; Mv = 0; sc += 64; }
-          ++blk; ++J; c = -1;
-        }
-        __syncwarp();
-      }
-      ++c;
-    }
+    uint64_t Pv, Mv;
+    int sc, blk, plast;
+    band_pass<G, EQ>(peq, q, t, m, n, rev, bp, hoP[wib], hoM[wib], hoS[wib], tabs, Pv, Mv, sc, blk, [&](int st, uint64_t pv, uint64_t ph) {
+      if (kind == 0) store[(size_t) st * G + p] = make_uint4((uint32_t) pv, (uint32_t) (pv >> 32), (uint32_t) ph, (uint32_t) (ph >> 32));
+    });
     __threadfence_block();
     __syncwarp();
 
     // corner: D[m][n] when the band holds it (a leaf's always does), reported as a score like the wavefront kernels do
-    {
-      const int tb = (m - 1) & 63;
-      const uint64_t below = tb == 63 ? 0ull : (~0ull << (tb + 1));
-      int s = sc - __popcll(Pv & below) + __popcll(Mv & below);
-      const int plast = (nblk - 1) - (Jend - bp.A);
-      s = __shfl_sync(0xffffffffu, s, (grp * G) + (plast & (G - 1)));
-      if (have && p == 0) a.corner[job] = (plast >= 0 && plast < G) ? -s : 1;
-    }
+    const int s = band_corner<G>(Pv, Mv, sc, m, n, bp, plast);
+    if (have && p == 0) a.corner[job] = (plast >= 0 && plast < G) ? -s : 1;
 
     if (kind == 1 && have) {
       int* colv = a.colbuf + a.out_off[job];
@@ -278,59 +237,12 @@ __global__ void __launch_bounds__(SEGB_WARPS * 32) seg_band_kernel(SegJobs a) {
       }
     }
 
-    // traceback of the leaves (src/edlib.cpp:1021-1131: up = insert 1, left = delete 2, diagonal = match 0 / mismatch 3)
-    {
-      const bool act = have && kind == 0;
-      int r = m - 1, cc = n - 1;
-      uint32_t k = 0;
-      const uint32_t cap = (uint32_t) (m + n);
-      uint8_t* out = a.tmp_ops + (have ? a.out_off[job] : 0);
-      int wb = -1, wc0 = -1;
-      while (__any_sync(0xffffffffu, act && r >= 0 && cc >= 0)) {
-        const bool go = act && r >= 0 && cc >= 0;
-        const int b = r >> 6;
-        const bool need = go && (b != wb || cc > wc0 || cc <= wc0 - WCOLS);
-        if (__any_sync(0xffffffffu, need)) {
-          if (need) {
-            for (int x = p; x < WCOLS; x += G) {
-              const int col = cc - x;
-              uint4 v = make_uint4(0, 0, 0, 0);
-              if (col >= 0) {
-                const int Jc = col >> 6, pp = b - (Jc - bp.A);
-                if (pp >= 0 && pp < G) v = __ldcg(store + ((size_t) (65 * Jc + (col & 63) + pp) * G + pp));
-              }
-              win[x] = v;
-            }
-            wb = b; wc0 = cc;
-          }
-          __syncwarp();
-        }
-        if (go) {
-          const uint4 w = win[wc0 - cc];
-          const int bit = r & 63;
-          const uint32_t pv = ((bit < 32 ? w.x : w.y) >> (bit & 31)) & 1u;
-          const uint32_t ph = ((bit < 32 ? w.z : w.w) >> (bit & 31)) & 1u;
-          uint8_t op;
-          if (pv) { op = 1; --r; }
-          else if (ph) { op = 2; --cc; }
-          else {
-            const uint32_t x = __ldg(rev ? q + (m - 1 - r) : q + r), y = __ldg(rev ? t + (n - 1 - cc) : t + cc);
-            op = (EQ ? a.eq.equal(x, y) : (x == y)) ? 0 : 3;
-            --r; --cc;
-          }
-          if (p == 0) out[cap - 1 - k] = op;
-          ++k;
-        }
-        __syncwarp();
-      }
-      if (act) {
-        for (int i = p; i <= r; i += G) out[cap - 1 - (k + (uint32_t) i)] = 1;    // column 0 reached: the remaining rows are inserts
-        if (r >= 0) k += (uint32_t) (r + 1);
-        for (int i = p; i <= cc; i += G) out[cap - 1 - (k + (uint32_t) i)] = 2;   // row 0 reached: the remaining columns are deletes
-        if (cc >= 0) k += (uint32_t) (cc + 1);
-        if (p == 0) a.out_len[job] = k;
-      }
-    }
+    const bool act = have && kind == 0;
+    const uint32_t k = leaf_trace<G, WCOLS, EQ>(act, q, t, m, n, rev, a.eq, win, a.tmp_ops + (have ? a.out_off[job] : 0), [&](int col, int b) {
+      const int Jc = col >> 6, pp = b - (Jc - bp.A);
+      return pp >= 0 && pp < G ? __ldcg(store + ((size_t) (65 * Jc + (col & 63) + pp) * G + pp)) : make_uint4(0, 0, 0, 0);
+    });
+    if (act && p == 0) a.out_len[job] = k;
     __syncwarp();
   }
 }
@@ -343,17 +255,17 @@ constexpr int EPL_WARPS = 2;     // warps per CTA of seg_leaf_wide_kernel
 constexpr int EPL_G = 2;         // lanes per leaf: one per 64-row block
 constexpr int EPL_WCOLS = 32;    // traceback window, columns
 
-// Half column (kind 1) of an unbanded segment: one warp per segment, one 64-row Myers block per lane, an anti-diagonal wavefront over
-// 2048-row stripes whose bottom horizontal deltas are parked in the warp's scratch row (n bytes), as ed_long_kernel computes edit distances.
-// NW top boundary (D[0][j] = j), rows / columns read back to front when rev. After each stripe the lanes' final Pv / Mv are the vertical
-// deltas of column n, which give colbuf[out_off + i] = -D[i][n] for every row of the stripe, run on from the stripe above; the column is
-// exact on every row.
+// Half column (kind 1) of an unbanded segment: one warp per segment on ed_long_kernel's striped wavefront (stripes), its bottom deltas
+// parked in the warp's scratch row (n bytes). NW top boundary (D[0][j] = j), rows / columns read back to front when rev. After each
+// stripe the lanes' final Pv / Mv are the vertical deltas of column n, which give colbuf[out_off + i] = -D[i][n] for every row of the
+// stripe, run on from the stripe above; the column is exact on every row.
 template <bool EQ>
 __global__ void __launch_bounds__(EPW_WARPS * 32) seg_half_wide_kernel(SegJobs a, size_t hrow_stride) {
   __shared__ uint64_t peq_s[EPW_WARPS][5][32];
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
   const uint32_t gwarp = blockIdx.x * EPW_WARPS + wib, nwarps = gridDim.x * EPW_WARPS;
   volatile int8_t* hrow = (volatile int8_t*) (a.work + (size_t) gwarp * hrow_stride);
+  const EqTabs tabs = {a.eq.f, a.eq.s, a.eq_cls};
   for (uint32_t idx = gwarp; idx < a.count; idx += nwarps) {
     const uint32_t job = a.list[idx];
     const uint32_t m = a.q_len[job], n = a.t_len[job];
@@ -363,93 +275,30 @@ __global__ void __launch_bounds__(EPW_WARPS * 32) seg_half_wide_kernel(SegJobs a
     int* colv = a.colbuf + a.out_off[job];
     if (lane == 0) colv[0] = -(int) n;
     int top = (int) n;   // D[s * 2048][n]: the column value above the current stripe
-    const uint32_t nstripes = (m + 2047) / 2048;
-    for (uint32_t s = 0; s < nstripes; ++s) {
-      const uint32_t row0 = s * 2048 + (uint32_t) lane * 64;
-      const int nb = (int) min(32u, (m - s * 2048 + 63) / 64);
-      const bool last_stripe = (s + 1 == nstripes), active = lane < nb;
-      const int rows = active ? (int) min(64u, m - row0) : 0;
-      uint64_t other = 0;   // rows holding a byte outside ACGTN: compared byte by byte (pair tables included under EQ)
-      {
-        uint64_t pm[5] = {0, 0, 0, 0, 0};
-        for (int i = 0; i < rows; ++i) {
-          const uint32_t code = dna_code(__ldg(rev ? q + (m - 1 - row0 - i) : q + row0 + i));
-#pragma unroll
-          for (int sy = 0; sy < 5; ++sy) pm[sy] |= (code == (uint32_t) sy) ? (1ull << i) : 0ull;
-          if (code == 5u) other |= 1ull << i;
-        }
-        __syncwarp();
-#pragma unroll
-        for (int sy = 0; sy < 5; ++sy) peq_s[wib][sy][lane] = pm[sy];
-        __syncwarp();
-      }
-      uint64_t Pv = ~0ull, Mv = 0;
-      int hout = 0;
-      uint32_t cbuf = 0, cchar = 0;
-      const uint32_t nsteps = n + (uint32_t) nb - 1;
-      for (uint32_t st = 0; st < nsteps; ++st) {
-        if ((st & 31u) == 0) {
-          const uint32_t p = st + (uint32_t) lane;
-          cbuf = (p < n) ? (uint32_t) __ldg(rev ? t + (n - 1 - p) : t + p) : 0u;
-        }
-        const uint32_t newc = __shfl_sync(0xffffffffu, cbuf, (int) (st & 31u));
-        const uint32_t upc = __shfl_up_sync(0xffffffffu, cchar, 1);
-        cchar = (lane == 0) ? newc : upc;
-        const int hin_sh = __shfl_up_sync(0xffffffffu, hout, 1);
-        const int col = (int) st - lane;
-        if (active && col >= 0 && col < (int) n) {
-          const int hin = lane ? hin_sh : (s == 0 ? 1 : (int) hrow[col]);
-          uint64_t Eq, rest = other;
-          if (EQ) {
-            const uint32_t cm = a.eq_cls[cchar & 0xffu];
-            Eq = 0;
-#pragma unroll
-            for (int sy = 0; sy < 5; ++sy)
-              if ((cm >> sy) & 1u) Eq |= peq_s[wib][sy][lane];
-          } else {
-            const uint32_t code = dna_code(cchar);
-            Eq = code < 5 ? peq_s[wib][code][lane] : 0ull;
-            if (code < 5) rest = 0;   // an ACGTN column byte equals no row outside ACGTN
-          }
-          if (rest) {
-            const uint32_t cf = EQ ? a.eq.f[cchar & 0xffu] : 0u, cs = EQ ? a.eq.s[cchar & 0xffu] : 0u;
-            while (rest) {
-              const int i = __ffsll((long long) rest) - 1;
-              rest &= rest - 1;
-              const uint32_t qb = __ldg(rev ? q + (m - 1 - row0 - i) : q + row0 + i);
-              if (qb == (cchar & 0xffu) || (EQ && ((a.eq.f[qb] & cs) || (a.eq.s[qb] & cf)))) Eq |= 1ull << i;
-            }
-          }
-          uint64_t Ph, Mh;
-          hout = block64(Pv, Mv, Eq, hin, Ph, Mh);
-          if (lane == nb - 1 && !last_stripe) hrow[col] = (int8_t) hout;
-        }
-      }
-      __syncwarp();
-      __threadfence_block();
-      // this stripe's rows of column n: exclusive prefix of the lanes' delta sums, then each lane writes its own rows
-      const uint64_t valid = rows == 64 ? ~0ull : ((1ull << rows) - 1);
-      const int sum = __popcll(Pv & valid) - __popcll(Mv & valid);
-      int incl = sum;
-      for (int o = 1; o < 32; o <<= 1) {
-        const int v = __shfl_up_sync(0xffffffffu, incl, o);
-        if (lane >= o) incl += v;
-      }
-      int v = top + incl - sum;
-      for (int j = 0; j < rows; ++j) {
-        v += (int) ((Pv >> j) & 1ull) - (int) ((Mv >> j) & 1ull);
-        colv[row0 + j + 1] = -v;
-      }
-      top += __shfl_sync(0xffffffffu, incl, 31);
-    }
+    stripes<EQ>(peq_s[wib], hrow, q, t, m, n, rev, 1, tabs, [](int, uint64_t, uint64_t) {},
+                [&](uint32_t row0, int rows, uint64_t Pv, uint64_t Mv) {
+                  // this stripe's rows of column n: exclusive prefix of the lanes' delta sums, then each lane writes its own rows
+                  const uint64_t valid = rows == 64 ? ~0ull : ((1ull << rows) - 1);
+                  const int sum = __popcll(Pv & valid) - __popcll(Mv & valid);
+                  int incl = sum;
+                  for (int o = 1; o < 32; o <<= 1) {
+                    const int v = __shfl_up_sync(0xffffffffu, incl, o);
+                    if (lane >= o) incl += v;
+                  }
+                  int v = top + incl - sum;
+                  for (int j = 0; j < rows; ++j) {
+                    v += (int) ((Pv >> j) & 1ull) - (int) ((Mv >> j) & 1ull);
+                    colv[row0 + j + 1] = -v;
+                  }
+                  top += __shfl_sync(0xffffffffu, incl, 31);
+                });
     if (lane == 0) a.corner[job] = -top;
   }
 }
 
 // Leaf (kind 0) of at most two 64-row blocks and any width: EPL_G = 2 lanes per leaf, 16 leaves per warp. Lane p holds block p over the
 // whole column (lane 1 one step behind lane 0, its horizontal delta arriving by shuffle) and stores (Pv after the column, Ph into the
-// column) for every column, 16 B per lane-column. The traceback is the one of seg_band_kernel (up > left > diagonal through a window of
-// EPL_WCOLS columns of the current block in shared memory); ops are written from the END of the job's slot backwards.
+// column) for every column, 16 B per lane-column. The traceback is seg_band_kernel's (leaf_trace, a window of EPL_WCOLS columns).
 template <bool EQ>
 __global__ void __launch_bounds__(EPL_WARPS * 32) seg_leaf_wide_kernel(SegJobs a) {
   constexpr int G = EPL_G, JPW = 32 / G;
@@ -503,51 +352,9 @@ __global__ void __launch_bounds__(EPL_WARPS * 32) seg_leaf_wide_kernel(SegJobs a
       if (have && p == 0) a.corner[job] = -s;
     }
 
-    // traceback (src/edlib.cpp:1021-1131: up = insert 1, left = delete 2, diagonal = match 0 / mismatch 3)
-    int r = m - 1, cc = n - 1;
-    uint32_t k = 0;
-    const uint32_t cap = (uint32_t) (m + n);
-    uint8_t* out = a.tmp_ops + (have ? a.out_off[job] : 0);
-    int wb = -1, wc0 = -1;
-    while (__any_sync(0xffffffffu, have && r >= 0 && cc >= 0)) {
-      const bool go = have && r >= 0 && cc >= 0;
-      const int b = r >> 6;
-      const bool need = go && (b != wb || cc > wc0 || cc <= wc0 - EPL_WCOLS);
-      if (__any_sync(0xffffffffu, need)) {
-        if (need) {
-          for (int x = p; x < EPL_WCOLS; x += G) {
-            const int col = cc - x;
-            win[x] = col >= 0 ? __ldcg(store + (size_t) col * nblk + b) : make_uint4(0, 0, 0, 0);
-          }
-          wb = b; wc0 = cc;
-        }
-        __syncwarp();
-      }
-      if (go) {
-        const uint4 w = win[wc0 - cc];
-        const int bit = r & 63;
-        const uint32_t pv = ((bit < 32 ? w.x : w.y) >> (bit & 31)) & 1u;
-        const uint32_t ph = ((bit < 32 ? w.z : w.w) >> (bit & 31)) & 1u;
-        uint8_t op;
-        if (pv) { op = 1; --r; }
-        else if (ph) { op = 2; --cc; }
-        else {
-          const uint32_t x = __ldg(rev ? q + (m - 1 - r) : q + r), y = __ldg(rev ? t + (n - 1 - cc) : t + cc);
-          op = (EQ ? a.eq.equal(x, y) : (x == y)) ? 0 : 3;
-          --r; --cc;
-        }
-        if (p == 0) out[cap - 1 - k] = op;
-        ++k;
-      }
-      __syncwarp();
-    }
-    if (have) {
-      for (int i = p; i <= r; i += G) out[cap - 1 - (k + (uint32_t) i)] = 1;    // column 0 reached: the remaining rows are inserts
-      if (r >= 0) k += (uint32_t) (r + 1);
-      for (int i = p; i <= cc; i += G) out[cap - 1 - (k + (uint32_t) i)] = 2;   // row 0 reached: the remaining columns are deletes
-      if (cc >= 0) k += (uint32_t) (cc + 1);
-      if (p == 0) a.out_len[job] = k;
-    }
+    const uint32_t k = leaf_trace<G, EPL_WCOLS, EQ>(have, q, t, m, n, rev, a.eq, win, a.tmp_ops + (have ? a.out_off[job] : 0),
+                                                    [&](int col, int b) { return __ldcg(store + (size_t) col * nblk + b); });
+    if (have && p == 0) a.out_len[job] = k;
     __syncwarp();
   }
 }
