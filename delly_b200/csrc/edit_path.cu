@@ -20,6 +20,8 @@
 #include "myers.cuh"
 #include "wavefront.cuh"
 #include <algorithm>
+#include <array>
+#include <utility>
 
 int dgpu_edit_distance_impl(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes, const uint32_t* q_off, const uint32_t* q_len,
                             const uint32_t* t_off, const uint32_t* t_len, const int32_t* k, int mode, uint64_t n, int32_t* dist,
@@ -87,13 +89,18 @@ struct SegJobs {
   const uint8_t* eq_cls;   // class table of the generalised equality (null: byte equality)
 };
 
-__host__ __device__ inline int seg_cols(int cls) { return cls <= 8 ? 8 * cls : 32; }
+// Geometry of the seg_kernel classes: a segment of n target columns takes the first row with n <= cap (class 0: n = 0), with C columns
+// per lane, T threads per CTA (MULTI: T > 32) and a grid of at most per_sm CTAs per SM.
+struct SegGeom { uint32_t cap; int C, T, per_sm; };
+constexpr int SEG_NCLS = 12;
+constexpr SegGeom SEG_GEOM[SEG_NCLS] = {{0, 0, 0, 0},
+                                        {256, 8, 32, 16}, {512, 16, 32, 16}, {768, 24, 32, 16}, {1024, 32, 32, 16},
+                                        {1280, 40, 32, 16}, {1536, 48, 32, 16}, {1792, 56, 32, 16}, {2048, 64, 32, 16},
+                                        {4096, 32, 128, 4}, {8192, 32, 256, 2}, {16384, 32, 512, 1}};
 __host__ __device__ inline uint32_t seg_dstride(uint32_t n, uint32_t C) { return ((n + C - 1) / C + 1) * (C / 8); }
 inline int seg_class(uint32_t n) {
-  if (n <= 2048) return (int) ((n + 255) / 256);
-  if (n <= 4096) return 9;
-  if (n <= 8192) return 10;
-  if (n <= 16384) return 11;
+  for (int c = 0; c < SEG_NCLS; ++c)
+    if (n <= SEG_GEOM[c].cap) return c;
   return -1;
 }
 
@@ -443,19 +450,14 @@ struct SegRunner {
   int run(uint8_t* tmp_ops, int* colbuf);
 };
 
-template <int C, bool MULTI>
-int seg_launch(dgpu_ctx* ctx, SegJobs& a, bool use_eq, unsigned grid, unsigned threads, size_t smem, cudaStream_t st) {
-  int rc;
-  if (use_eq) {
-    if ((rc = dgpu_smem_optin(ctx, seg_kernel<C, MULTI, true>, smem, "cudaFuncSetAttribute(seg_kernel)"))) return rc;
-    seg_kernel<C, MULTI, true><<<grid, threads, smem, st>>>(a);
-  } else {
-    if ((rc = dgpu_smem_optin(ctx, seg_kernel<C, MULTI, false>, smem, "cudaFuncSetAttribute(seg_kernel)"))) return rc;
-    seg_kernel<C, MULTI, false><<<grid, threads, smem, st>>>(a);
-  }
-  DGPU_LAUNCH_CHECK(ctx, "seg_kernel");
-  return DGPU_OK;
+// seg_kernel of each class, [0] without and [1] with equality tables, its template arguments read from SEG_GEOM
+using SegKernel = void (*)(SegJobs);
+template <bool EQ, size_t... G>
+constexpr std::array<SegKernel, SEG_NCLS> seg_kernels(std::index_sequence<G...>) {
+  return {{nullptr, seg_kernel<SEG_GEOM[G + 1].C, (SEG_GEOM[G + 1].T > 32), EQ>...}};
 }
+constexpr std::array<SegKernel, SEG_NCLS> SEG_KERNELS[2] = {seg_kernels<false>(std::make_index_sequence<SEG_NCLS - 1>()),
+                                                            seg_kernels<true>(std::make_index_sequence<SEG_NCLS - 1>())};
 
 template <int G>
 int seg_band_launch(dgpu_ctx* ctx, SegJobs& a, bool use_eq, unsigned grid, cudaStream_t st) {
@@ -479,15 +481,14 @@ inline int seg_band_class(uint32_t m, uint32_t pm, uint32_t pn, int32_t k) {
 // Whether seg_kernel cannot stage m query rows in shared memory: the launch's opt-in of (m + 15) & ~15 dynamic bytes would exceed the
 // device's per-block maximum less the kernel's static shared memory, and the whole call would fail. Such half columns (Hirschberg over a
 // query of more than ~230 kb) run on seg_half_wide_kernel instead; every segment seg_kernel can launch still runs there.
-bool seg_rows_exceed(dgpu_ctx* ctx, uint32_t m, bool multi, bool eq) {
-  static size_t room[2][2] = {{0, 0}, {0, 0}};   // [multi][eq]: dynamic shared memory seg_kernel may opt in to
-  size_t& r = room[multi][eq];
+bool seg_rows_exceed(dgpu_ctx* ctx, uint32_t m, int cls, bool eq) {
+  static size_t room[SEG_NCLS][2] = {};   // [class][eq]: dynamic shared memory the class's seg_kernel may opt in to
+  size_t& r = room[cls][eq];
   if (!r) {
     int optin = 0;
     cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device);
     cudaFuncAttributes fa{};
-    if (multi) cudaFuncGetAttributes(&fa, eq ? (const void*) seg_kernel<32, true, true> : (const void*) seg_kernel<32, true, false>);
-    else cudaFuncGetAttributes(&fa, eq ? (const void*) seg_kernel<8, false, true> : (const void*) seg_kernel<8, false, false>);
+    cudaFuncGetAttributes(&fa, (const void*) SEG_KERNELS[eq][cls]);
     r = (size_t) optin - fa.sharedSizeBytes;
   }
   const size_t smem = ((size_t) m + 15) & ~(size_t) 15;
@@ -521,26 +522,26 @@ int SegRunner::run(uint8_t* tmp_ops, int* colbuf) {
   DGPU_CUDA(ctx, cudaMemcpyAsync(d_rev, rev.data(), N, cudaMemcpyHostToDevice, st));
   DGPU_CUDA(ctx, cudaMemcpyAsync(d_kind, kind.data(), N, cudaMemcpyHostToDevice, st));
   // class lists
-  // lists[1..11]: wavefront classes by target length; lists[12..16]: band classes G = 2, 4, 8, 16, 32
+  // lists[1..11]: wavefront classes by target length (SEG_GEOM); lists[12..16]: band classes G = 2, 4, 8, 16, 32
   // wide_half / wide_leaf: unbanded segments wider than the wavefront classes (seg_half_wide_kernel, seg_leaf_wide_kernel)
-  std::vector<std::vector<uint32_t> > lists(12 + EDB_CLASSES);
+  std::vector<std::vector<uint32_t> > lists(SEG_NCLS + EDB_CLASSES);
   std::vector<uint32_t> wide_half, wide_leaf;
   tail_ops.assign(N, 0);
   static const bool no_band = getenv("DGPU_EP_NO_BAND") != nullptr;   // development switch: no band classes (wavefront and wide kernels only)
   for (size_t i = 0; i < N; ++i) {
     const int bc = no_band ? -1 : seg_band_class(qlen[i], plan_m[i], plan_n[i], bound[i]);
-    if (bc >= 0) { lists[12 + bc].push_back((uint32_t) i); tail_ops[i] = 1; continue; }
+    if (bc >= 0) { lists[SEG_NCLS + bc].push_back((uint32_t) i); tail_ops[i] = 1; continue; }
     const int c = seg_class(tlen[i]);
-    if (c > 0 && !(kind[i] == 1 && seg_rows_exceed(ctx, qlen[i], c > 8, use_eq))) { lists[c].push_back((uint32_t) i); continue; }
+    if (c > 0 && !(kind[i] == 1 && seg_rows_exceed(ctx, qlen[i], c, use_eq))) { lists[c].push_back((uint32_t) i); continue; }
     if (kind[i] == 1) { wide_half.push_back((uint32_t) i); continue; }
     if (qlen[i] > 64 * EPL_G) return DGPU_ERR_UNSUPPORTED;   // Hirschberg's split rule leaves no such leaf
     wide_leaf.push_back((uint32_t) i);
     tail_ops[i] = 1;
   }
   std::vector<uint32_t> flat;
-  std::vector<size_t> lo(13 + EDB_CLASSES, 0);
-  for (int c = 1; c < 12 + EDB_CLASSES; ++c) { lo[c] = flat.size(); flat.insert(flat.end(), lists[c].begin(), lists[c].end()); }
-  lo[12 + EDB_CLASSES] = flat.size();
+  std::vector<size_t> lo(SEG_NCLS + 1 + EDB_CLASSES, 0);
+  for (int c = 1; c < SEG_NCLS + EDB_CLASSES; ++c) { lo[c] = flat.size(); flat.insert(flat.end(), lists[c].begin(), lists[c].end()); }
+  lo[SEG_NCLS + EDB_CLASSES] = flat.size();
   const size_t lo_half = flat.size();
   flat.insert(flat.end(), wide_half.begin(), wide_half.end());
   const size_t lo_leaf = flat.size();
@@ -553,7 +554,7 @@ int SegRunner::run(uint8_t* tmp_ops, int* colbuf) {
   size_t free_b = 0, total_b = 0;
   cudaMemGetInfo(&free_b, &total_b);
   for (int bc = 0; bc < EDB_CLASSES; ++bc) {
-    std::vector<uint32_t> const& L = lists[12 + bc];
+    std::vector<uint32_t> const& L = lists[SEG_NCLS + bc];
     if (L.empty()) continue;
     const int G = edb_lanes(bc), jpw = 32 / G;
     size_t maxsteps = 0;   // trace storage of a leaf: one uint4 per lane and step
@@ -568,7 +569,7 @@ int SegRunner::run(uint8_t* tmp_ops, int* colbuf) {
     void* w;
     if ((rc = dgpu_reserve(ctx, SLOT_WAVEFRONT, std::max<size_t>(grid * per_block, 256), &w))) return rc;
     a.work = (uint8_t*) w;
-    a.list = d_list + lo[12 + bc];
+    a.list = d_list + lo[SEG_NCLS + bc];
     a.count = (uint32_t) L.size();
     switch (bc) {
       case 0: rc = seg_band_launch<2>(ctx, a, use_eq, (unsigned) grid, st); break;
@@ -614,22 +615,20 @@ int SegRunner::run(uint8_t* tmp_ops, int* colbuf) {
     else seg_leaf_wide_kernel<false><<<(unsigned) grid, EPL_WARPS * 32, 0, st>>>(a);
     DGPU_LAUNCH_CHECK(ctx, "seg_leaf_wide_kernel");
   }
-  for (int c = 1; c < 12; ++c) {
+  for (int c = 1; c < SEG_NCLS; ++c) {
     if (lists[c].empty()) continue;
-    const int C = seg_cols(c);
+    const SegGeom& g = SEG_GEOM[c];
     size_t maxwords = 0, mmax = 0, mnmax = 0;
     for (uint32_t i : lists[c]) {
-      if (kind[i] == 0) maxwords = std::max(maxwords, (size_t) (qlen[i] + 1) * seg_dstride(tlen[i], C));   // half columns store no directions
+      if (kind[i] == 0) maxwords = std::max(maxwords, (size_t) (qlen[i] + 1) * seg_dstride(tlen[i], g.C));   // half columns store no directions
       mmax = std::max<size_t>(mmax, qlen[i]);
       mnmax = std::max<size_t>(mnmax, (size_t) qlen[i] + tlen[i]);
     }
     auto al = [](size_t x) { return (x + 255) & ~(size_t) 255; };
     a.off_trace = al(maxwords * 4 + 1024);
     a.work_stride = a.off_trace + al(mnmax + 64);
-    const unsigned threads = c <= 8 ? 32u : (c == 9 ? 128u : (c == 10 ? 256u : 512u));
     const size_t smem = (mmax + 15) & ~(size_t) 15;
-    const int per_sm = c <= 8 ? 16 : (c == 9 ? 4 : (c == 10 ? 2 : 1));
-    size_t grid = std::min<size_t>(lists[c].size(), (size_t) ctx->num_sms * per_sm);
+    size_t grid = std::min<size_t>(lists[c].size(), (size_t) ctx->num_sms * g.per_sm);
     size_t budget = (size_t) ((double) free_b * 0.6) + ctx->bufs[SLOT_WAVEFRONT].cap;
     if (grid * a.work_stride > budget) grid = std::max<size_t>(1, budget / a.work_stride);
     void* w;
@@ -637,18 +636,10 @@ int SegRunner::run(uint8_t* tmp_ops, int* colbuf) {
     a.work = (uint8_t*) w;
     a.list = d_list + lo[c];
     a.count = (uint32_t) lists[c].size();
-    switch (c) {
-      case 1: rc = seg_launch<8, false>(ctx, a, use_eq, (unsigned) grid, threads, smem, st); break;
-      case 2: rc = seg_launch<16, false>(ctx, a, use_eq, (unsigned) grid, threads, smem, st); break;
-      case 3: rc = seg_launch<24, false>(ctx, a, use_eq, (unsigned) grid, threads, smem, st); break;
-      case 4: rc = seg_launch<32, false>(ctx, a, use_eq, (unsigned) grid, threads, smem, st); break;
-      case 5: rc = seg_launch<40, false>(ctx, a, use_eq, (unsigned) grid, threads, smem, st); break;
-      case 6: rc = seg_launch<48, false>(ctx, a, use_eq, (unsigned) grid, threads, smem, st); break;
-      case 7: rc = seg_launch<56, false>(ctx, a, use_eq, (unsigned) grid, threads, smem, st); break;
-      case 8: rc = seg_launch<64, false>(ctx, a, use_eq, (unsigned) grid, threads, smem, st); break;
-      default: rc = seg_launch<32, true>(ctx, a, use_eq, (unsigned) grid, threads, smem, st); break;
-    }
-    if (rc) return rc;
+    const SegKernel k = SEG_KERNELS[use_eq][c];
+    if ((rc = dgpu_smem_optin(ctx, k, smem, "cudaFuncSetAttribute(seg_kernel)"))) return rc;
+    k<<<(unsigned) grid, (unsigned) g.T, smem, st>>>(a);
+    DGPU_LAUNCH_CHECK(ctx, "seg_kernel");
   }
   return DGPU_OK;
 }

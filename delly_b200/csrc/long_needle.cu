@@ -21,9 +21,9 @@
 // reduced once at the end. refRight (needle.h:116-123) is recovered from the stored maxima and the
 // "equals maximum" bits. Workspace ~3 B per DP cell (0.8 MB for 300x1100; a batch in flight exceeds L2 and streams
 // through HBM at about 1 TB/s, far below the roof).
-// Job geometry (ln_class / ln_cols / ln_threads): up to 1273 reference columns one warp with C = 8..40 columns per lane;
-// up to 2041 two warps x C=32; up to 4089 four warps x C=32; up to 16377 eight warps x C = 24..64 (C >= 48 keeps the
-// previous-row state in shared memory), chosen so that at least 3/4 of the lanes own columns. Warps of one CTA hand the
+// Job geometry (ln_geom): up to 1273 reference columns one warp with C = 8..40 columns per lane;
+// up to 2041 two warps x C=32; up to 4089 four warps x C=32; up to 16377 eight warps x C = 24..64 (ln_ups: C >= 48 keeps the
+// scalar engine's previous-row state in shared memory), chosen so that at least 3/4 of the lanes own columns. Warps of one CTA hand the
 // boundary column over through a shared-memory ring (wavefront.cuh), not a block barrier. The two tracebacks are
 // warp-cooperative (a diagonal window of direction words per round of loads). Job classes of one call run concurrently on
 // forked streams.
@@ -31,12 +31,14 @@
 #include "wavefront.cuh"
 #include "wavefront2.cuh"
 #include <algorithm>
+#include <array>
 #include <string>
+#include <utility>
 #include <vector>
 
 namespace {
 
-constexpr int LN_NCLS = 16;  // 0 trivial; 1..8 one warp, C = 8*cls columns per lane; 9..15 multi-warp CTA (see ln_class)
+constexpr int LN_NCLS = 16;  // 0 trivial; 1..15 the rows of ln_geom
 constexpr int LN_GEN = 16;   // class + LN_GEN: the same geometry for jobs with a byte outside ACGTN (scalar engine, byte compares)
 
 struct LnArgs {
@@ -53,7 +55,8 @@ struct LnArgs {
   int32_t* info;            // optional per job [consLeft, refLeft, refRight, bestScore] (may be NULL)
   uint32_t* perm;
   uint32_t* counts;              // [0..31] class counts (16.. = generic), [32..63] starts, [64..95] cursors
-  unsigned long long* maxcells;  // [0..31] per class max (m+1)*bstride ; [32..63] per class max m+n ; [64..95] per class max m
+  unsigned long long* maxcells;  // per class max: [0..31] prefix-maxima bytes (wide class: slab bytes), [32..63] direction bytes of one pass,
+                                 // [64..95] m+n, [96..127] m
   uint8_t* jobcls;               // per job: its class (0..31), written by the count kernel
   uint8_t* work;                 // per-CTA workspace slabs
   size_t work_stride;
@@ -62,11 +65,27 @@ struct LnArgs {
   unsigned long long wide_budget;  // workspace bytes one wide job may take
 };
 
-// columns per thread of a class
-// classes 1..5: one warp, C = 8*cls; 6..8: two warps x C=32 (one warp with C = 48..64 would spill);
-// 9: four warps x C=32; 10..15: eight warps x C = 24..64
-__host__ __device__ inline int ln_cols(int cls) { return cls <= 5 ? 8 * cls : (cls <= 9 ? 32 : 8 * (cls - 7)); }
-__host__ __device__ inline int ln_threads(int cls) { return cls <= 5 ? 32 : (cls <= 8 ? 64 : (cls == 9 ? 128 : 256)); }
+// Geometry of the wavefront job classes: a job whose n reference columns satisfy n + 7 <= cap (7 columns of slack for the aligned
+// forward blocks) and not the previous row's cap takes the row's class, C columns per lane and T threads per CTA (MULTI: T > 32).
+// Classes 1..5 one warp; 6..8 two warps x C=32 (one warp with C = 48..64 would spill); 9 four warps; 10..15 eight warps. Multi-warp
+// CTAs are sized so that at least 3/4 of their lanes own columns (idle lanes are idle issue slots).
+struct LnGeom { uint32_t cap; int C, T; };
+__host__ __device__ constexpr LnGeom ln_geom(int cls) {
+  constexpr LnGeom rows[LN_NCLS] = {{0, 0, 0},
+                                    {256, 8, 32}, {512, 16, 32}, {768, 24, 32}, {1024, 32, 32}, {1280, 40, 32},
+                                    {1536, 32, 64}, {1792, 32, 64}, {2048, 32, 64},
+                                    {4096, 32, 128},
+                                    {6144, 24, 256}, {8192, 32, 256}, {10240, 40, 256}, {12288, 48, 256}, {14336, 56, 256}, {16384, 64, 256}};
+  return rows[cls];
+}
+// Packed engine: CTAs per SM its register allocation is sized for (12 warps per SM; one 8-warp CTA), and the depth of its partner ring
+// (wavefront2.cuh).
+__host__ __device__ constexpr int ln2_occ(int T) { return 12 * 32 / T; }
+constexpr int LN_PART_D = 2;
+// Scalar engine: CTAs per SM of the grid cap (8 warps per SM at up to 255 registers per thread), and whether the C columns of row state do
+// not fit the register file and live in shared memory (wavefront.cuh).
+__host__ __device__ constexpr int ln_per_sm(int T) { return T == 32 ? 16 : 256 / T; }
+__host__ __device__ constexpr bool ln_ups(int C, int T) { return T > 32 && C >= 48; }
 // row geometry for n reference columns with C columns per thread (see wavefront.cuh)
 __host__ __device__ inline uint32_t ln_nact(uint32_t n, uint32_t C) { return (n + C - 1) / C; }
 __host__ __device__ inline uint32_t ln_P(uint32_t n, uint32_t C) { return 1 + ln_nact(n, C) * C; }
@@ -77,11 +96,35 @@ __host__ __device__ inline uint32_t ln_dstride(uint32_t n, uint32_t C) { return 
 __host__ __device__ inline int ln_class(uint32_t m, uint32_t n) {
   if (m == 0 || n == 0) return 0;
   if ((uint64_t) m + n > 32000u) return -1;  // int16 score storage
-  if (n + 7 <= 2048) return (int) ((n + 7 + 255) / 256);  // 1..8 by 256 columns (7 columns of slack for the aligned forward blocks); geometry: ln_cols / ln_threads
-  // multi-warp CTAs: the CTA is sized so that at least 3/4 of its lanes own columns (idle lanes are idle issue slots)
-  if (n + 7 <= 4096) return 9;     // 4 warps x 32 lanes x C=32
-  if (n + 7 <= 16384) return 10 + (int) ((n + 7 - 4097) / 2048);  // 8 warps x 32 lanes x C = 24, 32, 40, 48, 56, 64
+  for (int c = 1; c < LN_NCLS; ++c)
+    if (n + 7 <= ln_geom(c).cap) return c;
   return -1;
+}
+
+// Dynamic shared memory of ln_kernel2, carved in this order: the partner ring of the forward pass (bytes), the row scratch of the join's
+// arg-max search (words), the row string of the current pass (m bytes).
+struct Ln2Smem {
+  size_t ring, scr;
+  size_t bytes(size_t mmax) const { return ring + scr * sizeof(uint32_t) + ((mmax + 15) & ~(size_t) 15); }
+};
+__host__ __device__ inline Ln2Smem ln2_smem(int C, int T) { return {(size_t) wf2::part_slots(C, LN_PART_D, T) * sizeof(uint4), (size_t) (C + 1) * T}; }
+// Dynamic shared memory of ln_kernel: the previous-row state (ln_ups classes), then the row string of the current pass (m bytes).
+__host__ __device__ constexpr size_t ln_smem_ups(int C, int T) { return ln_ups(C, T) ? (size_t) C * T * sizeof(int) : 0; }
+// Workspace of one job: the reverse pass's prefix maxima and the direction nibbles of one pass. The packed engine's workspace is step-major
+// (wavefront2.cuh), the scalar engine's row-major.
+struct LnParts { unsigned long long rev, dirs; };
+__host__ __device__ inline LnParts ln2_parts(int C, int T, uint32_t m) { return {wf2::ws_brev_bytes(C, (int) m, T), wf2::ws_dirs_bytes(C, (int) m, T)}; }
+__host__ __device__ inline LnParts ln_parts(int C, uint32_t m, uint32_t n) {
+  return {(m + 1ull) * ln_bstride(n, C) * sizeof(int16_t), (m + 1ull) * ln_dstride(n, C) * sizeof(uint32_t)};
+}
+// Slab layout of a class from the maxima over its jobs: prefix maxima, reverse direction nibbles, forward direction nibbles, then the four
+// trace strings of m + n bytes.
+inline void ln_slab(LnArgs& a, unsigned long long rev, unsigned long long dirs, unsigned long long mn) {
+  auto al = [](size_t x) { return (x + 255) & ~(size_t) 255; };
+  a.off_dirsR = al(rev + 1024);
+  a.off_dirsF = a.off_dirsR + al(dirs + 1024);
+  a.off_trace = a.off_dirsF + al(dirs + 1024);
+  a.work_stride = a.off_trace + al(4 * mn + 64);
 }
 
 // ---- wide-window engine geometry (lnw_kernel below) --------------------------------------------------------------------------------
@@ -154,15 +197,16 @@ __global__ void ln_count_kernel(LnArgs a, int* unsupported) {
   a.jobcls[i] = (uint8_t) c;
   atomicAdd(&a.counts[c], 1u);
   if (c == 0) { a.ok[i] = 0; a.aln_len[i] = 0; return; }
-  if (c == LN_WIDE) {   // slab bytes, not cells: the wide kernel lays its slab out per job (lnw_geom)
+  atomicMax(&a.maxcells[96 + c], (unsigned long long) m);
+  if (c == LN_WIDE) {   // slab bytes: the wide kernel lays its slab out per job (lnw_geom)
     atomicMax(&a.maxcells[c], lnw_geom(m, n).bytes);
-    atomicMax(&a.maxcells[64 + c], (unsigned long long) m);
     return;
   }
-  const int g = c & (LN_GEN - 1);
-  atomicMax(&a.maxcells[c], (unsigned long long) (m + 1) * ln_bstride(n, ln_cols(g)));
-  atomicMax(&a.maxcells[32 + c], (unsigned long long) (m + n));
-  atomicMax(&a.maxcells[64 + c], (unsigned long long) m);
+  const LnGeom g = ln_geom(c & (LN_GEN - 1));
+  const LnParts p = c < LN_GEN ? ln2_parts(g.C, g.T, m) : ln_parts(g.C, m, n);
+  atomicMax(&a.maxcells[c], p.rev);
+  atomicMax(&a.maxcells[32 + c], p.dirs);
+  atomicMax(&a.maxcells[64 + c], (unsigned long long) (m + n));
 }
 
 __global__ void ln_offsets_kernel(uint32_t* counts) {
@@ -273,20 +317,15 @@ __device__ __forceinline__ uint32_t ln_traceback_warp(const uint32_t* __restrict
   return k + (uint32_t) cc + (uint32_t) rr;
 }
 
-// multi-warp classes whose C columns of row state do not fit the register file keep it in shared memory
-#ifndef LN_UPS_COLS
-#define LN_UPS_COLS 48
-#endif
-constexpr int LN_UPS_FROM = 7 + LN_UPS_COLS / 8;  // first class with C >= LN_UPS_COLS
 // (a register cap tight enough for more single-warp CTAs per SM would spill the DP state that lives in registers)
 // MAXT = threads per CTA the register allocation is sized for: a multi-warp CTA of 8 warps may use 255 registers per
 // thread (the DP state of C columns lives in registers), 16 warps would be capped at 128 and spill.
 template <int C, bool MULTI, int MAXT>
 __global__ void __launch_bounds__(MAXT, 1) ln_kernel(LnArgs a, int cls) {
   extern __shared__ uint8_t sm_dyn[];
-  constexpr int UPS = (MULTI && C >= LN_UPS_COLS) ? MAXT : 0;   // wide column blocks: previous-row state in shared memory (wavefront.cuh)
+  constexpr int UPS = ln_ups(C, MAXT) ? MAXT : 0;   // wide column blocks: previous-row state in shared memory (wavefront.cuh)
   int* sm_up = (int*) sm_dyn;                         // [C][UPS]
-  uint8_t* sm_rows = sm_dyn + (size_t) C * UPS * sizeof(int);  // row string of the current pass (m bytes)
+  uint8_t* sm_rows = sm_dyn + ln_smem_ups(C, MAXT);  // row string of the current pass (m bytes)
   __shared__ int sm_x[wf::WF_SMX];
   __shared__ int sm_pub[8];
   __shared__ uint32_t sm_win[128];  // traceback windows (one per tracing warp)
@@ -485,25 +524,16 @@ __device__ __forceinline__ uint32_t ln_traceback_warp2(const uint32_t* __restric
   return k + (uint32_t) cc + (uint32_t) rr;
 }
 
-#ifndef LN2_OCC
-#define LN2_OCC 12   // single-warp CTAs per SM the register allocation is sized for
-#endif
 template <int C, bool MULTI, int MAXT>
-__global__ void __launch_bounds__(MAXT, (MAXT == 32 ? LN2_OCC : (MAXT == 64 ? LN2_OCC / 2 : (MAXT == 128 ? LN2_OCC / 4 : 1)))) ln_kernel2(LnArgs a, int cls) {
+__global__ void __launch_bounds__(MAXT, ln2_occ(MAXT)) ln_kernel2(LnArgs a, int cls) {
   extern __shared__ uint8_t sm_dyn[];
   const int tid = threadIdx.x;
   const int T = blockDim.x;
   const int lane = tid & 31;
-  uint4* sm_part = (uint4*) sm_dyn;                                                    // partner ring of the forward pass
-#ifndef LN2_PD_SMALL
-#define LN2_PD_SMALL 2
-#endif
-#ifndef LN2_PD_C40
-#define LN2_PD_C40 2
-#endif
-  constexpr int PD = (MAXT == 256) ? 2 : ((C >= 40) ? LN2_PD_C40 : LN2_PD_SMALL);         // partner ring depth (wavefront2.cuh)
-  uint32_t* sm_scr = (uint32_t*) (sm_dyn + (size_t) wf2::part_slots<C, PD>(T) * sizeof(uint4));   // row scratch of the join's arg-max search
-  uint8_t* sm_rows = (uint8_t*) (sm_scr + (size_t) (C + 1) * T);                         // one-hot codes of the row string of the current pass
+  const Ln2Smem L = ln2_smem(C, T);
+  uint4* sm_part = (uint4*) sm_dyn;                  // partner ring of the forward pass
+  uint32_t* sm_scr = (uint32_t*) (sm_dyn + L.ring);  // row scratch of the join's arg-max search
+  uint8_t* sm_rows = (uint8_t*) (sm_scr + L.scr);    // one-hot codes of the row string of the current pass
   __shared__ int sm_x[wf::WF_SMX];
   __shared__ int sm_pub[8];
   __shared__ uint32_t sm_win[128];
@@ -530,16 +560,8 @@ __global__ void __launch_bounds__(MAXT, (MAXT == 32 ? LN2_OCC : (MAXT == 64 ? LN
     __syncthreads();
     wf::Best dummy;
     int revCorner, matCorner;
-#ifndef LN2_SKIP_REV   // (development switches LN2_SKIP_*: timing experiments only, results are wrong with them)
-    wf2::pass<C, MULTI, wf2::REV, PD>(sm_rows, [&](int i) { return revcomp_at(s2, n, (uint32_t) i); }, (int) m, (int) n, 1, dirsR, brev4, P, sm_x, sm_part, sm_scr, dummy, revCorner);
-#else
-    revCorner = 0;
-#endif
+    wf2::pass<C, MULTI, wf2::REV, LN_PART_D>(sm_rows, [&](int i) { return revcomp_at(s2, n, (uint32_t) i); }, (int) m, (int) n, 1, dirsR, brev4, P, sm_x, sm_part, sm_scr, dummy, revCorner);
     __syncthreads();
-#ifdef LN2_SKIP_FWD
-    if (tid == 0) { a.ok[job] = 0; a.aln_len[job] = (uint32_t) revCorner; }
-    continue;
-#endif
     // ---- forward pass with the fused join ----
     for (uint32_t i = tid; i < m; i += T) sm_rows[i] = (uint8_t) wf2::hot(s1[i]);
     wf2::synth_groups<C>(brev4, (int) m);
@@ -554,7 +576,7 @@ __global__ void __launch_bounds__(MAXT, (MAXT == 32 ? LN2_OCC : (MAXT == 64 ? LN
     }
     __syncthreads();
     wf::Best best;
-    wf2::pass<C, MULTI, wf2::FWD, PD>(sm_rows, [&](int i) { return s2[i]; }, (int) m, (int) n, cstartF, dirsF, brev4, P, sm_x, sm_part, sm_scr, best, matCorner);
+    wf2::pass<C, MULTI, wf2::FWD, LN_PART_D>(sm_rows, [&](int i) { return s2[i]; }, (int) m, (int) n, cstartF, dirsF, brev4, P, sm_x, sm_part, sm_scr, best, matCorner);
 #pragma unroll
     for (int d = 16; d >= 1; d >>= 1) {
       wf::Best o;
@@ -940,23 +962,15 @@ __global__ void __launch_bounds__(LNW_THREADS, 1) lnw_kernel(LnArgs a) {
   }
 }
 
-template <int C, bool MULTI, int MAXT = 32>
-int ln_launch2(dgpu_ctx* ctx, LnArgs& a, int cls, unsigned grid, unsigned threads, size_t smem, cudaStream_t st) {
-  int rc = dgpu_smem_optin(ctx, ln_kernel2<C, MULTI, MAXT>, smem, "cudaFuncSetAttribute(ln_kernel2)");
-  if (rc) return rc;
-  ln_kernel2<C, MULTI, MAXT><<<grid, threads, smem, st>>>(a, cls);
-  DGPU_LAUNCH_CHECK(ctx, "ln_kernel2");
-  return DGPU_OK;
+// The wavefront kernel of each job class, its template arguments read from ln_geom: classes 1..15 on the packed engine, 17..31 the same
+// geometries on the scalar engine.
+using LnKernel = void (*)(LnArgs, int);
+template <size_t... G>
+constexpr std::array<LnKernel, 2 * LN_NCLS> ln_kernels(std::index_sequence<G...>) {
+  return {{nullptr, ln_kernel2<ln_geom(G + 1).C, (ln_geom(G + 1).T > 32), ln_geom(G + 1).T>..., nullptr,
+           ln_kernel<ln_geom(G + 1).C, (ln_geom(G + 1).T > 32), ln_geom(G + 1).T>...}};
 }
-
-template <int C, bool MULTI, int MAXT = 32>
-int ln_launch(dgpu_ctx* ctx, LnArgs& a, int cls, unsigned grid, unsigned threads, size_t smem, cudaStream_t st) {
-  int rc = dgpu_smem_optin(ctx, ln_kernel<C, MULTI, MAXT>, smem, "cudaFuncSetAttribute(ln_kernel)");
-  if (rc) return rc;
-  ln_kernel<C, MULTI, MAXT><<<grid, threads, smem, st>>>(a, cls);
-  DGPU_LAUNCH_CHECK(ctx, "ln_kernel");
-  return DGPU_OK;
-}
+constexpr std::array<LnKernel, 2 * LN_NCLS> LN_KERNELS = ln_kernels(std::make_index_sequence<LN_NCLS - 1>());
 
 int check_max_ref(dgpu_ctx* ctx, uint32_t max_ref) {
   if (max_ref >= 1 && max_ref <= DGPU_LN_MAX_REF) return DGPU_OK;
@@ -989,8 +1003,8 @@ int ln_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes, const uint32
   a.perm = (uint32_t*) p;
   if ((rc = dgpu_reserve(ctx, SLOT_COUNTS, 2048, &p))) return rc;
   a.counts = (uint32_t*) p;                                   // 96 uint32 = 384 B
-  a.maxcells = (unsigned long long*) ((uint8_t*) p + 512);     // 96 uint64 = 768 B
-  int* d_unsupported = (int*) ((uint8_t*) p + 1280);
+  a.maxcells = (unsigned long long*) ((uint8_t*) p + 512);     // 128 uint64 = 1024 B
+  int* d_unsupported = (int*) ((uint8_t*) p + 1536);
   DGPU_CUDA(ctx, cudaMemsetAsync(p, 0, 2048, st));
   void* pc;
   if ((rc = dgpu_reserve(ctx, SLOT_LN_JOBCLS, n + 64, &pc))) return rc;
@@ -1002,7 +1016,7 @@ int ln_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes, const uint32
   DGPU_LAUNCH_CHECK(ctx, "ln_offsets");
   ln_scatter_kernel<<<cb, 256, 0, st>>>(a);
   DGPU_LAUNCH_CHECK(ctx, "ln_scatter");
-  struct { uint32_t counts[128]; unsigned long long maxc[96]; int unsupported; } h;
+  struct { uint32_t counts[128]; unsigned long long maxc[128]; int unsupported; } h;
   DGPU_CUDA(ctx, cudaMemcpyAsync(&h, p, sizeof(h), cudaMemcpyDeviceToHost, st));
   DGPU_CUDA(ctx, cudaStreamSynchronize(st));
   if (h.unsupported) {   // per-item refusal: those jobs come back with ok = 0 (and info[2] = -1); never a silent approximation, never a failed batch
@@ -1018,54 +1032,33 @@ int ln_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes, const uint32
   // streams forked from `st` (each class has its own region of the workspace): a batch of a few hundred SVs spread over
   // several classes would otherwise run as a sequence of under-filled launches.
   // Classes 1..15: jobs over ACGTN only -> packed two-row engine (ln_kernel2); 17..31: the same geometries for jobs with other bytes -> scalar engine.
-  struct Plan { int c; LnArgs a; size_t grid, off; unsigned threads; size_t smem; };
+  struct Plan { int c; LnArgs a; size_t grid; unsigned threads; size_t smem; };
   std::vector<Plan> plans;
   size_t total = 0;
   for (int c = 1; c < 2 * LN_NCLS; ++c) {
     if (!h.counts[c]) continue;
     Plan pl;
     pl.c = c; pl.a = a;
+    const size_t mmax = (size_t) h.maxc[96 + c];
+    int per_sm;
     if (c == LN_WIDE) {   // one 512-thread CTA per SM; the slab is the largest job's (lnw_geom), laid out per job by the kernel
       pl.a.work_stride = (size_t) h.maxc[c];
       pl.threads = LNW_THREADS;
-      pl.smem = lnw_smem(max_ref, (size_t) h.maxc[64 + c]);
-      pl.grid = std::min<size_t>(h.counts[c], (size_t) ctx->num_sms);
-      pl.off = 0;
-      total += pl.grid * pl.a.work_stride;
-      plans.push_back(pl);
-      continue;
-    }
-    const int g = c & (LN_GEN - 1);
-    const bool packed = c < LN_GEN;
-    const size_t cells = (size_t) h.maxc[c];
-    const size_t mn = (size_t) h.maxc[32 + c];
-    const size_t mmax = (size_t) h.maxc[64 + c];
-    auto al = [](size_t x) { return (x + 255) & ~(size_t) 255; };
-    size_t b_rev = al(cells * 2 + 1024);
-    size_t b_dirs = al(cells / 2 + 64 * mmax + 1024);  // (m+1) * dstride words, dstride <= bstride/8 + C/8
-    if (packed) {   // step-major workspace of the packed engine (wavefront2.cuh): sized by the row pairs, not by the columns
-      const size_t steps = (mmax + 1) / 2 + ln_threads(g) + 1;
-      b_rev = al((steps * 2 * (ln_cols(g) / 8) + ln_cols(g) / 8 + 1) * ln_threads(g) * 16 + 1024);   // rows + the constant groups of synth_groups()
-      b_dirs = al(steps * 2 * (ln_cols(g) / 8) * ln_threads(g) * 4 + 1024);
-    }
-    const size_t b_trace = al(4 * mn + 64);
-    pl.a.off_dirsR = b_rev;
-    pl.a.off_dirsF = b_rev + b_dirs;
-    pl.a.off_trace = b_rev + 2 * b_dirs;
-    pl.a.work_stride = pl.a.off_trace + b_trace;
-    pl.threads = (unsigned) ln_threads(g);
-    int per_sm;
-    if (packed) {
-      pl.smem = ((mmax + 15) & ~(size_t) 15) + (size_t) (ln_threads(g) == 256 ? 2 : (ln_cols(g) >= 40 ? LN2_PD_C40 : LN2_PD_SMALL)) * 2 * (ln_cols(g) / 8) * ln_threads(g) * sizeof(uint4) +
-                (size_t) (ln_cols(g) + 1) * ln_threads(g) * sizeof(uint32_t);
-      per_sm = ln_threads(g) == 32 ? LN2_OCC : (ln_threads(g) == 64 ? LN2_OCC / 2 : (ln_threads(g) == 128 ? LN2_OCC / 4 : 1));
-      per_sm = std::max(1, std::min<int>(per_sm, (int) ((200 * 1024) / (pl.smem + 2048))));
+      pl.smem = lnw_smem(max_ref, mmax);
+      per_sm = 1;
     } else {
-      pl.smem = ((mmax + 15) & ~(size_t) 15) + (g >= LN_UPS_FROM ? (size_t) ln_cols(g) * 256 * sizeof(int) : 0);
-      per_sm = ln_threads(g) == 32 ? 16 : 256 / ln_threads(g);  // multi-warp CTAs: 8 warps per SM at up to 255 registers per thread
+      const LnGeom g = ln_geom(c & (LN_GEN - 1));
+      ln_slab(pl.a, h.maxc[c], h.maxc[32 + c], h.maxc[64 + c]);
+      pl.threads = (unsigned) g.T;
+      if (c < LN_GEN) {
+        pl.smem = ln2_smem(g.C, g.T).bytes(mmax);
+        per_sm = std::max(1, std::min<int>(ln2_occ(g.T), (int) ((200 * 1024) / (pl.smem + 2048))));
+      } else {
+        pl.smem = ln_smem_ups(g.C, g.T) + ((mmax + 15) & ~(size_t) 15);
+        per_sm = ln_per_sm(g.T);
+      }
     }
     pl.grid = std::min<size_t>(h.counts[c], (size_t) ctx->num_sms * per_sm);
-    pl.off = 0;
     total += pl.grid * pl.a.work_stride;
     plans.push_back(pl);
   }
@@ -1104,40 +1097,16 @@ int ln_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes, const uint32
     }
     const unsigned grid = (unsigned) pl.grid, threads = pl.threads;
     const size_t smem = pl.smem;
-    switch (c) {
-      case 1: rc = ln_launch2<8, false>(ctx, pl.a, c, grid, threads, smem, cs); break;
-      case 2: rc = ln_launch2<16, false>(ctx, pl.a, c, grid, threads, smem, cs); break;
-      case 3: rc = ln_launch2<24, false>(ctx, pl.a, c, grid, threads, smem, cs); break;
-      case 4: rc = ln_launch2<32, false>(ctx, pl.a, c, grid, threads, smem, cs); break;
-      case 5: rc = ln_launch2<40, false>(ctx, pl.a, c, grid, threads, smem, cs); break;
-      case 6: case 7: case 8: rc = ln_launch2<32, true, 64>(ctx, pl.a, c, grid, threads, smem, cs); break;
-      case 9: rc = ln_launch2<32, true, 128>(ctx, pl.a, c, grid, threads, smem, cs); break;
-      case 10: rc = ln_launch2<24, true, 256>(ctx, pl.a, c, grid, threads, smem, cs); break;
-      case 11: rc = ln_launch2<32, true, 256>(ctx, pl.a, c, grid, threads, smem, cs); break;
-      case 12: rc = ln_launch2<40, true, 256>(ctx, pl.a, c, grid, threads, smem, cs); break;
-      case 13: rc = ln_launch2<48, true, 256>(ctx, pl.a, c, grid, threads, smem, cs); break;
-      case 14: rc = ln_launch2<56, true, 256>(ctx, pl.a, c, grid, threads, smem, cs); break;
-      case 15: rc = ln_launch2<64, true, 256>(ctx, pl.a, c, grid, threads, smem, cs); break;
-      case LN_WIDE:
-        if ((rc = dgpu_smem_optin(ctx, lnw_kernel, smem, "cudaFuncSetAttribute(lnw_kernel)"))) break;
-        lnw_kernel<<<grid, threads, smem, cs>>>(pl.a);
-        DGPU_LAUNCH_CHECK(ctx, "lnw_kernel");
-        break;
-      case 17: rc = ln_launch<8, false>(ctx, pl.a, c, grid, threads, smem, cs); break;
-      case 18: rc = ln_launch<16, false>(ctx, pl.a, c, grid, threads, smem, cs); break;
-      case 19: rc = ln_launch<24, false>(ctx, pl.a, c, grid, threads, smem, cs); break;
-      case 20: rc = ln_launch<32, false>(ctx, pl.a, c, grid, threads, smem, cs); break;
-      case 21: rc = ln_launch<40, false>(ctx, pl.a, c, grid, threads, smem, cs); break;
-      case 22: case 23: case 24: rc = ln_launch<32, true, 64>(ctx, pl.a, c, grid, threads, smem, cs); break;  // 2 warps x C=32: n <= 2041 without spills
-      case 25: rc = ln_launch<32, true, 128>(ctx, pl.a, c, grid, threads, smem, cs); break;
-      case 26: rc = ln_launch<24, true, 256>(ctx, pl.a, c, grid, threads, smem, cs); break;
-      case 27: rc = ln_launch<32, true, 256>(ctx, pl.a, c, grid, threads, smem, cs); break;
-      case 28: rc = ln_launch<40, true, 256>(ctx, pl.a, c, grid, threads, smem, cs); break;
-      case 29: rc = ln_launch<48, true, 256>(ctx, pl.a, c, grid, threads, smem, cs); break;
-      case 30: rc = ln_launch<56, true, 256>(ctx, pl.a, c, grid, threads, smem, cs); break;
-      default: rc = ln_launch<64, true, 256>(ctx, pl.a, c, grid, threads, smem, cs); break;
+    if (c == LN_WIDE) {
+      if ((rc = dgpu_smem_optin(ctx, lnw_kernel, smem, "cudaFuncSetAttribute(lnw_kernel)"))) return rc;
+      lnw_kernel<<<grid, threads, smem, cs>>>(pl.a);
+      DGPU_LAUNCH_CHECK(ctx, "lnw_kernel");
+    } else {
+      const LnKernel k = LN_KERNELS[c];
+      if ((rc = dgpu_smem_optin(ctx, k, smem, c < LN_GEN ? "cudaFuncSetAttribute(ln_kernel2)" : "cudaFuncSetAttribute(ln_kernel)"))) return rc;
+      k<<<grid, threads, smem, cs>>>(pl.a, c);
+      DGPU_LAUNCH_CHECK(ctx, c < LN_GEN ? "ln_kernel2" : "ln_kernel");
     }
-    if (rc) return rc;
   }
   if (fork) {  // join
     const size_t used = std::min<size_t>(plans.size(), DGPU_FORK_STREAMS);

@@ -38,8 +38,7 @@ namespace wf2 {
 using wf::Best;
 using wf::best_before;
 
-// partner-row ring depth in steps (FWD): rows are fetched PART_D - 1 steps ahead with cp.async (template parameter of pass(): 3, or 2 where
-// shared memory is short: the 8-warp classes)
+// partner-row ring depth in steps (FWD): rows are fetched PART_D - 1 steps ahead with cp.async (template parameter of pass())
 constexpr int BIAS = 8;          // U = H + row + BIAS
 constexpr uint32_t NEG16x2 = 0x80008000u;
 
@@ -73,7 +72,7 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N)); }
 
 // shared memory a pass needs for the partner ring (FWD), in uint4
-template <int C, int PART_D> __host__ __device__ constexpr int part_slots(int T) { return PART_D * 2 * (C / 8) * T; }
+__host__ __device__ constexpr int part_slots(int C, int part_d, int T) { return part_d * 2 * (C / 8) * T; }
 
 // ---- workspace layout: STEP-MAJOR ("diagonal") ---------------------------------------------------------------------------
 // At one step of the wavefront the threads of a warp work on DIFFERENT rows (thread t on row pair s - t), so a row-major workspace makes
@@ -84,10 +83,12 @@ template <int C, int PART_D> __host__ __device__ constexpr int part_slots(int T)
 //     nibble words  (uint32 units): ((step * 2 + ab) * T + t) * WPT + w
 // so that what the 32 lanes of a warp store in one instruction is contiguous. The forward pass reads the partner row m - r of its own row r;
 // under the mirroring all lanes of a warp then read groups of the SAME reverse step, again contiguous. Row 0 is "pair 0, lane B".
-// Sizes: (K + T + 1) * 2 * WPT * T groups resp. * T * WPT words with K = (m + 1) / 2 row pairs.
-template <int C> __host__ __device__ __forceinline__ size_t ws_steps(int m, int T) { return (size_t) ((m + 1) / 2 + T + 1); }
-template <int C> __host__ __device__ __forceinline__ size_t ws_brev_bytes(int m, int T) { return ws_steps<C>(m, T) * 2 * (C / 8) * T * 16; }
-template <int C> __host__ __device__ __forceinline__ size_t ws_dirs_bytes(int m, int T) { return ws_steps<C>(m, T) * 2 * (C / 8) * T * 4; }
+// Sizes: (K + T + 1) * 2 * WPT * T groups resp. * T * WPT words with K = (m + 1) / 2 row pairs, and behind the groups the
+// (WPT + 1) * T constant groups of synth_groups().
+__host__ __device__ __forceinline__ size_t ws_steps(int m, int T) { return (size_t) ((m + 1) / 2 + T + 1); }
+__host__ __device__ __forceinline__ int ws_synth_groups(int C, int T) { return (C / 8 + 1) * T; }
+__host__ __device__ __forceinline__ size_t ws_brev_bytes(int C, int m, int T) { return (ws_steps(m, T) * 2 * (C / 8) * T + ws_synth_groups(C, T)) * 16; }
+__host__ __device__ __forceinline__ size_t ws_dirs_bytes(int C, int m, int T) { return ws_steps(m, T) * 2 * (C / 8) * T * 4; }
 template <int C> __device__ __forceinline__ size_t grp_index(int r, int t, int w, int T) {
   return ((size_t) ((((r + 1) >> 1) + t) * 2 + ((r & 1) ^ 1)) * (C / 8) + w) * T + t;
 }
@@ -112,8 +113,8 @@ template <int C> __device__ __forceinline__ void synth_groups(uint4* __restrict_
   constexpr int WPT = C / 8;
   constexpr uint32_t NEG2 = 0x80008000u;
   const int T = blockDim.x, tid = threadIdx.x;
-  uint4* g = brev4 + ws_steps<C>(m, T) * 2 * WPT * T;
-  for (int i = tid; i < (WPT + 1) * T; i += T) g[i] = make_uint4(i == 0 ? ((NEG2 & 0xffff0000u) | (uint32_t) BIAS) : NEG2, NEG2, NEG2, NEG2);
+  uint4* g = brev4 + ws_steps(m, T) * 2 * WPT * T;
+  for (int i = tid; i < ws_synth_groups(C, T); i += T) g[i] = make_uint4(i == 0 ? ((NEG2 & 0xffff0000u) | (uint32_t) BIAS) : NEG2, NEG2, NEG2, NEG2);
 }
 
 // rowHot: one-hot codes of the row string (shared memory, m bytes); colChar(c-1) = column byte.
@@ -123,7 +124,7 @@ template <int C> __device__ __forceinline__ void synth_groups(uint4* __restrict_
 template <int C, bool MULTI, int MODE, int PART_D, typename TB>
 __device__ __forceinline__ void pass(const uint8_t* rowHot, TB colChar, const int m, const int n, const int cstart, uint32_t* __restrict__ dirs,
                                      uint4* __restrict__ brev4, const int P, int* sm_x /* MULTI: WF_SMX ints */,
-                                     uint4* sm_part /* FWD: part_slots<C, PART_D>(T) uint4 */, uint32_t* sm_scr /* FWD: (C + 1) * T words */, Best& best, int& corner) {
+                                     uint4* sm_part /* FWD: part_slots(C, PART_D, T) uint4 */, uint32_t* sm_scr /* FWD: (C + 1) * T words */, Best& best, int& corner) {
   const int tid = threadIdx.x;
   const int lane = tid & 31;
   const int T = blockDim.x;
@@ -185,7 +186,7 @@ __device__ __forceinline__ void pass(const uint8_t* rowHot, TB colChar, const in
   // As uint4 indices relative to brev4 a group's source is base + w*T (+ the row's base when a reverse thread stored it). Groups nobody stored
   // (column 0: U = BIAS as first element; beyond the row: no partner) are read from a small constant region behind the job's rows
   // (synth_groups below: entry 0 = the column-0 group, every other entry = "no partner"), so that the prefetch is branch-free.
-  const int synth0 = (int) (ws_steps<C>(m, T) * 2 * WPT * T);
+  const int synth0 = (int) (ws_steps(m, T) * 2 * WPT * T);
   const bool dynA = tqa >= 0, dynB = tqa >= 1;
   const int baseA = dynA ? (2 * tqa * WPT + wa0) * T + tqa : ((tqa == -1 && wa0 == 0) ? synth0 : synth0 + 1);
   const int baseB = dynB ? (2 * (tqa - 1) * WPT - split) * T + (tqa - 1) : ((tqa == 0) ? synth0 - split * T : synth0 + 1);
@@ -343,7 +344,6 @@ __device__ __forceinline__ void pass(const uint8_t* rowHot, TB colChar, const in
       prevRecvHi = rH >> 16;
       // ---- nibble rows --------------------------------------------------------------------------------------------------
       {
-#ifndef LN2_NO_NIB_STORE
         uint32_t* dA = dirs + ((size_t) (s * 2 + 0) * T + tid) * WPT;
 #pragma unroll
         for (int w = 0; w < WPT; ++w) dA[w] = __byte_perm(acc[2 * w], acc[2 * w + 1], 0x5410);
@@ -352,12 +352,6 @@ __device__ __forceinline__ void pass(const uint8_t* rowHot, TB colChar, const in
 #pragma unroll
           for (int w = 0; w < WPT; ++w) dB[w] = __byte_perm(acc[2 * w], acc[2 * w + 1], 0x7632);
         }
-#else
-        uint32_t z = 0;
-#pragma unroll
-        for (int w = 0; w < C / 4; ++w) z ^= acc[w];
-        if (z == 0x12345678u) dirs[0] = 1;
-#endif
       }
       if (MODE == FWD) {
         const int off = m + 2 * BIAS;

@@ -157,6 +157,16 @@ def test_cuda_non_acgtn_jobs_take_the_scalar_engine(ctx):
     b1 = synth.k3_consref_batch(40, seed=12, cons_range=(60, 200), ref_cap=900)
     b2 = _edge_batch(seed=5)
     jobs = [j for j in list(_jobs(b1)) + list(_jobs(b2)) if len(j[0]) and len(j[1])]
+    # one job on each side of every class bound on n + 7, over ACGTN (packed engine) and with one lower-case byte (scalar engine)
+    rng = np.random.default_rng(77)
+    bounds = [b for k in range(1, 9) for b in (256 * k, 256 * k + 1)] + [b for k in range(4096, 16384, 2048) for b in (k, k + 1)] + [16384]
+    for n in (b - 7 for b in bounds):
+        ref = synth._ACGT[rng.integers(0, 4, size=n, dtype=np.uint8)]
+        a = int(rng.integers(0, n // 3)); b = int(rng.integers(2 * n // 3, n - 60))
+        cons = synth.sub_noise(rng, np.concatenate([ref[a:a + 60], ref[b:b + 60]]), 0.03)
+        low = ref.copy()
+        low[n // 2] += 32
+        jobs += [(cons.tobytes(), ref.tobytes()), (cons.tobytes(), low.tobytes())]
     arena, off, ln = synth.pack([x for cr in jobs for x in cr])
     ok, alen, rows = ctx.long_needle(arena, off[0::2].copy(), ln[0::2].copy(), off[1::2].copy(), ln[1::2].copy())
     for i, (c, r) in enumerate(jobs):
