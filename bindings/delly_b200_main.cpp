@@ -17,6 +17,7 @@
 #include <unistd.h>
 #include <thread>
 #include <vector>
+#include <zlib.h>
 
 #include "hts_io.hpp"
 #include "../delly_b200/host/gather.hpp"
@@ -67,8 +68,8 @@ bool svTypesToCompute(Config& c, std::string const& svtype) {
 
 void usage(Options const& o) {
   std::cerr << "\nUsage: delly_b200 " << (o.lr ? "lr" : "sr") << " [OPTIONS] -g <ref.fa> <sample1.sort.bam> <sample2.sort.bam> ...\n"
-            << "  options follow `delly " << (o.lr ? "lr" : "sr") << "` (same letters and defaults); extra: --device N, --io-threads N"
-            << (o.lr ? ", --mei <templates.fa>" : "") << "\n";
+            << "  options follow `delly " << (o.lr ? "lr" : "sr") << "` (same letters and defaults), including -d <reads.gz> (gzipped list of the reads"
+            << " that support each SV); extra: --device N, --io-threads N" << (o.lr ? ", --mei <templates.fa>" : "") << "\n";
 }
 
 // `delly sr` (src/delly.h:207-246) and `delly lr` (src/tegua.h:215-275) share most letters; the long names are the reference's.
@@ -130,6 +131,11 @@ bool parse(int argc, char** argv, Options& o) {
     else if (o.lr && a == "--mei") o.meifile = val();
     else if (o.lr && is("-l", "--alt-align")) { std::cerr << "alternate alignments (-l) are outside the accelerated path (SURVEY section 2)" << std::endl; return false; }
     else { std::cerr << "unrecognised option '" << argv[i] << "'" << std::endl; return false; }
+  }
+  if (!o.dumpfile.empty() && o.nranks > 1) {
+    std::cerr << "the SV-read dump (-d) needs a single process: over --nranks > 1 every rank genotypes a part of the SV list, and the order of"
+                 " the dump lines depends on the whole list" << std::endl;
+    return false;
   }
   return true;
 }
@@ -251,6 +257,17 @@ bool openInputs(Options& o, Inputs& in) {
 }
 
 
+// The SV-read dump (-d) as one gzip stream; render(put) hands it the text.
+template <typename TRender> bool writeDump(std::string const& path, TRender render) {
+  gzFile gz = gzopen(path.c_str(), "wb");
+  if (!gz) { std::cerr << "cannot open the SV-read dump file " << path << std::endl; return false; }
+  bool ok = true;
+  render([&](const char* p, std::size_t n) { if (ok && gzwrite(gz, p, (unsigned) n) != (int) n) ok = false; });
+  if (gzclose(gz) != Z_OK) ok = false;
+  if (!ok) std::cerr << "cannot write the SV-read dump file " << path << std::endl;
+  return ok;
+}
+
 void writeTiming(Options const& o, StageClock const& clock, std::size_t nsv) {
   if (o.timingFile.empty()) return;
   std::ofstream f((o.timingFile + (o.nranks > 1 ? "." + std::to_string(o.rank) : std::string())).c_str());
@@ -304,11 +321,16 @@ int runSr(Options& o, DeviceSession& dev) {
   clock.lap("open_inputs");
   Config& c = o.c;
   const std::size_t F = in.files.size();
+  const bool dump = !o.dumpfile.empty();
+  std::vector<std::vector<std::string> > names(dump ? F : 0);   // query names of the genotyped records (-d)
   // records of every file, as the reference's iterators return them
   std::vector<std::vector<SrRecord> > recs(F);
   std::vector<std::vector<SrRecord> const*> samples;
   for (std::size_t f = 0; f < F; ++f) {
-    if (!in.files[f].readRegionsParallel(o.genome, in.validRegions, recs[f], io::toSrRecord, o.ioThreads)) { std::cerr << "cannot read " << o.files[f] << std::endl; return 1; }
+    if (!in.files[f].readRegionsParallel(o.genome, in.validRegions, recs[f], io::toSrRecord, o.ioThreads, nullptr, nullptr, 0, (dump && !o.hasExclude) ? &names[f] : nullptr)) {
+      std::cerr << "cannot read " << o.files[f] << std::endl;
+      return 1;
+    }
     samples.push_back(&recs[f]);
   }
   // exclude file: scan, clustering, assembly and the library estimate see the valid regions (src/shortpe.h:349, src/util.h:810), the genotyping pass
@@ -317,7 +339,10 @@ int runSr(Options& o, DeviceSession& dev) {
   std::vector<std::vector<SrRecord> const*> genoSamples;
   if (o.hasExclude) {
     for (std::size_t f = 0; f < F; ++f) {
-      if (!in.files[f].readRegionsParallel(o.genome, in.wholeContigs, recsWhole[f], io::toSrRecord, o.ioThreads)) { std::cerr << "cannot read " << o.files[f] << std::endl; return 1; }
+      if (!in.files[f].readRegionsParallel(o.genome, in.wholeContigs, recsWhole[f], io::toSrRecord, o.ioThreads, nullptr, nullptr, 0, dump ? &names[f] : nullptr)) {
+        std::cerr << "cannot read " << o.files[f] << std::endl;
+        return 1;
+      }
       genoSamples.push_back(&recsWhole[f]);
     }
     c.contigExcluded.assign(in.validRegions.size(), 0);
@@ -335,17 +360,25 @@ int runSr(Options& o, DeviceSession& dev) {
   dgpu_ctx* ctx = dev.ctx();
   const Shard shard = dev.shard();
   SrMultiCallSet cs;
+  SvReadDump reads;
   int rc;
-  if (!o.hasVcf) rc = dellySrCallSharded(ctx, c, libs, in.target_len, in.target_name, in.genome.cseq, samples, shard, cs, &clock, o.hasExclude ? &genoSamples : nullptr);
+  if (!o.hasVcf)
+    rc = dellySrCallSharded(ctx, c, libs, in.target_len, in.target_name, in.genome.cseq, samples, shard, cs, &clock, o.hasExclude ? &genoSamples : nullptr, dump ? &reads : nullptr);
   else {
     std::vector<VcfSite> sites;
     bool hasConsBp = false;
     if (!io::readSites(o.vcffile, sites, hasConsBp)) return 1;
-    rc = dellySrGenotypeSharded(ctx, c, libs, in.target_len, in.target_name, in.genome.cseq, sites, hasConsBp, o.hasExclude ? genoSamples : samples, shard, cs, &clock);
+    rc = dellySrGenotypeSharded(ctx, c, libs, in.target_len, in.target_name, in.genome.cseq, sites, hasConsBp, o.hasExclude ? genoSamples : samples, shard, cs, &clock,
+                                dump ? &reads : nullptr);
     if (rc == DGPU_ERR_ARG && !cs.sample.empty()) { std::cerr << "Error: Delly genotyping requires a Delly BCF file from v1.1.7 or later!" << std::endl; rc = DGPU_OK; }
   }
   if (rc) { std::cerr << "delly_b200: device path failed (" << rc << "): " << dgpu_last_error(ctx) << std::endl; return 1; }
   if (o.rank != 0) { writeTiming(o, clock, cs.svs.size()); return 0; }   // every rank holds the complete call set; rank 0 writes it
+  if (dump && !cs.svs.empty()) {   // the reference opens the dump in annotateCoverage, which an empty SV list skips (src/delly.h:176)
+    std::vector<std::vector<SrRecord> const*> const& geno = o.hasExclude ? genoSamples : samples;
+    if (!writeDump(o.dumpfile, [&](auto put) { writeSrReadDump(put, reads, o.files, geno, names, in.target_name); })) return 1;
+    clock.lap("write_dump");
+  }
   // src/delly.h:161-178: the count maps stay empty (and the header gets no sample column) when there is nothing to genotype
   std::vector<VcfSample> vs;
   if (!cs.svs.empty())
@@ -374,11 +407,16 @@ int runLr(Options& o, DeviceSession& dev, const char* argv0) {
   MeiTemplates mei;
   const std::string meiPath = o.meifile.empty() ? exeDir(argv0) + "/../data/_mei_templates.fa" : o.meifile;
   if (!loadMei(meiPath, mei)) { std::cerr << "cannot read the annotation templates " << meiPath << " (see --mei)" << std::endl; return 1; }
+  const bool dump = !o.dumpfile.empty();
+  std::vector<std::vector<std::string> > names(dump ? F : 0);   // query names of the genotyped records (-d)
   std::vector<std::vector<LrRecord> > recs(F);
   std::vector<std::vector<std::size_t> > ids(F);
   std::vector<LrSample> samples;
   for (std::size_t f = 0; f < F; ++f) {
-    if (!in.files[f].readRegionsParallel(o.genome, in.validRegions, recs[f], io::toLrRecord, o.ioThreads, &ids[f], io::hashLr)) { std::cerr << "cannot read " << o.files[f] << std::endl; return 1; }
+    if (!in.files[f].readRegionsParallel(o.genome, in.validRegions, recs[f], io::toLrRecord, o.ioThreads, &ids[f], io::hashLr, 0, (dump && !o.hasExclude) ? &names[f] : nullptr)) {
+      std::cerr << "cannot read " << o.files[f] << std::endl;
+      return 1;
+    }
     samples.push_back(LrSample{&recs[f], &ids[f]});
   }
   std::vector<std::vector<LrRecord> > recsWhole(o.hasExclude ? F : 0);   // exclude file: the genotyping pass still reads whole contigs
@@ -386,24 +424,36 @@ int runLr(Options& o, DeviceSession& dev, const char* argv0) {
   std::vector<LrSample> genoSamples;
   if (o.hasExclude)
     for (std::size_t f = 0; f < F; ++f) {
-      if (!in.files[f].readRegionsParallel(o.genome, in.wholeContigs, recsWhole[f], io::toLrRecord, o.ioThreads, &idsWhole[f], io::hashLr)) { std::cerr << "cannot read " << o.files[f] << std::endl; return 1; }
+      if (!in.files[f].readRegionsParallel(o.genome, in.wholeContigs, recsWhole[f], io::toLrRecord, o.ioThreads, &idsWhole[f], io::hashLr, 0, dump ? &names[f] : nullptr)) {
+        std::cerr << "cannot read " << o.files[f] << std::endl;
+        return 1;
+      }
       genoSamples.push_back(LrSample{&recsWhole[f], &idsWhole[f]});
     }
   if (!dev.wait()) return 3;
   dgpu_ctx* ctx = dev.ctx();
   LrMultiCallSet cs;
+  SvReadDump reads;
   int rc;
   const Shard shard = dev.shard();
-  if (!o.hasVcf) rc = dellyLrCallSharded(ctx, c, o.indelExtension, in.target_len, in.target_name, in.genome.cseq, samples, shard, cs, &mei, o.anno, &o.methyl, o.hasExclude ? &genoSamples : nullptr);
+  if (!o.hasVcf)
+    rc = dellyLrCallSharded(ctx, c, o.indelExtension, in.target_len, in.target_name, in.genome.cseq, samples, shard, cs, &mei, o.anno, &o.methyl,
+                            o.hasExclude ? &genoSamples : nullptr, dump ? &reads : nullptr);
   else {
     std::vector<VcfSite> sites;
     bool hasConsBp = false;
     if (!io::readSites(o.vcffile, sites, hasConsBp)) return 1;
-    rc = dellyLrGenotypeSharded(ctx, c, in.target_len, in.target_name, in.genome.cseq, sites, hasConsBp, o.hasExclude ? genoSamples : samples, shard, cs, &mei, o.anno, &o.methyl);
+    rc = dellyLrGenotypeSharded(ctx, c, in.target_len, in.target_name, in.genome.cseq, sites, hasConsBp, o.hasExclude ? genoSamples : samples, shard, cs, &mei, o.anno,
+                                &o.methyl, dump ? &reads : nullptr);
     if (rc == DGPU_ERR_ARG && !cs.sample.empty()) { std::cerr << "Error: Delly genotyping requires a Delly BCF file from v1.1.7 or later!" << std::endl; rc = DGPU_OK; }
   }
   if (rc) { std::cerr << "delly_b200: device path failed (" << rc << "): " << dgpu_last_error(ctx) << std::endl; return 1; }
   if (o.rank != 0) return 0;   // every rank holds the complete call set; rank 0 writes it
+  if (dump && !cs.svs.empty()) {   // genotypeLR returns before it opens the dump when the SV list is empty (src/genotype.h:97, :127-133)
+    std::vector<std::vector<LrRecord> const*> geno;
+    for (LrSample const& s : (o.hasExclude ? genoSamples : samples)) geno.push_back(s.recs);
+    if (!writeDump(o.dumpfile, [&](auto put) { writeLrReadDump(put, reads, o.files, geno, names, in.target_name); })) return 1;
+  }
   // long reads have no spanning pairs: empty lists per SV (src/tegua.h:173-190)
   std::vector<SpanningCount> noSpan(cs.svs.size());
   std::vector<VcfSample> vs;
@@ -432,7 +482,6 @@ int main(int argc, char** argv) {
   if (o.c.minCliqueSize < 2) o.c.minCliqueSize = 2;
   if (o.c.minMapQual > o.c.minTraQual) o.c.minTraQual = o.c.minMapQual;
   if (o.c.minGenoQual < 5 && !o.lr) o.c.minGenoQual = 5;   // src/delly.h:386
-  if (!o.dumpfile.empty()) { std::cerr << "the SV-read dump file (-d) is outside the accelerated path" << std::endl; return 1; }
   DeviceSession dev(o);
   const int r = o.lr ? runLr(o, dev, argv[0]) : runSr(o, dev);
   DeviceLimitLog const& lim = deviceLimitLog();

@@ -129,20 +129,21 @@ struct AlignmentFile {
   // region is cut into chunks of `chunk` bp, each chunk is read through its own file handle and iterator, and a record belongs to the chunk that
   // contains its start position (an iterator also returns the reads that merely overlap its interval; of those a later chunk keeps only what
   // starts inside it, the first chunk of a region keeps everything — exactly what the single iterator over the region returns, in its order).
+  // names: the query name of every record, kept only for the SV-read dump (a sample has millions of records).
   template <typename TRec, typename TFill>
   bool readRegionsParallel(std::string const& genome, TRegionsGenome const& regions, std::vector<TRec>& out, TFill fill, int threads, std::vector<std::size_t>* ids = nullptr,
-                           std::size_t (*idfn)(bam1_t const*) = nullptr, uint32_t chunk = 0) {
+                           std::size_t (*idfn)(bam1_t const*) = nullptr, uint32_t chunk = 0, std::vector<std::string>* names = nullptr) {
     if (!chunk) {   // about four chunks per thread, between 256 kbp and 4 Mbp
       uint64_t total = 0;
       for (auto const& v : regions) for (Interval const& iv : v) total += iv.hi - iv.lo;
       chunk = (uint32_t) std::min<uint64_t>(4000000, std::max<uint64_t>(262144, total / (4 * (uint64_t) std::max(1, threads))));
     }
-    struct Task { int32_t tid; uint32_t lo, hi; bool firstOfRegion; std::vector<TRec> recs; std::vector<std::size_t> ids; };
+    struct Task { int32_t tid; uint32_t lo, hi; bool firstOfRegion; std::vector<TRec> recs; std::vector<std::size_t> ids; std::vector<std::string> names; };
     std::vector<Task> tasks;
     for (int32_t refIndex = 0; refIndex < hdr->n_targets; ++refIndex)
       for (Interval const& iv : regions[refIndex])
         for (uint32_t b = iv.lo; b < iv.hi; b += chunk) { Task t; t.tid = refIndex; t.lo = b; t.hi = std::min<uint64_t>((uint64_t) b + chunk, iv.hi); t.firstOfRegion = (b == iv.lo); tasks.push_back(std::move(t)); }
-    if (threads < 2 || tasks.size() < 2) { readRegions(regions, out, fill, ids, idfn); return true; }
+    if (threads < 2 || tasks.size() < 2) { readRegions(regions, out, fill, ids, idfn, names); return true; }
     std::atomic<std::size_t> next(0);
     std::atomic<bool> failed(false);
     auto worker = [&]() {
@@ -161,6 +162,7 @@ struct AlignmentFile {
           t.recs.emplace_back();
           fill(rec, t.recs.back());
           if (ids) t.ids.push_back(idfn(rec));
+          if (names) t.names.emplace_back(bam_get_qname(rec));
         }
         hts_itr_destroy(iter);
       }
@@ -175,11 +177,13 @@ struct AlignmentFile {
     for (std::size_t k = 0; k < tasks.size(); ++k) off[k + 1] = off[k] + tasks[k].recs.size();
     out.resize(off[tasks.size()]);
     if (ids) ids->resize(off[tasks.size()]);
+    if (names) names->resize(off[tasks.size()]);
     std::atomic<std::size_t> nextMove(0);
     auto mover = [&]() {
       for (std::size_t k = nextMove++; k < tasks.size(); k = nextMove++) {
         std::move(tasks[k].recs.begin(), tasks[k].recs.end(), out.begin() + (std::ptrdiff_t) off[k]);
         if (ids) std::copy(tasks[k].ids.begin(), tasks[k].ids.end(), ids->begin() + (std::ptrdiff_t) off[k]);
+        if (names) std::move(tasks[k].names.begin(), tasks[k].names.end(), names->begin() + (std::ptrdiff_t) off[k]);
         std::vector<TRec>().swap(tasks[k].recs);
       }
     };
@@ -191,7 +195,8 @@ struct AlignmentFile {
   }
   // every record the reference's iterators return: contig by contig, region by region (a read over two regions comes twice, as there)
   template <typename TRec, typename TFill>
-  void readRegions(TRegionsGenome const& regions, std::vector<TRec>& out, TFill fill, std::vector<std::size_t>* ids = nullptr, std::size_t (*idfn)(bam1_t const*) = nullptr) {
+  void readRegions(TRegionsGenome const& regions, std::vector<TRec>& out, TFill fill, std::vector<std::size_t>* ids = nullptr, std::size_t (*idfn)(bam1_t const*) = nullptr,
+                   std::vector<std::string>* names = nullptr) {
     bam1_t* rec = bam_init1();
     for (int32_t refIndex = 0; refIndex < hdr->n_targets; ++refIndex) {
       for (Interval const& iv : regions[refIndex]) {
@@ -200,6 +205,7 @@ struct AlignmentFile {
           out.emplace_back();
           fill(rec, out.back());
           if (ids) ids->push_back(idfn(rec));
+          if (names) names->emplace_back(bam_get_qname(rec));
         }
         hts_itr_destroy(iter);
       }

@@ -151,11 +151,15 @@ inline uint64_t genotypingCost(StructuralVariantRecord const& sv, Config const& 
 
 // ---- sharded genotyping of a sorted, renumbered SV list (one or several samples) ---------------------------------------------------
 // in/out: cs.svs = the COMPLETE list, sorted and renumbered, identical on every rank. On return every rank holds the complete result.
+// dump: the SV-read events of every sample (one process only: the order of tied breakpoints depends on the whole SV list, see DESIGN §8).
 inline int genotypeSrSitesSharded(dgpu_ctx* ctx, Config const& c, std::vector<LibraryInfo> const& libs, std::vector<uint32_t> const& target_len,
                                   std::vector<std::string> const& target_name, std::vector<const char*> const& chrseq,
-                                  std::vector<std::vector<SrRecord> const*> const& samples, Shard const& shard, SrMultiCallSet& cs, StageClock* clock = nullptr) {
+                                  std::vector<std::vector<SrRecord> const*> const& samples, Shard const& shard, SrMultiCallSet& cs, StageClock* clock = nullptr,
+                                  SvReadDump* dump = nullptr) {
   const std::size_t F = samples.size();
+  if (dump && shard.active()) return DGPU_ERR_ARG;
   cs.sample.assign(F, SrSampleCounts());
+  if (dump) dump->file.assign(F, SvReadDump::File());
   if (cs.svs.empty()) return DGPU_OK;
   if (!shard.active()) {
     JunctionProbes probes;
@@ -164,7 +168,7 @@ inline int genotypeSrSitesSharded(dgpu_ctx* ctx, Config const& c, std::vector<Li
     if (clock) clock->lap("probes");
     for (std::size_t f = 0; f < F; ++f) {
       SrCallSet one; one.svs = cs.svs;
-      if ((rc = genotypeSrSites(ctx, c, libs[f], target_len, target_name, chrseq, *samples[f], one, &probes))) return rc;
+      if ((rc = genotypeSrSites(ctx, c, libs[f], target_len, target_name, chrseq, *samples[f], one, &probes, dump ? &dump->file[f] : nullptr))) return rc;
       cs.sample[f].jctMap.swap(one.jctMap); cs.sample[f].spanMap.swap(one.spanMap); cs.sample[f].rcMap.swap(one.rcMap); cs.sample[f].format.swap(one.format);
     }
     if (clock) clock->lap("genotype");
@@ -234,15 +238,16 @@ inline int genotypeSrSitesSharded(dgpu_ctx* ctx, Config const& c, std::vector<Li
 inline int dellySrGenotypeSharded(dgpu_ctx* ctx, Config const& c, std::vector<LibraryInfo> const& libs, std::vector<uint32_t> const& target_len,
                                   std::vector<std::string> const& target_name, std::vector<const char*> const& chrseq, std::vector<VcfSite> const& sites,
                                   bool headerHasConsBp, std::vector<std::vector<SrRecord> const*> const& samples, Shard const& shard, SrMultiCallSet& out,
-                                  StageClock* clock = nullptr) {
+                                  StageClock* clock = nullptr, SvReadDump* dump = nullptr) {
   out = SrMultiCallSet();
+  if (dump && shard.active()) return DGPU_ERR_ARG;
   const bool ok = vcfParseSites(sites, headerHasConsBp, target_name, out.svs);
   for (auto const& sv : out.svs)
     if (sv.chr < 0 || sv.chr2 < 0) return DGPU_ERR_ARG;
   std::sort(out.svs.begin(), out.svs.end());   // src/delly.h:155-158, on every rank identically, BEFORE the list is cut
   for (std::size_t i = 0; i < out.svs.size(); ++i) out.svs[i].id = (int32_t) i;
   if (clock) clock->lap("parse_sort_sites");
-  const int rc = genotypeSrSitesSharded(ctx, c, libs, target_len, target_name, chrseq, samples, shard, out, clock);
+  const int rc = genotypeSrSitesSharded(ctx, c, libs, target_len, target_name, chrseq, samples, shard, out, clock, dump);
   if (rc) return rc;
   return ok ? DGPU_OK : DGPU_ERR_ARG;
 }
@@ -253,12 +258,13 @@ inline AssembleShard makeAssembleShard(Shard const& shard);
 inline int dellySrCallSharded(dgpu_ctx* ctx, Config const& c, std::vector<LibraryInfo>& libs, std::vector<uint32_t> const& target_len,
                               std::vector<std::string> const& target_name, std::vector<const char*> const& chrseq,
                               std::vector<std::vector<SrRecord> const*> const& samples, Shard const& shard, SrMultiCallSet& out, StageClock* clock = nullptr,
-                              std::vector<std::vector<SrRecord> const*> const* genoSamples = nullptr) {
+                              std::vector<std::vector<SrRecord> const*> const* genoSamples = nullptr, SvReadDump* dump = nullptr) {
   // samples: the records of the valid regions (scan, clustering, assembly); genoSamples: the records of the whole contigs for the genotyping pass
-  // (src/coverage.h reads every contig end to end) — the same lists unless an exclude file is in play.
+  // (src/coverage.h reads every contig end to end) — the same lists unless an exclude file is in play. dump: indexes into genoSamples.
   std::vector<StructuralVariantRecord> srSVs;
   std::vector<TPosReadSV> srStore;
   out = SrMultiCallSet();
+  if (dump && shard.active()) return DGPU_ERR_ARG;
   int rc = scanPEandSRBatch(ctx, c, libs, target_len, samples, out.svs, srSVs, srStore);
   if (rc) return rc;
   if (clock) clock->lap("scan_cluster");
@@ -271,7 +277,7 @@ inline int dellySrCallSharded(dgpu_ctx* ctx, Config const& c, std::vector<Librar
   std::sort(out.svs.begin(), out.svs.end());
   for (std::size_t i = 0; i < out.svs.size(); ++i) out.svs[i].id = (int32_t) i;
   if (clock) clock->lap("merge_sort");
-  return genotypeSrSitesSharded(ctx, c, libs, target_len, target_name, chrseq, genoSamples ? *genoSamples : samples, shard, out, clock);
+  return genotypeSrSitesSharded(ctx, c, libs, target_len, target_name, chrseq, genoSamples ? *genoSamples : samples, shard, out, clock, dump);
 }
 
 // The exchange of an assembly queue cut by cost (AssembleShard): every rank sends the finished records of its range and receives all of them in
@@ -307,15 +313,19 @@ inline AssembleShard makeAssembleShard(Shard const& shard) {
 // ids become local index + range start, one all-gatherv of the complete records and count vectors, concatenation in rank order.
 inline int genotypeLrSitesSharded(dgpu_ctx* ctx, Config const& c, std::vector<uint32_t> const& target_len, std::vector<std::string> const& target_name,
                                   std::vector<const char*> const& chrseq, std::vector<LrSample> const& samples, Shard const& shard, LrMultiCallSet& cs,
-                                  MeiTemplates const* mei, AnnoConfig const& annoCfg, MethylConfig const* methylCfg, bool annotateBeforeFormat) {
+                                  MeiTemplates const* mei, AnnoConfig const& annoCfg, MethylConfig const* methylCfg, bool annotateBeforeFormat,
+                                  SvReadDump* dump = nullptr) {
   const std::size_t F = samples.size();
+  if (dump && shard.active()) return DGPU_ERR_ARG;
   cs.sample.assign(F, LrSampleCounts());
+  if (dump) dump->file.assign(F, SvReadDump::File());
   int rc;
   auto runRange = [&](std::vector<StructuralVariantRecord>& svs, std::vector<LrSampleCounts>& out) -> int {
     out.assign(F, LrSampleCounts());
     for (std::size_t f = 0; f < F; ++f) {
       LrSampleCounts& sc = out[f];
-      int r = genotypeLRBatch(ctx, c, target_len, target_name, chrseq, svs, *samples[f].recs, sc.jctMap, sc.rcMap, methylCfg, methylCfg ? &sc.methyl : nullptr);
+      int r = genotypeLRBatch(ctx, c, target_len, target_name, chrseq, svs, *samples[f].recs, sc.jctMap, sc.rcMap, methylCfg, methylCfg ? &sc.methyl : nullptr,
+                              dump ? &dump->file[f].sr : nullptr);
       if (r) return r;
     }
     if (mei) { int r = annotateSVs(ctx, annoCfg, *mei, chrseq, target_len, svs); if (r) return r; }
@@ -368,8 +378,9 @@ inline int genotypeLrSitesSharded(dgpu_ctx* ctx, Config const& c, std::vector<ui
 inline int dellyLrCallSharded(dgpu_ctx* ctx, Config const& c, float indelExtension, std::vector<uint32_t> const& target_len, std::vector<std::string> const& target_name,
                               std::vector<const char*> const& chrseq, std::vector<LrSample> const& samples, Shard const& shard, LrMultiCallSet& out,
                               MeiTemplates const* mei = nullptr, AnnoConfig const& annoCfg = AnnoConfig(), MethylConfig const* methylCfg = nullptr,
-                              std::vector<LrSample> const* genoSamples = nullptr) {
+                              std::vector<LrSample> const* genoSamples = nullptr, SvReadDump* dump = nullptr) {
   out = LrMultiCallSet();
+  if (dump && shard.active()) return DGPU_ERR_ARG;
   std::vector<LrRecord> stream;
   std::vector<std::size_t> streamIds;
   buildLrStream(target_len, samples, stream, streamIds);
@@ -377,21 +388,22 @@ inline int dellyLrCallSharded(dgpu_ctx* ctx, Config const& c, float indelExtensi
   if (shard.active()) as = makeAssembleShard(shard);
   int rc = discoverLrSVs(ctx, c, indelExtension, target_len, chrseq, stream, streamIds, out.svs, shard.active() ? &as : nullptr);
   if (rc) return rc;
-  return genotypeLrSitesSharded(ctx, c, target_len, target_name, chrseq, genoSamples ? *genoSamples : samples, shard, out, mei, annoCfg, methylCfg, true);
+  return genotypeLrSitesSharded(ctx, c, target_len, target_name, chrseq, genoSamples ? *genoSamples : samples, shard, out, mei, annoCfg, methylCfg, true, dump);
 }
 
 // `delly lr -v sites.bcf` over ranks (ids = file order, src/tegua.h:157)
 inline int dellyLrGenotypeSharded(dgpu_ctx* ctx, Config const& c, std::vector<uint32_t> const& target_len, std::vector<std::string> const& target_name,
                                   std::vector<const char*> const& chrseq, std::vector<VcfSite> const& sites, bool headerHasConsBp, std::vector<LrSample> const& samples,
                                   Shard const& shard, LrMultiCallSet& out, MeiTemplates const* mei = nullptr, AnnoConfig const& annoCfg = AnnoConfig(),
-                                  MethylConfig const* methylCfg = nullptr) {
+                                  MethylConfig const* methylCfg = nullptr, SvReadDump* dump = nullptr) {
   out = LrMultiCallSet();
+  if (dump && shard.active()) return DGPU_ERR_ARG;
   const bool ok = vcfParseSites(sites, headerHasConsBp, target_name, out.svs);
   for (auto const& sv : out.svs)
     if (sv.chr < 0 || sv.chr2 < 0) return DGPU_ERR_ARG;
   for (std::size_t i = 0; i < out.svs.size(); ++i)
     if (out.svs[i].id != (int32_t) i) return DGPU_ERR_ARG;   // the count vectors are indexed by id
-  const int rc = genotypeLrSitesSharded(ctx, c, target_len, target_name, chrseq, samples, shard, out, mei, annoCfg, methylCfg, false);
+  const int rc = genotypeLrSitesSharded(ctx, c, target_len, target_name, chrseq, samples, shard, out, mei, annoCfg, methylCfg, false, dump);
   if (rc) return rc;
   return ok ? DGPU_OK : DGPU_ERR_ARG;
 }

@@ -258,6 +258,13 @@ struct ReadCount {  // src/util.h:69-76
   int32_t leftRC = 0, rc = 0, rightRC = 0;
 };
 
+// One ALT-supporting read of an SV, for the SV-read dump (host/svreaddump.hpp)
+struct SvReadEvent {
+  uint32_t rec;    // index into the genotyped record list
+  uint32_t svid;
+  int32_t svt;     // the type the reference names the id after (_addID)
+};
+
 // src/genotype.h:30-41
 inline int32_t _readStart(LrRecord const& r) {
   uint32_t rp = (uint32_t) r.pos;
@@ -307,10 +314,11 @@ inline int32_t _findSeqBp(LrRecord const& r, uint32_t pos) {
 // The reference's first cap test (ref.size() + alt.size() >= maxGenoReadCount, :231) is implied by its second
 // (reads seen for this SV, :233) because a read adds at most one quality after it has been counted; only the second
 // is evaluated here, which is what makes the candidates independent of the scores.
+// dump: receives the ALT-supporting (read, SV) groups in evaluation order (src/genotype.h:325-331)
 inline int genotypeLRBatch(dgpu_ctx* ctx, Config const& c, std::vector<uint32_t> const& target_len, std::vector<std::string> const& target_name,
                            std::vector<const char*> const& chrseq, std::vector<StructuralVariantRecord>& svs, std::vector<LrRecord> const& recs,
                            std::vector<JunctionCount>& jctMap, std::vector<ReadCount>& covMap, MethylConfig const* methylCfg = nullptr,
-                           std::vector<MethylInfo>* methylMap = nullptr) {
+                           std::vector<MethylInfo>* methylMap = nullptr, std::vector<SvReadEvent>* dump = nullptr) {
   jctMap.assign(svs.size(), JunctionCount());
   covMap.assign(svs.size(), ReadCount());
   const bool wantMethyl = (methylCfg != nullptr) && (methylMap != nullptr);
@@ -477,6 +485,7 @@ inline int genotypeLRBatch(dgpu_ctx* ctx, Config const& c, std::vector<uint32_t>
       if (rec.hp == 1) jc.hp1ref.push_back(qual);
       else if (rec.hp == 2) jc.hp2ref.push_back(qual);
     } else {
+      if (dump) dump->push_back(SvReadEvent{groupKey[g].first, groupKey[g].second, svs[groupKey[g].second].svt});
       jc.alt.push_back(qual);
       if (rec.hp == 1) jc.hp1alt.push_back(qual);
       else if (rec.hp == 2) jc.hp2alt.push_back(qual);
@@ -548,15 +557,15 @@ inline int prepareJunctionProbes(dgpu_ctx* ctx, Config const& c, std::vector<uin
 }
 
 inline int annotateJunctionReadsWithProbes(dgpu_ctx* ctx, Config const& c, std::vector<uint32_t> const& target_len, JunctionProbes const& probes, std::size_t nSv,
-                                           std::vector<SrRecord> const& recs, std::vector<JunctionCount>& countMap);
+                                           std::vector<SrRecord> const& recs, std::vector<JunctionCount>& countMap, std::vector<SvReadEvent>* dump = nullptr);
 
 inline int annotateJunctionReadsBatch(dgpu_ctx* ctx, Config const& c, std::vector<uint32_t> const& target_len, std::vector<std::string> const& target_name,
                                       std::vector<const char*> const& chrseq, std::vector<StructuralVariantRecord>& svs, std::vector<SrRecord> const& recs,
-                                      std::vector<JunctionCount>& countMap) {
+                                      std::vector<JunctionCount>& countMap, std::vector<SvReadEvent>* dump = nullptr) {
   JunctionProbes probes;
   int rc = prepareJunctionProbes(ctx, c, target_len, target_name, chrseq, svs, probes);
   if (rc) return rc;
-  return annotateJunctionReadsWithProbes(ctx, c, target_len, probes, svs.size(), recs, countMap);
+  return annotateJunctionReadsWithProbes(ctx, c, target_len, probes, svs.size(), recs, countMap, dump);
 }
 
 // the per-file pass (src/coverage.h:346-548, :671-675) over probes prepared once.
@@ -568,8 +577,10 @@ inline int annotateJunctionReadsBatch(dgpu_ctx* ctx, Config const& c, std::vecto
 //    all jobs go to the device in as few dgpu_edit_distance calls as the 4 GiB arena allows, and the merge applies the cap in job order;
 //  * the arena holds every probe once and every read once per orientation (the ALT and REF job of a read share it; BAM_FREVERSE-dependent
 //    orientation per breakpoint is src/split.h:55-68), instead of three strings per job.
+// dump: receives the ALT junction reads in job order (src/coverage.h:528-532). The reference aligns one job at a time when it dumps and checks
+// the cap against exact counts before each alignment; the merge below applies the same check to the same jobs in the same order.
 inline int annotateJunctionReadsWithProbes(dgpu_ctx* ctx, Config const& c, std::vector<uint32_t> const& target_len, JunctionProbes const& probes, std::size_t nSv,
-                                           std::vector<SrRecord> const& recs, std::vector<JunctionCount>& countMap) {
+                                           std::vector<SrRecord> const& recs, std::vector<JunctionCount>& countMap, std::vector<SvReadEvent>* dump) {
   std::vector<std::vector<std::string> > const& refProbeArr = probes.refProbeArr;
   std::vector<std::vector<std::string> > const& consProbeArr = probes.consProbeArr;
   std::vector<std::vector<BpRegion> > const& bpRegion = probes.bpRegion;
@@ -696,8 +707,10 @@ inline int annotateJunctionReadsWithProbes(dgpu_ctx* ctx, Config const& c, std::
       const uint8_t qual = (uint8_t) std::min(255, std::min((int) ((isRef ? scoreRef : scoreAlt) * 35), (int) j.qual));
       JunctionCount& jc = countMap[j.svId];
       if ((jc.ref.size() + jc.alt.size()) >= c.maxGenoReadCount) continue;
-      if (!isRef) jc.alt.push_back(qual);
-      else if (++refAlignedReadCount[j.svId] % 2) jc.ref.push_back(qual);
+      if (!isRef) {
+        jc.alt.push_back(qual);
+        if (dump) dump->push_back(SvReadEvent{j.rec, j.svId, j.svt});
+      } else if (++refAlignedReadCount[j.svId] % 2) jc.ref.push_back(qual);
     }
     done = end;
   }
@@ -735,9 +748,10 @@ inline int32_t _isizeMappingPos(SrRecord const& r, int32_t isize) {
 // SV's type whose mate lands near the other breakpoint, and the left / body / right read-depth of every SV.
 // svOnChr as produced by generateProbesBatch. The reference keys its mate table by a hash of (name, tid, pos, mtid, mpos);
 // here the key is the tuple itself.
+// dump: receives the ALT-spanning pair events in contig order, record order within a contig (src/coverage.h:652-657)
 inline void annotateSpanningAndDepth(Config const& c, LibraryInfo const& lib, std::vector<uint32_t> const& target_len,
                                      std::vector<StructuralVariantRecord> const& svs, std::vector<bool> const& svOnChr, std::vector<SrRecord> const& recs,
-                                     std::vector<ReadCount>& covCount, std::vector<SpanningCount>& spanMap) {
+                                     std::vector<ReadCount>& covCount, std::vector<SpanningCount>& spanMap, std::vector<SvReadEvent>* dump = nullptr) {
   covCount.assign(svs.size(), ReadCount());
   spanMap.assign(svs.size(), SpanningCount());
   typedef std::tuple<uint64_t, int32_t, int32_t, int32_t, int32_t> TPairKey;
@@ -773,6 +787,7 @@ inline void annotateSpanningAndDepth(Config const& c, LibraryInfo const& lib, st
     }
   }
   std::vector<std::vector<SpanEvent> > events((std::size_t) nchr);
+  std::vector<std::vector<SvReadEvent> > dumpOf(dump ? (std::size_t) nchr : 0);
   auto doContig = [&](std::size_t refIndexU) {
     const int32_t refIndex = (int32_t) refIndexU;
     if (!svOnChr[refIndex]) return;
@@ -780,6 +795,7 @@ inline void annotateSpanningAndDepth(Config const& c, LibraryInfo const& lib, st
     TClipQual clip;
     TClipQual& cliptra = cliptraOf[refIndex];
     std::vector<SpanEvent>& ev = events[refIndex];
+    std::vector<SvReadEvent>* dumpEv = dump ? &dumpOf[refIndex] : nullptr;
     const int32_t tlen = (int32_t) target_len[refIndex];
     std::vector<uint16_t> covFragment((std::size_t) tlen, 0), covBases((std::size_t) tlen, 0);
     // base coverage as a difference array (one +1 / -1 per aligned block instead of one increment per base); the reference's saturating
@@ -858,8 +874,10 @@ inline void annotateSpanningAndDepth(Config const& c, LibraryInfo const& lib, st
         const bool spanvalid = (itSpan != spanPoint.end()) && (itSpan->bppos < pend);
         if (spanvalid) {
           for (; (itSpan != spanPoint.end()) && (pend >= itSpan->bppos); ++itSpan)
-            if ((svt == itSpan->svt) && (rec.mtid == itSpan->chr2) && (std::abs(rec.mpos - itSpan->otherBppos) < lib.maxNormalISize))
+            if ((svt == itSpan->svt) && (rec.mtid == itSpan->chr2) && (std::abs(rec.mpos - itSpan->otherBppos) < lib.maxNormalISize)) {
               ev.push_back(SpanEvent{itSpan->id, 1, pairQuality});
+              if (dumpEv) dumpEv->push_back(SvReadEvent{(uint32_t) q, itSpan->id, itSpan->svt});
+            }
         }
       }
     }
@@ -906,6 +924,7 @@ inline void annotateSpanningAndDepth(Config const& c, LibraryInfo const& lib, st
       if (e.alt) spanMap[e.id].alt.push_back(e.quality);
       else if (++refAlignedSpanCount[e.id] % 2) spanMap[e.id].ref.push_back(e.quality);
     }
+  for (auto const& v : dumpOf) dump->insert(dump->end(), v.begin(), v.end());
 }
 
 }  // namespace dellyb200

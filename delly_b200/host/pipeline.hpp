@@ -9,6 +9,7 @@
 #include "gl.hpp"
 #include "scan.hpp"
 #include "svanno.hpp"
+#include "svreaddump.hpp"
 #include "vcfparse.hpp"
 
 namespace dellyb200 {
@@ -24,8 +25,10 @@ struct SrCallSet {
 // The part of dellyRun after the SV list exists (src/delly.h:155-178): sort + renumber, annotateCoverage, per-sample genotype fields.
 // out.svs holds the SVs on entry (from discovery or from a site list).
 // `probes`: the junction probes of the (already sorted and renumbered) SV list when the caller prepared them once for several samples.
+// `dump`: receives this sample's SV-read events.
 inline int genotypeSrSites(dgpu_ctx* ctx, Config const& c, LibraryInfo const& lib, std::vector<uint32_t> const& target_len, std::vector<std::string> const& target_name,
-                           std::vector<const char*> const& chrseq, std::vector<SrRecord> const& recs, SrCallSet& out, JunctionProbes const* probes = nullptr) {
+                           std::vector<const char*> const& chrseq, std::vector<SrRecord> const& recs, SrCallSet& out, JunctionProbes const* probes = nullptr,
+                           SvReadDump::File* dump = nullptr) {
   int rc = DGPU_OK;
   if (!probes) {
     std::sort(out.svs.begin(), out.svs.end());
@@ -33,12 +36,12 @@ inline int genotypeSrSites(dgpu_ctx* ctx, Config const& c, LibraryInfo const& li
   }
   if (out.svs.empty()) return DGPU_OK;
   // annotateCoverage = junction-read half + spanning / read-depth half (independent of each other)
-  if (probes) rc = annotateJunctionReadsWithProbes(ctx, c, target_len, *probes, out.svs.size(), recs, out.jctMap);
-  else rc = annotateJunctionReadsBatch(ctx, c, target_len, target_name, chrseq, out.svs, recs, out.jctMap);
+  if (probes) rc = annotateJunctionReadsWithProbes(ctx, c, target_len, *probes, out.svs.size(), recs, out.jctMap, dump ? &dump->sr : nullptr);
+  else rc = annotateJunctionReadsBatch(ctx, c, target_len, target_name, chrseq, out.svs, recs, out.jctMap, dump ? &dump->sr : nullptr);
   if (rc) return rc;
   std::vector<bool> svOnChr(target_len.size(), false);
   for (auto const& sv : out.svs) { svOnChr[sv.chr] = true; svOnChr[sv.chr2] = true; }
-  annotateSpanningAndDepth(c, lib, target_len, out.svs, svOnChr, recs, out.rcMap, out.spanMap);
+  annotateSpanningAndDepth(c, lib, target_len, out.svs, svOnChr, recs, out.rcMap, out.spanMap, dump ? &dump->pe : nullptr);
   static const BoLog bl;
   out.format.resize(out.svs.size());
   for (std::size_t i = 0; i < out.svs.size(); ++i) {
