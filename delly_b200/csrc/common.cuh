@@ -96,6 +96,42 @@ int dgpu_reserve(dgpu_ctx* ctx, int slot, size_t bytes, void** out);
     if (_e != cudaSuccess) return dgpu_set_cuda_error((ctx), _e, name); \
   } while (0)
 
+// Bytes a planner may reserve in workspace `slot`: 60 % of the free device memory (cudaMemGetInfo) plus what the slot already holds.
+inline size_t dgpu_workspace_budget(const dgpu_ctx* ctx, int slot, size_t free_bytes) { return (size_t) ((double) free_bytes * 0.6) + ctx->bufs[slot].cap; }
+
+// Independent launches of one batch call, side by side on the context's fork/join pool inside the profiling bracket on `st`. begin() records
+// the fork event on st; next() gives launch k pool stream k % DGPU_FORK_STREAMS, whose first launch waits for the fork event; end() makes st
+// wait for every pool stream used. A caller that synchronises st therefore sees every result, and last_kernel_ms spans all launches. With
+// one launch or none nothing forks and every launch goes on st.
+struct DgpuFork {
+  dgpu_ctx* ctx;
+  cudaStream_t st;
+  bool fork;
+  int k = 0;  // launches handed out so far
+  DgpuFork(dgpu_ctx* c, cudaStream_t s, size_t launches) : ctx(c), st(s), fork(launches > 1) {}
+  int begin() {
+    int rc;
+    if (fork && (rc = dgpu_fork_init(ctx))) return rc;
+    dgpu_prof_begin(ctx, st);
+    if (fork) DGPU_CUDA(ctx, cudaEventRecord(ctx->fork_events[0], st));
+    return DGPU_OK;
+  }
+  int next(cudaStream_t& cs) {
+    cs = fork ? ctx->fork_streams[k % DGPU_FORK_STREAMS] : st;
+    if (fork && k < DGPU_FORK_STREAMS) DGPU_CUDA(ctx, cudaStreamWaitEvent(cs, ctx->fork_events[0], 0));
+    ++k;
+    return DGPU_OK;
+  }
+  int end() {
+    for (int s = 0; fork && s < k && s < DGPU_FORK_STREAMS; ++s) {
+      DGPU_CUDA(ctx, cudaEventRecord(ctx->fork_events[1 + s], ctx->fork_streams[s]));
+      DGPU_CUDA(ctx, cudaStreamWaitEvent(st, ctx->fork_events[1 + s], 0));
+    }
+    dgpu_prof_end(ctx, st);
+    return DGPU_OK;
+  }
+};
+
 // Lets `kernel` launch with `smem` bytes of dynamic shared memory (an opt-in above 48 KiB).
 template <typename K>
 int dgpu_smem_optin(dgpu_ctx* ctx, K* kernel, size_t smem, const char* name) {

@@ -32,7 +32,9 @@
 #include "common.cuh"
 #include "myers.cuh"
 #include <algorithm>
+#include <array>
 #include <cstdio>
+#include <utility>
 
 namespace {
 
@@ -998,6 +1000,31 @@ int dgpu_pipe_init(dgpu_ctx* ctx) {
   return DGPU_OK;
 }
 
+// The class kernels that take EdArgs alone, [class][want_end]: ed_small for classes 1..4, ed_pair and ed_pack for the target-sharing
+// pairs. Pairs return no end locations (EdArgs::pair needs end_loc == nullptr), so their kernel fills both columns. Class 5 is a chain of
+// its own (launch_mode).
+using EdKernel = void (*)(EdArgs);
+template <int MODE>
+constexpr EdKernel ED_KERNELS[ED_NCLS][2] = {
+    {nullptr, nullptr},
+    {ed_small_kernel<1, MODE, false>, ed_small_kernel<1, MODE, true>}, {ed_small_kernel<2, MODE, false>, ed_small_kernel<2, MODE, true>},
+    {ed_small_kernel<3, MODE, false>, ed_small_kernel<3, MODE, true>}, {ed_small_kernel<4, MODE, false>, ed_small_kernel<4, MODE, true>},
+    {nullptr, nullptr},
+    {ed_pair_kernel<1>, ed_pair_kernel<1>}, {ed_pair_kernel<2>, ed_pair_kernel<2>}, {ed_pair_kernel<3>, ed_pair_kernel<3>},
+    {ed_pair_kernel<4>, ed_pair_kernel<4>}, {ed_pack_kernel<3, 1>, ed_pack_kernel<3, 1>}, {ed_pack_kernel<5, 2>, ed_pack_kernel<5, 2>}};
+
+// Class 5's kernels: the band pass of each band class and the full matrix, [0] without and [1] with equality tables
+using EdBandKernel = void (*)(EdArgs, uint32_t*, uint32_t);
+template <bool EQ, size_t... C>
+constexpr std::array<EdBandKernel, EDB_CLASSES> ed_band_kernels(std::index_sequence<C...>) {
+  return {{ed_band_kernel<edb_lanes(C), EQ>...}};
+}
+constexpr std::array<EdBandKernel, EDB_CLASSES> ED_BAND_KERNELS[2] = {ed_band_kernels<false>(std::make_index_sequence<EDB_CLASSES>()),
+                                                                      ed_band_kernels<true>(std::make_index_sequence<EDB_CLASSES>())};
+using EdLongKernel = void (*)(EdArgs, const uint32_t*, const uint32_t*);
+template <int MODE>
+constexpr EdLongKernel ED_LONG_KERNELS[2] = {ed_long_kernel<MODE, false>, ed_long_kernel<MODE, true>};
+
 template <int MODE>
 int launch_mode(dgpu_ctx* ctx, EdArgs& a, const uint32_t* hc, cudaStream_t st) {
   const int sms = ctx->num_sms;
@@ -1007,6 +1034,7 @@ int launch_mode(dgpu_ctx* ctx, EdArgs& a, const uint32_t* hc, cudaStream_t st) {
     return need < cap ? need : cap;
   };
   const bool want_end = (a.end_loc != nullptr);
+  const bool eq = (a.eq_cls != nullptr);
   // Scratch of class 5, reserved before any class kernel of this call is launched (see the note on dgpu_reserve where perm is reserved).
   const bool band = MODE == DGPU_MODE_NW && !ctx->no_band;
   const uint32_t g5 = grid_for(hc[5], EDL_WARPS, 8);
@@ -1030,97 +1058,46 @@ int launch_mode(dgpu_ctx* ctx, EdArgs& a, const uint32_t* hc, cudaStream_t st) {
   // one class on stream cs: ed_small / ed_pair / ed_pack, or class 5's chain in order on one stream (band passes narrowest first, as a
   // pass queues what it could not certify for the next one, then the full matrix; without band passes the full matrix alone)
   auto launch = [&](int c, cudaStream_t cs) -> int {
-    const uint32_t g = grid_for(hc[c], ED_THREADS, ED_CTAS_PER_SM);
-    switch (c) {
-#define ED_CASE_SMALL(NWV)                                                                  \
-      case NWV:                                                                             \
-        if (want_end) ed_small_kernel<NWV, MODE, true><<<g, ED_THREADS, 0, cs>>>(a);        \
-        else ed_small_kernel<NWV, MODE, false><<<g, ED_THREADS, 0, cs>>>(a);                \
-        DGPU_LAUNCH_CHECK(ctx, "ed_small");                                                 \
-        return DGPU_OK;
-      ED_CASE_SMALL(1)
-      ED_CASE_SMALL(2)
-      ED_CASE_SMALL(3)
-      ED_CASE_SMALL(4)
-#undef ED_CASE_SMALL
-#define ED_CASE_PAIR(NWV)                                                                   \
-      case ED_PAIR + NWV:                                                                   \
-        ed_pair_kernel<NWV><<<g, ED_THREADS, 0, cs>>>(a);                                   \
-        DGPU_LAUNCH_CHECK(ctx, "ed_pair");                                                  \
-        return DGPU_OK;
-      ED_CASE_PAIR(1)
-      ED_CASE_PAIR(2)
-      ED_CASE_PAIR(3)
-      ED_CASE_PAIR(4)
-#undef ED_CASE_PAIR
-      case ED_PACK:
-        ed_pack_kernel<3, 1><<<g, ED_THREADS, 0, cs>>>(a);
-        DGPU_LAUNCH_CHECK(ctx, "ed_pack");
-        return DGPU_OK;
-      case ED_PACK + 1:
-        ed_pack_kernel<5, 2><<<g, ED_THREADS, 0, cs>>>(a);
-        DGPU_LAUNCH_CHECK(ctx, "ed_pack");
-        return DGPU_OK;
-      default:
-        break;
+    if (c != 5) {
+      const EdKernel k = ED_KERNELS<MODE>[c][want_end];
+      k<<<grid_for(hc[c], ED_THREADS, ED_CTAS_PER_SM), ED_THREADS, 0, cs>>>(a);
+      DGPU_LAUNCH_CHECK(ctx, c <= 4 ? "ed_small" : c < ED_PACK ? "ed_pair" : "ed_pack");
+      return DGPU_OK;
     }
+    const uint32_t *list = nullptr, *list_cnt = nullptr;   // ed_long_kernel's jobs: class 5 of perm, or what the band passes left
     if (band) {
       const uint32_t cap = hc[5];
       ed_band_plan_kernel<<<grid_for(hc[5], 8, 8), 256, 0, cs>>>(a, lists, cap);
       DGPU_LAUNCH_CHECK(ctx, "ed_band_plan");
-#define ED_LAUNCH_BAND(GV)                                                                                                    \
-      if (a.eq_cls) ed_band_kernel<GV, true><<<grid_for(hc[5], EDB_WARPS * (32 / GV), 5), EDB_WARPS * 32, 0, cs>>>(a, lists, cap);  \
-      else ed_band_kernel<GV, false><<<grid_for(hc[5], EDB_WARPS * (32 / GV), 5), EDB_WARPS * 32, 0, cs>>>(a, lists, cap);         \
-      DGPU_LAUNCH_CHECK(ctx, "ed_band");
-      ED_LAUNCH_BAND(2)
-      ED_LAUNCH_BAND(4)
-      ED_LAUNCH_BAND(8)
-      ED_LAUNCH_BAND(16)
-      ED_LAUNCH_BAND(32)
-#undef ED_LAUNCH_BAND
-      if (a.eq_cls) ed_long_kernel<MODE, true><<<g5, EDL_WARPS * 32, 0, cs>>>(a, lists + (size_t) EDB_CLASSES * cap, a.counts + ED_BANDQ + EDB_CLASSES);
-      else ed_long_kernel<MODE, false><<<g5, EDL_WARPS * 32, 0, cs>>>(a, lists + (size_t) EDB_CLASSES * cap, a.counts + ED_BANDQ + EDB_CLASSES);
-    } else if (a.eq_cls) {
-      ed_long_kernel<MODE, true><<<g5, EDL_WARPS * 32, 0, cs>>>(a, nullptr, nullptr);
-    } else {
-      ed_long_kernel<MODE, false><<<g5, EDL_WARPS * 32, 0, cs>>>(a, nullptr, nullptr);
+      for (int bc = 0; bc < EDB_CLASSES; ++bc) {
+        const EdBandKernel k = ED_BAND_KERNELS[eq][bc];
+        k<<<grid_for(hc[5], EDB_WARPS * (32 / edb_lanes(bc)), 5), EDB_WARPS * 32, 0, cs>>>(a, lists, cap);
+        DGPU_LAUNCH_CHECK(ctx, "ed_band");
+      }
+      list = lists + (size_t) EDB_CLASSES * cap;
+      list_cnt = a.counts + ED_BANDQ + EDB_CLASSES;
     }
+    const EdLongKernel k = ED_LONG_KERNELS<MODE>[eq];
+    k<<<g5, EDL_WARPS * 32, 0, cs>>>(a, list, list_cnt);
     DGPU_LAUNCH_CHECK(ctx, "ed_long");
     return DGPU_OK;
   };
 
-  // The classes are independent once perm is scattered, so they run side by side: the k-th class launched goes to pool stream
-  // k % DGPU_FORK_STREAMS, each stream's first class waits for the fork event recorded on st, and st waits for every pool stream used
-  // before the profiling bracket closes. A caller that synchronises st therefore sees every result, and last_kernel_ms spans all classes.
+  // The classes are independent once perm is scattered, so they run side by side on the fork/join pool (DgpuFork).
   // Costliest class per job first: the block scheduler starts the CTAs of earlier launches first, so the classes launched last fill the
   // SMs while the long ones drain, where one stream let every class drain the GPU alone.
   static constexpr int order[] = {ED_PACK + 1, ED_PAIR + 2, ED_PAIR + 3, ED_PAIR + 4, ED_PACK, ED_PAIR + 1, 4, 3, 2, 1, 5};
   int nl = 0;
   for (int c : order) nl += hc[c] != 0;
-  const bool fork = nl > 1;
+  DgpuFork fork(ctx, st, nl);
   int rc;
-  if (fork && (rc = dgpu_fork_init(ctx))) return rc;
-  dgpu_prof_begin(ctx, st);
-  if (fork) DGPU_CUDA(ctx, cudaEventRecord(ctx->fork_events[0], st));
-  int k = 0;
+  if ((rc = fork.begin())) return rc;
   for (int c : order) {
     if (!hc[c]) continue;
-    cudaStream_t cs = st;
-    if (fork) {
-      cs = ctx->fork_streams[k % DGPU_FORK_STREAMS];
-      if (k < DGPU_FORK_STREAMS) DGPU_CUDA(ctx, cudaStreamWaitEvent(cs, ctx->fork_events[0], 0));
-    }
-    ++k;
-    if ((rc = launch(c, cs))) return rc;
+    cudaStream_t cs;
+    if ((rc = fork.next(cs)) || (rc = launch(c, cs))) return rc;
   }
-  if (fork) {  // join
-    for (int s = 0; s < std::min(k, DGPU_FORK_STREAMS); ++s) {
-      DGPU_CUDA(ctx, cudaEventRecord(ctx->fork_events[1 + s], ctx->fork_streams[s]));
-      DGPU_CUDA(ctx, cudaStreamWaitEvent(st, ctx->fork_events[1 + s], 0));
-    }
-  }
-  dgpu_prof_end(ctx, st);
-  return DGPU_OK;
+  return fork.end();
 }
 
 }  // namespace

@@ -416,11 +416,6 @@ __global__ void hb_concat_kernel(const uint8_t* tmp_ops, const uint32_t* job_lea
   if (lane == 0) ops_len[w] = pos;
 }
 
-template <typename T> struct HostDev {  // small host vector mirrored on the device for one launch round
-  std::vector<T> h;
-  T* d = nullptr;
-};
-
 struct Seg { uint32_t job, qoff, qlen, toff, tlen; int32_t score; };
 
 // Runs a set of SegJobs (already on the host) class by class.
@@ -459,13 +454,17 @@ constexpr std::array<SegKernel, SEG_NCLS> seg_kernels(std::index_sequence<G...>)
 constexpr std::array<SegKernel, SEG_NCLS> SEG_KERNELS[2] = {seg_kernels<false>(std::make_index_sequence<SEG_NCLS - 1>()),
                                                             seg_kernels<true>(std::make_index_sequence<SEG_NCLS - 1>())};
 
-template <int G>
-int seg_band_launch(dgpu_ctx* ctx, SegJobs& a, bool use_eq, unsigned grid, cudaStream_t st) {
-  if (use_eq) seg_band_kernel<G, true><<<grid, SEGB_WARPS * 32, 0, st>>>(a);
-  else seg_band_kernel<G, false><<<grid, SEGB_WARPS * 32, 0, st>>>(a);
-  DGPU_LAUNCH_CHECK(ctx, "seg_band_kernel");
-  return DGPU_OK;
+// seg_band_kernel of each band class (G = edb_lanes), [0] without and [1] with equality tables
+template <bool EQ, size_t... C>
+constexpr std::array<SegKernel, EDB_CLASSES> segb_kernels(std::index_sequence<C...>) {
+  return {{seg_band_kernel<edb_lanes(C), EQ>...}};
 }
+constexpr std::array<SegKernel, EDB_CLASSES> SEGB_KERNELS[2] = {segb_kernels<false>(std::make_index_sequence<EDB_CLASSES>()),
+                                                                segb_kernels<true>(std::make_index_sequence<EDB_CLASSES>())};
+// the segments wider than the wavefront classes, [eq]
+using SegHalfKernel = void (*)(SegJobs, size_t);
+constexpr SegHalfKernel SEG_HALF_WIDE_KERNELS[2] = {seg_half_wide_kernel<false>, seg_half_wide_kernel<true>};
+constexpr SegKernel SEG_LEAF_WIDE_KERNELS[2] = {seg_leaf_wide_kernel<false>, seg_leaf_wide_kernel<true>};
 
 // narrowest band class that holds the segment's rows and certifies the optimum `k` of the problem (pm x pn) it belongs to; -1: none
 inline int seg_band_class(uint32_t m, uint32_t pm, uint32_t pn, int32_t k) {
@@ -551,8 +550,16 @@ int SegRunner::run(uint8_t* tmp_ops, int* colbuf) {
   a.seqs = seqs; a.q_off = d_qoff; a.q_len = d_qlen; a.t_off = d_toff; a.t_len = d_tlen; a.rev = d_rev; a.kind = d_kind; a.out_off = d_oo;
   a.out_len = d_out_len; a.corner = d_corner; a.tmp_ops = tmp_ops; a.colbuf = colbuf; a.eq = eq;
   a.plan_m = d_pm; a.plan_n = d_pn; a.eq_cls = eq_cls;
-  size_t free_b = 0, total_b = 0;
-  cudaMemGetInfo(&free_b, &total_b);
+  // One launch per kind of segment, in turn on st: band classes G = 2 .. 32, wide half columns, wide leaves, seg_kernel classes. A kind's CTA
+  // takes `per_cta` jobs, each with `stride` bytes of workspace in `slot` (a wide half column's scratch row, a leaf's trace storage, a
+  // seg_kernel job's directions and, from off_trace on, its trace); the grid is at most per_sm CTAs per SM, shrunk to the workspace budget.
+  struct Kind {
+    const std::vector<uint32_t>* jobs; size_t lo;   // the jobs and their offset in d_list
+    size_t per_cta; int per_sm, slot; size_t stride, off_trace; unsigned threads; size_t smem;
+    SegKernel k; SegHalfKernel half;                 // seg_half_wide_kernel (half) takes the stride as its row stride
+    const char* name;
+  };
+  std::vector<Kind> kinds;
   for (int bc = 0; bc < EDB_CLASSES; ++bc) {
     std::vector<uint32_t> const& L = lists[SEG_NCLS + bc];
     if (L.empty()) continue;
@@ -560,60 +567,20 @@ int SegRunner::run(uint8_t* tmp_ops, int* colbuf) {
     size_t maxsteps = 0;   // trace storage of a leaf: one uint4 per lane and step
     for (uint32_t i : L)
       if (kind[i] == 0) maxsteps = std::max<size_t>(maxsteps, 65 * (size_t) ((tlen[i] - 1) >> 6) + ((tlen[i] - 1) & 63) + G);
-    a.off_trace = 0;
-    a.work_stride = maxsteps * G * sizeof(uint4);
-    size_t grid = std::min<size_t>((L.size() + (size_t) jpw * SEGB_WARPS - 1) / ((size_t) jpw * SEGB_WARPS), (size_t) ctx->num_sms * 8);
-    const size_t per_block = (size_t) SEGB_WARPS * jpw * a.work_stride;
-    const size_t budget = (size_t) ((double) free_b * 0.6) + ctx->bufs[SLOT_WAVEFRONT].cap;
-    if (per_block && grid * per_block > budget) grid = std::max<size_t>(1, budget / per_block);
-    void* w;
-    if ((rc = dgpu_reserve(ctx, SLOT_WAVEFRONT, std::max<size_t>(grid * per_block, 256), &w))) return rc;
-    a.work = (uint8_t*) w;
-    a.list = d_list + lo[SEG_NCLS + bc];
-    a.count = (uint32_t) L.size();
-    switch (bc) {
-      case 0: rc = seg_band_launch<2>(ctx, a, use_eq, (unsigned) grid, st); break;
-      case 1: rc = seg_band_launch<4>(ctx, a, use_eq, (unsigned) grid, st); break;
-      case 2: rc = seg_band_launch<8>(ctx, a, use_eq, (unsigned) grid, st); break;
-      case 3: rc = seg_band_launch<16>(ctx, a, use_eq, (unsigned) grid, st); break;
-      default: rc = seg_band_launch<32>(ctx, a, use_eq, (unsigned) grid, st); break;
-    }
-    if (rc) return rc;
+    kinds.push_back({&L, lo[SEG_NCLS + bc], (size_t) jpw * SEGB_WARPS, 8, SLOT_WAVEFRONT, maxsteps * G * sizeof(uint4), 0, SEGB_WARPS * 32, 0,
+                     SEGB_KERNELS[use_eq][bc], nullptr, "seg_band_kernel"});
   }
-  if (!wide_half.empty()) {   // one warp per half column, a scratch row of n bytes per warp (SLOT_EP_HROW)
+  if (!wide_half.empty()) {   // one warp per half column, a scratch row of n bytes per warp
     size_t nmax = 0;
     for (uint32_t i : wide_half) nmax = std::max<size_t>(nmax, tlen[i]);
-    const size_t stride = (nmax + 255) & ~(size_t) 255;
-    size_t grid = std::min<size_t>((wide_half.size() + EPW_WARPS - 1) / EPW_WARPS, (size_t) ctx->num_sms * 4);
-    const size_t budget = (size_t) ((double) free_b * 0.6) + ctx->bufs[SLOT_EP_HROW].cap;
-    if (grid * EPW_WARPS * stride > budget) grid = std::max<size_t>(1, budget / (EPW_WARPS * stride));
-    void* w;
-    if ((rc = dgpu_reserve(ctx, SLOT_EP_HROW, grid * EPW_WARPS * stride, &w))) return rc;
-    a.work = (uint8_t*) w;
-    a.list = d_list + lo_half;
-    a.count = (uint32_t) wide_half.size();
-    if (use_eq) seg_half_wide_kernel<true><<<(unsigned) grid, EPW_WARPS * 32, 0, st>>>(a, stride);
-    else seg_half_wide_kernel<false><<<(unsigned) grid, EPW_WARPS * 32, 0, st>>>(a, stride);
-    DGPU_LAUNCH_CHECK(ctx, "seg_half_wide_kernel");
+    kinds.push_back({&wide_half, lo_half, EPW_WARPS, 4, SLOT_EP_HROW, (nmax + 255) & ~(size_t) 255, 0, EPW_WARPS * 32, 0, nullptr,
+                     SEG_HALF_WIDE_KERNELS[use_eq], "seg_half_wide_kernel"});
   }
   if (!wide_leaf.empty()) {   // trace storage of a leaf: one uint4 per block and column
-    constexpr int jpw = 32 / EPL_G;
     size_t maxcells = 0;
     for (uint32_t i : wide_leaf) maxcells = std::max<size_t>(maxcells, (size_t) tlen[i] * ((qlen[i] + 63) >> 6));
-    a.off_trace = 0;
-    a.work_stride = maxcells * sizeof(uint4);
-    size_t grid = std::min<size_t>((wide_leaf.size() + (size_t) jpw * EPL_WARPS - 1) / ((size_t) jpw * EPL_WARPS), (size_t) ctx->num_sms * 8);
-    const size_t per_block = (size_t) EPL_WARPS * jpw * a.work_stride;
-    const size_t budget = (size_t) ((double) free_b * 0.6) + ctx->bufs[SLOT_WAVEFRONT].cap;
-    if (grid * per_block > budget) grid = std::max<size_t>(1, budget / per_block);
-    void* w;
-    if ((rc = dgpu_reserve(ctx, SLOT_WAVEFRONT, grid * per_block, &w))) return rc;
-    a.work = (uint8_t*) w;
-    a.list = d_list + lo_leaf;
-    a.count = (uint32_t) wide_leaf.size();
-    if (use_eq) seg_leaf_wide_kernel<true><<<(unsigned) grid, EPL_WARPS * 32, 0, st>>>(a);
-    else seg_leaf_wide_kernel<false><<<(unsigned) grid, EPL_WARPS * 32, 0, st>>>(a);
-    DGPU_LAUNCH_CHECK(ctx, "seg_leaf_wide_kernel");
+    kinds.push_back({&wide_leaf, lo_leaf, (size_t) (32 / EPL_G) * EPL_WARPS, 8, SLOT_WAVEFRONT, maxcells * sizeof(uint4), 0, EPL_WARPS * 32, 0,
+                     SEG_LEAF_WIDE_KERNELS[use_eq], nullptr, "seg_leaf_wide_kernel"});
   }
   for (int c = 1; c < SEG_NCLS; ++c) {
     if (lists[c].empty()) continue;
@@ -625,21 +592,28 @@ int SegRunner::run(uint8_t* tmp_ops, int* colbuf) {
       mnmax = std::max<size_t>(mnmax, (size_t) qlen[i] + tlen[i]);
     }
     auto al = [](size_t x) { return (x + 255) & ~(size_t) 255; };
-    a.off_trace = al(maxwords * 4 + 1024);
-    a.work_stride = a.off_trace + al(mnmax + 64);
-    const size_t smem = (mmax + 15) & ~(size_t) 15;
-    size_t grid = std::min<size_t>(lists[c].size(), (size_t) ctx->num_sms * g.per_sm);
-    size_t budget = (size_t) ((double) free_b * 0.6) + ctx->bufs[SLOT_WAVEFRONT].cap;
-    if (grid * a.work_stride > budget) grid = std::max<size_t>(1, budget / a.work_stride);
-    void* w;
-    if ((rc = dgpu_reserve(ctx, SLOT_WAVEFRONT, grid * a.work_stride, &w))) return rc;
+    const size_t off_trace = al(maxwords * 4 + 1024);
+    kinds.push_back({&lists[c], lo[c], 1, g.per_sm, SLOT_WAVEFRONT, off_trace + al(mnmax + 64), off_trace, (unsigned) g.T, (mmax + 15) & ~(size_t) 15,
+                     SEG_KERNELS[use_eq][c], nullptr, "seg_kernel"});
+  }
+  size_t free_b = 0, total_b = 0;
+  cudaMemGetInfo(&free_b, &total_b);
+  for (Kind const& k : kinds) {
+    size_t grid = std::min<size_t>((k.jobs->size() + k.per_cta - 1) / k.per_cta, (size_t) ctx->num_sms * k.per_sm);
+    const size_t per_block = k.per_cta * k.stride;
+    const size_t budget = dgpu_workspace_budget(ctx, k.slot, free_b);
+    if (per_block && grid * per_block > budget) grid = std::max<size_t>(1, budget / per_block);
+    void* w;   // at least 256 bytes: a band class of half columns alone stores no trace (the other kinds always take more)
+    if ((rc = dgpu_reserve(ctx, k.slot, std::max<size_t>(grid * per_block, 256), &w))) return rc;
     a.work = (uint8_t*) w;
-    a.list = d_list + lo[c];
-    a.count = (uint32_t) lists[c].size();
-    const SegKernel k = SEG_KERNELS[use_eq][c];
-    if ((rc = dgpu_smem_optin(ctx, k, smem, "cudaFuncSetAttribute(seg_kernel)"))) return rc;
-    k<<<(unsigned) grid, (unsigned) g.T, smem, st>>>(a);
-    DGPU_LAUNCH_CHECK(ctx, "seg_kernel");
+    a.list = d_list + k.lo;
+    a.count = (uint32_t) k.jobs->size();
+    a.work_stride = k.stride;
+    a.off_trace = k.off_trace;
+    if (!k.half && (rc = dgpu_smem_optin(ctx, k.k, k.smem, "cudaFuncSetAttribute(seg_kernel)"))) return rc;
+    if (k.half) k.half<<<(unsigned) grid, k.threads, 0, st>>>(a, k.stride);
+    else k.k<<<(unsigned) grid, k.threads, k.smem, st>>>(a);
+    DGPU_LAUNCH_CHECK(ctx, k.name);
   }
   return DGPU_OK;
 }
@@ -659,107 +633,75 @@ int check_max_slice(dgpu_ctx* ctx, uint32_t max_slice) {
   return DGPU_ERR_ARG;
 }
 
-// The device form of every entry point: a job whose aligned target slice is wider than max_slice gets status 2 alone.
-int ep_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
-           const uint32_t* q_off, const uint32_t* q_len, const uint32_t* t_off, const uint32_t* t_len,
-           int mode, const uint8_t* eq_pairs, uint32_t n_eq, uint64_t n, int32_t* dist, int32_t* start_loc, int32_t* end_loc,
-           uint8_t* ops, const uint64_t* ops_off, uint32_t* ops_len, uint32_t* status, uint32_t max_slice, void* stream) {
-  if (!ctx) return DGPU_ERR_ARG;
-  if (n == 0) return DGPU_OK;
-  if (n >= (1ull << 31) || seqs_bytes >= (1ull << 32)) return DGPU_ERR_ARG;
-  if (mode != DGPU_MODE_NW && mode != DGPU_MODE_SHW && mode != DGPU_MODE_HW) return DGPU_ERR_ARG;
-  if (!seqs || !q_off || !q_len || !t_off || !t_len || !dist || !start_loc || !end_loc || !ops || !ops_off || !ops_len || !status) return DGPU_ERR_ARG;
-  if (n_eq > 32 || (n_eq && !eq_pairs)) return DGPU_ERR_ARG;
-  DGPU_CUDA(ctx, cudaSetDevice(ctx->device));
-  cudaStream_t st = stream ? (cudaStream_t) stream : ctx->stream;
+// Distance and first end location of every job, then its start location (HW: a reversed SHW pass per mirror run); host copies of all three.
+int ep_locate(dgpu_ctx* ctx, cudaStream_t st, const uint8_t* seqs, uint64_t seqs_bytes, const uint32_t* q_off, const uint32_t* q_len,
+              const uint32_t* t_off, const uint32_t* t_len, int mode, const uint32_t* d_eqtabs, uint64_t n, std::vector<uint32_t> const& h_qlen,
+              std::vector<uint32_t> const& h_tlen, int32_t* dist, int32_t* start_loc, int32_t* end_loc, std::vector<int32_t>& h_dist,
+              std::vector<int32_t>& h_start, std::vector<int32_t>& h_end) {
   int rc;
   const uint32_t nb = (uint32_t) ((n + 255) / 256);
-  // host copies of the job geometry
-  std::vector<uint32_t> h_qoff(n), h_qlen(n), h_toff(n), h_tlen(n);
-  std::vector<uint64_t> h_opsoff(n);
-  DGPU_CUDA(ctx, cudaMemcpyAsync(h_qoff.data(), q_off, n * 4, cudaMemcpyDeviceToHost, st));
-  DGPU_CUDA(ctx, cudaMemcpyAsync(h_qlen.data(), q_len, n * 4, cudaMemcpyDeviceToHost, st));
-  DGPU_CUDA(ctx, cudaMemcpyAsync(h_toff.data(), t_off, n * 4, cudaMemcpyDeviceToHost, st));
-  DGPU_CUDA(ctx, cudaMemcpyAsync(h_tlen.data(), t_len, n * 4, cudaMemcpyDeviceToHost, st));
-  DGPU_CUDA(ctx, cudaMemcpyAsync(h_opsoff.data(), ops_off, n * 8, cudaMemcpyDeviceToHost, st));
-  SegRunner R;
-  R.ctx = ctx; R.st = st; R.seqs = seqs; R.use_eq = n_eq > 0; R.eq.f = nullptr; R.eq.s = nullptr;
-  const uint32_t* d_eqtabs = nullptr;  // f[256], s[256], cls[256 bytes]
-  if (n_eq) {
-    uint32_t tab[512 + 64] = {0};
-    for (uint32_t p = 0; p < n_eq; ++p) { tab[eq_pairs[2 * p]] |= 1u << p; tab[256 + eq_pairs[2 * p + 1]] |= 1u << p; }
-    uint8_t* cls = (uint8_t*) (tab + 512);
-    static const uint8_t sym[5] = {'A', 'C', 'G', 'T', 'N'};
-    for (uint32_t b = 0; b < 256; ++b)
-      for (int sy = 0; sy < 5; ++sy)
-        if (b == sym[sy] || (tab[b] & tab[256 + sym[sy]]) || (tab[256 + b] & tab[sym[sy]])) cls[b] |= (uint8_t) (1u << sy);
-    void* d_tab;
-    if ((rc = dgpu_reserve(ctx, SLOT_EP_EQTAB, sizeof(tab), &d_tab))) return rc;
-    DGPU_CUDA(ctx, cudaMemcpyAsync(d_tab, tab, sizeof(tab), cudaMemcpyHostToDevice, st));
-    DGPU_CUDA(ctx, cudaStreamSynchronize(st));  // tab is a stack array
-    R.eq.f = (const uint32_t*) d_tab; R.eq.s = (const uint32_t*) d_tab + 256; R.eq_cls = (const uint8_t*) ((const uint32_t*) d_tab + 512);
-    d_eqtabs = (const uint32_t*) d_tab;
-  }
-  std::vector<int32_t> h_dist(n), h_start(n), h_end(n);
-  {
-    // 1. distance + first end location (k = -1 at every PATH call site of the reference); generalised equalities ride along as tables
-    if ((rc = dgpu_edit_distance_impl(ctx, seqs, seqs_bytes, q_off, q_len, t_off, t_len, nullptr, mode, n, dist, end_loc, st, 0, d_eqtabs))) return rc;
-    void* d_rev = nullptr;
-    // mirror layout of the HW start pass: job i's reversed query at mq[i], its reversed target right after it, jobs back to back in runs
-    // of at most EP_MIRROR_RUN bytes; each run is mirrored and searched in one SHW pass (offsets relative to the run)
-    std::vector<uint32_t> h_moff;
-    std::vector<uint64_t> run_lo, run_bytes;
-    if (mode == DGPU_MODE_HW) {
-      h_moff.resize(2 * n);
-      uint64_t pos = 0;
-      for (uint64_t i = 0; i < n; ++i) {
-        const uint64_t need = (uint64_t) h_qlen[i] + h_tlen[i];
-        if (need > EP_MIRROR_RUN) { ctx->last_error = "dgpu_edit_path: a HW job's query and target exceed the start-pass mirror"; return DGPU_ERR_CAPACITY; }
-        if (i == 0 || pos + need > EP_MIRROR_RUN) {
-          if (i) run_bytes.push_back(pos);
-          run_lo.push_back(i);
-          pos = 0;
-        }
-        h_moff[i] = (uint32_t) pos; h_moff[n + i] = (uint32_t) (pos + h_qlen[i]);
-        pos += need;
+  // 1. distance + first end location (k = -1 at every PATH call site of the reference); generalised equalities ride along as tables
+  if ((rc = dgpu_edit_distance_impl(ctx, seqs, seqs_bytes, q_off, q_len, t_off, t_len, nullptr, mode, n, dist, end_loc, st, 0, d_eqtabs))) return rc;
+  void* d_rev = nullptr;
+  // mirror layout of the HW start pass: job i's reversed query at mq[i], its reversed target right after it, jobs back to back in runs
+  // of at most EP_MIRROR_RUN bytes; each run is mirrored and searched in one SHW pass (offsets relative to the run)
+  std::vector<uint32_t> h_moff;
+  std::vector<uint64_t> run_lo, run_bytes;
+  if (mode == DGPU_MODE_HW) {
+    h_moff.resize(2 * n);
+    uint64_t pos = 0;
+    for (uint64_t i = 0; i < n; ++i) {
+      const uint64_t need = (uint64_t) h_qlen[i] + h_tlen[i];
+      if (need > EP_MIRROR_RUN) { ctx->last_error = "dgpu_edit_path: a HW job's query and target exceed the start-pass mirror"; return DGPU_ERR_CAPACITY; }
+      if (i == 0 || pos + need > EP_MIRROR_RUN) {
+        if (i) run_bytes.push_back(pos);
+        run_lo.push_back(i);
+        pos = 0;
       }
-      run_bytes.push_back(pos);
-      run_lo.push_back(n);
-      const uint64_t run_max = *std::max_element(run_bytes.begin(), run_bytes.end());
-      // 2. start location: reversed query vs reversed target prefix, SHW, k = distance, LAST optimal end
-      void *d_mirror, *d_t2off, *d_t2len, *d_k2;
-      if ((rc = dgpu_reserve(ctx, SLOT_EP_MIRROR, run_max + 64, &d_mirror))) return rc;
-      if ((rc = dgpu_reserve(ctx, SLOT_EP_TABLE, n * 12, &d_t2off))) return rc;
-      if ((rc = dgpu_reserve(ctx, SLOT_EP_COLS, n * 4, &d_t2len))) return rc;
-      if ((rc = dgpu_reserve(ctx, SLOT_EP_BOUNDS, n * 8, &d_k2))) return rc;
-      d_rev = (uint8_t*) d_k2 + n * 4;
-      uint32_t* d_mq = (uint32_t*) d_t2off + n;
-      uint32_t* d_mt = d_mq + n;
-      DGPU_CUDA(ctx, cudaMemcpyAsync(d_mq, h_moff.data(), 2 * n * 4, cudaMemcpyHostToDevice, st));
-      ep_hwstart_jobs_kernel<<<nb, 256, 0, st>>>(d_mt, t_len, dist, end_loc, (uint32_t) n, (uint32_t*) d_t2off, (uint32_t*) d_t2len, (int32_t*) d_k2);
-      DGPU_LAUNCH_CHECK(ctx, "ep_hwstart_jobs");
-      for (size_t r = 0; r + 1 < run_lo.size(); ++r) {   // a run reuses the mirror after the previous run's pass on the same stream
-        const uint64_t j0 = run_lo[r], cnt = run_lo[r + 1] - j0;
-        const uint32_t wb = (uint32_t) ((cnt * 32 + 255) / 256);
-        ep_mirror_kernel<<<wb, 256, 0, st>>>(seqs, (uint8_t*) d_mirror, q_off + j0, q_len + j0, d_mq + j0, (uint32_t) cnt);
-        DGPU_LAUNCH_CHECK(ctx, "ep_mirror(q)");
-        ep_mirror_kernel<<<wb, 256, 0, st>>>(seqs, (uint8_t*) d_mirror, t_off + j0, t_len + j0, d_mt + j0, (uint32_t) cnt);
-        DGPU_LAUNCH_CHECK(ctx, "ep_mirror(t)");
-        if ((rc = dgpu_edit_distance_impl(ctx, (const uint8_t*) d_mirror, run_bytes[r], d_mq + j0, q_len + j0, (const uint32_t*) d_t2off + j0,
-                                          (const uint32_t*) d_t2len + j0, (const int32_t*) d_k2 + j0, DGPU_MODE_SHW, cnt, start_loc + j0,
-                                          (int32_t*) d_rev + j0, st, 1, d_eqtabs))) return rc;
-      }
+      h_moff[i] = (uint32_t) pos; h_moff[n + i] = (uint32_t) (pos + h_qlen[i]);
+      pos += need;
     }
-    ep_start_kernel<<<nb, 256, 0, st>>>(mode, q_len, t_len, dist, end_loc, (const int32_t*) d_rev, (uint32_t) n, start_loc);
-    DGPU_LAUNCH_CHECK(ctx, "ep_start");
-    DGPU_CUDA(ctx, cudaMemcpyAsync(h_dist.data(), dist, n * 4, cudaMemcpyDeviceToHost, st));
-    DGPU_CUDA(ctx, cudaMemcpyAsync(h_start.data(), start_loc, n * 4, cudaMemcpyDeviceToHost, st));
-    DGPU_CUDA(ctx, cudaMemcpyAsync(h_end.data(), end_loc, n * 4, cudaMemcpyDeviceToHost, st));
-    DGPU_CUDA(ctx, cudaStreamSynchronize(st));
+    run_bytes.push_back(pos);
+    run_lo.push_back(n);
+    const uint64_t run_max = *std::max_element(run_bytes.begin(), run_bytes.end());
+    // 2. start location: reversed query vs reversed target prefix, SHW, k = distance, LAST optimal end
+    void *d_mirror, *d_t2off, *d_t2len, *d_k2;
+    if ((rc = dgpu_reserve(ctx, SLOT_EP_MIRROR, run_max + 64, &d_mirror))) return rc;
+    if ((rc = dgpu_reserve(ctx, SLOT_EP_TABLE, n * 12, &d_t2off))) return rc;
+    if ((rc = dgpu_reserve(ctx, SLOT_EP_COLS, n * 4, &d_t2len))) return rc;
+    if ((rc = dgpu_reserve(ctx, SLOT_EP_BOUNDS, n * 8, &d_k2))) return rc;
+    d_rev = (uint8_t*) d_k2 + n * 4;
+    uint32_t* d_mq = (uint32_t*) d_t2off + n;
+    uint32_t* d_mt = d_mq + n;
+    DGPU_CUDA(ctx, cudaMemcpyAsync(d_mq, h_moff.data(), 2 * n * 4, cudaMemcpyHostToDevice, st));
+    ep_hwstart_jobs_kernel<<<nb, 256, 0, st>>>(d_mt, t_len, dist, end_loc, (uint32_t) n, (uint32_t*) d_t2off, (uint32_t*) d_t2len, (int32_t*) d_k2);
+    DGPU_LAUNCH_CHECK(ctx, "ep_hwstart_jobs");
+    for (size_t r = 0; r + 1 < run_lo.size(); ++r) {   // a run reuses the mirror after the previous run's pass on the same stream
+      const uint64_t j0 = run_lo[r], cnt = run_lo[r + 1] - j0;
+      const uint32_t wb = (uint32_t) ((cnt * 32 + 255) / 256);
+      ep_mirror_kernel<<<wb, 256, 0, st>>>(seqs, (uint8_t*) d_mirror, q_off + j0, q_len + j0, d_mq + j0, (uint32_t) cnt);
+      DGPU_LAUNCH_CHECK(ctx, "ep_mirror(q)");
+      ep_mirror_kernel<<<wb, 256, 0, st>>>(seqs, (uint8_t*) d_mirror, t_off + j0, t_len + j0, d_mt + j0, (uint32_t) cnt);
+      DGPU_LAUNCH_CHECK(ctx, "ep_mirror(t)");
+      if ((rc = dgpu_edit_distance_impl(ctx, (const uint8_t*) d_mirror, run_bytes[r], d_mq + j0, q_len + j0, (const uint32_t*) d_t2off + j0,
+                                        (const uint32_t*) d_t2len + j0, (const int32_t*) d_k2 + j0, DGPU_MODE_SHW, cnt, start_loc + j0,
+                                        (int32_t*) d_rev + j0, st, 1, d_eqtabs))) return rc;
+    }
   }
-  // 3. Hirschberg splitting on the host geometry, half columns + split rows on the device, level by level
-  std::vector<std::vector<Seg> > perjob(n);
-  std::vector<uint32_t> h_status(n, 0);
+  ep_start_kernel<<<nb, 256, 0, st>>>(mode, q_len, t_len, dist, end_loc, (const int32_t*) d_rev, (uint32_t) n, start_loc);
+  DGPU_LAUNCH_CHECK(ctx, "ep_start");
+  DGPU_CUDA(ctx, cudaMemcpyAsync(h_dist.data(), dist, n * 4, cudaMemcpyDeviceToHost, st));
+  DGPU_CUDA(ctx, cudaMemcpyAsync(h_start.data(), start_loc, n * 4, cudaMemcpyDeviceToHost, st));
+  DGPU_CUDA(ctx, cudaMemcpyAsync(h_end.data(), end_loc, n * 4, cudaMemcpyDeviceToHost, st));
+  DGPU_CUDA(ctx, cudaStreamSynchronize(st));
+  return DGPU_OK;
+}
+
+// Hirschberg splitting of every job's aligned slice, level by level, until each segment is a leaf (status 2: slice wider than max_slice).
+int ep_split(dgpu_ctx* ctx, cudaStream_t st, SegRunner& R, uint64_t n, std::vector<uint32_t> const& h_qoff, std::vector<uint32_t> const& h_qlen,
+             std::vector<uint32_t> const& h_toff, std::vector<uint32_t> const& h_tlen, std::vector<int32_t> const& h_dist, std::vector<int32_t> const& h_start,
+             std::vector<int32_t> const& h_end, uint32_t max_slice, std::vector<std::vector<Seg> >& perjob, std::vector<uint32_t>& h_status) {
+  int rc;
   bool any_split = false;
   for (uint64_t i = 0; i < n; ++i) {
     if (h_qlen[i] == 0 || h_tlen[i] == 0 || h_dist[i] < 0) continue;  // no path at all (edlib returns early)
@@ -832,7 +774,13 @@ int ep_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
       for (Seg const& g : perjob[i])
         if (g.qlen && g.tlen && seg_needs_split(g.qlen, g.tlen)) { any_split = true; break; }
   }
-  // 4. leaves: traceback (or trivial runs) and concatenation per job
+  return DGPU_OK;
+}
+
+// Traceback (or trivial run) of every leaf, the check that it reproduces its distance, the concatenation per job into ops, then status.
+int ep_leaves(dgpu_ctx* ctx, cudaStream_t st, SegRunner& R, uint64_t n, std::vector<std::vector<Seg> > const& perjob, std::vector<uint32_t>& h_status,
+              uint8_t* ops, const uint64_t* ops_off, uint32_t* ops_len, uint32_t* status) {
+  int rc;
   R.clear();
   std::vector<uint32_t> job_lo(n + 1, 0), leaf_kind, leaf_len_h;
   std::vector<uint64_t> leaf_off;
@@ -898,6 +846,55 @@ int ep_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
   DGPU_CUDA(ctx, cudaMemcpyAsync(status, h_status.data(), n * 4, cudaMemcpyHostToDevice, st));
   DGPU_CUDA(ctx, cudaStreamSynchronize(st));  // host vectors above are copy sources
   return DGPU_OK;
+}
+
+// The device form of every entry point: a job whose aligned target slice is wider than max_slice gets status 2 alone.
+int ep_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
+           const uint32_t* q_off, const uint32_t* q_len, const uint32_t* t_off, const uint32_t* t_len,
+           int mode, const uint8_t* eq_pairs, uint32_t n_eq, uint64_t n, int32_t* dist, int32_t* start_loc, int32_t* end_loc,
+           uint8_t* ops, const uint64_t* ops_off, uint32_t* ops_len, uint32_t* status, uint32_t max_slice, void* stream) {
+  if (!ctx) return DGPU_ERR_ARG;
+  if (n == 0) return DGPU_OK;
+  if (n >= (1ull << 31) || seqs_bytes >= (1ull << 32)) return DGPU_ERR_ARG;
+  if (mode != DGPU_MODE_NW && mode != DGPU_MODE_SHW && mode != DGPU_MODE_HW) return DGPU_ERR_ARG;
+  if (!seqs || !q_off || !q_len || !t_off || !t_len || !dist || !start_loc || !end_loc || !ops || !ops_off || !ops_len || !status) return DGPU_ERR_ARG;
+  if (n_eq > 32 || (n_eq && !eq_pairs)) return DGPU_ERR_ARG;
+  DGPU_CUDA(ctx, cudaSetDevice(ctx->device));
+  cudaStream_t st = stream ? (cudaStream_t) stream : ctx->stream;
+  int rc;
+  // host copies of the job geometry
+  std::vector<uint32_t> h_qoff(n), h_qlen(n), h_toff(n), h_tlen(n);
+  std::vector<uint64_t> h_opsoff(n);
+  DGPU_CUDA(ctx, cudaMemcpyAsync(h_qoff.data(), q_off, n * 4, cudaMemcpyDeviceToHost, st));
+  DGPU_CUDA(ctx, cudaMemcpyAsync(h_qlen.data(), q_len, n * 4, cudaMemcpyDeviceToHost, st));
+  DGPU_CUDA(ctx, cudaMemcpyAsync(h_toff.data(), t_off, n * 4, cudaMemcpyDeviceToHost, st));
+  DGPU_CUDA(ctx, cudaMemcpyAsync(h_tlen.data(), t_len, n * 4, cudaMemcpyDeviceToHost, st));
+  DGPU_CUDA(ctx, cudaMemcpyAsync(h_opsoff.data(), ops_off, n * 8, cudaMemcpyDeviceToHost, st));
+  SegRunner R;
+  R.ctx = ctx; R.st = st; R.seqs = seqs; R.use_eq = n_eq > 0; R.eq.f = nullptr; R.eq.s = nullptr;
+  const uint32_t* d_eqtabs = nullptr;  // f[256], s[256], cls[256 bytes]
+  if (n_eq) {
+    uint32_t tab[512 + 64] = {0};
+    for (uint32_t p = 0; p < n_eq; ++p) { tab[eq_pairs[2 * p]] |= 1u << p; tab[256 + eq_pairs[2 * p + 1]] |= 1u << p; }
+    uint8_t* cls = (uint8_t*) (tab + 512);
+    static const uint8_t sym[5] = {'A', 'C', 'G', 'T', 'N'};
+    for (uint32_t b = 0; b < 256; ++b)
+      for (int sy = 0; sy < 5; ++sy)
+        if (b == sym[sy] || (tab[b] & tab[256 + sym[sy]]) || (tab[256 + b] & tab[sym[sy]])) cls[b] |= (uint8_t) (1u << sy);
+    void* d_tab;
+    if ((rc = dgpu_reserve(ctx, SLOT_EP_EQTAB, sizeof(tab), &d_tab))) return rc;
+    DGPU_CUDA(ctx, cudaMemcpyAsync(d_tab, tab, sizeof(tab), cudaMemcpyHostToDevice, st));
+    DGPU_CUDA(ctx, cudaStreamSynchronize(st));  // tab is a stack array
+    R.eq.f = (const uint32_t*) d_tab; R.eq.s = (const uint32_t*) d_tab + 256; R.eq_cls = (const uint8_t*) ((const uint32_t*) d_tab + 512);
+    d_eqtabs = (const uint32_t*) d_tab;
+  }
+  std::vector<int32_t> h_dist(n), h_start(n), h_end(n);
+  if ((rc = ep_locate(ctx, st, seqs, seqs_bytes, q_off, q_len, t_off, t_len, mode, d_eqtabs, n, h_qlen, h_tlen, dist, start_loc, end_loc, h_dist,
+                      h_start, h_end))) return rc;
+  std::vector<std::vector<Seg> > perjob(n);
+  std::vector<uint32_t> h_status(n, 0);
+  if ((rc = ep_split(ctx, st, R, n, h_qoff, h_qlen, h_toff, h_tlen, h_dist, h_start, h_end, max_slice, perjob, h_status))) return rc;
+  return ep_leaves(ctx, st, R, n, perjob, h_status, ops, ops_off, ops_len, status);
 }
 
 // The host form of every entry point.

@@ -997,7 +997,7 @@ int ln_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes, const uint32
   if (max_ref) {   // a wide job may take half of the workspace budget below; one that needs more is refused alone
     size_t free0 = 0, total0 = 0;
     cudaMemGetInfo(&free0, &total0);
-    a.wide_budget = (unsigned long long) (((double) free0 * 0.6 + (double) ctx->bufs[SLOT_WAVEFRONT].cap) * 0.5);
+    a.wide_budget = dgpu_workspace_budget(ctx, SLOT_WAVEFRONT, free0) / 2;
   }
   if ((rc = dgpu_reserve(ctx, SLOT_JOB_PERM, n * sizeof(uint32_t), &p))) return rc;
   a.perm = (uint32_t*) p;
@@ -1062,7 +1062,7 @@ int ln_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes, const uint32
     total += pl.grid * pl.a.work_stride;
     plans.push_back(pl);
   }
-  const size_t budget = (size_t) ((double) free_b * 0.6) + ctx->bufs[SLOT_WAVEFRONT].cap;
+  const size_t budget = dgpu_workspace_budget(ctx, SLOT_WAVEFRONT, free_b);
   // The wide class's slabs are hundreds of MB: left in the common shrink, a few wide jobs would cut the grids of every ordinary class. So
   // the ordinary classes keep what they ask for, up to half of the budget, and the wide class is sized within the rest (all of it when
   // the batch has only wide jobs).
@@ -1083,18 +1083,12 @@ int ln_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes, const uint32
   total += wide_total;
   if ((rc = dgpu_reserve(ctx, SLOT_WAVEFRONT, total, &p))) return rc;
   { size_t off = 0; for (auto& pl : plans) { pl.a.work = (uint8_t*) p + off; off += pl.grid * pl.a.work_stride; } }
-  const bool fork = plans.size() > 1;
-  if (fork && (rc = dgpu_fork_init(ctx))) return rc;
-  dgpu_prof_begin(ctx, st);
-  if (fork) DGPU_CUDA(ctx, cudaEventRecord(ctx->fork_events[0], st));
-  for (size_t k = 0; k < plans.size(); ++k) {
-    Plan& pl = plans[k];
+  DgpuFork fork(ctx, st, plans.size());
+  if ((rc = fork.begin())) return rc;
+  for (Plan& pl : plans) {
     const int c = pl.c;
-    cudaStream_t cs = st;
-    if (fork) {
-      cs = ctx->fork_streams[k % DGPU_FORK_STREAMS];
-      if (k < DGPU_FORK_STREAMS) DGPU_CUDA(ctx, cudaStreamWaitEvent(cs, ctx->fork_events[0], 0));
-    }
+    cudaStream_t cs;
+    if ((rc = fork.next(cs))) return rc;
     const unsigned grid = (unsigned) pl.grid, threads = pl.threads;
     const size_t smem = pl.smem;
     if (c == LN_WIDE) {
@@ -1108,15 +1102,7 @@ int ln_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes, const uint32
       DGPU_LAUNCH_CHECK(ctx, c < LN_GEN ? "ln_kernel2" : "ln_kernel");
     }
   }
-  if (fork) {  // join
-    const size_t used = std::min<size_t>(plans.size(), DGPU_FORK_STREAMS);
-    for (size_t k = 0; k < used; ++k) {
-      DGPU_CUDA(ctx, cudaEventRecord(ctx->fork_events[1 + k], ctx->fork_streams[k]));
-      DGPU_CUDA(ctx, cudaStreamWaitEvent(st, ctx->fork_events[1 + k], 0));
-    }
-  }
-  dgpu_prof_end(ctx, st);
-  return DGPU_OK;
+  return fork.end();
 }
 
 // the host form of both entry points (max_ref = 0: dgpu_long_needle)
