@@ -9,10 +9,12 @@
 // No CPU fallback: without an sm_90 device dgpu_ctx_create fails and so does this program.
 #include <condition_variable>
 #include <cstdlib>
+#include <map>
 #include <mutex>
 #include <cstring>
 #include <iostream>
 #include <string>
+#include <sys/resource.h>
 #include <sys/stat.h>
 #include <unistd.h>
 #include <thread>
@@ -36,6 +38,8 @@ struct Options {
   int device = 0, ioThreads = 16;
   int rank = 0, nranks = 1;          // one process per GPU: --rank r --nranks N --comm-file path (rank 0 publishes the NCCL id there)
   std::string commFile, timingFile;  // --timing file: stage wall-clock times as one JSON object
+  std::string shardBy = "svs";       // --shard-by svs|contig: what the ranks divide (sr only)
+  bool readShareOnly = false;        // --read-share-only: read this rank's share of the alignments, write --timing, stop (measuring a share alone)
   float indelExtension = 0.5f;
   MethylConfig methyl;
   AnnoConfig anno;
@@ -69,7 +73,9 @@ bool svTypesToCompute(Config& c, std::string const& svtype) {
 void usage(Options const& o) {
   std::cerr << "\nUsage: delly_b200 " << (o.lr ? "lr" : "sr") << " [OPTIONS] -g <ref.fa> <sample1.sort.bam> <sample2.sort.bam> ...\n"
             << "  options follow `delly " << (o.lr ? "lr" : "sr") << "` (same letters and defaults), including -d <reads.gz> (gzipped list of the reads"
-            << " that support each SV); extra: --device N, --io-threads N" << (o.lr ? ", --mei <templates.fa>" : "") << "\n";
+            << " that support each SV); extra: --device N, --io-threads N" << (o.lr ? ", --mei <templates.fa>" : "") << "\n"
+            << "  several GPUs, one process each: --rank r --nranks N --comm-file <path>" << (o.lr ? "" : " [--shard-by svs|contig]") << " [--timing <file>]\n"
+            << (o.lr ? "" : "  --read-share-only: read this rank's share (--shard-by contig), write --timing and stop: no device, no exchange\n");
 }
 
 // `delly sr` (src/delly.h:207-246) and `delly lr` (src/tegua.h:215-275) share most letters; the long names are the reference's.
@@ -110,6 +116,8 @@ bool parse(int argc, char** argv, Options& o) {
     else if (a == "--nranks") o.nranks = std::stoi(val());
     else if (a == "--comm-file") o.commFile = val();
     else if (a == "--timing") o.timingFile = val();
+    else if (!o.lr && a == "--shard-by") o.shardBy = val();
+    else if (!o.lr && a == "--read-share-only") o.readShareOnly = true;
     else if (!o.lr && is("-h", "--threads")) c.maxThreads = (uint32_t) std::stoul(val());
     else if (!o.lr && is("-r", "--qual-tra")) c.minTraQual = (uint16_t) std::stoi(val());
     else if (!o.lr && is("-s", "--mad-cutoff")) c.madCutoff = (uint16_t) std::stoi(val());
@@ -131,6 +139,12 @@ bool parse(int argc, char** argv, Options& o) {
     else if (o.lr && a == "--mei") o.meifile = val();
     else if (o.lr && is("-l", "--alt-align")) { std::cerr << "alternate alignments (-l) are outside the accelerated path (SURVEY section 2)" << std::endl; return false; }
     else { std::cerr << "unrecognised option '" << argv[i] << "'" << std::endl; return false; }
+  }
+  if (o.shardBy != "svs" && o.shardBy != "contig") { std::cerr << "--shard-by takes svs or contig" << std::endl; return false; }
+  if (o.readShareOnly && o.shardBy != "contig") { std::cerr << "--read-share-only measures a share of --shard-by contig" << std::endl; return false; }
+  if (!o.dumpfile.empty() && o.shardBy == "contig") {
+    std::cerr << "the SV-read dump (-d) needs --shard-by svs: the order of the dump lines depends on the whole SV list and the whole record list" << std::endl;
+    return false;
   }
   if (!o.dumpfile.empty() && o.nranks > 1) {
     std::cerr << "the SV-read dump (-d) needs a single process: over --nranks > 1 every rank genotypes a part of the SV list, and the order of"
@@ -268,13 +282,32 @@ template <typename TRender> bool writeDump(std::string const& path, TRender rend
   return ok;
 }
 
-void writeTiming(Options const& o, StageClock const& clock, std::size_t nsv) {
+// what this rank holds and sends (--timing): its records (both lists with -x), its peak resident memory, and the bytes it contributed to the
+// exchanges of each stage (the stage clock's lap names)
+struct ShareStats {
+  std::size_t records = 0;
+  std::map<std::size_t, uint64_t> sentAtLap;   // bytes handed to the gather while the stage clock had k laps: the stage of lap k sent them
+};
+
+void writeTiming(Options const& o, StageClock const& clock, std::size_t nsv, ShareStats const* share = nullptr) {
   if (o.timingFile.empty()) return;
   std::ofstream f((o.timingFile + (o.nranks > 1 ? "." + std::to_string(o.rank) : std::string())).c_str());
   double total = 0;
   f << "{\"rank\": " << o.rank << ", \"nranks\": " << o.nranks << ", \"svs\": " << nsv << ", \"stages_ms\": {";
   for (std::size_t i = 0; i < clock.ms.size(); ++i) { f << (i ? ", " : "") << "\"" << clock.ms[i].first << "\": " << clock.ms[i].second; total += clock.ms[i].second; }
-  f << "}, \"total_ms\": " << total << "}" << std::endl;
+  f << "}, \"total_ms\": " << total;
+  if (share) {
+    struct rusage ru;
+    getrusage(RUSAGE_SELF, &ru);
+    f << ", \"records\": " << share->records << ", \"peak_rss_kb\": " << ru.ru_maxrss << ", \"sent_bytes\": {";
+    bool first = true;
+    for (auto const& kv : share->sentAtLap) {
+      f << (first ? "" : ", ") << "\"" << (kv.first < clock.ms.size() ? clock.ms[kv.first].first : std::string("end")) << "\": " << kv.second;
+      first = false;
+    }
+    f << "}";
+  }
+  f << "}" << std::endl;
 }
 
 // One process per GPU: rank 0 creates the NCCL id and publishes it in --comm-file (written under a temporary name, then renamed); the other
@@ -301,6 +334,7 @@ bool initComm(Options const& o, dgpu_ctx* ctx, void** comm) {
 }
 
 void DeviceSession::start() {
+  if (o_.readShareOnly) { reach(2); return; }   // nothing on the device
   const int rc = dgpu_ctx_create(o_.device, &ctx_);
   if (rc != DGPU_OK) { std::cerr << "delly_b200: no usable sm_90 device (dgpu_ctx_create = " << rc << "); there is no CPU fallback on this path" << std::endl; ctx_ = nullptr; reach(2); return; }
   reach(1);
@@ -314,6 +348,21 @@ void DeviceSession::start() {
   reach(2);
 }
 
+// --shard-by contig: the contig ranges of the ranks, balanced by the mapped reads of the BAM indexes summed over the files; by the contig
+// lengths when an index has no read counts (one unit for every contig). Every rank computes the same cut from the same files.
+std::vector<std::size_t> contigCut(Options const& o, Inputs const& in) {
+  std::vector<uint64_t> w(in.target_len.size(), 0);
+  bool counted = true;
+  for (auto const& f : in.files)
+    for (int32_t t = 0; t < (int32_t) w.size() && counted; ++t) {
+      uint64_t mapped = 0, unmapped = 0;
+      if (hts_idx_get_stat(f.idx, t, &mapped, &unmapped) != 0) counted = false;
+      else w[t] += mapped;
+    }
+  if (!counted) w.assign(in.target_len.begin(), in.target_len.end());
+  return partitionContigs(w, o.nranks);
+}
+
 int runSr(Options& o, DeviceSession& dev) {
   StageClock clock;
   Inputs in;
@@ -321,6 +370,21 @@ int runSr(Options& o, DeviceSession& dev) {
   clock.lap("open_inputs");
   Config& c = o.c;
   const std::size_t F = in.files.size();
+  const bool byContig = o.shardBy == "contig";
+  Shard shard = dev.shard();
+  ShareStats share;
+  // exclude file: contigs without a valid region are excluded as a whole; the scan skips pairs whose mate is there (src/shortpe.h:399)
+  if (o.hasExclude) c.contigExcluded = excludedContigs(in.validRegions);
+  if (byContig) {   // this rank reads its own contigs only (the exclude flags above are the whole genome's)
+    shard.contigBounds = contigCut(o, in);
+    if (o.nranks == 1) shard.gather = [](std::string const& local, std::vector<std::string>& parts) { parts.assign(1, local); return (int) DGPU_OK; };
+    keepOwnContigs(shard.contigBounds, o.rank, in.validRegions, in.wholeContigs);
+    GatherFn g = shard.gather;
+    shard.gather = [g, &share, &clock](std::string const& local, std::vector<std::string>& parts) {
+      share.sentAtLap[clock.ms.size()] += local.size();
+      return g(local, parts);
+    };
+  }
   const bool dump = !o.dumpfile.empty();
   std::vector<std::vector<std::string> > names(dump ? F : 0);   // query names of the genotyped records (-d)
   // records of every file, as the reference's iterators return them
@@ -345,20 +409,31 @@ int runSr(Options& o, DeviceSession& dev) {
       }
       genoSamples.push_back(&recsWhole[f]);
     }
-    c.contigExcluded.assign(in.validRegions.size(), 0);
-    for (std::size_t r = 0; r < in.validRegions.size(); ++r) c.contigExcluded[r] = in.validRegions[r].empty();
   }
   clock.lap("read_bam");
+  if (byContig) {
+    const std::size_t lo = shard.contigBounds[o.rank], hi = shard.contigBounds[o.rank + 1];
+    std::size_t n = 0;
+    for (std::size_t f = 0; f < F; ++f) n += recs[f].size() + (o.hasExclude ? recsWhole[f].size() : 0);
+    std::cerr << "rank " << o.rank << "/" << o.nranks << ": contigs ";
+    if (lo < hi) std::cerr << lo << "-" << hi - 1 << " (" << in.target_name[lo] << ".." << in.target_name[hi - 1] << ")";
+    else std::cerr << "none";
+    std::cerr << ", " << n << " records" << std::endl;
+    share.records = n;
+    if (o.readShareOnly) { writeTiming(o, clock, 0, &share); return 0; }
+  }
   std::vector<LibraryInfo> libs(F);
   for (std::size_t f = 0; f < F; ++f) {
-    getLibraryParams(c, in.target_len, recs[f], libs[f]);
+    if (byContig) {   // the first alignments in contig order may lie on other ranks' contigs: the screen continues rank after rank
+      const int lrc = getLibraryParamsSharded(c, in.target_len, recs[f], shard.contigShard(), libs[f]);
+      if (lrc) { std::cerr << "delly_b200: the library exchange failed (" << lrc << ")" << std::endl; return 1; }
+    } else getLibraryParams(c, in.target_len, recs[f], libs[f]);
     if (libs[f].rs == 0) { std::cerr << "Sample has not enough data to estimate library parameters! File: " << o.files[f] << std::endl; return 1; }
   }
   clock.lap("library");
   if (!dev.wait()) return 3;
   clock.lap("wait_device");
   dgpu_ctx* ctx = dev.ctx();
-  const Shard shard = dev.shard();
   SrMultiCallSet cs;
   SvReadDump reads;
   int rc;
@@ -373,7 +448,7 @@ int runSr(Options& o, DeviceSession& dev) {
     if (rc == DGPU_ERR_ARG && !cs.sample.empty()) { std::cerr << "Error: Delly genotyping requires a Delly BCF file from v1.1.7 or later!" << std::endl; rc = DGPU_OK; }
   }
   if (rc) { std::cerr << "delly_b200: device path failed (" << rc << "): " << dgpu_last_error(ctx) << std::endl; return 1; }
-  if (o.rank != 0) { writeTiming(o, clock, cs.svs.size()); return 0; }   // every rank holds the complete call set; rank 0 writes it
+  if (o.rank != 0) { writeTiming(o, clock, cs.svs.size(), byContig ? &share : nullptr); return 0; }   // every rank holds the complete call set; rank 0 writes it
   if (dump && !cs.svs.empty()) {   // the reference opens the dump in annotateCoverage, which an empty SV list skips (src/delly.h:176)
     std::vector<std::vector<SrRecord> const*> const& geno = o.hasExclude ? genoSamples : samples;
     if (!writeDump(o.dumpfile, [&](auto put) { writeSrReadDump(put, reads, o.files, geno, names, in.target_name); })) return 1;
@@ -391,7 +466,7 @@ int runSr(Options& o, DeviceSession& dev) {
   vcfRecordsTo(w, cs.svs, vs, in.target_name, in.target_len, o.genome, io::todayIso(), o.hasVcf, 0);
   w.close();
   clock.lap("write_bcf");
-  writeTiming(o, clock, cs.svs.size());
+  writeTiming(o, clock, cs.svs.size(), byContig ? &share : nullptr);
   for (std::size_t f = 0; f < F; ++f)
     std::cerr << "Sample:" << in.sampleName[f] << ",ReadSize=" << libs[f].rs << ",Median=" << libs[f].median << ",MAD=" << libs[f].mad << ",UniqueDiscordantPairs=" << libs[f].abnormal_pairs << std::endl;
   return 0;

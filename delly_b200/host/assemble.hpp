@@ -25,15 +25,20 @@ inline std::size_t srSeed(SrRecord const& r) { return r.seed ? r.seed : (std::si
 
 // samples: the alignment lists of all input files, in file order (the reference walks contig by contig and, inside a contig, file by
 // file: src/shortpe.h:81-156), each sorted like a coordinate-sorted BAM.
+// cs != nullptr (contig sharding): samples hold this rank's contigs only and an SV belongs to the rank of sv.chr. The split reads a rank
+// collects for a translocation on its contigs are gathered by every rank and replayed in contig order into the owner's read set, so msa sees
+// the set of the single-process walk; the owner assembles its SVs and the finished records of all ranks are gathered.
 inline int assembleSplitReadsBatch(dgpu_ctx* ctx, Config const& c, std::vector<uint32_t> const& target_len, std::vector<const char*> const& chrseq,
                                    std::vector<TPosReadSV> const& srStore, std::vector<StructuralVariantRecord>& svs,
-                                   std::vector<std::vector<SrRecord> const*> const& samples, AssembleShard const* shard = nullptr) {
+                                   std::vector<std::vector<SrRecord> const*> const& samples, AssembleShard const* shard = nullptr,
+                                   ContigShard const* cs = nullptr) {
   // The reference keeps the reads of an SV in a std::unordered_set<std::string>; its iteration order is the order msa() sees
   // (and it de-duplicates identical reads). The same container with the same insertion sequence gives the same order.
   typedef std::unordered_set<std::string> TSequences;
   const std::size_t N = svs.size();
   std::vector<TSequences> traStore(N);
   std::vector<std::vector<uint8_t> > traQualStore(N);
+  std::vector<std::vector<std::string> > traOrder(cs ? N : 0);   // contig sharding: the translocation reads in insertion order
   std::vector<uint32_t> queued;                          // SV ids that reach msa + alignConsensus
   std::vector<std::vector<std::string> > clusters;       // their reads, in the set's iteration order
   std::vector<std::vector<uint8_t> > quals;
@@ -45,7 +50,7 @@ inline int assembleSplitReadsBatch(dgpu_ctx* ctx, Config const& c, std::vector<u
       rlo[f] = ri[f];
       while (ri[f] < recs.size() && recs[ri[f]].tid == refIndex) ++ri[f];
     }
-    if (srStore[refIndex].empty()) continue;
+    if (srStore[refIndex].empty() || (cs && !cs->owns(refIndex))) continue;
     std::vector<bool> hits(target_len[refIndex], false);
     for (auto const& kv : srStore[refIndex]) hits[(std::size_t) kv.first.first] = true;
     std::vector<TSequences> seqStore(N);
@@ -68,7 +73,10 @@ inline int assembleSplitReadsBatch(dgpu_ctx* ctx, Config const& c, std::vector<u
       else if (sv.svt == 1) bpPoint = (rec.pos + 25 > sv.svEnd);
       _adjustOrientation(sequence, bpPoint ? 1u : 0u, sv.svt);
       if (seqStore[svid].size() < c.maxReadPerSV) {   // (the cap looks at seqStore for translocations too, :140)
-        if (_translocation(sv.svt)) { if (traStore[svid].insert(std::move(sequence)).second) traQualStore[svid].push_back(rec.mapq); }
+        if (_translocation(sv.svt)) {
+          if (cs) { if (traStore[svid].insert(sequence).second) { traQualStore[svid].push_back(rec.mapq); traOrder[svid].push_back(std::move(sequence)); } }
+          else if (traStore[svid].insert(std::move(sequence)).second) traQualStore[svid].push_back(rec.mapq);
+        }
         else { if (seqStore[svid].insert(std::move(sequence)).second) qualStore[svid].push_back(rec.mapq); }
       }
     }
@@ -81,17 +89,42 @@ inline int assembleSplitReadsBatch(dgpu_ctx* ctx, Config const& c, std::vector<u
       quals.push_back(qualStore[svid]);
     }
   }
+  int rc = DGPU_OK;
+  if (cs) {   // every rank's translocation reads, replayed in rank (= contig) order into the read sets of this rank's translocations
+    ByteWriter w;
+    for (uint32_t svid = 0; svid < N; ++svid) {
+      if (traOrder[svid].empty()) continue;
+      w.pod(svid); w.pod<uint32_t>((uint32_t) traOrder[svid].size());
+      for (std::size_t k = 0; k < traOrder[svid].size(); ++k) { w.str(traOrder[svid][k]); w.pod(traQualStore[svid][k]); }
+    }
+    std::vector<std::string> parts;
+    if ((rc = cs->exchange(DGPU_OK, w.buf, parts))) return rc;
+    for (uint32_t svid = 0; svid < N; ++svid) { traStore[svid].clear(); traQualStore[svid].clear(); }
+    for (int r = 0; r < cs->nranks; ++r) {
+      ByteReader rd(parts[r].data(), parts[r].size());
+      while (rd.ok() && !rd.done()) {
+        const uint32_t svid = rd.pod<uint32_t>(), n = rd.pod<uint32_t>();
+        if (svid >= N) return DGPU_ERR_NCCL;
+        for (uint32_t k = 0; k < n && rd.ok(); ++k) {
+          std::string sq = rd.str();
+          const uint8_t q = rd.pod<uint8_t>();
+          if (cs->owns(svs[svid].chr) && traStore[svid].insert(std::move(sq)).second) traQualStore[svid].push_back(q);
+        }
+      }
+      if (!rd.ok()) return DGPU_ERR_NCCL;
+    }
+  }
   for (int32_t refIndex2 = 0; refIndex2 < (int32_t) target_len.size(); ++refIndex2)
     for (int32_t refIndex = refIndex2 + 1; refIndex < (int32_t) target_len.size(); ++refIndex)
       for (uint32_t svid = 0; svid < N; ++svid) {
-        if (!_translocation(svs[svid].svt)) continue;
+        if (!_translocation(svs[svid].svt) || (cs && !cs->owns(refIndex))) continue;
         if ((svs[svid].chr != refIndex) || (svs[svid].chr2 != refIndex2)) continue;
         if (traStore[svid].size() <= 1) { reset(svs[svid]); continue; }
         queued.push_back(svid);
         clusters.push_back(std::vector<std::string>(traStore[svid].begin(), traStore[svid].end()));
         quals.push_back(traQualStore[svid]);
       }
-  if (queued.empty()) return DGPU_OK;
+  if (queued.empty() && !cs) return DGPU_OK;
   // The two device batches — msa() and alignConsensus() of every queued SV — are what a rank shards (SURVEY §8e): the read collection above is
   // host work every rank repeats; of the queue a rank processes one contiguous range, cut by cost (all-pairs LCS + progressive alignment grow with
   // reads^2 x length^2), and the finished records of all ranks are exchanged once.
@@ -109,14 +142,16 @@ inline int assembleSplitReadsBatch(dgpu_ctx* ctx, Config const& c, std::vector<u
   }
   std::vector<std::string> consensus;
   std::vector<int> rows;
-  int rc = DGPU_OK;
   std::vector<StructuralVariantRecord> work(hi - lo);
   std::vector<uint8_t> ok;
   if (hi > lo) {
     std::vector<std::vector<std::string> > mine(clusters.begin() + lo, clusters.begin() + hi);
-    if ((rc = msaBatch(ctx, c, mine, consensus, rows))) return rc;
-    for (std::size_t k = lo; k < hi; ++k) { work[k - lo] = svs[queued[k]]; work[k - lo].consensus = consensus[k - lo]; }
-    if ((rc = alignConsensusBatch(ctx, c, target_len, chrseq, work, false, ok))) return rc;
+    rc = msaBatch(ctx, c, mine, consensus, rows);
+    if (!rc) {
+      for (std::size_t k = lo; k < hi; ++k) { work[k - lo] = svs[queued[k]]; work[k - lo].consensus = consensus[k - lo]; }
+      rc = alignConsensusBatch(ctx, c, target_len, chrseq, work, false, ok);
+    }
+    if (rc && !cs) return rc;   // (contig sharding: the error travels with the exchange below)
   }
   if (shard && shard->nranks > 1) {
     std::vector<StructuralVariantRecord> allWork;
@@ -125,7 +160,7 @@ inline int assembleSplitReadsBatch(dgpu_ctx* ctx, Config const& c, std::vector<u
     if (allWork.size() != queued.size()) return DGPU_ERR_NCCL;
     work.swap(allWork); ok.swap(allOk);
   }
-  for (std::size_t k = 0; k < queued.size(); ++k) {
+  for (std::size_t k = 0; k < queued.size() && !rc; ++k) {
     StructuralVariantRecord& sv = svs[queued[k]];
     sv = work[k];
     if (!ok[k]) { reset(sv); continue; }
@@ -135,6 +170,22 @@ inline int assembleSplitReadsBatch(dgpu_ctx* ctx, Config const& c, std::vector<u
     if (!qv.empty()) { const std::size_t n = qv.size() / 2; std::nth_element(qv.begin(), qv.begin() + n, qv.end()); sv.srMapQuality = qv[n]; }   // medianVector, src/util.h:78-84
     else sv.srMapQuality = 0;
     sv.srSupport = (int32_t) clusters[k].size();
+  }
+  if (cs) {   // the records of every rank's SVs
+    ByteWriter w;
+    for (uint32_t svid = 0; svid < N; ++svid)
+      if (cs->owns(svs[svid].chr)) putSv(w, svs[svid]);
+    std::vector<std::string> parts;
+    if ((rc = cs->exchange(rc, w.buf, parts))) return rc;
+    for (int r = 0; r < cs->nranks; ++r) {
+      if (r == cs->rank) continue;
+      ByteReader rd(parts[r].data(), parts[r].size());
+      for (uint32_t svid = 0; svid < N; ++svid) {
+        if (svs[svid].chr < (int32_t) cs->bounds[r] || svs[svid].chr >= (int32_t) cs->bounds[r + 1]) continue;
+        getSv(rd, svs[svid]);
+      }
+      if (!rd.ok() || !rd.done()) return DGPU_ERR_NCCL;
+    }
   }
   return DGPU_OK;
 }

@@ -12,6 +12,9 @@
 // What is replicated on every rank: reading the alignments, the junction scan and the (sequential, order-dependent) clustering — host work
 // whose result every rank needs in full. What is sharded: every device batch (msa, longNeedle / splitAlign, probe generation, the junction
 // read realignment, read-depth and spanning-pair bookkeeping of the rank's own SVs).
+// The contig-sharded form (Shard::contigBounds, `--shard-by contig`) removes the replicated reading and scan: a rank holds the alignments of its
+// own contigs only and the per-contig logs of every stage travel between the ranks (genotypeSrSitesByContig below, host/scan.hpp,
+// host/assemble.hpp, host/genotype.hpp); only junction selection, clustering, mergeSort and the sort stay replicated.
 //
 // Exactness: the N-rank result equals the 1-rank result record for record, unconditionally. The only cross-SV coupling in the genotyping
 // pass is the batching of the junction-read jobs (flushed every 131072 x threads jobs and at the end of a contig, src/coverage.h:271,446,671):
@@ -32,13 +35,15 @@
 
 namespace dellyb200 {
 
-// all-gatherv of one byte string per rank: parts[r] = rank r's payload, same on every rank. Returns DGPU_OK or an error code.
-typedef std::function<int(std::string const& local, std::vector<std::string>& parts)> GatherFn;
-
 struct Shard {
   int rank = 0, nranks = 1;
   GatherFn gather;   // empty = single process
+  // --shard-by contig: the contig ranges of the ranks (partitionContigs); empty = the SV list is cut by cost (--shard-by svs). The contig
+  // mode holds from one rank up (one rank owns every contig and exchanges with itself).
+  std::vector<std::size_t> contigBounds;
   bool active() const { return nranks > 1 && (bool) gather; }
+  bool byContig() const { return !contigBounds.empty() && (bool) gather; }
+  ContigShard contigShard() const { ContigShard cs; cs.rank = rank; cs.nranks = nranks; cs.bounds = contigBounds; cs.gather = gather; return cs; }
 };
 
 // wall-clock of the chain's stages (for the pipeline-level benchmark): name -> milliseconds, in call order
@@ -52,46 +57,7 @@ struct StageClock {
   }
 };
 
-// ---- wire format (little endian, host order; all ranks are the same binary on the same box) ----------------------------------------
-class ByteWriter {
- public:
-  std::string buf;
-  template <typename T> void pod(T const& v) { buf.append(reinterpret_cast<const char*>(&v), sizeof(T)); }
-  void str(std::string const& s) { pod<uint32_t>((uint32_t) s.size()); buf.append(s); }
-  void bytes(std::vector<uint8_t> const& v) { pod<uint32_t>((uint32_t) v.size()); if (!v.empty()) buf.append(reinterpret_cast<const char*>(v.data()), v.size()); }
-};
-class ByteReader {
- public:
-  ByteReader(const char* p, std::size_t n) : p_(p), end_(p + n) {}
-  bool ok() const { return ok_; }
-  bool done() const { return p_ >= end_; }
-  template <typename T> T pod() { T v = T(); if (p_ + sizeof(T) > end_) { ok_ = false; return v; } std::memcpy(&v, p_, sizeof(T)); p_ += sizeof(T); return v; }
-  std::string str() { const uint32_t n = pod<uint32_t>(); if (!ok_ || p_ + n > end_) { ok_ = false; return std::string(); } std::string s(p_, n); p_ += n; return s; }
-  std::vector<uint8_t> bytes() { const uint32_t n = pod<uint32_t>(); if (!ok_ || p_ + n > end_) { ok_ = false; return {}; } std::vector<uint8_t> v(p_, p_ + n); p_ += n; return v; }
- private:
-  const char* p_; const char* end_; bool ok_ = true;
-};
-
-inline void putSv(ByteWriter& w, StructuralVariantRecord const& v) {
-  const int32_t f[20] = {v.chr, v.svStart, v.chr2, v.svEnd, v.ciposlow, v.ciposhigh, v.ciendlow, v.ciendhigh, v.srSupport, v.srMapQuality,
-                         v.mapq, v.insLen, v.svt, v.id, v.homLen, v.peSupport, v.peMapQuality, v.consBp, v.alleleid, v.nallele};
-  for (int32_t x : f) w.pod(x);
-  w.pod(v.srAlignQuality);
-  w.pod<uint8_t>(v.precise ? 1 : 0);
-  w.pod<uint8_t>(v.anno.isRC ? 1 : 0); w.pod(v.anno.seqType); w.pod(v.anno.homLen); w.pod(v.anno.trPeriod); w.pod(v.anno.trCopies);   // SVAnno (src/tags.h:82-91)
-  w.str(v.alleles); w.str(v.consensus);
-}
-inline void getSv(ByteReader& r, StructuralVariantRecord& v) {
-  int32_t f[20];
-  for (int32_t& x : f) x = r.pod<int32_t>();
-  v.chr = f[0]; v.svStart = f[1]; v.chr2 = f[2]; v.svEnd = f[3]; v.ciposlow = f[4]; v.ciposhigh = f[5]; v.ciendlow = f[6]; v.ciendhigh = f[7]; v.srSupport = f[8];
-  v.srMapQuality = f[9]; v.mapq = f[10]; v.insLen = f[11]; v.svt = f[12]; v.id = f[13]; v.homLen = f[14]; v.peSupport = f[15]; v.peMapQuality = f[16]; v.consBp = f[17];
-  v.alleleid = f[18]; v.nallele = f[19];
-  v.srAlignQuality = r.pod<float>();
-  v.precise = r.pod<uint8_t>() != 0;
-  v.anno.isRC = r.pod<uint8_t>() != 0; v.anno.seqType = r.pod<int32_t>(); v.anno.homLen = r.pod<int32_t>(); v.anno.trPeriod = r.pod<int32_t>(); v.anno.trCopies = r.pod<float>();
-  v.alleles = r.str(); v.consensus = r.str();
-}
+// ---- wire format (ByteWriter / ByteReader, host/shard.hpp) --------------------------------------------------------------------------
 inline void putJct(ByteWriter& w, JunctionCount const& j) { w.bytes(j.ref); w.bytes(j.alt); w.bytes(j.hp1ref); w.bytes(j.hp1alt); w.bytes(j.hp2ref); w.bytes(j.hp2alt); w.pod(j.ps); }
 inline void getJct(ByteReader& r, JunctionCount& j) { j.ref = r.bytes(); j.alt = r.bytes(); j.hp1ref = r.bytes(); j.hp1alt = r.bytes(); j.hp2ref = r.bytes(); j.hp2alt = r.bytes(); j.ps = r.pod<int32_t>(); }
 inline void putMethyl(ByteWriter& w, MethylInfo const& m) { for (int k = 0; k < 4; ++k) { w.pod(m.alt[k]); w.pod(m.ref[k]); w.pod(m.mnc[k]); w.pod(m.mdp[k]); } }
@@ -149,6 +115,51 @@ inline uint64_t genotypingCost(StructuralVariantRecord const& sv, Config const& 
   return cost;
 }
 
+// the genotype fields of one sample from its count vectors (src/modvcf.h:667-715): precise SVs from junction reads, imprecise ones from
+// spanning pairs
+inline void srSampleFormat(std::vector<StructuralVariantRecord> const& svs, SrSampleCounts& sc) {
+  static const BoLog bl;
+  sc.format.resize(svs.size());
+  for (std::size_t i = 0; i < svs.size(); ++i) {
+    JunctionCount const& j = sc.jctMap[i];
+    std::vector<uint8_t> const& rr = svs[i].precise ? j.ref : sc.spanMap[i].ref;
+    std::vector<uint8_t> const& aa = svs[i].precise ? j.alt : sc.spanMap[i].alt;
+    sc.format[i] = sampleFormat(bl, rr, aa, j.ps, (int32_t) j.hp1alt.size(), (int32_t) j.hp2alt.size(), sc.rcMap[i].leftRC, sc.rcMap[i].rc, sc.rcMap[i].rightRC);
+  }
+}
+
+// ---- contig-sharded genotyping (--shard-by contig) -----------------------------------------------------------------------------------
+// The complete, sorted and renumbered SV list on a rank that holds the alignments of its own contigs only: the probes of the SVs with a
+// breakpoint on those contigs, then per sample the junction-read pass and the spanning-pair / read-depth pass over the rank's contigs, each
+// with its exchange (host/genotype.hpp). Every rank ends with the complete count vectors and genotype fields.
+inline int genotypeSrSitesByContig(dgpu_ctx* ctx, Config const& c, std::vector<LibraryInfo> const& libs, std::vector<uint32_t> const& target_len,
+                                   std::vector<std::string> const& target_name, std::vector<const char*> const& chrseq,
+                                   std::vector<std::vector<SrRecord> const*> const& samples, ContigShard const& cs, SrMultiCallSet& out, StageClock* clock) {
+  const std::size_t F = samples.size();
+  out.sample.assign(F, SrSampleCounts());
+  if (out.svs.empty()) return DGPU_OK;
+  std::vector<uint8_t> want(out.svs.size());
+  for (std::size_t i = 0; i < out.svs.size(); ++i) want[i] = cs.owns(out.svs[i].chr) || cs.owns(out.svs[i].chr2);
+  JunctionProbes probes;
+  int rc = prepareJunctionProbes(ctx, c, target_len, target_name, chrseq, out.svs, probes, &want);
+  if (rc) {   // this rank alone may fail (a probe cut outside its consensus): the first exchange of the other ranks carries the error to them
+    std::vector<std::string> parts;
+    cs.exchange(rc, std::string(), parts);
+    return rc;
+  }
+  if (clock) clock->lap("probes");
+  std::vector<bool> svOnChr(target_len.size(), false);
+  for (auto const& sv : out.svs) { svOnChr[sv.chr] = true; svOnChr[sv.chr2] = true; }
+  for (std::size_t f = 0; f < F; ++f) {
+    SrSampleCounts& sc = out.sample[f];
+    if ((rc = annotateJunctionReadsWithProbes(ctx, c, target_len, probes, out.svs.size(), *samples[f], sc.jctMap, nullptr, &cs))) return rc;
+    if ((rc = annotateSpanningAndDepth(c, libs[f], target_len, out.svs, svOnChr, *samples[f], sc.rcMap, sc.spanMap, nullptr, &cs))) return rc;
+    srSampleFormat(out.svs, sc);
+  }
+  if (clock) clock->lap("genotype");
+  return DGPU_OK;
+}
+
 // ---- sharded genotyping of a sorted, renumbered SV list (one or several samples) ---------------------------------------------------
 // in/out: cs.svs = the COMPLETE list, sorted and renumbered, identical on every rank. On return every rank holds the complete result.
 // dump: the SV-read events of every sample (one process only: the order of tied breakpoints depends on the whole SV list, see DESIGN §8).
@@ -157,7 +168,8 @@ inline int genotypeSrSitesSharded(dgpu_ctx* ctx, Config const& c, std::vector<Li
                                   std::vector<std::vector<SrRecord> const*> const& samples, Shard const& shard, SrMultiCallSet& cs, StageClock* clock = nullptr,
                                   SvReadDump* dump = nullptr) {
   const std::size_t F = samples.size();
-  if (dump && shard.active()) return DGPU_ERR_ARG;
+  if (dump && (shard.active() || shard.byContig())) return DGPU_ERR_ARG;
+  if (shard.byContig()) return genotypeSrSitesByContig(ctx, c, libs, target_len, target_name, chrseq, samples, shard.contigShard(), cs, clock);
   cs.sample.assign(F, SrSampleCounts());
   if (dump) dump->file.assign(F, SvReadDump::File());
   if (cs.svs.empty()) return DGPU_OK;
@@ -220,17 +232,7 @@ inline int genotypeSrSitesSharded(dgpu_ctx* ctx, Config const& c, std::vector<Li
   }
   if (all.size() != cs.svs.size()) return DGPU_ERR_NCCL;
   cs.svs.swap(all);
-  static const BoLog bl;
-  for (std::size_t f = 0; f < F; ++f) {
-    SrSampleCounts& sc = cs.sample[f];
-    sc.format.resize(cs.svs.size());
-    for (std::size_t i = 0; i < cs.svs.size(); ++i) {
-      JunctionCount const& j = sc.jctMap[i];
-      std::vector<uint8_t> const& rr = cs.svs[i].precise ? j.ref : sc.spanMap[i].ref;
-      std::vector<uint8_t> const& aa = cs.svs[i].precise ? j.alt : sc.spanMap[i].alt;
-      sc.format[i] = sampleFormat(bl, rr, aa, j.ps, (int32_t) j.hp1alt.size(), (int32_t) j.hp2alt.size(), sc.rcMap[i].leftRC, sc.rcMap[i].rc, sc.rcMap[i].rightRC);
-    }
-  }
+  for (std::size_t f = 0; f < F; ++f) srSampleFormat(cs.svs, cs.sample[f]);
   return DGPU_OK;
 }
 
@@ -240,7 +242,7 @@ inline int dellySrGenotypeSharded(dgpu_ctx* ctx, Config const& c, std::vector<Li
                                   bool headerHasConsBp, std::vector<std::vector<SrRecord> const*> const& samples, Shard const& shard, SrMultiCallSet& out,
                                   StageClock* clock = nullptr, SvReadDump* dump = nullptr) {
   out = SrMultiCallSet();
-  if (dump && shard.active()) return DGPU_ERR_ARG;
+  if (dump && (shard.active() || shard.byContig())) return DGPU_ERR_ARG;
   const bool ok = vcfParseSites(sites, headerHasConsBp, target_name, out.svs);
   for (auto const& sv : out.svs)
     if (sv.chr < 0 || sv.chr2 < 0) return DGPU_ERR_ARG;
@@ -254,7 +256,9 @@ inline int dellySrGenotypeSharded(dgpu_ctx* ctx, Config const& c, std::vector<Li
 
 inline AssembleShard makeAssembleShard(Shard const& shard);
 
-// `delly sr` discovery + genotyping sharded over ranks: scan + clustering replicated (host), split-read assembly and genotyping sharded.
+// `delly sr` discovery + genotyping sharded over ranks. --shard-by svs: scan + clustering replicated (host), split-read assembly and genotyping
+// cut by cost. --shard-by contig: every rank holds, scans, assembles and genotypes the alignments of its own contigs, the per-contig logs are
+// exchanged (host/scan.hpp, host/assemble.hpp, host/genotype.hpp), junction selection, clustering, mergeSort and the sort run on every rank.
 inline int dellySrCallSharded(dgpu_ctx* ctx, Config const& c, std::vector<LibraryInfo>& libs, std::vector<uint32_t> const& target_len,
                               std::vector<std::string> const& target_name, std::vector<const char*> const& chrseq,
                               std::vector<std::vector<SrRecord> const*> const& samples, Shard const& shard, SrMultiCallSet& out, StageClock* clock = nullptr,
@@ -264,11 +268,14 @@ inline int dellySrCallSharded(dgpu_ctx* ctx, Config const& c, std::vector<Librar
   std::vector<StructuralVariantRecord> srSVs;
   std::vector<TPosReadSV> srStore;
   out = SrMultiCallSet();
-  if (dump && shard.active()) return DGPU_ERR_ARG;
-  int rc = scanPEandSRBatch(ctx, c, libs, target_len, samples, out.svs, srSVs, srStore);
+  if (dump && (shard.active() || shard.byContig())) return DGPU_ERR_ARG;
+  const ContigShard cs = shard.contigShard();
+  int rc = scanPEandSRBatch(ctx, c, libs, target_len, samples, out.svs, srSVs, srStore, shard.byContig() ? &cs : nullptr);
   if (rc) return rc;
   if (clock) clock->lap("scan_cluster");
-  if (shard.active()) {
+  if (shard.byContig()) {
+    if ((rc = assembleSplitReadsBatch(ctx, c, target_len, chrseq, srStore, srSVs, samples, nullptr, &cs))) return rc;
+  } else if (shard.active()) {
     AssembleShard as = makeAssembleShard(shard);
     if ((rc = assembleSplitReadsBatch(ctx, c, target_len, chrseq, srStore, srSVs, samples, &as))) return rc;
   } else if ((rc = assembleSplitReadsBatch(ctx, c, target_len, chrseq, srStore, srSVs, samples))) return rc;

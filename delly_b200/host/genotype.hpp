@@ -14,9 +14,10 @@
 #include <vector>
 
 #include "../../include/dgpu.h"
+#include "methyl.hpp"
+#include "shard.hpp"
 #include "split.hpp"
 #include "types.hpp"
-#include "methyl.hpp"
 
 namespace dellyb200 {
 
@@ -149,10 +150,13 @@ inline bool _substrChecked(std::string const& s, int32_t start, int32_t len, std
 //   refProbeArr / consProbeArr   [2][svs.size()], indexed by sv.id like the reference
 //   bpRegion       [n_targets], each sorted by bppos; svOnChr[n_targets]
 //   bad            ids whose probe cut fell outside the string (the reference would have thrown)
+//   want           (may be null) the SVs whose probes are needed, by index; the others get their alleles only. A rank of a contig-sharded run
+//                  wants the SVs with a breakpoint on its contigs: the breakpoint regions of those contigs are then the single-process ones.
 inline int generateProbesBatch(dgpu_ctx* ctx, Config const& c, std::vector<uint32_t> const& target_len, std::vector<std::string> const& target_name,
                                std::vector<const char*> const& chrseq, std::vector<StructuralVariantRecord>& svs,
                                std::vector<std::vector<std::string> >& refProbeArr, std::vector<std::vector<std::string> >& consProbeArr,
-                               std::vector<std::vector<BpRegion> >& bpRegion, std::vector<bool>& svOnChr, std::vector<uint32_t>& bad) {
+                               std::vector<std::vector<BpRegion> >& bpRegion, std::vector<bool>& svOnChr, std::vector<uint32_t>& bad,
+                               std::vector<uint8_t> const* want = nullptr) {
   const std::size_t N = svs.size();
   refProbeArr.assign(2, std::vector<std::string>(N));
   consProbeArr.assign(2, std::vector<std::string>(N));
@@ -166,7 +170,7 @@ inline int generateProbesBatch(dgpu_ctx* ctx, Config const& c, std::vector<uint3
     svOnChr[sv.chr] = true;
     svOnChr[sv.chr2] = true;
     if (sv.alleles.empty()) sv.alleles = _addAlleles(detail::upperSlice(chrseq[sv.chr], sv.svStart - 1, sv.svStart), target_name[sv.chr2], sv, sv.svt);
-    if (!sv.precise) continue;
+    if (!sv.precise || (want && !(*want)[i])) continue;
     Breakpoint bp(sv);
     if (sv.svt == 4) _initBreakpoint(target_len, bp, std::max((int32_t) ((sv.consensus.size() - sv.insLen) / 3), c.minimumFlankSize), sv.svt);
     else _initBreakpoint(target_len, bp, (int32_t) sv.consensus.size(), sv.svt);
@@ -548,16 +552,18 @@ struct JunctionProbes {
   std::vector<bool> svOnChr;
 };
 inline int prepareJunctionProbes(dgpu_ctx* ctx, Config const& c, std::vector<uint32_t> const& target_len, std::vector<std::string> const& target_name,
-                                 std::vector<const char*> const& chrseq, std::vector<StructuralVariantRecord>& svs, JunctionProbes& p) {
+                                 std::vector<const char*> const& chrseq, std::vector<StructuralVariantRecord>& svs, JunctionProbes& p,
+                                 std::vector<uint8_t> const* want = nullptr) {
   std::vector<uint32_t> bad;
-  int rc = generateProbesBatch(ctx, c, target_len, target_name, chrseq, svs, p.refProbeArr, p.consProbeArr, p.bpRegion, p.svOnChr, bad);
+  int rc = generateProbesBatch(ctx, c, target_len, target_name, chrseq, svs, p.refProbeArr, p.consProbeArr, p.bpRegion, p.svOnChr, bad, want);
   if (rc) return rc;
   if (!bad.empty()) return DGPU_ERR_ARG;  // the reference would have thrown (std::out_of_range in substr)
   return DGPU_OK;
 }
 
 inline int annotateJunctionReadsWithProbes(dgpu_ctx* ctx, Config const& c, std::vector<uint32_t> const& target_len, JunctionProbes const& probes, std::size_t nSv,
-                                           std::vector<SrRecord> const& recs, std::vector<JunctionCount>& countMap, std::vector<SvReadEvent>* dump = nullptr);
+                                           std::vector<SrRecord> const& recs, std::vector<JunctionCount>& countMap, std::vector<SvReadEvent>* dump = nullptr,
+                                           ContigShard const* cs = nullptr);
 
 inline int annotateJunctionReadsBatch(dgpu_ctx* ctx, Config const& c, std::vector<uint32_t> const& target_len, std::vector<std::string> const& target_name,
                                       std::vector<const char*> const& chrseq, std::vector<StructuralVariantRecord>& svs, std::vector<SrRecord> const& recs,
@@ -579,8 +585,11 @@ inline int annotateJunctionReadsBatch(dgpu_ctx* ctx, Config const& c, std::vecto
 //    orientation per breakpoint is src/split.h:55-68), instead of three strings per job.
 // dump: receives the ALT junction reads in job order (src/coverage.h:528-532). The reference aligns one job at a time when it dumps and checks
 // the cap against exact counts before each alignment; the merge below applies the same check to the same jobs in the same order.
+// cs != nullptr (contig sharding): recs holds this rank's contigs only; the rank aligns the jobs of its contigs, and the decided jobs of all
+// ranks (SV, REF / ALT, quality) are gathered and merged in job order — contig order is rank order — on every rank.
 inline int annotateJunctionReadsWithProbes(dgpu_ctx* ctx, Config const& c, std::vector<uint32_t> const& target_len, JunctionProbes const& probes, std::size_t nSv,
-                                           std::vector<SrRecord> const& recs, std::vector<JunctionCount>& countMap, std::vector<SvReadEvent>* dump) {
+                                           std::vector<SrRecord> const& recs, std::vector<JunctionCount>& countMap, std::vector<SvReadEvent>* dump,
+                                           ContigShard const* cs) {
   std::vector<std::vector<std::string> > const& refProbeArr = probes.refProbeArr;
   std::vector<std::vector<std::string> > const& consProbeArr = probes.consProbeArr;
   std::vector<std::vector<BpRegion> > const& bpRegion = probes.bpRegion;
@@ -596,7 +605,7 @@ inline int annotateJunctionReadsWithProbes(dgpu_ctx* ctx, Config const& c, std::
   }
   std::vector<std::vector<LightJob> > jobsOf((std::size_t) nchr);
   auto scanContig = [&](int32_t refIndex) {
-    if (!svOnChr[refIndex]) return;
+    if (!svOnChr[refIndex] || (cs && !cs->owns(refIndex))) return;
     const int32_t tlen = (int32_t) target_len[refIndex];
     // the union of the breakpoint regions as sorted disjoint intervals: "does the read touch a region" is one binary search
     std::vector<std::pair<int32_t, int32_t> > iv;
@@ -648,6 +657,16 @@ inline int annotateJunctionReadsWithProbes(dgpu_ctx* ctx, Config const& c, std::
   }
   // ---- arena: probes once, reads once per orientation; jobs in the reference's order (contig, read, breakpoint) ------------------------------
   std::vector<uint32_t> refAlignedReadCount(nSv, 0);
+  // the merge of one decided job into the SV's lists (src/coverage.h:442-453); true = an ALT read was added
+  auto merge = [&](uint32_t svId, bool isRef, uint8_t qual) {
+    JunctionCount& jc = countMap[svId];
+    if ((jc.ref.size() + jc.alt.size()) >= c.maxGenoReadCount) return false;
+    if (!isRef) { jc.alt.push_back(qual); return true; }
+    if (++refAlignedReadCount[svId] % 2) jc.ref.push_back(qual);
+    return false;
+  };
+  ByteWriter votes;   // contig sharding: this rank's decided jobs, in job order
+  int rc = DGPU_OK;
   std::vector<LightJob> jobs;
   for (auto& v : jobsOf) { jobs.insert(jobs.end(), v.begin(), v.end()); std::vector<LightJob>().swap(v); }
   const std::size_t J = jobs.size();
@@ -695,9 +714,10 @@ inline int annotateJunctionReadsWithProbes(dgpu_ctx* ctx, Config const& c, std::
     }
     const std::size_t n = end - done;
     std::vector<int32_t> dist(2 * n);
-    const int rc = dgpu_edit_distance(ctx, (const uint8_t*) arena.data(), arena.size(), qo.data(), ql.data(), to.data(), tl.data(), k.data(), DGPU_MODE_HW, 2 * n,
-                                      dist.data(), nullptr);
-    if (rc) return rc;
+    rc = dgpu_edit_distance(ctx, (const uint8_t*) arena.data(), arena.size(), qo.data(), ql.data(), to.data(), tl.data(), k.data(), DGPU_MODE_HW, 2 * n,
+                            dist.data(), nullptr);
+    if (rc && !cs) return rc;
+    if (rc) break;
     for (std::size_t i = 0; i < n; ++i) {   // processBatch scoring (src/coverage.h:412-441) and the merge (:442-453), in job order
       LightJob const& j = jobs[done + i];
       const double scoreAlt = _hwScore(c, ql[2 * i], dist[2 * i]);
@@ -705,14 +725,24 @@ inline int annotateJunctionReadsWithProbes(dgpu_ctx* ctx, Config const& c, std::
       if (!((scoreRef > 0.7) || (scoreAlt > 0.7))) continue;
       const bool isRef = scoreRef > scoreAlt;
       const uint8_t qual = (uint8_t) std::min(255, std::min((int) ((isRef ? scoreRef : scoreAlt) * 35), (int) j.qual));
-      JunctionCount& jc = countMap[j.svId];
-      if ((jc.ref.size() + jc.alt.size()) >= c.maxGenoReadCount) continue;
-      if (!isRef) {
-        jc.alt.push_back(qual);
-        if (dump) dump->push_back(SvReadEvent{j.rec, j.svId, j.svt});
-      } else if (++refAlignedReadCount[j.svId] % 2) jc.ref.push_back(qual);
+      if (cs) { votes.pod(j.svId); votes.pod<uint8_t>(isRef); votes.pod(qual); continue; }
+      if (merge(j.svId, isRef, qual) && dump) dump->push_back(SvReadEvent{j.rec, j.svId, j.svt});
     }
     done = end;
+  }
+  if (cs) {
+    std::vector<std::string> parts;
+    if ((rc = cs->exchange(rc, votes.buf, parts))) return rc;
+    for (std::string const& part : parts) {
+      ByteReader rd(part.data(), part.size());
+      while (rd.ok() && !rd.done()) {
+        const uint32_t svId = rd.pod<uint32_t>();
+        const bool isRef = rd.pod<uint8_t>() != 0;
+        const uint8_t qual = rd.pod<uint8_t>();
+        if (!rd.ok() || svId >= nSv) return DGPU_ERR_NCCL;
+        merge(svId, isRef, qual);
+      }
+    }
   }
   return DGPU_OK;
 }
@@ -749,12 +779,15 @@ inline int32_t _isizeMappingPos(SrRecord const& r, int32_t isize) {
 // svOnChr as produced by generateProbesBatch. The reference keys its mate table by a hash of (name, tid, pos, mtid, mpos);
 // here the key is the tuple itself.
 // dump: receives the ALT-spanning pair events in contig order, record order within a contig (src/coverage.h:652-657)
-inline void annotateSpanningAndDepth(Config const& c, LibraryInfo const& lib, std::vector<uint32_t> const& target_len,
-                                     std::vector<StructuralVariantRecord> const& svs, std::vector<bool> const& svOnChr, std::vector<SrRecord> const& recs,
-                                     std::vector<ReadCount>& covCount, std::vector<SpanningCount>& spanMap, std::vector<SvReadEvent>* dump = nullptr) {
+// cs != nullptr (contig sharding): recs holds this rank's contigs only. The inter-chromosomal first observations go to the rank of the mate's
+// contig, the rank walks its own contigs, and the events of every contig and the read-depth of every SV (counted on contig sv.chr) are gathered
+// and replayed in contig order on every rank.
+inline int annotateSpanningAndDepth(Config const& c, LibraryInfo const& lib, std::vector<uint32_t> const& target_len,
+                                    std::vector<StructuralVariantRecord> const& svs, std::vector<bool> const& svOnChr, std::vector<SrRecord> const& recs,
+                                    std::vector<ReadCount>& covCount, std::vector<SpanningCount>& spanMap, std::vector<SvReadEvent>* dump = nullptr,
+                                    ContigShard const* cs = nullptr) {
   covCount.assign(svs.size(), ReadCount());
   spanMap.assign(svs.size(), SpanningCount());
-  typedef std::tuple<uint64_t, int32_t, int32_t, int32_t, int32_t> TPairKey;
   typedef std::map<TPairKey, std::pair<bool, uint8_t> > TClipQual;
   struct SpanPoint { int32_t bppos, svt; uint32_t id; int32_t chr2, otherBppos; bool operator<(SpanPoint const& o) const { return bppos < o.bppos; } };
   struct SpanEvent { uint32_t id; uint8_t alt, quality; };   // one push_back of the reference, replayed in contig order below
@@ -786,11 +819,13 @@ inline void annotateSpanningAndDepth(Config const& c, LibraryInfo const& lib, st
       cliptraOf[rec.mtid][TPairKey(rec.name, rec.tid, rec.pos, rec.mtid, rec.mpos)] = std::make_pair(softClipped(rec), rec.mapq);
     }
   }
+  int rc = DGPU_OK;
+  if (cs && (rc = shareMateTables(*cs, DGPU_OK, cliptraOf))) return rc;
   std::vector<std::vector<SpanEvent> > events((std::size_t) nchr);
   std::vector<std::vector<SvReadEvent> > dumpOf(dump ? (std::size_t) nchr : 0);
   auto doContig = [&](std::size_t refIndexU) {
     const int32_t refIndex = (int32_t) refIndexU;
-    if (!svOnChr[refIndex]) return;
+    if (!svOnChr[refIndex] || (cs && !cs->owns(refIndex))) return;
     const std::size_t rlo = lo[refIndex], ri = lo[refIndex + 1];
     TClipQual clip;
     TClipQual& cliptra = cliptraOf[refIndex];
@@ -918,6 +953,32 @@ inline void annotateSpanningAndDepth(Config const& c, LibraryInfo const& lib, st
     worker();
     for (auto& th : pool) th.join();
   }
+  if (cs) {   // the other ranks' contig events and read-depth
+    ByteWriter w;
+    for (std::size_t refIndex = cs->lo(); refIndex < cs->hi(); ++refIndex) {
+      w.pod<uint64_t>((uint64_t) events[refIndex].size());
+      for (SpanEvent const& e : events[refIndex]) { w.pod(e.id); w.pod(e.alt); w.pod(e.quality); }
+    }
+    for (auto const& sv : svs) if (cs->owns(sv.chr)) w.pod(covCount[sv.id]);
+    std::vector<std::string> parts;
+    if ((rc = cs->exchange(DGPU_OK, w.buf, parts))) return rc;
+    for (int r = 0; r < cs->nranks; ++r) {
+      if (r == cs->rank) continue;
+      ByteReader rd(parts[r].data(), parts[r].size());
+      for (std::size_t refIndex = cs->bounds[r]; refIndex < cs->bounds[r + 1]; ++refIndex) {
+        const uint64_t n = rd.pod<uint64_t>();
+        for (uint64_t k = 0; k < n && rd.ok(); ++k) {
+          SpanEvent e;
+          e.id = rd.pod<uint32_t>(); e.alt = rd.pod<uint8_t>(); e.quality = rd.pod<uint8_t>();
+          if (e.id >= svs.size()) return DGPU_ERR_NCCL;
+          events[refIndex].push_back(e);
+        }
+      }
+      for (auto const& sv : svs)
+        if (sv.chr >= (int32_t) cs->bounds[r] && sv.chr < (int32_t) cs->bounds[r + 1]) covCount[sv.id] = rd.pod<ReadCount>();
+      if (!rd.ok() || !rd.done()) return DGPU_ERR_NCCL;
+    }
+  }
   std::vector<uint32_t> refAlignedSpanCount(svs.size(), 0);
   for (int32_t refIndex = 0; refIndex < nchr; ++refIndex)
     for (SpanEvent const& e : events[refIndex]) {
@@ -925,6 +986,7 @@ inline void annotateSpanningAndDepth(Config const& c, LibraryInfo const& lib, st
       else if (++refAlignedSpanCount[e.id] % 2) spanMap[e.id].ref.push_back(e.quality);
     }
   for (auto const& v : dumpOf) dump->insert(dump->end(), v.begin(), v.end());
+  return DGPU_OK;
 }
 
 }  // namespace dellyb200

@@ -28,9 +28,10 @@ namespace dellyb200 {
 // hash_string(qname) in a set that scanPEandSR fills with hash_sr ids (:409), so it only fires on a hash coincidence.
 // The per-file half of scanPEandSR (:318-463): junction scan and abnormal-pair bookkeeping of ONE sample, junction selection; the
 // sample's split-read and paired-end records are appended to srBR / bamRecord (the reference concatenates the files in order, :468-477).
-inline void scanSamplePEandSR(Config const& c, LibraryInfo& lib, std::vector<uint32_t> const& target_len, std::vector<SrRecord> const& recs, TSvtSRBamRecord& srBRAll,
-                              std::vector<std::vector<BamAlignRecord> >& bamRecord) {
-  typedef std::tuple<uint64_t, int32_t, int32_t, int32_t, int32_t> TPairKey;
+// cs != nullptr (contig sharding): recs holds this rank's contigs only; the inter-chromosomal first observations go to the rank of the mate's
+// contig before the contig logs are built, and the logs of all ranks are gathered and replayed in contig order on every rank.
+inline int scanSamplePEandSR(Config const& c, LibraryInfo& lib, std::vector<uint32_t> const& target_len, std::vector<SrRecord> const& recs, TSvtSRBamRecord& srBRAll,
+                             std::vector<std::vector<BamAlignRecord> >& bamRecord, ContigShard const* cs = nullptr) {
   typedef std::map<TPairKey, std::pair<uint8_t, int32_t> > TMateMap;
   std::unordered_map<std::size_t, TJunctionVector> readBp;
   TSvtSRBamRecord srBR(2 * DELLY_SVT_TRANS);
@@ -78,6 +79,8 @@ inline void scanSamplePEandSR(Config const& c, LibraryInfo& lib, std::vector<uin
       if (pairType(rec) < 0) continue;
       matetraOf[rec.mtid][TPairKey(rec.name, rec.tid, rec.pos, rec.mtid, rec.mpos)] = std::make_pair(rec.mapq, (int32_t) alignmentLength(rec));
     }
+  int rc = DGPU_OK;
+  if (cs && (rc = shareMateTables(*cs, DGPU_OK, matetraOf))) return rc;
   struct JunctionLog {   // stands in for the per-read table inside cigarJunctions: records (read id, junction) in insertion order
     std::vector<std::pair<std::size_t, Junction> > ev;
     struct Slot { JunctionLog* log; std::size_t seed; void push_back(Junction const& j) { log->ev.emplace_back(seed, j); } };
@@ -87,6 +90,7 @@ inline void scanSamplePEandSR(Config const& c, LibraryInfo& lib, std::vector<uin
   std::vector<ContigLog> logs((std::size_t) nchr);
   parallelFor((std::size_t) nchr, [&](std::size_t refIndexU) {
     const int32_t refIndex = (int32_t) refIndexU;
+    if (cs && !cs->owns(refIndex)) return;
     ContigLog& log = logs[refIndexU];
     TMateMap mateMap;
     TMateMap& matetra = matetraOf[refIndexU];
@@ -123,6 +127,39 @@ inline void scanSamplePEandSR(Config const& c, LibraryInfo& lib, std::vector<uin
       }
     }
   });
+  if (cs) {   // the logs of the other ranks' contigs
+    ByteWriter w;
+    for (std::size_t refIndex = cs->lo(); refIndex < cs->hi(); ++refIndex) {
+      ContigLog const& log = logs[refIndex];
+      w.pod<uint64_t>((uint64_t) log.junctions.ev.size());
+      for (auto const& e : log.junctions.ev) {
+        Junction const& j = e.second;
+        w.pod<uint64_t>((uint64_t) e.first); w.pod<uint8_t>(j.forward); w.pod<uint8_t>(j.scleft); w.pod(j.refidx); w.pod(j.rstart); w.pod(j.refpos); w.pod(j.seqpos); w.pod(j.qual);
+      }
+      w.pod<uint64_t>((uint64_t) log.pairs.size());
+      for (auto const& pr : log.pairs) { w.pod(pr.first); w.pod(pr.second); }
+    }
+    std::vector<std::string> parts;
+    if ((rc = cs->exchange(DGPU_OK, w.buf, parts))) return rc;
+    for (int r = 0; r < cs->nranks; ++r) {
+      if (r == cs->rank) continue;
+      ByteReader rd(parts[r].data(), parts[r].size());
+      for (std::size_t refIndex = cs->bounds[r]; refIndex < cs->bounds[r + 1]; ++refIndex) {
+        ContigLog& log = logs[refIndex];
+        const uint64_t nj = rd.pod<uint64_t>();
+        for (uint64_t k = 0; k < nj && rd.ok(); ++k) {
+          const std::size_t seed = (std::size_t) rd.pod<uint64_t>();
+          const bool fw = rd.pod<uint8_t>() != 0, cl = rd.pod<uint8_t>() != 0;
+          const int32_t refidx = rd.pod<int32_t>(), rstart = rd.pod<int32_t>(), refpos = rd.pod<int32_t>(), seqpos = rd.pod<int32_t>();
+          const uint16_t qual = rd.pod<uint16_t>();
+          log.junctions.ev.emplace_back(seed, Junction(fw, cl, refidx, rstart, refpos, seqpos, qual));
+        }
+        const uint64_t np = rd.pod<uint64_t>();
+        for (uint64_t k = 0; k < np && rd.ok(); ++k) { const int32_t svt = rd.pod<int32_t>(); log.pairs.emplace_back(svt, rd.pod<BamAlignRecord>()); }
+      }
+      if (!rd.ok() || !rd.done()) return DGPU_ERR_NCCL;
+    }
+  }
   for (int32_t refIndex = 0; refIndex < nchr; ++refIndex) {
     for (auto const& e : logs[refIndex].junctions.ev) readBp[e.first].push_back(e.second);
     for (auto const& pr : logs[refIndex].pairs) { bamRecord[pr.first].push_back(pr.second); ++lib.abnormal_pairs; }
@@ -134,6 +171,7 @@ inline void scanSamplePEandSR(Config const& c, LibraryInfo& lib, std::vector<uin
   if (c.wantSvt(4)) selectInsertions(c, readBp, srBR);
   if (c.svtset.empty() || c.svtset.count(5) || c.svtset.count(6) || c.svtset.count(7) || c.svtset.count(8)) selectTranslocations(c, readBp, srBR);
   for (std::size_t svt = 0; svt < srBR.size(); ++svt) srBRAll[svt].insert(srBRAll[svt].end(), srBR[svt].begin(), srBR[svt].end());
+  return DGPU_OK;
 }
 
 // The joint half (:479-527): per SV type sort + cluster of the pooled records, and the read store assembleSplitReads consumes.
@@ -167,17 +205,24 @@ inline int clusterScannedPEandSR(dgpu_ctx* ctx, Config const& c, int32_t varisiz
 }
 
 // scanPEandSR over the samples of a call set (libs[f] belongs to samples[f]).
+// cs: contig sharding (scanSamplePEandSR); the pooled records and the clustering are then the same on every rank.
 inline int scanPEandSRBatch(dgpu_ctx* ctx, Config const& c, std::vector<LibraryInfo>& libs, std::vector<uint32_t> const& target_len,
                             std::vector<std::vector<SrRecord> const*> const& samples, std::vector<StructuralVariantRecord>& svs,
-                            std::vector<StructuralVariantRecord>& srSVs, std::vector<TPosReadSV>& srStore) {
+                            std::vector<StructuralVariantRecord>& srSVs, std::vector<TPosReadSV>& srStore, ContigShard const* cs = nullptr) {
   TSvtSRBamRecord srBR(2 * DELLY_SVT_TRANS);
   std::vector<std::vector<BamAlignRecord> > bamRecord(2 * DELLY_SVT_TRANS);
   int32_t varisize = 0;
   for (std::size_t f = 0; f < samples.size(); ++f) {
-    scanSamplePEandSR(c, libs[f], target_len, *samples[f], srBR, bamRecord);
+    const int rc = scanSamplePEandSR(c, libs[f], target_len, *samples[f], srBR, bamRecord, cs);
+    if (rc) return rc;
     varisize = std::max(varisize, std::max(libs[f].maxNormalISize, libs[f].rs));
   }
-  return clusterScannedPEandSR(ctx, c, varisize, target_len, srBR, bamRecord, svs, srSVs, srStore);
+  const int rc = clusterScannedPEandSR(ctx, c, varisize, target_len, srBR, bamRecord, svs, srSVs, srStore);
+  if (rc && cs) {   // a device failure of this rank alone: the next exchange of the other ranks (the assembly's) carries it to them
+    std::vector<std::string> parts;
+    cs->exchange(rc, std::string(), parts);
+  }
+  return rc;
 }
 
 inline int scanPEandSRBatch(dgpu_ctx* ctx, Config const& c, LibraryInfo& lib, std::vector<uint32_t> const& target_len, std::vector<SrRecord> const& recs,
@@ -251,43 +296,55 @@ inline void mergeSort(std::vector<StructuralVariantRecord>& pe, std::vector<Stru
 // up to 10^6 read-1 alignments (primary, mapped, not duplicate / QC-fail), the normal-pair window and the deletion cut-off
 // derived from them. A library whose pairs are mostly not in FR orientation keeps median = 0 (the reference warns and treats
 // it as single-end). recs sorted like a coordinate-sorted BAM.
-inline void getLibraryParams(Config const& c, std::vector<uint32_t> const& target_len, std::vector<SrRecord> const& recs, LibraryInfo& lib) {
-  lib = LibraryInfo();
-  const uint32_t maxAlignmentsScreened = 10000000, maxNumAlignments = 1000000, minNumAlignments = 1000;
+// The screen is a state (LibraryScreen) so that it can be continued: a contig-sharded run (getLibraryParamsSharded) continues it rank after
+// rank, where the ranks of the lower contigs left it. The screened values are kept as histograms (value -> count): the medians are order
+// statistics, which a histogram gives exactly, and a histogram of insert sizes is a few kB where the values are millions.
+struct LibraryScreen {
   uint32_t alignmentCount = 0, processedNumPairs = 0, processedNumReads = 0, rplus = 0, nonrplus = 0;
-  std::vector<uint32_t> vecISize, readSize;
-  bool libCharacterized = false;
+  bool characterized = false;
+  std::unordered_map<uint32_t, uint32_t> readSize, isize;
+};
+inline void continueLibraryScreen(std::vector<uint32_t> const& target_len, std::vector<SrRecord> const& recs, LibraryScreen& s) {
+  const uint32_t maxAlignmentsScreened = 10000000, maxNumAlignments = 1000000;
   std::size_t ri = 0;
-  for (int32_t refIndex = 0; (refIndex < (int32_t) target_len.size()) && !libCharacterized; ++refIndex) {
+  for (int32_t refIndex = 0; (refIndex < (int32_t) target_len.size()) && !s.characterized; ++refIndex) {
     const std::size_t rlo = ri;
     while (ri < recs.size() && recs[ri].tid == refIndex) ++ri;
     for (std::size_t q = rlo; q < ri; ++q) {
       SrRecord const& rec = recs[q];
-      if ((rec.flag & 0x80) || !(rec.lqseq < 65000)) continue;   // BAM_FREAD2
+      if ((rec.flag & 0x80) || !(rec.lqseq < 65000)) continue;
       if (rec.flag & (BAMF_SECONDARY | BAMF_QCFAIL | BAMF_DUP | BAMF_SUPPLEMENTARY | BAMF_UNMAP)) continue;
-      if ((alignmentCount > maxAlignmentsScreened) || ((processedNumReads >= maxNumAlignments) && (processedNumPairs == 0)) || (processedNumPairs >= maxNumAlignments)) {
-        libCharacterized = true;
+      if ((s.alignmentCount > maxAlignmentsScreened) || ((s.processedNumReads >= maxNumAlignments) && (s.processedNumPairs == 0)) ||
+          (s.processedNumPairs >= maxNumAlignments)) {
+        s.characterized = true;
         break;
       }
-      ++alignmentCount;
-      if (processedNumReads < maxNumAlignments) { readSize.push_back((uint32_t) rec.lqseq); ++processedNumReads; }
-      if ((rec.flag & 0x1) && !(rec.flag & BAMF_MUNMAP) && (rec.tid == rec.mtid) && (processedNumPairs < maxNumAlignments)) {
-        vecISize.push_back((uint32_t) std::abs(rec.isize));
-        if (getSVType(rec) == 2) ++rplus; else ++nonrplus;
-        ++processedNumPairs;
+      ++s.alignmentCount;
+      if (s.processedNumReads < maxNumAlignments) { ++s.readSize[(uint32_t) rec.lqseq]; ++s.processedNumReads; }
+      if ((rec.flag & 0x1) && !(rec.flag & BAMF_MUNMAP) && (rec.tid == rec.mtid) && (s.processedNumPairs < maxNumAlignments)) {
+        ++s.isize[(uint32_t) std::abs(rec.isize)];
+        if (getSVType(rec) == 2) ++s.rplus; else ++s.nonrplus;
+        ++s.processedNumPairs;
       }
     }
   }
-  // medians = the element a full sort would put at size / 2: selection instead of three sorts of up to a million values
-  auto medianOf = [](std::vector<uint32_t>& v) { std::nth_element(v.begin(), v.begin() + v.size() / 2, v.end()); return v[v.size() / 2]; };
-  if (processedNumReads >= minNumAlignments) lib.rs = (int32_t) medianOf(readSize);
-  if (processedNumPairs >= minNumAlignments) {
-    const int32_t median = (int32_t) medianOf(vecISize);
-    std::vector<uint32_t> absDev;
-    absDev.reserve(vecISize.size());
-    for (uint32_t v : vecISize) absDev.push_back((uint32_t) std::abs((int32_t) v - median));
-    const int32_t mad = (int32_t) medianOf(absDev);
-    if ((median >= 50) && (median <= 100000) && !(rplus < nonrplus)) {
+}
+inline void libraryFromScreen(Config const& c, LibraryScreen const& s, LibraryInfo& lib) {
+  const uint32_t minNumAlignments = 1000;
+  lib = LibraryInfo();
+  auto kth = [](std::unordered_map<uint32_t, uint32_t> const& h, uint64_t k) {   // the element a full sort would put at index k
+    std::vector<std::pair<uint32_t, uint32_t> > v(h.begin(), h.end());
+    std::sort(v.begin(), v.end());
+    for (auto const& kv : v) { if (k < kv.second) return kv.first; k -= kv.second; }
+    return 0u;
+  };
+  if (s.processedNumReads >= minNumAlignments) lib.rs = (int32_t) kth(s.readSize, s.processedNumReads / 2);
+  if (s.processedNumPairs >= minNumAlignments) {
+    const int32_t median = (int32_t) kth(s.isize, s.processedNumPairs / 2);
+    std::unordered_map<uint32_t, uint32_t> absDev;
+    for (auto const& kv : s.isize) absDev[(uint32_t) std::abs((int32_t) kv.first - median)] += kv.second;
+    const int32_t mad = (int32_t) kth(absDev, s.processedNumPairs / 2);
+    if ((median >= 50) && (median <= 100000) && !(s.rplus < s.nonrplus)) {
       lib.median = median; lib.mad = mad;
       lib.maxNormalISize = median + (c.madNormalCutoff * mad);
       lib.minNormalISize = std::max(median - (c.madNormalCutoff * mad), 0);
@@ -298,6 +355,46 @@ inline void getLibraryParams(Config const& c, std::vector<uint32_t> const& targe
       if (lib.minISizeCutoff < 0) lib.minISizeCutoff = 0;
     }
   }
+}
+inline void getLibraryParams(Config const& c, std::vector<uint32_t> const& target_len, std::vector<SrRecord> const& recs, LibraryInfo& lib) {
+  LibraryScreen s;
+  continueLibraryScreen(target_len, recs, s);
+  libraryFromScreen(c, s, lib);
+}
+
+// the screen over a contig-sharded genome: rank r continues it (over its own contigs) from the state rank r - 1 left, until the library is
+// characterized — usually inside the first rank's contigs: one exchange
+inline int getLibraryParamsSharded(Config const& c, std::vector<uint32_t> const& target_len, std::vector<SrRecord> const& recs, ContigShard const& cs,
+                                   LibraryInfo& lib) {
+  LibraryScreen s;
+  for (int r = 0; r < cs.nranks && !s.characterized; ++r) {
+    ByteWriter w;
+    if (r == cs.rank) {
+      continueLibraryScreen(target_len, recs, s);
+      const uint32_t f[5] = {s.alignmentCount, s.processedNumPairs, s.processedNumReads, s.rplus, s.nonrplus};
+      for (uint32_t x : f) w.pod(x);
+      w.pod<uint8_t>(s.characterized);
+      for (auto const* h : {&s.readSize, &s.isize}) {
+        w.pod<uint64_t>((uint64_t) h->size());
+        for (auto const& kv : *h) { w.pod(kv.first); w.pod(kv.second); }
+      }
+    }
+    std::vector<std::string> parts;
+    const int rc = cs.exchange(DGPU_OK, w.buf, parts);
+    if (rc) return rc;
+    ByteReader rd(parts[r].data(), parts[r].size());
+    s.alignmentCount = rd.pod<uint32_t>(); s.processedNumPairs = rd.pod<uint32_t>(); s.processedNumReads = rd.pod<uint32_t>(); s.rplus = rd.pod<uint32_t>();
+    s.nonrplus = rd.pod<uint32_t>();
+    s.characterized = rd.pod<uint8_t>() != 0;
+    for (auto* h : {&s.readSize, &s.isize}) {
+      h->clear();
+      const uint64_t n = rd.pod<uint64_t>();
+      for (uint64_t k = 0; k < n && rd.ok(); ++k) { const uint32_t v = rd.pod<uint32_t>(); (*h)[v] = rd.pod<uint32_t>(); }
+    }
+    if (!rd.ok() || !rd.done()) return DGPU_ERR_NCCL;
+  }
+  libraryFromScreen(c, s, lib);
+  return DGPU_OK;
 }
 
 }  // namespace dellyb200
