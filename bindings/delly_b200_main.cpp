@@ -38,7 +38,7 @@ struct Options {
   int device = 0, ioThreads = 16;
   int rank = 0, nranks = 1;          // one process per GPU: --rank r --nranks N --comm-file path (rank 0 publishes the NCCL id there)
   std::string commFile, timingFile;  // --timing file: stage wall-clock times as one JSON object
-  std::string shardBy = "svs";       // --shard-by svs|contig: what the ranks divide (sr only)
+  std::string shardBy = "svs";       // --shard-by svs|contig: what the ranks divide
   bool readShareOnly = false;        // --read-share-only: read this rank's share of the alignments, write --timing, stop (measuring a share alone)
   float indelExtension = 0.5f;
   MethylConfig methyl;
@@ -74,8 +74,8 @@ void usage(Options const& o) {
   std::cerr << "\nUsage: delly_b200 " << (o.lr ? "lr" : "sr") << " [OPTIONS] -g <ref.fa> <sample1.sort.bam> <sample2.sort.bam> ...\n"
             << "  options follow `delly " << (o.lr ? "lr" : "sr") << "` (same letters and defaults), including -d <reads.gz> (gzipped list of the reads"
             << " that support each SV); extra: --device N, --io-threads N" << (o.lr ? ", --mei <templates.fa>" : "") << "\n"
-            << "  several GPUs, one process each: --rank r --nranks N --comm-file <path>" << (o.lr ? "" : " [--shard-by svs|contig]") << " [--timing <file>]\n"
-            << (o.lr ? "" : "  --read-share-only: read this rank's share (--shard-by contig), write --timing and stop: no device, no exchange\n");
+            << "  several GPUs, one process each: --rank r --nranks N --comm-file <path> [--shard-by svs|contig] [--timing <file>]\n"
+            << "  --read-share-only: read this rank's share (--shard-by contig), write --timing and stop: no device, no exchange\n";
 }
 
 // `delly sr` (src/delly.h:207-246) and `delly lr` (src/tegua.h:215-275) share most letters; the long names are the reference's.
@@ -116,8 +116,8 @@ bool parse(int argc, char** argv, Options& o) {
     else if (a == "--nranks") o.nranks = std::stoi(val());
     else if (a == "--comm-file") o.commFile = val();
     else if (a == "--timing") o.timingFile = val();
-    else if (!o.lr && a == "--shard-by") o.shardBy = val();
-    else if (!o.lr && a == "--read-share-only") o.readShareOnly = true;
+    else if (a == "--shard-by") o.shardBy = val();
+    else if (a == "--read-share-only") o.readShareOnly = true;
     else if (!o.lr && is("-h", "--threads")) c.maxThreads = (uint32_t) std::stoul(val());
     else if (!o.lr && is("-r", "--qual-tra")) c.minTraQual = (uint16_t) std::stoi(val());
     else if (!o.lr && is("-s", "--mad-cutoff")) c.madCutoff = (uint16_t) std::stoi(val());
@@ -473,8 +473,10 @@ int runSr(Options& o, DeviceSession& dev) {
 }
 
 int runLr(Options& o, DeviceSession& dev, const char* argv0) {
+  StageClock clock;
   Inputs in;
   if (!openInputs(o, in)) return 1;
+  clock.lap("open_inputs");
   Config& c = o.c;
   const std::size_t F = in.files.size();
   if (o.mode == "pb") o.indelExtension = 0.7f;
@@ -482,6 +484,19 @@ int runLr(Options& o, DeviceSession& dev, const char* argv0) {
   MeiTemplates mei;
   const std::string meiPath = o.meifile.empty() ? exeDir(argv0) + "/../data/_mei_templates.fa" : o.meifile;
   if (!loadMei(meiPath, mei)) { std::cerr << "cannot read the annotation templates " << meiPath << " (see --mei)" << std::endl; return 1; }
+  const bool byContig = o.shardBy == "contig";
+  Shard shard = dev.shard();
+  ShareStats share;
+  if (byContig) {   // this rank reads its own contigs only: its valid regions, and its whole contigs with -x
+    shard.contigBounds = contigCut(o, in);
+    if (o.nranks == 1) shard.gather = [](std::string const& local, std::vector<std::string>& parts) { parts.assign(1, local); return (int) DGPU_OK; };
+    keepOwnContigs(shard.contigBounds, o.rank, in.validRegions, in.wholeContigs);
+    GatherFn g = shard.gather;
+    shard.gather = [g, &share, &clock](std::string const& local, std::vector<std::string>& parts) {
+      share.sentAtLap[clock.ms.size()] += local.size();
+      return g(local, parts);
+    };
+  }
   const bool dump = !o.dumpfile.empty();
   std::vector<std::vector<std::string> > names(dump ? F : 0);   // query names of the genotyped records (-d)
   std::vector<std::vector<LrRecord> > recs(F);
@@ -505,29 +520,42 @@ int runLr(Options& o, DeviceSession& dev, const char* argv0) {
       }
       genoSamples.push_back(LrSample{&recsWhole[f], &idsWhole[f]});
     }
+  clock.lap("read_bam");
+  if (byContig) {
+    const std::size_t lo = shard.contigBounds[o.rank], hi = shard.contigBounds[o.rank + 1];
+    std::size_t n = 0;
+    for (std::size_t f = 0; f < F; ++f) n += recs[f].size() + (o.hasExclude ? recsWhole[f].size() : 0);
+    std::cerr << "rank " << o.rank << "/" << o.nranks << ": contigs ";
+    if (lo < hi) std::cerr << lo << "-" << hi - 1 << " (" << in.target_name[lo] << ".." << in.target_name[hi - 1] << ")";
+    else std::cerr << "none";
+    std::cerr << ", " << n << " records" << std::endl;
+    share.records = n;
+    if (o.readShareOnly) { writeTiming(o, clock, 0, &share); return 0; }
+  }
   if (!dev.wait()) return 3;
+  clock.lap("wait_device");
   dgpu_ctx* ctx = dev.ctx();
   LrMultiCallSet cs;
   SvReadDump reads;
   int rc;
-  const Shard shard = dev.shard();
   if (!o.hasVcf)
     rc = dellyLrCallSharded(ctx, c, o.indelExtension, in.target_len, in.target_name, in.genome.cseq, samples, shard, cs, &mei, o.anno, &o.methyl,
-                            o.hasExclude ? &genoSamples : nullptr, dump ? &reads : nullptr);
+                            o.hasExclude ? &genoSamples : nullptr, dump ? &reads : nullptr, &clock);
   else {
     std::vector<VcfSite> sites;
     bool hasConsBp = false;
     if (!io::readSites(o.vcffile, sites, hasConsBp)) return 1;
     rc = dellyLrGenotypeSharded(ctx, c, in.target_len, in.target_name, in.genome.cseq, sites, hasConsBp, o.hasExclude ? genoSamples : samples, shard, cs, &mei, o.anno,
-                                &o.methyl, dump ? &reads : nullptr);
+                                &o.methyl, dump ? &reads : nullptr, &clock);
     if (rc == DGPU_ERR_ARG && !cs.sample.empty()) { std::cerr << "Error: Delly genotyping requires a Delly BCF file from v1.1.7 or later!" << std::endl; rc = DGPU_OK; }
   }
   if (rc) { std::cerr << "delly_b200: device path failed (" << rc << "): " << dgpu_last_error(ctx) << std::endl; return 1; }
-  if (o.rank != 0) return 0;   // every rank holds the complete call set; rank 0 writes it
+  if (o.rank != 0) { writeTiming(o, clock, cs.svs.size(), byContig ? &share : nullptr); return 0; }   // every rank holds the complete call set; rank 0 writes it
   if (dump && !cs.svs.empty()) {   // genotypeLR returns before it opens the dump when the SV list is empty (src/genotype.h:97, :127-133)
     std::vector<std::vector<LrRecord> const*> geno;
     for (LrSample const& s : (o.hasExclude ? genoSamples : samples)) geno.push_back(s.recs);
     if (!writeDump(o.dumpfile, [&](auto put) { writeLrReadDump(put, reads, o.files, geno, names, in.target_name); })) return 1;
+    clock.lap("write_dump");
   }
   // long reads have no spanning pairs: empty lists per SV (src/tegua.h:173-190)
   std::vector<SpanningCount> noSpan(cs.svs.size());
@@ -540,6 +568,8 @@ int runLr(Options& o, DeviceSession& dev, const char* argv0) {
   if (!w.ok()) { std::cerr << "cannot open " << o.outfile << std::endl; return 1; }
   vcfRecordsTo(w, cs.svs, vs, in.target_name, in.target_len, o.genome, io::todayIso(), o.hasVcf, o.methyl.minCpgDepth);
   w.close();
+  clock.lap("write_bcf");
+  writeTiming(o, clock, cs.svs.size(), byContig ? &share : nullptr);
   return 0;
 }
 

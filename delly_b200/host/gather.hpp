@@ -380,14 +380,80 @@ inline int genotypeLrSitesSharded(dgpu_ctx* ctx, Config const& c, std::vector<ui
   return DGPU_OK;
 }
 
-// `delly lr` over ranks: the record stream, the junction clustering and the read collection replicated (host), the per-SV consensus + consensus
-// alignment and the genotyping / annotation sharded by cost.
+// ---- contig-sharded long reads (`delly_b200 lr --shard-by contig`) ---------------------------------------------------------------------
+// A rank holds the long reads of its own contigs only. Discovery: the junction logs are gathered and replayed in contig order
+// (clusterSRReadsLR), the read collection of an SV ends on the rank of sv.chr, which receives the lower ranks' candidates and builds the
+// consensus (assembleLRBatch). Genotyping per file: the cap counts of SVs split over two ranks, then the decided qualities, read-depth and
+// methylation sums (genotypeLRBatch). Annotation below. Junction selection, clustering, the sort, the near-duplicate filter and the
+// renumbering run on every rank over the same inputs.
+
+// annotateSVs over the SVs whose first breakpoint is on this rank's contigs; the annotations of every rank's SVs are exchanged
+inline int annotateSVsByContig(dgpu_ctx* ctx, AnnoConfig const& annoCfg, MeiTemplates const& mei, std::vector<const char*> const& chrseq,
+                               std::vector<uint32_t> const& target_len, std::vector<StructuralVariantRecord>& svs, ContigShard const& cs) {
+  std::vector<int32_t> which;
+  for (std::size_t i = 0; i < svs.size(); ++i)
+    if (!_translocation(svs[i].svt) && cs.owns(svs[i].chr)) which.push_back((int32_t) i);
+  int rc = which.empty() ? DGPU_OK : annotateSVBatch(ctx, annoCfg, mei, chrseq, target_len, svs, which);
+  ByteWriter w;
+  for (int32_t i : which) { SVAnno const& a = svs[i].anno; w.pod<uint8_t>(a.isRC ? 1 : 0); w.pod(a.seqType); w.pod(a.homLen); w.pod(a.trPeriod); w.pod(a.trCopies); }
+  std::vector<std::string> parts;
+  if ((rc = cs.exchange(rc, w.buf, parts))) return rc;
+  for (int r = 0; r < cs.nranks; ++r) {
+    if (r == cs.rank) continue;
+    ByteReader rd(parts[r].data(), parts[r].size());
+    for (StructuralVariantRecord& sv : svs) {
+      if (_translocation(sv.svt) || cs.owner(sv.chr) != r) continue;
+      sv.anno.isRC = rd.pod<uint8_t>() != 0; sv.anno.seqType = rd.pod<int32_t>(); sv.anno.homLen = rd.pod<int32_t>(); sv.anno.trPeriod = rd.pod<int32_t>();
+      sv.anno.trCopies = rd.pod<float>();
+    }
+    if (!rd.ok() || !rd.done()) return DGPU_ERR_NCCL;
+  }
+  return DGPU_OK;
+}
+
+// genotyping (every file) + annotation of a complete SV list whose ids are its indices, on a rank that holds its own contigs' reads
+inline int genotypeLrSitesByContig(dgpu_ctx* ctx, Config const& c, std::vector<uint32_t> const& target_len, std::vector<std::string> const& target_name,
+                                   std::vector<const char*> const& chrseq, std::vector<LrSample> const& samples, ContigShard const& cs, LrMultiCallSet& out,
+                                   MeiTemplates const* mei, AnnoConfig const& annoCfg, MethylConfig const* methylCfg, StageClock* clock) {
+  out.sample.assign(samples.size(), LrSampleCounts());
+  int rc;
+  for (std::size_t f = 0; f < samples.size(); ++f) {
+    LrSampleCounts& sc = out.sample[f];
+    if ((rc = genotypeLRBatch(ctx, c, target_len, target_name, chrseq, out.svs, *samples[f].recs, sc.jctMap, sc.rcMap, methylCfg, methylCfg ? &sc.methyl : nullptr,
+                              nullptr, &cs)))
+      return rc;
+    lrSampleFormat(out.svs, sc.jctMap, sc.rcMap, sc.format);
+  }
+  if (mei && (rc = annotateSVsByContig(ctx, annoCfg, *mei, chrseq, target_len, out.svs, cs))) return rc;
+  if (clock) clock->lap("genotype");
+  return DGPU_OK;
+}
+
+// `delly lr` discovery + genotyping, contig-sharded: the result equals dellyLrCallMulti's on every rank
+inline int dellyLrCallByContig(dgpu_ctx* ctx, Config const& c, float indelExtension, std::vector<uint32_t> const& target_len, std::vector<std::string> const& target_name,
+                               std::vector<const char*> const& chrseq, std::vector<LrSample> const& samples, ContigShard const& cs, LrMultiCallSet& out,
+                               MeiTemplates const* mei, AnnoConfig const& annoCfg, MethylConfig const* methylCfg, std::vector<LrSample> const* genoSamples,
+                               StageClock* clock) {
+  out = LrMultiCallSet();
+  std::vector<LrRecord> stream;
+  std::vector<std::size_t> streamIds;
+  buildLrStream(target_len, samples, stream, streamIds);
+  int rc = discoverLrSVs(ctx, c, indelExtension, target_len, chrseq, stream, streamIds, out.svs, nullptr, &cs);
+  if (rc) return rc;
+  if (clock) clock->lap("discover");
+  return genotypeLrSitesByContig(ctx, c, target_len, target_name, chrseq, genoSamples ? *genoSamples : samples, cs, out, mei, annoCfg, methylCfg, clock);
+}
+
+// `delly lr` over ranks. --shard-by svs: the record stream, the junction clustering and the read collection replicated (host), the per-SV
+// consensus + consensus alignment and the genotyping / annotation sharded by cost. --shard-by contig: dellyLrCallByContig.
 inline int dellyLrCallSharded(dgpu_ctx* ctx, Config const& c, float indelExtension, std::vector<uint32_t> const& target_len, std::vector<std::string> const& target_name,
                               std::vector<const char*> const& chrseq, std::vector<LrSample> const& samples, Shard const& shard, LrMultiCallSet& out,
                               MeiTemplates const* mei = nullptr, AnnoConfig const& annoCfg = AnnoConfig(), MethylConfig const* methylCfg = nullptr,
-                              std::vector<LrSample> const* genoSamples = nullptr, SvReadDump* dump = nullptr) {
+                              std::vector<LrSample> const* genoSamples = nullptr, SvReadDump* dump = nullptr, StageClock* clock = nullptr) {
   out = LrMultiCallSet();
-  if (dump && shard.active()) return DGPU_ERR_ARG;
+  if (dump && (shard.active() || shard.byContig())) return DGPU_ERR_ARG;
+  if (shard.byContig())
+    return dellyLrCallByContig(ctx, c, indelExtension, target_len, target_name, chrseq, samples, shard.contigShard(), out, mei, annoCfg, methylCfg, genoSamples, clock);
   std::vector<LrRecord> stream;
   std::vector<std::size_t> streamIds;
   buildLrStream(target_len, samples, stream, streamIds);
@@ -395,23 +461,30 @@ inline int dellyLrCallSharded(dgpu_ctx* ctx, Config const& c, float indelExtensi
   if (shard.active()) as = makeAssembleShard(shard);
   int rc = discoverLrSVs(ctx, c, indelExtension, target_len, chrseq, stream, streamIds, out.svs, shard.active() ? &as : nullptr);
   if (rc) return rc;
-  return genotypeLrSitesSharded(ctx, c, target_len, target_name, chrseq, genoSamples ? *genoSamples : samples, shard, out, mei, annoCfg, methylCfg, true, dump);
+  if (clock) clock->lap("discover");
+  rc = genotypeLrSitesSharded(ctx, c, target_len, target_name, chrseq, genoSamples ? *genoSamples : samples, shard, out, mei, annoCfg, methylCfg, true, dump);
+  if (!rc && clock) clock->lap("genotype");
+  return rc;
 }
 
 // `delly lr -v sites.bcf` over ranks (ids = file order, src/tegua.h:157)
 inline int dellyLrGenotypeSharded(dgpu_ctx* ctx, Config const& c, std::vector<uint32_t> const& target_len, std::vector<std::string> const& target_name,
                                   std::vector<const char*> const& chrseq, std::vector<VcfSite> const& sites, bool headerHasConsBp, std::vector<LrSample> const& samples,
                                   Shard const& shard, LrMultiCallSet& out, MeiTemplates const* mei = nullptr, AnnoConfig const& annoCfg = AnnoConfig(),
-                                  MethylConfig const* methylCfg = nullptr, SvReadDump* dump = nullptr) {
+                                  MethylConfig const* methylCfg = nullptr, SvReadDump* dump = nullptr, StageClock* clock = nullptr) {
   out = LrMultiCallSet();
-  if (dump && shard.active()) return DGPU_ERR_ARG;
+  if (dump && (shard.active() || shard.byContig())) return DGPU_ERR_ARG;
   const bool ok = vcfParseSites(sites, headerHasConsBp, target_name, out.svs);
   for (auto const& sv : out.svs)
     if (sv.chr < 0 || sv.chr2 < 0) return DGPU_ERR_ARG;
   for (std::size_t i = 0; i < out.svs.size(); ++i)
     if (out.svs[i].id != (int32_t) i) return DGPU_ERR_ARG;   // the count vectors are indexed by id
-  const int rc = genotypeLrSitesSharded(ctx, c, target_len, target_name, chrseq, samples, shard, out, mei, annoCfg, methylCfg, false, dump);
+  if (clock) clock->lap("parse_sites");
+  const int rc = shard.byContig()
+                     ? genotypeLrSitesByContig(ctx, c, target_len, target_name, chrseq, samples, shard.contigShard(), out, mei, annoCfg, methylCfg, clock)
+                     : genotypeLrSitesSharded(ctx, c, target_len, target_name, chrseq, samples, shard, out, mei, annoCfg, methylCfg, false, dump);
   if (rc) return rc;
+  if (clock && !shard.byContig()) clock->lap("genotype");
   return ok ? DGPU_OK : DGPU_ERR_ARG;
 }
 

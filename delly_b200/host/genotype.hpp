@@ -309,6 +309,60 @@ inline int32_t _findSeqBp(LrRecord const& r, uint32_t pos) {
   return -1;
 }
 
+// The exchange of a contig-sharded genotypeLR: every rank sends, for the SVs with a breakpoint on its contigs, its decided qualities in job
+// order (REF / ALT, per haplotype, the phase set of its first phased ALT read), the read-depth (non-zero on the rank of sv.chr only) and its
+// methylation sums; the lists are concatenated in rank order, the sums added (finalizeMethylInfo sorts the CpG positions, so the sum of the
+// per-rank counts is exact).
+inline int mergeLrGenotypes(ContigShard const& cs, int localRc, std::vector<StructuralVariantRecord> const& svs, bool wantMethyl, std::vector<JunctionCount>& jctMap,
+                            std::vector<ReadCount>& covMap, std::vector<MethylAccum>& acc) {
+  ByteWriter w;
+  auto putQ = [&](std::vector<uint8_t> const& v) { w.bytes(v); };
+  for (uint32_t i = 0; i < svs.size(); ++i) {
+    if (!cs.owns(svs[i].chr) && !cs.owns(svs[i].chr2)) continue;
+    JunctionCount const& j = jctMap[i];
+    w.pod(i);
+    putQ(j.ref); putQ(j.alt); putQ(j.hp1ref); putQ(j.hp1alt); putQ(j.hp2ref); putQ(j.hp2alt); w.pod(j.ps);
+    w.pod(covMap[i].leftRC); w.pod(covMap[i].rc); w.pod(covMap[i].rightRC);
+    if (wantMethyl) {
+      MethylAccum const& a = acc[i];
+      for (int f = 0; f < 4; ++f) {
+        w.pod(a.altM[f]); w.pod(a.altT[f]); w.pod(a.refM[f]); w.pod(a.refT[f]);
+        w.pod<uint32_t>((uint32_t) a.cpg[f].size());
+        for (auto const& kv : a.cpg[f]) { w.pod(kv.first); w.pod(kv.second); }
+      }
+    }
+  }
+  std::vector<std::string> parts;
+  int rc = cs.exchange(localRc, w.buf, parts);
+  if (rc) return rc;
+  jctMap.assign(svs.size(), JunctionCount());
+  covMap.assign(svs.size(), ReadCount());
+  if (wantMethyl) acc.assign(svs.size(), MethylAccum());
+  auto add = [](std::vector<uint8_t>& to, std::vector<uint8_t> const& v) { to.insert(to.end(), v.begin(), v.end()); };
+  for (int r = 0; r < cs.nranks; ++r) {
+    ByteReader rd(parts[r].data(), parts[r].size());
+    while (rd.ok() && !rd.done()) {
+      const uint32_t i = rd.pod<uint32_t>();
+      if (!rd.ok() || i >= svs.size()) return DGPU_ERR_NCCL;
+      JunctionCount& j = jctMap[i];
+      add(j.ref, rd.bytes()); add(j.alt, rd.bytes()); add(j.hp1ref, rd.bytes()); add(j.hp1alt, rd.bytes()); add(j.hp2ref, rd.bytes()); add(j.hp2alt, rd.bytes());
+      const int32_t ps = rd.pod<int32_t>();
+      if (j.ps < 0) j.ps = ps;
+      covMap[i].leftRC += rd.pod<int32_t>(); covMap[i].rc += rd.pod<int32_t>(); covMap[i].rightRC += rd.pod<int32_t>();
+      if (wantMethyl) {
+        MethylAccum& a = acc[i];
+        for (int f = 0; f < 4; ++f) {
+          a.altM[f] += rd.pod<uint32_t>(); a.altT[f] += rd.pod<uint32_t>(); a.refM[f] += rd.pod<uint32_t>(); a.refT[f] += rd.pod<uint32_t>();
+          const uint32_t n = rd.pod<uint32_t>();
+          for (uint32_t k = 0; k < n && rd.ok(); ++k) { const int32_t pos = rd.pod<int32_t>(); a.cpg[f][pos] += rd.pod<uint32_t>(); }
+        }
+      }
+    }
+    if (!rd.ok()) return DGPU_ERR_NCCL;
+  }
+  return DGPU_OK;
+}
+
 // genotypeLR for ONE sample: records sorted like a coordinate-sorted BAM (by tid, then pos). The read scan, the
 // coverage track and the candidate selection run on the host exactly as the reference does; every
 // (read, SV, breakpoint) candidate contributes two global edit distances (REF window vs read window, ALT window vs read
@@ -319,15 +373,83 @@ inline int32_t _findSeqBp(LrRecord const& r, uint32_t pos) {
 // (reads seen for this SV, :233) because a read adds at most one quality after it has been counted; only the second
 // is evaluated here, which is what makes the candidates independent of the scores.
 // dump: receives the ALT-supporting (read, SV) groups in evaluation order (src/genotype.h:325-331)
+// cs != nullptr (contig sharding): recs holds this rank's contigs only. A read only ever counts toward the SVs with a breakpoint on its own
+// contig, so the per-SV cap needs a count from another rank only for an SV whose two breakpoints lie on two ranks' contigs (a translocation,
+// or a BND site): the rank of the lower contig first sends the number of reads it will count for it (no alignment is needed for that), the
+// rank of the higher contig starts its cap there. Every rank then realigns the reads of its contigs and sends, per SV, its decided qualities
+// in job order, the read-depth of the SVs whose first breakpoint is on its contigs, and its methylation sums; every rank merges them in rank
+// order (= contig order).
 inline int genotypeLRBatch(dgpu_ctx* ctx, Config const& c, std::vector<uint32_t> const& target_len, std::vector<std::string> const& target_name,
                            std::vector<const char*> const& chrseq, std::vector<StructuralVariantRecord>& svs, std::vector<LrRecord> const& recs,
                            std::vector<JunctionCount>& jctMap, std::vector<ReadCount>& covMap, MethylConfig const* methylCfg = nullptr,
-                           std::vector<MethylInfo>* methylMap = nullptr, std::vector<SvReadEvent>* dump = nullptr) {
+                           std::vector<MethylInfo>* methylMap = nullptr, std::vector<SvReadEvent>* dump = nullptr, ContigShard const* cs = nullptr) {
   jctMap.assign(svs.size(), JunctionCount());
   covMap.assign(svs.size(), ReadCount());
   const bool wantMethyl = (methylCfg != nullptr) && (methylMap != nullptr);
   if (wantMethyl) methylMap->assign(svs.size(), MethylInfo());
   if (svs.empty()) return DGPU_OK;
+  if (cs && dump) return DGPU_ERR_ARG;
+  auto bpMapOf = [&](int32_t refIndex, std::multimap<int32_t, int32_t>& bpMap) {
+    for (auto const& sv : svs) {
+      if (sv.chr == refIndex) bpMap.insert(std::make_pair(sv.svStart, sv.id));
+      if (sv.chr2 == refIndex) bpMap.insert(std::make_pair(sv.svEnd, sv.id));
+    }
+  };
+  // the SVs whose breakpoints a genotyping read spans (:189-222); false for a read that decides nothing
+  auto spanned = [&](LrRecord const& rec, std::multimap<int32_t, int32_t> const& bpMap, std::set<int32_t>& process, int32_t& rStart, int32_t& rEnd) {
+    if (rec.flag & (BAMF_QCFAIL | BAMF_DUP | BAMF_UNMAP | BAMF_SUPPLEMENTARY | BAMF_SECONDARY)) return false;
+    if (rec.mapq < c.minMapQual) return false;
+    if ((int32_t) rec.seq.size() < 2 * c.minimumFlankSize) return false;
+    rStart = _readStart(rec) + c.minimumFlankSize;
+    rEnd = _readEnd(rec);
+    if (rEnd > c.minimumFlankSize) {
+      rEnd -= c.minimumFlankSize;
+      if (rStart < rEnd) {
+        auto itB = bpMap.lower_bound(rStart);
+        auto itE = bpMap.upper_bound(rEnd);
+        for (; (itB != itE) && (itB != bpMap.end()); ++itB) process.insert(itB->second);
+      }
+    }
+    return true;
+  };
+  std::vector<uint32_t> readSV(svs.size(), 0);
+  int rc = DGPU_OK;
+  if (cs) {   // the counts of the SVs whose lower breakpoint contig is this rank's and whose other one a higher rank's
+    auto split = [&](StructuralVariantRecord const& sv) { return cs->owner(sv.chr) != cs->owner(sv.chr2); };
+    std::vector<uint32_t> lowerCount(svs.size(), 0);
+    std::size_t ri = 0;
+    for (int32_t refIndex = 0; refIndex < (int32_t) target_len.size(); ++refIndex) {
+      const std::size_t rlo = ri;
+      while (ri < recs.size() && recs[ri].tid == refIndex) ++ri;
+      if (rlo == ri || !cs->owns(refIndex)) continue;
+      std::multimap<int32_t, int32_t> bpMap;
+      for (auto const& sv : svs)
+        if (split(sv) && std::min(sv.chr, sv.chr2) == refIndex) {
+          if (sv.chr == refIndex) bpMap.insert(std::make_pair(sv.svStart, sv.id));
+          if (sv.chr2 == refIndex) bpMap.insert(std::make_pair(sv.svEnd, sv.id));
+        }
+      if (bpMap.empty()) continue;
+      for (std::size_t k = rlo; k < ri; ++k) {
+        std::set<int32_t> process;
+        int32_t rStart, rEnd;
+        if (!spanned(recs[k], bpMap, process, rStart, rEnd)) continue;
+        for (int32_t svid : process) if (lowerCount[svid] < c.maxGenoReadCount) ++lowerCount[svid];
+      }
+    }
+    ByteWriter w;
+    for (uint32_t i = 0; i < svs.size(); ++i) if (lowerCount[i]) { w.pod(i); w.pod(lowerCount[i]); }
+    std::vector<std::string> parts;
+    if ((rc = cs->exchange(DGPU_OK, w.buf, parts))) return rc;
+    for (int r = 0; r < cs->nranks; ++r) {
+      ByteReader rd(parts[r].data(), parts[r].size());
+      while (rd.ok() && !rd.done()) {
+        const uint32_t i = rd.pod<uint32_t>(), n = rd.pod<uint32_t>();
+        if (!rd.ok() || i >= svs.size()) return DGPU_ERR_NCCL;
+        if (cs->owns(std::max(svs[i].chr, svs[i].chr2))) readSV[i] = n;
+      }
+      if (!rd.ok()) return DGPU_ERR_NCCL;
+    }
+  }
   std::vector<std::vector<int32_t> > groupCands;  // the breakpoints of the SV each (read, SV) group spans (methylation windows)
   struct Cand { uint32_t rec, svid; uint32_t refSize, altSize; };
   std::vector<Cand> cands;                 // in the reference's evaluation order
@@ -335,21 +457,18 @@ inline int genotypeLRBatch(dgpu_ctx* ctx, Config const& c, std::vector<uint32_t>
   std::vector<std::pair<uint32_t, uint32_t> > groupKey;  // (record, svid) per group
   std::string arena;
   std::vector<uint32_t> qo, ql, to, tl;
-  std::vector<uint32_t> readSV(svs.size(), 0);
   std::size_t ri = 0;
   for (int32_t refIndex = 0; refIndex < (int32_t) target_len.size(); ++refIndex) {
     std::size_t rlo = ri;
     while (ri < recs.size() && recs[ri].tid == refIndex) ++ri;   // this contig's records (tid < 0 never matches)
     std::multimap<int32_t, int32_t> bpMap;
-    for (auto const& sv : svs) {
-      if (sv.chr == refIndex) bpMap.insert(std::make_pair(sv.svStart, sv.id));
-      if (sv.chr2 == refIndex) bpMap.insert(std::make_pair(sv.svEnd, sv.id));
-    }
+    bpMapOf(refIndex, bpMap);
     if (bpMap.empty()) continue;
     const char* seq = chrseq[refIndex];
-    for (auto& sv : svs)
+    for (auto& sv : svs)   // the alleles only slice the reference: every rank fills them for every SV
       if ((sv.chr == refIndex) && sv.alleles.empty())
         sv.alleles = _addAlleles(detail::upperSlice(seq, sv.svStart - 1, sv.svStart), target_name[sv.chr2], sv, sv.svt);
+    if (cs && !cs->owns(refIndex)) continue;
     const uint32_t tlen = target_len[refIndex];
     std::vector<uint16_t> covBases(tlen, 0);
     const uint32_t maxCoverage = 65535;
@@ -366,20 +485,10 @@ inline int genotypeLRBatch(dgpu_ctx* ctx, Config const& c, std::vector<uint32_t>
           } else if (cg.first == 2 || cg.first == 3) rp += cg.second;
         }
       }
-      if (rec.flag & (BAMF_QCFAIL | BAMF_DUP | BAMF_UNMAP | BAMF_SUPPLEMENTARY | BAMF_SECONDARY)) continue;
-      const int32_t lq = (int32_t) rec.seq.size();
-      if (lq < 2 * c.minimumFlankSize) continue;
       std::set<int32_t> process;
-      const int32_t rStart = _readStart(rec) + c.minimumFlankSize;
-      int32_t rEnd = _readEnd(rec);
-      if (rEnd > c.minimumFlankSize) {
-        rEnd -= c.minimumFlankSize;
-        if (rStart < rEnd) {
-          auto itB = bpMap.lower_bound(rStart);
-          auto itE = bpMap.upper_bound(rEnd);
-          for (; (itB != itE) && (itB != bpMap.end()); ++itB) process.insert(itB->second);
-        }
-      }
+      int32_t rStart, rEnd;
+      if (!spanned(rec, bpMap, process, rStart, rEnd)) continue;
+      const int32_t lq = (int32_t) rec.seq.size();
       for (int32_t svid : process) {
         if (readSV[svid] >= c.maxGenoReadCount) continue;
         ++readSV[svid];
@@ -436,14 +545,11 @@ inline int genotypeLRBatch(dgpu_ctx* ctx, Config const& c, std::vector<uint32_t>
       }
     }
   }
-  if (cands.empty()) {   // no read reached a decision
-    if (wantMethyl) for (std::size_t i = 0; i < svs.size(); ++i) finalizeMethylInfo(MethylAccum(), (*methylMap)[i], methylCfg->minCpgDepth);
-    return DGPU_OK;
-  }
   std::vector<int32_t> dist(qo.size());
-  int rc = dgpu_edit_distance(ctx, (const uint8_t*) arena.data(), arena.size(), qo.data(), ql.data(), to.data(), tl.data(), nullptr, DGPU_MODE_NW,
-                              qo.size(), dist.data(), nullptr);
-  if (rc) return rc;
+  if (!cands.empty())   // (no device call when no read reached a decision)
+    rc = dgpu_edit_distance(ctx, (const uint8_t*) arena.data(), arena.size(), qo.data(), ql.data(), to.data(), tl.data(), nullptr, DGPU_MODE_NW,
+                            qo.size(), dist.data(), nullptr);
+  if (rc && !cs) return rc;
   // fold the distances back per (read, SV) in evaluation order (:283-337)
   std::size_t ci = 0;
   std::vector<MethylAccum> methylAccum(wantMethyl ? svs.size() : 0);
@@ -451,7 +557,7 @@ inline int genotypeLRBatch(dgpu_ctx* ctx, Config const& c, std::vector<uint32_t>
   std::vector<int8_t> methCall;          // calls of the record methCallRec (built once per read, :309-313)
   int64_t methCallRec = -1;
   bool hasMethyl = false;
-  for (std::size_t g = 0; g < groupEnd.size(); ++g) {
+  for (std::size_t g = 0; g < groupEnd.size() && !rc; ++g) {
     int32_t refedsum = 0, altedsum = 0, nInform = 0;
     for (; ci < groupEnd[g]; ++ci) {
       const int32_t refScore = dist[2 * ci], altScore = dist[2 * ci + 1];
@@ -496,10 +602,11 @@ inline int genotypeLRBatch(dgpu_ctx* ctx, Config const& c, std::vector<uint32_t>
       if ((rec.hp > 0) && (rec.ps >= 0) && (jc.ps < 0)) jc.ps = rec.ps;
     }
   }
-  if (wantMethyl) {
-    if ((rc = flushInsertionJobs(ctx, *methylCfg, insQueue, methylAccum))) return rc;
+  if (wantMethyl && !rc) rc = flushInsertionJobs(ctx, *methylCfg, insQueue, methylAccum);
+  if (rc && !cs) return rc;
+  if (cs && (rc = mergeLrGenotypes(*cs, rc, svs, wantMethyl, jctMap, covMap, methylAccum))) return rc;
+  if (wantMethyl)
     for (std::size_t i = 0; i < svs.size(); ++i) finalizeMethylInfo(methylAccum[i], (*methylMap)[i], methylCfg->minCpgDepth);
-  }
   return DGPU_OK;
 }
 

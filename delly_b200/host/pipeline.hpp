@@ -150,13 +150,39 @@ inline int dellySrGenotypeMulti(dgpu_ctx* ctx, Config const& c, std::vector<Libr
 // ids[i] = read id of recs[i] (hash_lr in the reference). ctx != nullptr: pair scans on the device.
 inline int clusterSRReadsLR(dgpu_ctx* ctx, Config const& c, std::vector<uint32_t> const& target_len, std::vector<LrRecord> const& recs,
                             std::vector<std::size_t> const& ids, float indelExtension, std::vector<StructuralVariantRecord>& svc,
-                            std::vector<TPosReadSlices>& srStore) {
+                            std::vector<TPosReadSlices>& srStore, ContigShard const* cs = nullptr) {
   std::unordered_map<std::size_t, TJunctionVector> readBp;
-  for (std::size_t i = 0; i < recs.size(); ++i) {
-    LrRecord const& rec = recs[i];
-    if (rec.flag & (BAMF_QCFAIL | BAMF_DUP | BAMF_UNMAP)) continue;
-    if ((rec.mapq < c.minMapQual) || (rec.tid < 0)) continue;
-    cigarJunctionsLR(readBp, ids[i], rec.flag, rec.tid, rec.pos, rec.mapq, rec.cigar, c.minClip, c.minRefSep, indelExtension);
+  if (!cs) {
+    for (std::size_t i = 0; i < recs.size(); ++i) {
+      LrRecord const& rec = recs[i];
+      if (rec.flag & (BAMF_QCFAIL | BAMF_DUP | BAMF_UNMAP)) continue;
+      if ((rec.mapq < c.minMapQual) || (rec.tid < 0)) continue;
+      cigarJunctionsLR(readBp, ids[i], rec.flag, rec.tid, rec.pos, rec.mapq, rec.cigar, c.minClip, c.minRefSep, indelExtension);
+    }
+  } else {
+    // contig sharding: the records (this rank's contigs, in stream order) fill one insertion log per contig; the logs of every rank are
+    // gathered and replayed in contig order, which is the sequence of insertions of the walk over the whole stream. A read's supplementary
+    // alignments on other ranks' contigs join its junctions there.
+    std::vector<JunctionLog> logs(target_len.size());
+    for (std::size_t i = 0; i < recs.size(); ++i) {
+      LrRecord const& rec = recs[i];
+      if (rec.flag & (BAMF_QCFAIL | BAMF_DUP | BAMF_UNMAP)) continue;
+      if ((rec.mapq < c.minMapQual) || !cs->owns(rec.tid)) continue;
+      cigarJunctionsLR(logs[rec.tid], ids[i], rec.flag, rec.tid, rec.pos, rec.mapq, rec.cigar, c.minClip, c.minRefSep, indelExtension);
+    }
+    ByteWriter w;
+    for (std::size_t t = cs->lo(); t < cs->hi(); ++t) putJunctionLog(w, logs[t]);
+    std::vector<std::string> parts;
+    int rc = cs->exchange(DGPU_OK, w.buf, parts);
+    if (rc) return rc;
+    for (int r = 0; r < cs->nranks; ++r) {
+      if (r == cs->rank) continue;
+      ByteReader rd(parts[r].data(), parts[r].size());
+      for (std::size_t t = cs->bounds[r]; t < cs->bounds[r + 1]; ++t) getJunctionLog(rd, logs[t]);
+      if (!rd.ok() || !rd.done()) return DGPU_ERR_NCCL;
+    }
+    for (auto const& log : logs)
+      for (auto const& e : log.ev) readBp[e.first].push_back(e.second);
   }
   for (auto& kv : readBp) std::sort(kv.second.begin(), kv.second.end());
   TSvtSRBamRecord srBR(2 * DELLY_SVT_TRANS);
@@ -165,7 +191,14 @@ inline int clusterSRReadsLR(dgpu_ctx* ctx, Config const& c, std::vector<uint32_t
   for (uint32_t svt = 0; svt < srBR.size(); ++svt) {
     if (srBR[svt].empty()) continue;
     std::sort(srBR[svt].begin(), srBR[svt].end());
-    if (ctx) { int rc = clusterGpu(ctx, c, srBR[svt], svc, (int32_t) svt); if (rc) return rc; }
+    if (ctx) {
+      const int rc = clusterGpu(ctx, c, srBR[svt], svc, (int32_t) svt);
+      if (rc && cs) {   // a device failure of this rank alone: the next exchange of the other ranks (the assembly's) carries it to them
+        std::vector<std::string> parts;
+        cs->exchange(rc, std::string(), parts);
+      }
+      if (rc) return rc;
+    }
     else cluster(c, srBR[svt], svc, (int32_t) svt);
     for (SRBamRecord const& r : srBR[svt]) {
       if ((r.svid == -1) || (r.rstart == -1)) continue;
@@ -189,13 +222,13 @@ struct LrCallSet {
 // discovery half: the SV list, sorted and renumbered
 inline int discoverLrSVs(dgpu_ctx* ctx, Config const& c, float indelExtension, std::vector<uint32_t> const& target_len, std::vector<const char*> const& chrseq,
                          std::vector<LrRecord> const& recs, std::vector<std::size_t> const& ids, std::vector<StructuralVariantRecord>& svsOut,
-                         AssembleShard const* shard = nullptr) {
+                         AssembleShard const* shard = nullptr, ContigShard const* cs = nullptr) {
   struct { std::vector<StructuralVariantRecord> svs; } out;
   std::vector<StructuralVariantRecord> svc;
   std::vector<TPosReadSlices> srStore;
-  int rc = clusterSRReadsLR(ctx, c, target_len, recs, ids, indelExtension, svc, srStore);
+  int rc = clusterSRReadsLR(ctx, c, target_len, recs, ids, indelExtension, svc, srStore, cs);
   if (rc) return rc;
-  if ((rc = assembleLRBatch(ctx, c, target_len, chrseq, svc, srStore, recs, ids, shard))) return rc;
+  if ((rc = assembleLRBatch(ctx, c, target_len, chrseq, svc, srStore, recs, ids, shard, cs))) return rc;
   std::sort(svc.begin(), svc.end());
   std::map<int32_t, StructuralVariantRecord> lastSVperType;
   for (auto const& sv : svc) {

@@ -81,11 +81,6 @@ inline int scanSamplePEandSR(Config const& c, LibraryInfo& lib, std::vector<uint
     }
   int rc = DGPU_OK;
   if (cs && (rc = shareMateTables(*cs, DGPU_OK, matetraOf))) return rc;
-  struct JunctionLog {   // stands in for the per-read table inside cigarJunctions: records (read id, junction) in insertion order
-    std::vector<std::pair<std::size_t, Junction> > ev;
-    struct Slot { JunctionLog* log; std::size_t seed; void push_back(Junction const& j) { log->ev.emplace_back(seed, j); } };
-    Slot operator[](std::size_t seed) { return Slot{this, seed}; }
-  };
   struct ContigLog { JunctionLog junctions; std::vector<std::pair<int32_t, BamAlignRecord> > pairs; };
   std::vector<ContigLog> logs((std::size_t) nchr);
   parallelFor((std::size_t) nchr, [&](std::size_t refIndexU) {
@@ -131,11 +126,7 @@ inline int scanSamplePEandSR(Config const& c, LibraryInfo& lib, std::vector<uint
     ByteWriter w;
     for (std::size_t refIndex = cs->lo(); refIndex < cs->hi(); ++refIndex) {
       ContigLog const& log = logs[refIndex];
-      w.pod<uint64_t>((uint64_t) log.junctions.ev.size());
-      for (auto const& e : log.junctions.ev) {
-        Junction const& j = e.second;
-        w.pod<uint64_t>((uint64_t) e.first); w.pod<uint8_t>(j.forward); w.pod<uint8_t>(j.scleft); w.pod(j.refidx); w.pod(j.rstart); w.pod(j.refpos); w.pod(j.seqpos); w.pod(j.qual);
-      }
+      putJunctionLog(w, log.junctions);
       w.pod<uint64_t>((uint64_t) log.pairs.size());
       for (auto const& pr : log.pairs) { w.pod(pr.first); w.pod(pr.second); }
     }
@@ -146,14 +137,7 @@ inline int scanSamplePEandSR(Config const& c, LibraryInfo& lib, std::vector<uint
       ByteReader rd(parts[r].data(), parts[r].size());
       for (std::size_t refIndex = cs->bounds[r]; refIndex < cs->bounds[r + 1]; ++refIndex) {
         ContigLog& log = logs[refIndex];
-        const uint64_t nj = rd.pod<uint64_t>();
-        for (uint64_t k = 0; k < nj && rd.ok(); ++k) {
-          const std::size_t seed = (std::size_t) rd.pod<uint64_t>();
-          const bool fw = rd.pod<uint8_t>() != 0, cl = rd.pod<uint8_t>() != 0;
-          const int32_t refidx = rd.pod<int32_t>(), rstart = rd.pod<int32_t>(), refpos = rd.pod<int32_t>(), seqpos = rd.pod<int32_t>();
-          const uint16_t qual = rd.pod<uint16_t>();
-          log.junctions.ev.emplace_back(seed, Junction(fw, cl, refidx, rstart, refpos, seqpos, qual));
-        }
+        getJunctionLog(rd, log.junctions);
         const uint64_t np = rd.pod<uint64_t>();
         for (uint64_t k = 0; k < np && rd.ok(); ++k) { const int32_t svt = rd.pod<int32_t>(); log.pairs.emplace_back(svt, rd.pod<BamAlignRecord>()); }
       }

@@ -119,6 +119,11 @@ struct ContigShard {
   std::size_t lo() const { return bounds[rank]; }
   std::size_t hi() const { return bounds[rank + 1]; }
   bool owns(int32_t tid) const { return tid >= 0 && (std::size_t) tid >= lo() && (std::size_t) tid < hi(); }
+  // the rank whose range holds contig tid (the last rank of an empty range at tid never does)
+  int owner(int32_t tid) const {
+    for (int r = 0; r < nranks; ++r) if ((std::size_t) tid >= bounds[r] && (std::size_t) tid < bounds[r + 1]) return r;
+    return nranks;
+  }
   // One all-gather with a status word in front of every payload, so that a rank whose local work failed still takes part in the exchange
   // and every rank leaves it with the same error. parts[r] = rank r's payload without the status word.
   int exchange(int localRc, std::string const& payload, std::vector<std::string>& parts) const {
@@ -141,6 +146,32 @@ struct ContigShard {
     return DGPU_OK;
   }
 };
+
+// The per-read junction table of the scans (readBp, an unordered_map whose iteration order depends on the order of its insertions) as a log:
+// (read id, junction) in insertion order. A contig's log is built on its owner, and replaying the logs in contig order into one table repeats
+// the insertions of the sequential walk.
+struct JunctionLog {
+  std::vector<std::pair<std::size_t, Junction> > ev;
+  struct Slot { JunctionLog* log; std::size_t seed; void push_back(Junction const& j) { log->ev.emplace_back(seed, j); } };
+  Slot operator[](std::size_t seed) { return Slot{this, seed}; }
+};
+inline void putJunctionLog(ByteWriter& w, JunctionLog const& log) {
+  w.pod<uint64_t>((uint64_t) log.ev.size());
+  for (auto const& e : log.ev) {
+    Junction const& j = e.second;
+    w.pod<uint64_t>((uint64_t) e.first); w.pod<uint8_t>(j.forward); w.pod<uint8_t>(j.scleft); w.pod(j.refidx); w.pod(j.rstart); w.pod(j.refpos); w.pod(j.seqpos); w.pod(j.qual);
+  }
+}
+inline void getJunctionLog(ByteReader& rd, JunctionLog& log) {
+  const uint64_t nj = rd.pod<uint64_t>();
+  for (uint64_t k = 0; k < nj && rd.ok(); ++k) {
+    const std::size_t seed = (std::size_t) rd.pod<uint64_t>();
+    const bool fw = rd.pod<uint8_t>() != 0, cl = rd.pod<uint8_t>() != 0;
+    const int32_t refidx = rd.pod<int32_t>(), rstart = rd.pod<int32_t>(), refpos = rd.pod<int32_t>(), seqpos = rd.pod<int32_t>();
+    const uint16_t qual = rd.pod<uint16_t>();
+    log.ev.emplace_back(seed, Junction(fw, cl, refidx, rstart, refpos, seqpos, qual));
+  }
+}
 
 // The mate tables of inter-chromosomal pairs (scanPEandSR, annotateCoverage): the first observation of a pair (tid < mtid) is put, on the
 // contig of the read, into the table of the mate's contig, which is read when that contig is walked. `tables[mtid]` holds this rank's first
