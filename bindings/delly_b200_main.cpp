@@ -7,10 +7,15 @@
 // Parity: tests/test_bcf_parity.py compares the BCF written here byte for byte (uncompressed stream, ##fileDate aside) with the BCF the
 // reference's own drivers write (oracle/_ref/delly_ref = src/delly.h + src/tegua.h compiled verbatim against the same htslib).
 // No CPU fallback: without an sm_90 device dgpu_ctx_create fails and so does this program.
+#include <atomic>
+#include <chrono>
 #include <condition_variable>
+#include <cstdio>
 #include <cstdlib>
 #include <map>
+#include <memory>
 #include <mutex>
+#include <sstream>
 #include <cstring>
 #include <iostream>
 #include <string>
@@ -40,6 +45,7 @@ struct Options {
   std::string commFile, timingFile;  // --timing file: stage wall-clock times as one JSON object
   std::string shardBy = "svs";       // --shard-by svs|contig: what the ranks divide
   bool readShareOnly = false;        // --read-share-only: read this rank's share of the alignments, write --timing, stop (measuring a share alone)
+  std::vector<int> devices;          // --devices LIST: rank r runs on devices[r]; every rank is a thread of this process (no NCCL, no comm file)
   float indelExtension = 0.5f;
   MethylConfig methyl;
   AnnoConfig anno;
@@ -75,7 +81,33 @@ void usage(Options const& o) {
             << "  options follow `delly " << (o.lr ? "lr" : "sr") << "` (same letters and defaults), including -d <reads.gz> (gzipped list of the reads"
             << " that support each SV); extra: --device N, --io-threads N" << (o.lr ? ", --mei <templates.fa>" : "") << "\n"
             << "  several GPUs, one process each: --rank r --nranks N --comm-file <path> [--shard-by svs|contig] [--timing <file>]\n"
+            << "  several GPUs, one process: --devices LIST (e.g. 0-7 or 0,1,2,3; rank r runs on entry r, an index may repeat) [--shard-by svs|contig]\n"
+            << "    [--timing <file>]; not with --device, --rank, --nranks or --comm-file. The ranks split --io-threads and the host-stage threads"
+               " (DGPU_HOST_THREADS, default min(cores, 16)) evenly, at least one each; --shard-by svs reads the BAM once, with all --io-threads\n"
             << "  --read-share-only: read this rank's share (--shard-by contig), write --timing and stop: no device, no exchange\n";
+}
+
+// --devices LIST: comma-separated device indices and ranges a-b (a <= b); entry r is the device of rank r. At most 1024 ranks.
+bool parseDeviceList(std::string const& s, std::vector<int>& out) {
+  out.clear();
+  std::size_t b = 0;
+  auto number = [](std::string const& t, int& v) {
+    if (t.empty() || t.size() > 4 || t.find_first_not_of("0123456789") != std::string::npos) return false;
+    v = std::stoi(t);
+    return true;
+  };
+  while (b <= s.size()) {
+    std::size_t e = s.find(',', b);
+    if (e == std::string::npos) e = s.size();
+    const std::string t = s.substr(b, e - b);
+    const std::size_t dash = t.find('-');
+    int lo = 0, hi = 0;
+    if (dash == std::string::npos) { if (!number(t, lo)) return false; hi = lo; }
+    else if (!number(t.substr(0, dash), lo) || !number(t.substr(dash + 1), hi) || hi < lo) return false;
+    for (int d = lo; d <= hi; ++d) { if (out.size() >= 1024) return false; out.push_back(d); }
+    b = e + 1;
+  }
+  return !out.empty();
 }
 
 // `delly sr` (src/delly.h:207-246) and `delly lr` (src/tegua.h:215-275) share most letters; the long names are the reference's.
@@ -86,6 +118,9 @@ bool parse(int argc, char** argv, Options& o) {
   c.maxThreads = 4;
   o.methyl.methylProb = 128; o.methyl.methylWindow = 1000; o.methyl.minCpgDepth = 5;
   auto need = [&](int& i) -> const char* { if (i + 1 >= argc) { std::cerr << "missing value for " << argv[i] << std::endl; std::exit(2); } return argv[++i]; };
+  std::vector<std::string> processRank;   // the options of the one-process-per-GPU mode that were given (--devices excludes them)
+  bool hasDevices = false;
+  std::string deviceList;
   for (int i = 1; i < argc; ++i) {
     std::string a = argv[i];
     std::string v;
@@ -110,11 +145,12 @@ bool parse(int argc, char** argv, Options& o) {
     else if (is("-u", "--geno-qual")) c.minGenoQual = (uint16_t) std::stoi(val());
     else if (is("-d", "--dump")) o.dumpfile = val();
     else if (is("-w", "--cons-window")) c.minConsWindow = std::stoi(val());
-    else if (a == "--device") o.device = std::stoi(val());
+    else if (a == "--device") { o.device = std::stoi(val()); processRank.push_back(a); }
+    else if (a == "--devices") { deviceList = val(); hasDevices = true; }
     else if (a == "--io-threads") o.ioThreads = std::stoi(val());
-    else if (a == "--rank") o.rank = std::stoi(val());
-    else if (a == "--nranks") o.nranks = std::stoi(val());
-    else if (a == "--comm-file") o.commFile = val();
+    else if (a == "--rank") { o.rank = std::stoi(val()); processRank.push_back(a); }
+    else if (a == "--nranks") { o.nranks = std::stoi(val()); processRank.push_back(a); }
+    else if (a == "--comm-file") { o.commFile = val(); processRank.push_back(a); }
     else if (a == "--timing") o.timingFile = val();
     else if (a == "--shard-by") o.shardBy = val();
     else if (a == "--read-share-only") o.readShareOnly = true;
@@ -139,6 +175,24 @@ bool parse(int argc, char** argv, Options& o) {
     else if (o.lr && a == "--mei") o.meifile = val();
     else if (o.lr && is("-l", "--alt-align")) { std::cerr << "alternate alignments (-l) are outside the accelerated path (SURVEY section 2)" << std::endl; return false; }
     else { std::cerr << "unrecognised option '" << argv[i] << "'" << std::endl; return false; }
+  }
+  if (hasDevices) {
+    if (!processRank.empty()) {
+      std::cerr << "--devices cannot be combined with " << processRank[0] << ": --devices runs every rank in this process, --device / --rank / --nranks /"
+                   " --comm-file run one rank per process" << std::endl;
+      return false;
+    }
+    if (!parseDeviceList(deviceList, o.devices)) {
+      std::cerr << "--devices takes a comma-separated list of device indices and ranges a-b with a <= b (e.g. 0,1,2,3 or 0-7), not '" << deviceList << "'" << std::endl;
+      return false;
+    }
+    if (!o.dumpfile.empty() && o.devices.size() > 1) {
+      std::cerr << "the SV-read dump (-d) needs a single rank: over --devices with several entries every rank genotypes a part of the SV list, and the"
+                   " order of the dump lines depends on the whole list" << std::endl;
+      return false;
+    }
+    if (o.devices.size() == 1) { o.device = o.devices[0]; o.devices.clear(); }   // one rank: the single-process run on that device
+    else o.nranks = (int) o.devices.size();
   }
   if (o.shardBy != "svs" && o.shardBy != "contig") { std::cerr << "--shard-by takes svs or contig" << std::endl; return false; }
   if (o.readShareOnly && o.shardBy != "contig") { std::cerr << "--read-share-only measures a share of --shard-by contig" << std::endl; return false; }
@@ -180,11 +234,12 @@ std::string exeDir(const char* argv0) {
   return (k == std::string::npos) ? "." : p.substr(0, k);
 }
 
-// The device side of the process starts while the host reads its inputs: creating the CUDA context (and, with several ranks, the NCCL
+// The device side of a rank starts while the host reads its inputs: creating the CUDA context (and, with one process per rank, the NCCL
 // communicator plus one tiny warm-up exchange that sets up the NVLink connections) costs 0.5 - 2 s; a background thread pays it during the BAM scan.
+// With `ex` (--devices) the rank is a thread of a several-rank process and exchanges through it: no communicator.
 class DeviceSession {
  public:
-  DeviceSession(Options const& o) : o_(o) { th_ = std::thread([this] { start(); }); }
+  DeviceSession(Options const& o, SimExchange* ex = nullptr) : o_(o), ex_(ex) { th_ = std::thread([this] { start(); }); }
   ~DeviceSession() {
     if (th_.joinable()) th_.join();
     if (comm_) dgpu_comm_destroy(commCtx_, comm_);
@@ -197,7 +252,17 @@ class DeviceSession {
   dgpu_ctx* ctx() { return ctx_; }
   Shard shard() {
     Shard sh;
-    if (o_.nranks > 1) {
+    if (o_.nranks > 1 && ex_) {
+      sh.rank = o_.rank; sh.nranks = o_.nranks;
+      sh.gather = ex_->of(o_.rank);
+#ifdef DELLY_B200_FAIL_HOOK
+      // test builds only (tests/test_devices.py): DELLY_B200_FAIL_RANK=r makes rank r's first exchange fail on the host, so that the release
+      // of the other ranks can be checked without a device error
+      const char* failRank = getenv("DELLY_B200_FAIL_RANK");
+      if (failRank && std::atoi(failRank) == o_.rank)
+        sh.gather = [](std::string const&, std::vector<std::string>&) { std::cerr << "delly_b200: exchange failed (DELLY_B200_FAIL_RANK)" << std::endl; return (int) DGPU_ERR_NCCL; };
+#endif
+    } else if (o_.nranks > 1) {
       sh.rank = o_.rank; sh.nranks = o_.nranks;
       sh.gather = [this](std::string const& local, std::vector<std::string>& parts) -> int {
         if (!waitComm()) return DGPU_ERR_NCCL;
@@ -220,7 +285,8 @@ class DeviceSession {
   void start();
   void reach(int stage) { { std::lock_guard<std::mutex> g(m_); stage_ = stage; } cv_.notify_all(); }
   void waitFor(int stage) { std::unique_lock<std::mutex> g(m_); cv_.wait(g, [&] { return stage_ >= stage; }); }
-  Options const& o_;
+  const Options o_;   // a copy: the rank's options, whatever the caller does with its own afterwards
+  SimExchange* ex_;
   std::thread th_;
   std::mutex m_;
   std::condition_variable cv_;
@@ -338,7 +404,7 @@ void DeviceSession::start() {
   const int rc = dgpu_ctx_create(o_.device, &ctx_);
   if (rc != DGPU_OK) { std::cerr << "delly_b200: no usable sm_90 device (dgpu_ctx_create = " << rc << "); there is no CPU fallback on this path" << std::endl; ctx_ = nullptr; reach(2); return; }
   reach(1);
-  if (o_.nranks > 1) {
+  if (o_.nranks > 1 && !ex_) {
     std::vector<std::string> parts;
     if (dgpu_ctx_create(o_.device, &commCtx_) != DGPU_OK) { commCtx_ = nullptr; std::cerr << "delly_b200: cannot create the exchange context" << std::endl; }
     else if (!initComm(o_, commCtx_, &comm_)) { }
@@ -363,11 +429,112 @@ std::vector<std::size_t> contigCut(Options const& o, Inputs const& in) {
   return partitionContigs(w, o.nranks);
 }
 
-int runSr(Options& o, DeviceSession& dev) {
-  StageClock clock;
+// The record lists of an sr run, as the reference's iterators return them: the valid regions' (scan, clustering, assembly, library estimate,
+// src/shortpe.h:349, src/util.h:810) and, with an exclude file, the whole contigs' for the genotyping pass (src/coverage.h) — a second list.
+// names: the query names of the genotyped records (-d).
+struct SrReads {
+  std::vector<std::vector<SrRecord> > recs, recsWhole;
+  std::vector<std::vector<std::string> > names;
+};
+
+bool readSr(Options const& o, std::vector<io::AlignmentFile>& files, io::TRegionsGenome const& valid, io::TRegionsGenome const& whole, SrReads& r) {
+  const std::size_t F = files.size();
+  const bool dump = !o.dumpfile.empty();
+  r.recs.assign(F, std::vector<SrRecord>());
+  r.recsWhole.assign(o.hasExclude ? F : 0, std::vector<SrRecord>());
+  r.names.assign(dump ? F : 0, std::vector<std::string>());
+  for (std::size_t f = 0; f < F; ++f)
+    if (!files[f].readRegionsParallel(o.genome, valid, r.recs[f], io::toSrRecord, o.ioThreads, nullptr, nullptr, 0, (dump && !o.hasExclude) ? &r.names[f] : nullptr)) {
+      std::cerr << "cannot read " << o.files[f] << std::endl;
+      return false;
+    }
+  for (std::size_t f = 0; f < F && o.hasExclude; ++f)
+    if (!files[f].readRegionsParallel(o.genome, whole, r.recsWhole[f], io::toSrRecord, o.ioThreads, nullptr, nullptr, 0, dump ? &r.names[f] : nullptr)) {
+      std::cerr << "cannot read " << o.files[f] << std::endl;
+      return false;
+    }
+  return true;
+}
+
+// The long reads of an lr run with their read ids: the valid regions' and, with an exclude file, the whole contigs' (the genotyping pass).
+struct LrReads {
+  std::vector<std::vector<LrRecord> > recs, recsWhole;
+  std::vector<std::vector<std::size_t> > ids, idsWhole;
+  std::vector<std::vector<std::string> > names;
+};
+
+bool readLr(Options const& o, std::vector<io::AlignmentFile>& files, io::TRegionsGenome const& valid, io::TRegionsGenome const& whole, LrReads& r) {
+  const std::size_t F = files.size();
+  const bool dump = !o.dumpfile.empty();
+  r.recs.assign(F, std::vector<LrRecord>()); r.ids.assign(F, std::vector<std::size_t>());
+  r.recsWhole.assign(o.hasExclude ? F : 0, std::vector<LrRecord>()); r.idsWhole.assign(o.hasExclude ? F : 0, std::vector<std::size_t>());
+  r.names.assign(dump ? F : 0, std::vector<std::string>());
+  for (std::size_t f = 0; f < F; ++f)
+    if (!files[f].readRegionsParallel(o.genome, valid, r.recs[f], io::toLrRecord, o.ioThreads, &r.ids[f], io::hashLr, 0, (dump && !o.hasExclude) ? &r.names[f] : nullptr)) {
+      std::cerr << "cannot read " << o.files[f] << std::endl;
+      return false;
+    }
+  for (std::size_t f = 0; f < F && o.hasExclude; ++f)
+    if (!files[f].readRegionsParallel(o.genome, whole, r.recsWhole[f], io::toLrRecord, o.ioThreads, &r.idsWhole[f], io::hashLr, 0, dump ? &r.names[f] : nullptr)) {
+      std::cerr << "cannot read " << o.files[f] << std::endl;
+      return false;
+    }
+  return true;
+}
+
+// What the ranks of a --devices process share, read-only once they start: the inputs opened once (headers, region lists, the genome loaded
+// once) and, with --shard-by svs, where every rank needs every record, the record lists read once. clock: the stages the process ran for
+// all ranks before they started (every rank's --timing begins with them).
+struct SharedInputs {
   Inputs in;
-  if (!openInputs(o, in)) return 1;
-  clock.lap("open_inputs");
+  bool haveReads = false;
+  SrReads sr;
+  LrReads lr;
+  StageClock clock;
+  std::atomic<bool> outputOpened{false};   // rank 0 has created the BCF (removed again when another rank fails)
+};
+
+// The inputs of one rank: opened by the rank itself (one process per rank) or shared (--devices). A rank of a --devices process that reads
+// its own share (--shard-by contig) does so through its own file handles, beside the other ranks' reads.
+struct RankInputs {
+  Inputs own;
+  Inputs& in;
+  std::vector<io::AlignmentFile> ownFiles;
+  io::TRegionsGenome valid, whole;   // this rank's region lists (cut to its contigs by keepOwnContigs)
+  explicit RankInputs(SharedInputs* shared) : in(shared ? shared->in : own) {}
+  bool open(Options& o, SharedInputs* shared) {
+    if (!shared && !openInputs(o, own)) return false;
+    valid = in.validRegions; whole = in.wholeContigs;
+    return true;
+  }
+  std::vector<io::AlignmentFile>& files(Options const& o, SharedInputs* shared) {
+    if (!shared) return in.files;
+    if (ownFiles.empty()) {
+      ownFiles.resize(o.files.size());
+      for (std::size_t f = 0; f < o.files.size(); ++f) if (!ownFiles[f].open(o.files[f], o.genome, o.ioThreads)) { ownFiles.clear(); break; }
+    }
+    return ownFiles;
+  }
+};
+
+// this rank's contigs and records (--shard-by contig), one line on stderr
+void reportShare(Options const& o, Inputs const& in, std::vector<std::size_t> const& bounds, std::size_t n) {
+  const std::size_t lo = bounds[o.rank], hi = bounds[o.rank + 1];
+  std::ostringstream s;   // one write: the ranks of a --devices process report side by side
+  s << "rank " << o.rank << "/" << o.nranks << ": contigs ";
+  if (lo < hi) s << lo << "-" << hi - 1 << " (" << in.target_name[lo] << ".." << in.target_name[hi - 1] << ")";
+  else s << "none";
+  s << ", " << n << " records\n";
+  std::cerr << s.str() << std::flush;
+}
+
+int runSr(Options& o, DeviceSession& dev, SharedInputs* shared = nullptr) {
+  StageClock clock = shared ? shared->clock : StageClock();
+  clock.t0 = std::chrono::steady_clock::now();
+  RankInputs ri(shared);
+  if (!ri.open(o, shared)) return 1;
+  Inputs& in = ri.in;
+  if (!shared) clock.lap("open_inputs");
   Config& c = o.c;
   const std::size_t F = in.files.size();
   const bool byContig = o.shardBy == "contig";
@@ -378,7 +545,7 @@ int runSr(Options& o, DeviceSession& dev) {
   if (byContig) {   // this rank reads its own contigs only (the exclude flags above are the whole genome's)
     shard.contigBounds = contigCut(o, in);
     if (o.nranks == 1) shard.gather = [](std::string const& local, std::vector<std::string>& parts) { parts.assign(1, local); return (int) DGPU_OK; };
-    keepOwnContigs(shard.contigBounds, o.rank, in.validRegions, in.wholeContigs);
+    keepOwnContigs(shard.contigBounds, o.rank, ri.valid, ri.whole);
     GatherFn g = shard.gather;
     shard.gather = [g, &share, &clock](std::string const& local, std::vector<std::string>& parts) {
       share.sentAtLap[clock.ms.size()] += local.size();
@@ -386,48 +553,32 @@ int runSr(Options& o, DeviceSession& dev) {
     };
   }
   const bool dump = !o.dumpfile.empty();
-  std::vector<std::vector<std::string> > names(dump ? F : 0);   // query names of the genotyped records (-d)
-  // records of every file, as the reference's iterators return them
-  std::vector<std::vector<SrRecord> > recs(F);
-  std::vector<std::vector<SrRecord> const*> samples;
+  SrReads ownReads;
+  const bool readHere = !(shared && shared->haveReads);
+  if (readHere) {
+    std::vector<io::AlignmentFile>& files = ri.files(o, shared);
+    if (files.size() != F || !readSr(o, files, ri.valid, ri.whole, ownReads)) return 1;
+    clock.lap("read_bam");
+  }
+  SrReads const& rd = readHere ? ownReads : shared->sr;
+  std::vector<std::vector<SrRecord> const*> samples, genoSamples;
   for (std::size_t f = 0; f < F; ++f) {
-    if (!in.files[f].readRegionsParallel(o.genome, in.validRegions, recs[f], io::toSrRecord, o.ioThreads, nullptr, nullptr, 0, (dump && !o.hasExclude) ? &names[f] : nullptr)) {
-      std::cerr << "cannot read " << o.files[f] << std::endl;
-      return 1;
-    }
-    samples.push_back(&recs[f]);
+    samples.push_back(&rd.recs[f]);
+    if (o.hasExclude) genoSamples.push_back(&rd.recsWhole[f]);
   }
-  // exclude file: scan, clustering, assembly and the library estimate see the valid regions (src/shortpe.h:349, src/util.h:810), the genotyping pass
-  // the whole contigs (src/coverage.h) — a second record list
-  std::vector<std::vector<SrRecord> > recsWhole(o.hasExclude ? F : 0);
-  std::vector<std::vector<SrRecord> const*> genoSamples;
-  if (o.hasExclude) {
-    for (std::size_t f = 0; f < F; ++f) {
-      if (!in.files[f].readRegionsParallel(o.genome, in.wholeContigs, recsWhole[f], io::toSrRecord, o.ioThreads, nullptr, nullptr, 0, dump ? &names[f] : nullptr)) {
-        std::cerr << "cannot read " << o.files[f] << std::endl;
-        return 1;
-      }
-      genoSamples.push_back(&recsWhole[f]);
-    }
-  }
-  clock.lap("read_bam");
   if (byContig) {
-    const std::size_t lo = shard.contigBounds[o.rank], hi = shard.contigBounds[o.rank + 1];
     std::size_t n = 0;
-    for (std::size_t f = 0; f < F; ++f) n += recs[f].size() + (o.hasExclude ? recsWhole[f].size() : 0);
-    std::cerr << "rank " << o.rank << "/" << o.nranks << ": contigs ";
-    if (lo < hi) std::cerr << lo << "-" << hi - 1 << " (" << in.target_name[lo] << ".." << in.target_name[hi - 1] << ")";
-    else std::cerr << "none";
-    std::cerr << ", " << n << " records" << std::endl;
+    for (std::size_t f = 0; f < F; ++f) n += rd.recs[f].size() + (o.hasExclude ? rd.recsWhole[f].size() : 0);
+    reportShare(o, in, shard.contigBounds, n);
     share.records = n;
     if (o.readShareOnly) { writeTiming(o, clock, 0, &share); return 0; }
   }
   std::vector<LibraryInfo> libs(F);
   for (std::size_t f = 0; f < F; ++f) {
     if (byContig) {   // the first alignments in contig order may lie on other ranks' contigs: the screen continues rank after rank
-      const int lrc = getLibraryParamsSharded(c, in.target_len, recs[f], shard.contigShard(), libs[f]);
+      const int lrc = getLibraryParamsSharded(c, in.target_len, rd.recs[f], shard.contigShard(), libs[f]);
       if (lrc) { std::cerr << "delly_b200: the library exchange failed (" << lrc << ")" << std::endl; return 1; }
-    } else getLibraryParams(c, in.target_len, recs[f], libs[f]);
+    } else getLibraryParams(c, in.target_len, rd.recs[f], libs[f]);
     if (libs[f].rs == 0) { std::cerr << "Sample has not enough data to estimate library parameters! File: " << o.files[f] << std::endl; return 1; }
   }
   clock.lap("library");
@@ -451,7 +602,7 @@ int runSr(Options& o, DeviceSession& dev) {
   if (o.rank != 0) { writeTiming(o, clock, cs.svs.size(), byContig ? &share : nullptr); return 0; }   // every rank holds the complete call set; rank 0 writes it
   if (dump && !cs.svs.empty()) {   // the reference opens the dump in annotateCoverage, which an empty SV list skips (src/delly.h:176)
     std::vector<std::vector<SrRecord> const*> const& geno = o.hasExclude ? genoSamples : samples;
-    if (!writeDump(o.dumpfile, [&](auto put) { writeSrReadDump(put, reads, o.files, geno, names, in.target_name); })) return 1;
+    if (!writeDump(o.dumpfile, [&](auto put) { writeSrReadDump(put, reads, o.files, geno, rd.names, in.target_name); })) return 1;
     clock.lap("write_dump");
   }
   // src/delly.h:161-178: the count maps stay empty (and the header gets no sample column) when there is nothing to genotype
@@ -461,6 +612,7 @@ int runSr(Options& o, DeviceSession& dev) {
       VcfSample s; s.name = in.sampleName[f]; s.jctMap = &cs.sample[f].jctMap; s.rcMap = &cs.sample[f].rcMap; s.spanMap = &cs.sample[f].spanMap;
       vs.push_back(s);
     }
+  if (shared) shared->outputOpened = true;
   io::HtsVcfWriter w(o.outfile, in.target_name);
   if (!w.ok()) { std::cerr << "cannot open " << o.outfile << std::endl; return 1; }
   vcfRecordsTo(w, cs.svs, vs, in.target_name, in.target_len, o.genome, io::todayIso(), o.hasVcf, 0);
@@ -472,11 +624,13 @@ int runSr(Options& o, DeviceSession& dev) {
   return 0;
 }
 
-int runLr(Options& o, DeviceSession& dev, const char* argv0) {
-  StageClock clock;
-  Inputs in;
-  if (!openInputs(o, in)) return 1;
-  clock.lap("open_inputs");
+int runLr(Options& o, DeviceSession& dev, const char* argv0, SharedInputs* shared = nullptr) {
+  StageClock clock = shared ? shared->clock : StageClock();
+  clock.t0 = std::chrono::steady_clock::now();
+  RankInputs ri(shared);
+  if (!ri.open(o, shared)) return 1;
+  Inputs& in = ri.in;
+  if (!shared) clock.lap("open_inputs");
   Config& c = o.c;
   const std::size_t F = in.files.size();
   if (o.mode == "pb") o.indelExtension = 0.7f;
@@ -490,7 +644,7 @@ int runLr(Options& o, DeviceSession& dev, const char* argv0) {
   if (byContig) {   // this rank reads its own contigs only: its valid regions, and its whole contigs with -x
     shard.contigBounds = contigCut(o, in);
     if (o.nranks == 1) shard.gather = [](std::string const& local, std::vector<std::string>& parts) { parts.assign(1, local); return (int) DGPU_OK; };
-    keepOwnContigs(shard.contigBounds, o.rank, in.validRegions, in.wholeContigs);
+    keepOwnContigs(shard.contigBounds, o.rank, ri.valid, ri.whole);
     GatherFn g = shard.gather;
     shard.gather = [g, &share, &clock](std::string const& local, std::vector<std::string>& parts) {
       share.sentAtLap[clock.ms.size()] += local.size();
@@ -498,37 +652,23 @@ int runLr(Options& o, DeviceSession& dev, const char* argv0) {
     };
   }
   const bool dump = !o.dumpfile.empty();
-  std::vector<std::vector<std::string> > names(dump ? F : 0);   // query names of the genotyped records (-d)
-  std::vector<std::vector<LrRecord> > recs(F);
-  std::vector<std::vector<std::size_t> > ids(F);
-  std::vector<LrSample> samples;
-  for (std::size_t f = 0; f < F; ++f) {
-    if (!in.files[f].readRegionsParallel(o.genome, in.validRegions, recs[f], io::toLrRecord, o.ioThreads, &ids[f], io::hashLr, 0, (dump && !o.hasExclude) ? &names[f] : nullptr)) {
-      std::cerr << "cannot read " << o.files[f] << std::endl;
-      return 1;
-    }
-    samples.push_back(LrSample{&recs[f], &ids[f]});
+  LrReads ownReads;
+  const bool readHere = !(shared && shared->haveReads);
+  if (readHere) {
+    std::vector<io::AlignmentFile>& files = ri.files(o, shared);
+    if (files.size() != F || !readLr(o, files, ri.valid, ri.whole, ownReads)) return 1;
+    clock.lap("read_bam");
   }
-  std::vector<std::vector<LrRecord> > recsWhole(o.hasExclude ? F : 0);   // exclude file: the genotyping pass still reads whole contigs
-  std::vector<std::vector<std::size_t> > idsWhole(o.hasExclude ? F : 0);
-  std::vector<LrSample> genoSamples;
-  if (o.hasExclude)
-    for (std::size_t f = 0; f < F; ++f) {
-      if (!in.files[f].readRegionsParallel(o.genome, in.wholeContigs, recsWhole[f], io::toLrRecord, o.ioThreads, &idsWhole[f], io::hashLr, 0, dump ? &names[f] : nullptr)) {
-        std::cerr << "cannot read " << o.files[f] << std::endl;
-        return 1;
-      }
-      genoSamples.push_back(LrSample{&recsWhole[f], &idsWhole[f]});
-    }
-  clock.lap("read_bam");
+  LrReads const& rd = readHere ? ownReads : shared->lr;
+  std::vector<LrSample> samples, genoSamples;
+  for (std::size_t f = 0; f < F; ++f) {
+    samples.push_back(LrSample{&rd.recs[f], &rd.ids[f]});
+    if (o.hasExclude) genoSamples.push_back(LrSample{&rd.recsWhole[f], &rd.idsWhole[f]});
+  }
   if (byContig) {
-    const std::size_t lo = shard.contigBounds[o.rank], hi = shard.contigBounds[o.rank + 1];
     std::size_t n = 0;
-    for (std::size_t f = 0; f < F; ++f) n += recs[f].size() + (o.hasExclude ? recsWhole[f].size() : 0);
-    std::cerr << "rank " << o.rank << "/" << o.nranks << ": contigs ";
-    if (lo < hi) std::cerr << lo << "-" << hi - 1 << " (" << in.target_name[lo] << ".." << in.target_name[hi - 1] << ")";
-    else std::cerr << "none";
-    std::cerr << ", " << n << " records" << std::endl;
+    for (std::size_t f = 0; f < F; ++f) n += rd.recs[f].size() + (o.hasExclude ? rd.recsWhole[f].size() : 0);
+    reportShare(o, in, shard.contigBounds, n);
     share.records = n;
     if (o.readShareOnly) { writeTiming(o, clock, 0, &share); return 0; }
   }
@@ -554,7 +694,7 @@ int runLr(Options& o, DeviceSession& dev, const char* argv0) {
   if (dump && !cs.svs.empty()) {   // genotypeLR returns before it opens the dump when the SV list is empty (src/genotype.h:97, :127-133)
     std::vector<std::vector<LrRecord> const*> geno;
     for (LrSample const& s : (o.hasExclude ? genoSamples : samples)) geno.push_back(s.recs);
-    if (!writeDump(o.dumpfile, [&](auto put) { writeLrReadDump(put, reads, o.files, geno, names, in.target_name); })) return 1;
+    if (!writeDump(o.dumpfile, [&](auto put) { writeLrReadDump(put, reads, o.files, geno, rd.names, in.target_name); })) return 1;
     clock.lap("write_dump");
   }
   // long reads have no spanning pairs: empty lists per SV (src/tegua.h:173-190)
@@ -564,6 +704,7 @@ int runLr(Options& o, DeviceSession& dev, const char* argv0) {
     VcfSample s; s.name = in.sampleName[f]; s.jctMap = &cs.sample[f].jctMap; s.rcMap = &cs.sample[f].rcMap; s.spanMap = &noSpan; s.methylMap = &cs.sample[f].methyl;
     vs.push_back(s);
   }
+  if (shared) shared->outputOpened = true;
   io::HtsVcfWriter w(o.outfile, in.target_name);
   if (!w.ok()) { std::cerr << "cannot open " << o.outfile << std::endl; return 1; }
   vcfRecordsTo(w, cs.svs, vs, in.target_name, in.target_len, o.genome, io::todayIso(), o.hasVcf, o.methyl.minCpgDepth);
@@ -571,6 +712,46 @@ int runLr(Options& o, DeviceSession& dev, const char* argv0) {
   clock.lap("write_bcf");
   writeTiming(o, clock, cs.svs.size(), byContig ? &share : nullptr);
   return 0;
+}
+
+// --devices: every rank a host thread of this process, on its own device and context (sessions[r], started by main so that the contexts are
+// created while the inputs are read), exchanging through `ex`. The process opens the inputs once and, with --shard-by svs, reads the record
+// lists once; with --shard-by contig every rank reads its own contigs, all at the same time. The ranks split the IO and host-stage thread
+// budgets. The first rank to fail releases the others (ex.fail()); the process then reports that rank and leaves no BCF behind.
+int runDevices(Options& o, std::vector<std::unique_ptr<DeviceSession> >& sessions, SimExchange& ex, const char* argv0) {
+  const int N = (int) o.devices.size();
+  SharedInputs shared;
+  if (!openInputs(o, shared.in)) { ex.fail(); return 1; }
+  shared.clock.lap("open_inputs");
+  if (o.shardBy == "svs") {   // every rank needs every record: one read, with the whole IO budget
+    const bool ok = o.lr ? readLr(o, shared.in.files, shared.in.validRegions, shared.in.wholeContigs, shared.lr)
+                         : readSr(o, shared.in.files, shared.in.validRegions, shared.in.wholeContigs, shared.sr);
+    if (!ok) { ex.fail(); return 1; }
+    shared.haveReads = true;
+    shared.clock.lap("read_bam");
+  }
+  const unsigned hostShare = std::max(1u, processHostThreads() / (unsigned) N);
+  std::vector<int> rcs((std::size_t) N, 0);
+  std::atomic<int> firstFailed(-1);
+  std::vector<std::thread> th;
+  for (int r = 0; r < N; ++r)
+    th.emplace_back([&, r] {
+      rankHostThreads() = hostShare;
+      Options ro = o;
+      ro.rank = r; ro.device = o.devices[r]; ro.ioThreads = std::max(1, o.ioThreads / N);
+      rcs[r] = o.lr ? runLr(ro, *sessions[r], argv0, &shared) : runSr(ro, *sessions[r], &shared);
+      if (rcs[r]) {
+        int none = -1;
+        firstFailed.compare_exchange_strong(none, r);
+        ex.fail();
+      }
+    });
+  for (auto& t : th) t.join();
+  const int bad = firstFailed.load();
+  if (bad < 0) return 0;
+  std::cerr << "delly_b200: rank " << bad << " of " << N << " (device " << o.devices[bad] << ") failed; the other ranks were stopped" << std::endl;
+  if (shared.outputOpened && o.outfile != "-") { std::remove(o.outfile.c_str()); std::remove((o.outfile + ".csi").c_str()); }
+  return rcs[bad];
 }
 
 }  // namespace
@@ -587,9 +768,24 @@ int main(int argc, char** argv) {
   if (o.c.minCliqueSize < 2) o.c.minCliqueSize = 2;
   if (o.c.minMapQual > o.c.minTraQual) o.c.minTraQual = o.c.minMapQual;
   if (o.c.minGenoQual < 5 && !o.lr) o.c.minGenoQual = 5;   // src/delly.h:386
-  DeviceSession dev(o);
-  const int r = o.lr ? runLr(o, dev, argv[0]) : runSr(o, dev);
-  DeviceLimitLog const& lim = deviceLimitLog();
+  if (!o.devices.empty()) {   // before any input is read
+    const int ndev = dgpu_device_count();   // < 0: no CUDA driver here; creating the contexts reports that
+    for (int d : o.devices)
+      if (ndev >= 0 && d >= ndev) { std::cerr << "--devices: there is no device " << d << " (this process sees " << ndev << ")" << std::endl; return 1; }
+  }
+  std::unique_ptr<SimExchange> ex;
+  std::vector<std::unique_ptr<DeviceSession> > sessions;   // one per rank, creating its context from here on
+  if (o.devices.empty()) sessions.emplace_back(new DeviceSession(o));
+  else {
+    ex.reset(new SimExchange((int) o.devices.size()));
+    for (std::size_t k = 0; k < o.devices.size(); ++k) {
+      Options ro = o;
+      ro.rank = (int) k; ro.device = o.devices[k];
+      sessions.emplace_back(new DeviceSession(ro, ex.get()));
+    }
+  }
+  const int r = !o.devices.empty() ? runDevices(o, sessions, *ex, argv[0]) : o.lr ? runLr(o, *sessions[0], argv[0]) : runSr(o, *sessions[0]);
+  DeviceLimitLog const& lim = deviceLimitLog();   // the sum over the ranks of a --devices run
   if (lim.total())
     std::cerr << "Warning: " << lim.msaClusters.load() << " read cluster(s) (over " << DGPU_MSA_LARGE_MAXR << " reads, over 1023 alignment columns or a byte"
               << " outside ACGTN), " << lim.pathJobs.load() << " edit-path job(s) (an aligned target slice over " << DGPU_EP_MAX_SLICE

@@ -32,6 +32,7 @@ struct dgpu_ctx {
   uint32_t async_bound = 0;  // dgpu_set_async_bound: > 0 = the caller guarantees no sequence is longer; device-form calls then never synchronise
   bool no_band = false;      // development switch (DGPU_ED_NO_BAND): long NW jobs straight to the full-matrix kernel
   uint64_t unsupported = 0;  // jobs refused per item because they exceed a device limit (dgpu_unsupported_count)
+  std::vector<size_t> seg_room;  // seg_rows_exceed (edit_path.cu): the shared memory each seg_kernel class may opt in to, asked once per context
   // optional CUDA-event timing of the dominant kernels of the last batch call
   bool profiling = false;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
@@ -132,12 +133,14 @@ struct DgpuFork {
   }
 };
 
-// Lets `kernel` launch with `smem` bytes of dynamic shared memory (an opt-in above 48 KiB).
+// Lets `kernel` launch with `smem` bytes of dynamic shared memory (an opt-in above 48 KiB). The opt-in belongs to the kernel on its device,
+// not to a context: every host thread with a context on that device shares it. So it is only ever raised, under a lock (ctx.cu), and a thread
+// that needs less never lowers it under another thread's launch.
+int dgpu_smem_optin_raise(dgpu_ctx* ctx, const void* kernel, size_t smem, const char* name);
 template <typename K>
 int dgpu_smem_optin(dgpu_ctx* ctx, K* kernel, size_t smem, const char* name) {
   if (smem <= 48 * 1024) return DGPU_OK;
-  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
-  return e == cudaSuccess ? DGPU_OK : dgpu_set_cuda_error(ctx, e, name);
+  return dgpu_smem_optin_raise(ctx, (const void*) kernel, smem, name);
 }
 
 // The device side of one host-pointer call (a host form of the C ABI): the device and stream, the staged copies of the caller's arrays

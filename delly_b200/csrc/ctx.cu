@@ -4,6 +4,8 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <map>
+#include <mutex>
 
 int dgpu_set_cuda_error(dgpu_ctx* ctx, cudaError_t e, const char* what) {
   if (ctx) {
@@ -37,6 +39,18 @@ int dgpu_reserve(dgpu_ctx* ctx, int slot, size_t bytes, void** out) {
   return DGPU_OK;
 }
 
+int dgpu_smem_optin_raise(dgpu_ctx* ctx, const void* kernel, size_t smem, const char* name) {
+  static std::mutex mu;
+  static std::map<std::pair<const void*, int>, size_t> granted;   // (kernel, device) -> the opt-in set so far
+  std::lock_guard<std::mutex> g(mu);
+  size_t& have = granted[std::make_pair(kernel, ctx->device)];
+  if (smem <= have) return DGPU_OK;
+  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
+  if (e != cudaSuccess) return dgpu_set_cuda_error(ctx, e, name);
+  have = smem;
+  return DGPU_OK;
+}
+
 int dgpu_fork_init(dgpu_ctx* ctx) {
   while (ctx->fork_streams.size() < DGPU_FORK_STREAMS) {
     cudaStream_t s;
@@ -53,7 +67,13 @@ int dgpu_fork_init(dgpu_ctx* ctx) {
 
 extern "C" {
 
-int dgpu_version(void) { return 1004; }
+int dgpu_version(void) { return 1005; }
+
+int dgpu_device_count(void) {
+  int n = 0;
+  if (cudaGetDeviceCount(&n) != cudaSuccess) { cudaGetLastError(); return DGPU_ERR_NODEVICE; }
+  return n;
+}
 
 const char* dgpu_strerror(int code) {
   switch (code) {

@@ -481,8 +481,8 @@ inline int seg_band_class(uint32_t m, uint32_t pm, uint32_t pn, int32_t k) {
 // device's per-block maximum less the kernel's static shared memory, and the whole call would fail. Such half columns (Hirschberg over a
 // query of more than ~230 kb) run on seg_half_wide_kernel instead; every segment seg_kernel can launch still runs there.
 bool seg_rows_exceed(dgpu_ctx* ctx, uint32_t m, int cls, bool eq) {
-  static size_t room[SEG_NCLS][2] = {};   // [class][eq]: dynamic shared memory the class's seg_kernel may opt in to
-  size_t& r = room[cls][eq];
+  if (ctx->seg_room.empty()) ctx->seg_room.assign(SEG_NCLS * 2, 0);
+  size_t& r = ctx->seg_room[cls * 2 + eq];   // [class][eq]: dynamic shared memory the class's seg_kernel may opt in to
   if (!r) {
     int optin = 0;
     cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device);

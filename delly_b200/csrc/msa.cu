@@ -1083,7 +1083,7 @@ int dgpu_msa_ex_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
   A.work_stride = A.off_spans + al((size_t) MSA_N * 2 * MSA_MAXR * 2);
   const int per_sm = MSA_PER_SM;  // CTAs of four independent warps
   const size_t smem = sizeof(WarpSm) * MSA_WARPS;
-  if ((rc = dgpu_smem_optin(ctx, msa_kernel, smem, "cudaFuncSetAttribute(msa_kernel)"))) return rc;   // per device and cheap: set on every call
+  if ((rc = dgpu_smem_optin(ctx, msa_kernel, smem, "cudaFuncSetAttribute(msa_kernel)"))) return rc;   // per device: set on the first call
   size_t grid = std::min<size_t>((nclusters + MSA_WARPS - 1) / MSA_WARPS, (size_t) ctx->num_sms * per_sm);
   void* p;
   if ((rc = dgpu_reserve(ctx, SLOT_MSA_SEGJOBS, grid * MSA_WARPS * A.work_stride, &p))) return rc;

@@ -1,6 +1,7 @@
 // edlib_compat.hpp — implementation of include/dgpu_edlib.h: the edlib C API (src/edlib.h) as single-job calls into the
 // batched C ABI. See the header for the contract (per-thread context, no CPU fallback, first location only).
 #pragma once
+#include <atomic>
 #include <cstdlib>
 #include <cstring>
 #include <string>
@@ -14,8 +15,8 @@
 namespace dellyb200 {
 namespace detail {
 // Test seam: the context the compat layer uses instead of creating its own (set by the CPU stand-in build, whose device entry points
-// ignore it). Null = create one on first use.
-inline dgpu_ctx*& edlibCompatCtxOverride() { static dgpu_ctx* p = nullptr; return p; }
+// ignore it). Null = create one on first use. One per process, read by every thread that aligns through the compat layer: atomic.
+inline std::atomic<dgpu_ctx*>& edlibCompatCtxOverride() { static std::atomic<dgpu_ctx*> p{nullptr}; return p; }
 inline dgpu_ctx* edlibCompatCtx() {
   if (edlibCompatCtxOverride()) return edlibCompatCtxOverride();
   thread_local dgpu_ctx* ctx = nullptr;

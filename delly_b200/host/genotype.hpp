@@ -753,7 +753,7 @@ inline int annotateJunctionReadsWithProbes(dgpu_ctx* ctx, Config const& c, std::
     }
   };
   {
-    const unsigned hw = std::max(1u, std::min<unsigned>(std::thread::hardware_concurrency() ? std::thread::hardware_concurrency() : 1u, 16u));
+    const unsigned hw = hostThreads();
     std::atomic<int32_t> next(0);
     auto worker = [&]() { for (int32_t r = next++; r < nchr; r = next++) scanContig(r); };
     std::vector<std::thread> pool;

@@ -1,11 +1,14 @@
 // shard.hpp — cutting a batch of independent jobs into contiguous per-rank ranges (SURVEY §8e), shared by the sharded stage mirrors; the
-// wire format and the all-gather every exchange between ranks goes through; the contig partition of the contig-sharded `delly sr`.
+// wire format and the all-gather every exchange between ranks goes through, and its in-process form (SimExchange); the contig partition of
+// the contig-sharded `delly sr`.
 #pragma once
 #include <algorithm>
+#include <condition_variable>
 #include <cstdint>
 #include <cstring>
 #include <functional>
 #include <map>
+#include <mutex>
 #include <string>
 #include <tuple>
 #include <vector>
@@ -43,6 +46,30 @@ struct AssembleShard {
 
 // all-gatherv of one byte string per rank: parts[r] = rank r's payload, same on every rank. Returns DGPU_OK or an error code.
 typedef std::function<int(std::string const& local, std::vector<std::string>& parts)> GatherFn;
+
+// The all-gatherv between N ranks that are host threads of one process (`delly_b200 --devices`, the in-process test hooks): every rank
+// leaves its payload in its slot, the last one to arrive publishes all slots. fail() releases every rank waiting now or later with
+// DGPU_ERR_NCCL, so that one rank's error never leaves the others blocked in an exchange it will not join.
+struct SimExchange {
+  std::mutex mu; std::condition_variable cv;
+  std::vector<std::string> slots; int arrived = 0; long generation = 0; int n;
+  bool failed = false;
+  explicit SimExchange(int nranks) : slots(nranks), n(nranks) {}
+  int gather(int rank, std::string const& local, std::vector<std::string>& parts) {
+    std::unique_lock<std::mutex> lk(mu);
+    if (failed) return DGPU_ERR_NCCL;
+    const long gen = generation;
+    slots[rank] = local;
+    if (++arrived == n) { published = slots; arrived = 0; ++generation; cv.notify_all(); }
+    else cv.wait(lk, [&] { return generation != gen || failed; });
+    if (failed) return DGPU_ERR_NCCL;
+    parts = published;
+    return DGPU_OK;
+  }
+  void fail() { std::lock_guard<std::mutex> lk(mu); failed = true; cv.notify_all(); }
+  GatherFn of(int rank) { return [this, rank](std::string const& local, std::vector<std::string>& parts) { return gather(rank, local, parts); }; }
+  std::vector<std::string> published;
+};
 
 // ---- wire format (little endian, host order; all ranks are the same binary on the same box) ----------------------------------------
 class ByteWriter {

@@ -26,7 +26,9 @@ namespace dellyb200 {
 
 // Host-side loop over independent items (per-SV folding between device rounds): up to 16 threads (DGPU_HOST_THREADS overrides), the calling
 // thread included; fn(i) must only touch item i. The reference runs these loops serially per SV; the results do not depend on the order.
-inline unsigned hostThreads() {
+// The budget is the process's; a rank thread of a several-rank process (`delly_b200 --devices`) sets its share of it (rankHostThreads), so
+// that the ranks together run no more host threads than one rank alone.
+inline unsigned processHostThreads() {
   static const unsigned n = [] {
     const char* e = getenv("DGPU_HOST_THREADS");
     if (e && atoi(e) > 0) return (unsigned) atoi(e);
@@ -35,6 +37,8 @@ inline unsigned hostThreads() {
   }();
   return n;
 }
+inline unsigned& rankHostThreads() { thread_local unsigned n = 0; return n; }   // 0 = the whole process budget
+inline unsigned hostThreads() { return rankHostThreads() ? rankHostThreads() : processHostThreads(); }
 template <typename F>
 inline void parallelFor(std::size_t n, F&& fn, std::size_t minPerThread = 1) {
   const std::size_t nth = std::min<std::size_t>(hostThreads(), std::max<std::size_t>(1, n / std::max<std::size_t>(1, minPerThread)));
@@ -51,6 +55,7 @@ inline void parallelFor(std::size_t n, F&& fn, std::size_t minPerThread = 1) {
 // Items that exceeded a device limit (include/dgpu.h, "Device limits"). The reference has no such limits; an item beyond one is never
 // computed some other way and never aborts the run: it is treated as a FAILED alignment of that one SV / read (the reference's own
 // behaviour when an alignment fails: the SV stays imprecise or is dropped), counted here, and the binding reports the counts on stderr.
+// One log per process: the ranks of a several-rank process (`delly_b200 --devices`) all count into it, so it holds the sum over the ranks.
 struct DeviceLimitLog {
   std::atomic<uint64_t> msaClusters{0};   // dgpu_msa_ex status != 0: > DGPU_MSA_LARGE_MAXR reads, > 1023 alignment columns, a byte outside ACGTN
   std::atomic<uint64_t> pathJobs{0};      // dgpu_edit_path[_wide] status != 0: target slice beyond DGPU_EP_MAX_SLICE columns

@@ -64,6 +64,8 @@ const char* dgpu_last_error(dgpu_ctx* ctx);
 const char* dgpu_strerror(int code);
 /* ABI version (major*1000+minor). */
 int dgpu_version(void);
+/* Number of CUDA devices this process can see (any architecture), or DGPU_ERR_NODEVICE when the runtime cannot count them (no driver). */
+int dgpu_device_count(void);
 /* Number of kernel launches issued through this context so far (bench accounting). */
 uint64_t dgpu_launch_count(dgpu_ctx* ctx);
 /* jobs refused PER ITEM so far because they exceed a device limit (the call still succeeds; the item comes back flagged: ok = 0 / status != 0) */
