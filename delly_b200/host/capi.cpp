@@ -30,6 +30,231 @@
 
 using namespace dellyb200;
 
+// ---- the flat rows of the hooks below --------------------------------------------------------------------------------------------------
+
+// CIGAR of a record row: r[5] = first op in the packed array (BAM encoding: length << 4 | op), r[6] = number of ops
+static std::vector<std::pair<uint8_t, uint32_t> > row_cigar(const int32_t* r, const uint32_t* cigar) {
+  std::vector<std::pair<uint8_t, uint32_t> > cg;
+  for (int k = 0; k < r[6]; ++k) cg.push_back(std::make_pair((uint8_t) (cigar[r[5] + k] & 0xf), cigar[r[5] + k] >> 4));
+  return cg;
+}
+
+// Short-read row i (tid, pos, flag, mapq, length, cigar first, cigar count, read offset, mtid, mpos, isize, name id). cigar, reads, seeds and
+// name_hash may be NULL: the fields they fill keep their defaults.
+static SrRecord sr_record(const int32_t* r, const uint32_t* cigar, const char* reads, const uint64_t* seeds, const uint32_t* name_hash, std::size_t i) {
+  SrRecord rec;
+  rec.tid = r[0]; rec.pos = r[1]; rec.flag = (uint32_t) r[2]; rec.mapq = (uint8_t) r[3];
+  if (cigar) rec.cigar = row_cigar(r, cigar);
+  if (reads) rec.seq.assign(reads + r[7], (std::size_t) r[4]);
+  rec.lqseq = r[4]; rec.mtid = r[8]; rec.mpos = r[9]; rec.isize = r[10]; rec.name = (uint64_t) r[11];
+  if (seeds) rec.seed = (std::size_t) seeds[i];
+  if (name_hash) rec.nameHash32 = name_hash[i];
+  return rec;
+}
+
+// MM / ML tags of long-read rows (flags NULL = none): flags[i] bit 0 = MM, bit 1 = ML, each the arena slice [off[i], off[i + 1])
+struct LrTags { const uint8_t* flags; const char* mm; const uint32_t* mm_off; const uint8_t* ml; const uint32_t* ml_off; };
+
+// Long-read row i: [0..7] as sr_record; with hpps, [8] = HP tag (0 = none) and [9] = PS tag (-1 = none). reads may be NULL.
+static LrRecord lr_record(const int32_t* r, const uint32_t* cigar, const char* reads, bool hpps, LrTags const& tags, std::size_t i) {
+  LrRecord rec;
+  rec.tid = r[0]; rec.pos = r[1]; rec.flag = (uint32_t) r[2]; rec.mapq = (uint8_t) r[3];
+  rec.cigar = row_cigar(r, cigar);
+  if (reads) rec.seq.assign(reads + r[7], (std::size_t) r[4]);
+  if (hpps) { rec.hp = (uint8_t) (r[8] > 0 ? r[8] : 0); rec.ps = r[9]; }
+  if (tags.flags && (tags.flags[i] & 1)) { rec.hasMM = true; rec.mm.assign(tags.mm + tags.mm_off[i], tags.mm + tags.mm_off[i + 1]); }
+  if (tags.flags && (tags.flags[i] & 2)) { rec.hasML = true; rec.ml.assign(tags.ml + tags.ml_off[i], tags.ml + tags.ml_off[i + 1]); }
+  return rec;
+}
+
+// contigs "chr0", "chr1", ... as arena + offsets + lengths
+struct Genome {
+  std::vector<uint32_t> tl; std::vector<std::string> names; std::vector<const char*> chr;
+  Genome(const char* arena, const uint32_t* off, const uint32_t* len, int n) {
+    for (int k = 0; k < n; ++k) { tl.push_back(len[k]); names.push_back("chr" + std::to_string(k)); chr.push_back(arena + off[k]); }
+  }
+};
+
+// mobile-element templates: arena slices off[t - 1] .. off[t] are sequences 1..6, off[6] .. off[7] the polyA tail
+static void load_mei(MeiTemplates& mei, const char* arena, const uint32_t* off) {
+  for (int t = 1; t <= 6; ++t) mei.seq[t].assign(arena + off[t - 1], arena + off[t]);
+  mei.polyA.assign(arena + off[6], arena + off[7]);
+}
+
+// the 20-int SV row: chr, start, chr2, end, ciposlow/high, ciendlow/high, PE, SR, PE mapq, SR mapq, mapq, insLen, homLen, svt, precise,
+// consBp, id, srAlignQuality (float bits)
+static void put_sv(int32_t* o, StructuralVariantRecord const& v) {
+  o[0] = v.chr; o[1] = v.svStart; o[2] = v.chr2; o[3] = v.svEnd; o[4] = v.ciposlow; o[5] = v.ciposhigh; o[6] = v.ciendlow; o[7] = v.ciendhigh;
+  o[8] = v.peSupport; o[9] = v.srSupport; o[10] = v.peMapQuality; o[11] = v.srMapQuality; o[12] = v.mapq; o[13] = v.insLen; o[14] = v.homLen; o[15] = v.svt;
+  o[16] = v.precise ? 1 : 0; o[17] = v.consBp; o[18] = v.id;
+  memcpy(o + 19, &v.srAlignQuality, 4);
+}
+
+// the 14-int FORMAT row: gt0, gt1, gq, pl0..2, rcn, pass, [8] and [9] as the chain defines them (c89), junction REF / ALT reads, rc,
+// left + right rc; and the GL triple
+static void put_format(int32_t* q, float* gl, SampleFormat const& f, std::pair<int32_t, int32_t> c89, JunctionCount const& j, ReadCount const& rc) {
+  q[0] = f.gt[0]; q[1] = f.gt[1]; q[2] = f.gq; q[3] = f.pl[0]; q[4] = f.pl[1]; q[5] = f.pl[2]; q[6] = f.rcn; q[7] = f.pass ? 1 : 0;
+  q[8] = c89.first; q[9] = c89.second; q[10] = (int32_t) j.ref.size(); q[11] = (int32_t) j.alt.size(); q[12] = rc.rc; q[13] = rc.leftRC + rc.rightRC;
+  for (int k = 0; k < 3; ++k) gl[k] = f.gl[k];
+}
+
+// FORMAT [8], [9]: spanning REF / ALT pairs (sr); zeros (lr); ALT reads of haplotype 1 + 100 x those of haplotype 2 and the phase set (the
+// lr contig hooks)
+static std::pair<int32_t, int32_t> cols_spanning(SrSampleCounts const& s, int i) { return {(int32_t) s.spanMap[i].ref.size(), (int32_t) s.spanMap[i].alt.size()}; }
+static std::pair<int32_t, int32_t> cols_zero(LrSampleCounts const&, int) { return {0, 0}; }
+static std::pair<int32_t, int32_t> cols_haplotype(LrSampleCounts const& s, int i) {
+  JunctionCount const& j = s.jctMap[i];
+  return {(int32_t) j.hp1alt.size() + 100 * (int32_t) j.hp2alt.size(), j.ps};
+}
+
+// fixed-stride string slot i, cut at the stride; len[i] = the full length
+static void put_bytes(char* out, int stride, int32_t* len, std::size_t i, std::string const& s) {
+  len[i] = (int32_t) s.size();
+  memcpy(out + i * stride, s.data(), std::min<size_t>(s.size(), stride));
+}
+
+// the assembled SVs of dh_assemble_split_reads / dh_assemble_lr: 13-int rows (start, end, SR, mapq, SR mapq, insLen, homLen, consBp, precise,
+// ciposlow/high, ciendlow/high), srAlignQuality, consensus and alleles
+static void put_assembled(std::vector<StructuralVariantRecord> const& svs, int32_t* sv_out, float* srq, char* cons_out, int cons_stride, int32_t* cons_len,
+                          char* alleles_out, int alleles_stride, int32_t* alleles_len) {
+  for (std::size_t i = 0; i < svs.size(); ++i) {
+    StructuralVariantRecord const& sv = svs[i];
+    int32_t* o = sv_out + 13 * i;
+    o[0] = sv.svStart; o[1] = sv.svEnd; o[2] = sv.srSupport; o[3] = sv.mapq; o[4] = sv.srMapQuality; o[5] = sv.insLen; o[6] = sv.homLen; o[7] = sv.consBp;
+    o[8] = sv.precise ? 1 : 0; o[9] = sv.ciposlow; o[10] = sv.ciposhigh; o[11] = sv.ciendlow; o[12] = sv.ciendhigh;
+    srq[i] = sv.srAlignQuality;
+    put_bytes(cons_out, cons_stride, cons_len, i, sv.consensus);
+    put_bytes(alleles_out, alleles_stride, alleles_len, i, sv.alleles);
+  }
+}
+
+// one MethylInfo as 16 ints: alt, ref, mnc, mdp
+static void put_methyl(int32_t* m, MethylInfo const& mi) { memcpy(m, mi.alt, 16); memcpy(m + 4, mi.ref, 16); memcpy(m + 8, mi.mnc, 16); memcpy(m + 12, mi.mdp, 16); }
+
+// per-SV quality lists (T: JunctionCount / SpanningCount) as one arena: the REF lists of all SVs, then the ALT lists; ref_off / alt_off[nsv + 1].
+// Returns the arena size, or -1 when it exceeds cap.
+template <typename T>
+static int put_qual_lists(std::vector<T> const& v, int nsv, uint8_t* out, int cap, uint32_t* ref_off, uint32_t* alt_off) {
+  int pos = 0;
+  for (int pass = 0; pass < 2; ++pass) {
+    uint32_t* off = pass ? alt_off : ref_off;
+    for (int i = 0; i < nsv; ++i) {
+      off[i] = (uint32_t) pos;
+      std::vector<uint8_t> const& q = pass ? v[i].alt : v[i].ref;
+      if (pos + (int) q.size() > cap) return -1;
+      for (uint8_t x : q) out[pos++] = x;
+    }
+    off[nsv] = (uint32_t) pos;
+  }
+  return pos;
+}
+
+// Where a chain hook writes its n SVs: sv[cap][20]; per file, file-major with stride cap, fmt[nfile][cap][14] and gl[nfile][cap][3]; the
+// consensus cons[cap][cons_stride] + cons_len[cap] (cons may be NULL). The lr extras, each may be NULL: anno[cap][5], methyl[nfile][cap][16],
+// alleles[cap][alleles_stride] + alleles_len[cap]. A single-sample hook is nfile = 1.
+struct ChainOut {
+  int32_t* sv; int cap; int32_t* fmt; float* gl; char* cons; int cons_stride; int32_t* cons_len;
+  int nfile = 1;
+  int32_t* anno = nullptr; int32_t* methyl = nullptr; char* alleles = nullptr; int alleles_stride = 0; int32_t* alleles_len = nullptr;
+};
+
+// The SV rows, FORMAT rows + GLs of every file and consensus of a multi-sample call set; cols89(sample, i) gives FORMAT [8], [9].
+// Returns the number of SVs, or -1 (nothing written) when they exceed cap.
+template <typename TCallSet, typename TCols89>
+static int write_calls(TCallSet const& cs, ChainOut const& o, TCols89 cols89) {
+  const int n = (int) cs.svs.size();
+  if (n > o.cap) return -1;
+  for (int i = 0; i < n; ++i) {
+    put_sv(o.sv + 20 * i, cs.svs[i]);
+    for (std::size_t f = 0; f < cs.sample.size(); ++f) {
+      const std::size_t row = f * o.cap + i;
+      put_format(o.fmt + 14 * row, o.gl + 3 * row, cs.sample[f].format[i], cols89(cs.sample[f], i), cs.sample[f].jctMap[i], cs.sample[f].rcMap[i]);
+    }
+    if (o.cons) put_bytes(o.cons, o.cons_stride, o.cons_len, i, cs.svs[i].consensus);
+  }
+  return n;
+}
+
+// the lr extras the hook has: annotation (isRC, seqType, homLen, trPeriod, trCopies as float bits), the methylation of every file that has
+// one, the alleles
+static void write_lr_extras(LrMultiCallSet const& cs, ChainOut const& o) {
+  for (std::size_t i = 0; i < cs.svs.size(); ++i) {
+    StructuralVariantRecord const& v = cs.svs[i];
+    if (o.anno) {
+      int32_t* a = o.anno + 5 * i;
+      a[0] = v.anno.isRC ? 1 : 0; a[1] = v.anno.seqType; a[2] = v.anno.homLen; a[3] = v.anno.trPeriod; memcpy(a + 4, &v.anno.trCopies, 4);
+    }
+    if (o.methyl)
+      for (std::size_t f = 0; f < cs.sample.size(); ++f)
+        if (!cs.sample[f].methyl.empty()) put_methyl(o.methyl + 16 * (f * o.cap + i), cs.sample[f].methyl[v.id]);
+    if (o.alleles) put_bytes(o.alleles, o.alleles_stride, o.alleles_len, i, v.alleles);
+  }
+}
+
+// a single-sample call set as the one-file multi-sample set
+static SrMultiCallSet one_sample(SrCallSet& cs) {
+  SrMultiCallSet m; m.svs.swap(cs.svs); m.sample.resize(1);
+  m.sample[0].jctMap.swap(cs.jctMap); m.sample[0].spanMap.swap(cs.spanMap); m.sample[0].rcMap.swap(cs.rcMap); m.sample[0].format.swap(cs.format);
+  return m;
+}
+static LrMultiCallSet one_sample(LrCallSet& cs) {
+  LrMultiCallSet m; m.svs.swap(cs.svs); m.sample.resize(1);
+  m.sample[0].jctMap.swap(cs.jctMap); m.sample[0].rcMap.swap(cs.rcMap); m.sample[0].format.swap(cs.format); m.sample[0].methyl.swap(cs.methyl);
+  return m;
+}
+
+// ---- in-process ranks ------------------------------------------------------------------------------------------------------------------
+
+// N ranks as N host threads of one process, exchanging through a SimExchange: rank r runs run(r, gather, outs[r]) -> rc. The first rank to
+// fail releases the others. Returns the first negative rank code; -100 when a rank's code or output differs from rank 0's (same(a, b) =
+// equal); else rank 0's code, with its output moved to out0.
+template <typename TOut, typename TRun, typename TSame>
+static int run_ranks(int nranks, TRun run, TSame same, TOut& out0) {
+  SimExchange ex(nranks);
+  std::vector<TOut> outs((size_t) nranks);
+  std::vector<int> rcs((size_t) nranks, 0);
+  std::vector<std::thread> th;
+  for (int r = 0; r < nranks; ++r) th.emplace_back([&, r] { rcs[r] = run(r, ex.of(r), outs[r]); if (rcs[r] < 0) ex.fail(); });
+  for (auto& t : th) t.join();
+  for (int r = 0; r < nranks; ++r) if (rcs[r] < 0) return rcs[r];
+  for (int r = 1; r < nranks; ++r) if (rcs[r] != rcs[0] || !same(outs[r], outs[0])) return -100;
+  out0 = std::move(outs[0]);
+  return rcs[0];
+}
+
+// A rank's own zeroed copy of a chain hook's outputs, shaped by the hook's ChainOut (with every lr extra; copy_to copies those the hook
+// has); compared with GL bits
+struct ChainCopy {
+  std::vector<int32_t> sv, fmt, cl, anno, methyl, al; std::vector<float> gl; std::vector<char> cons, alleles;
+  ChainOut view(ChainOut const& like) {
+    const std::size_t C = (std::size_t) like.cap, F = (std::size_t) like.nfile;
+    sv.assign(C * 20, 0); fmt.assign(F * C * 14, 0); gl.assign(F * C * 3, 0.f); cons.assign(C * like.cons_stride, 0); cl.assign(C, 0);
+    anno.assign(C * 5, 0); methyl.assign(F * C * 16, 0); alleles.assign(C * std::max(like.alleles_stride, 1), 0); al.assign(C, 0);
+    return ChainOut{sv.data(), like.cap, fmt.data(), gl.data(), cons.data(), like.cons_stride, cl.data(), like.nfile, anno.data(), methyl.data(), alleles.data(),
+                    like.alleles_stride, al.data()};
+  }
+  bool operator==(ChainCopy const& o) const {
+    return sv == o.sv && fmt == o.fmt && cl == o.cl && cons == o.cons && anno == o.anno && methyl == o.methyl && alleles == o.alleles && al == o.al &&
+           gl.size() == o.gl.size() && !memcmp(gl.data(), o.gl.data(), gl.size() * 4);
+  }
+  void copy_to(ChainOut const& d) const {
+    memcpy(d.sv, sv.data(), sv.size() * 4); memcpy(d.fmt, fmt.data(), fmt.size() * 4); memcpy(d.gl, gl.data(), gl.size() * 4);
+    memcpy(d.cons, cons.data(), cons.size()); memcpy(d.cons_len, cl.data(), cl.size() * 4);
+    if (d.anno) memcpy(d.anno, anno.data(), anno.size() * 4);
+    if (d.methyl) memcpy(d.methyl, methyl.data(), methyl.size() * 4);
+    if (d.alleles) { memcpy(d.alleles, alleles.data(), (size_t) d.cap * d.alleles_stride); memcpy(d.alleles_len, al.data(), al.size() * 4); }
+  }
+};
+
+// run_ranks over a chain hook: run(r, gather, out) writes rank r's outputs to out; rank 0's reach dst
+template <typename TRun>
+static int run_chain_ranks(int nranks, ChainOut const& dst, TRun run) {
+  ChainCopy out;
+  const int n = run_ranks(nranks, [&](int r, GatherFn gather, ChainCopy& o) { return run(r, gather, o.view(dst)); }, std::equal_to<ChainCopy>(), out);
+  if (n >= 0) out.copy_to(dst);
+  return n;
+}
+
 extern "C" {
 
 // cluster(c, br, sv, svt) — layout as oracle/ref_wrap2.cpp::ref_cluster_sr
@@ -126,8 +351,7 @@ int dh_find_junctions(const int32_t* rec7, const uint64_t* seeds, int n, const u
     const uint32_t flag = (uint32_t) r[2];
     if (flag & (0x200 | 0x400 | 0x4)) continue;                 // BAM_FQCFAIL | BAM_FDUP | BAM_FUNMAP
     if ((r[3] < minMapQual) || (r[0] < 0)) continue;
-    std::vector<std::pair<uint8_t, uint32_t> > cg;
-    for (int k = 0; k < r[6]; ++k) cg.push_back(std::make_pair((uint8_t) (cigar[r[5] + k] & 0xf), cigar[r[5] + k] >> 4));
+    const std::vector<std::pair<uint8_t, uint32_t> > cg = row_cigar(r, cigar);
     if (lr) cigarJunctionsLR(readBp, (std::size_t) seeds[i], flag, r[0], r[1], (uint8_t) r[3], cg, (uint32_t) minClip, (uint32_t) minRefSep, indelExtension);
     else cigarJunctions(readBp, (std::size_t) seeds[i], flag, r[0], r[1], (uint8_t) r[3], cg, (uint32_t) minClip, (uint32_t) minRefSep);
   }
@@ -330,14 +554,8 @@ int dh_annotate_junction_reads(dgpu_ctx* ctx, const char* seq0, int len0, const 
   std::vector<uint32_t> tl = {(uint32_t) len0, (uint32_t) len1};
   std::vector<std::string> names = {"chrA", "chrB"};
   std::vector<const char*> chr = {seq0, seq1};
-  std::vector<SrRecord> recs(nrec);
-  for (int i = 0; i < nrec; ++i) {
-    const int32_t* r = rec10 + 12 * i;
-    recs[i].tid = r[0]; recs[i].pos = r[1]; recs[i].flag = (uint32_t) r[2]; recs[i].mapq = (uint8_t) r[3];
-    for (int k = 0; k < r[6]; ++k) recs[i].cigar.push_back(std::make_pair((uint8_t) (cigar[r[5] + k] & 0xf), cigar[r[5] + k] >> 4));
-    recs[i].seq.assign(reads + r[7], (std::size_t) r[4]);
-    recs[i].lqseq = r[4]; recs[i].mtid = r[8]; recs[i].mpos = r[9]; recs[i].isize = r[10]; recs[i].name = (uint64_t) r[11];
-  }
+  std::vector<SrRecord> recs;
+  for (int i = 0; i < nrec; ++i) recs.push_back(sr_record(rec10 + 12 * i, cigar, reads, nullptr, nullptr, i));
   std::vector<StructuralVariantRecord> svs(nsv);
   for (int i = 0; i < nsv; ++i) {
     const int32_t* s = sv9 + 9 * i;
@@ -348,18 +566,7 @@ int dh_annotate_junction_reads(dgpu_ctx* ctx, const char* seq0, int len0, const 
   std::vector<JunctionCount> countMap;
   int rc = annotateJunctionReadsBatch(ctx, c, tl, names, chr, svs, recs, countMap);
   if (rc) return rc - 2;
-  int pos = 0;
-  for (int pass = 0; pass < 2; ++pass) {
-    uint32_t* off = pass ? alt_off : ref_off;
-    for (int i = 0; i < nsv; ++i) {
-      off[i] = (uint32_t) pos;
-      std::vector<uint8_t> const& v = pass ? countMap[i].alt : countMap[i].ref;
-      if (pos + (int) v.size() > qual_cap) return -1;
-      for (uint8_t q : v) qual_out[pos++] = q;
-    }
-    off[nsv] = (uint32_t) pos;
-  }
-  return pos;
+  return put_qual_lists(countMap, nsv, qual_out, qual_cap, ref_off, alt_off);
 }
 
 // annotateSpanningAndDepth — the spanning-pair / read-depth outputs of oracle/ref_wrap3.cpp::ref_annotate_junction_reads (pure host).
@@ -369,13 +576,8 @@ int dh_annotate_spanning(int len0, int len1, const int32_t* rec12, int nrec, con
   Config c; c.indelsize = indelsize; c.minGenoQual = (uint16_t) minGenoQual;
   LibraryInfo lib; lib.median = lib4[0]; lib.minNormalISize = lib4[1]; lib.maxNormalISize = lib4[2]; lib.maxISizeCutoff = lib4[3];
   std::vector<uint32_t> tl = {(uint32_t) len0, (uint32_t) len1};
-  std::vector<SrRecord> recs(nrec);
-  for (int i = 0; i < nrec; ++i) {
-    const int32_t* r = rec12 + 12 * i;
-    recs[i].tid = r[0]; recs[i].pos = r[1]; recs[i].flag = (uint32_t) r[2]; recs[i].mapq = (uint8_t) r[3];
-    for (int k = 0; k < r[6]; ++k) recs[i].cigar.push_back(std::make_pair((uint8_t) (cigar[r[5] + k] & 0xf), cigar[r[5] + k] >> 4));
-    recs[i].lqseq = r[4]; recs[i].mtid = r[8]; recs[i].mpos = r[9]; recs[i].isize = r[10]; recs[i].name = (uint64_t) r[11];
-  }
+  std::vector<SrRecord> recs;
+  for (int i = 0; i < nrec; ++i) recs.push_back(sr_record(rec12 + 12 * i, cigar, nullptr, nullptr, nullptr, i));
   std::vector<StructuralVariantRecord> svs(nsv);
   std::vector<bool> svOnChr(2, false);
   for (int i = 0; i < nsv; ++i) {
@@ -386,17 +588,8 @@ int dh_annotate_spanning(int len0, int len1, const int32_t* rec12, int nrec, con
   }
   std::vector<ReadCount> cov; std::vector<SpanningCount> span;
   annotateSpanningAndDepth(c, lib, tl, svs, svOnChr, recs, cov, span);
-  int sp = 0;
-  for (int pass = 0; pass < 2; ++pass) {
-    uint32_t* off = pass ? salt_off : sref_off;
-    for (int i = 0; i < nsv; ++i) {
-      off[i] = (uint32_t) sp;
-      std::vector<uint8_t> const& v = pass ? span[i].alt : span[i].ref;
-      if (sp + (int) v.size() > span_cap) return -1;
-      for (uint8_t q : v) span_out[sp++] = q;
-    }
-    off[nsv] = (uint32_t) sp;
-  }
+  const int sp = put_qual_lists(span, nsv, span_out, span_cap, sref_off, salt_off);
+  if (sp < 0) return sp;
   for (int i = 0; i < nsv; ++i) { rc_out[3 * i] = cov[i].leftRC; rc_out[3 * i + 1] = cov[i].rc; rc_out[3 * i + 2] = cov[i].rightRC; }
   return sp;
 }
@@ -408,16 +601,9 @@ int dh_assemble_split_reads(dgpu_ctx* ctx, const char* contig_arena, const uint3
                             float* srq, char* cons_out, int cons_stride, int32_t* cons_len, char* alleles_out, int alleles_stride, int32_t* alleles_len) {
   Config c; c.maxReadPerSV = (uint32_t) maxReadPerSV; c.minMapQual = (uint16_t) minMapQual; c.minCliqueSize = (uint16_t) minCliqueSize;
   c.flankQuality = flankQuality; c.minimumFlankSize = minimumFlankSize; c.indelsize = indelsize; c.minConsWindow = minConsWindow;
-  std::vector<uint32_t> tl; std::vector<const char*> chr;
-  for (int k = 0; k < ncontig; ++k) { tl.push_back(contig_len[k]); chr.push_back(contig_arena + contig_off[k]); }
-  std::vector<SrRecord> recs(nrec);
-  for (int i = 0; i < nrec; ++i) {
-    const int32_t* r = rec12 + 12 * i;
-    recs[i].tid = r[0]; recs[i].pos = r[1]; recs[i].flag = (uint32_t) r[2]; recs[i].mapq = (uint8_t) r[3];
-    for (int k = 0; k < r[6]; ++k) recs[i].cigar.push_back(std::make_pair((uint8_t) (cigar[r[5] + k] & 0xf), cigar[r[5] + k] >> 4));
-    recs[i].seq.assign(reads + r[7], (std::size_t) r[4]);
-    recs[i].lqseq = r[4]; recs[i].mtid = r[8]; recs[i].mpos = r[9]; recs[i].isize = r[10]; recs[i].name = (uint64_t) r[11];
-  }
+  const Genome g(contig_arena, contig_off, contig_len, ncontig);
+  std::vector<SrRecord> recs;
+  for (int i = 0; i < nrec; ++i) recs.push_back(sr_record(rec12 + 12 * i, cigar, reads, nullptr, nullptr, i));
   std::vector<StructuralVariantRecord> svs(nsv);
   for (int i = 0; i < nsv; ++i) {
     const int32_t* s = sv7 + 7 * i;
@@ -429,19 +615,9 @@ int dh_assemble_split_reads(dgpu_ctx* ctx, const char* contig_arena, const uint3
     const int32_t* e = store5 + 5 * i;
     srStore[e[0]].insert(std::make_pair(std::make_pair(e[1], (std::size_t) e[2] * 2 + (e[3] ? 1 : 0)), e[4]));
   }
-  int rc = assembleSplitReadsBatch(ctx, c, tl, chr, srStore, svs, recs);
+  int rc = assembleSplitReadsBatch(ctx, c, g.tl, g.chr, srStore, svs, recs);
   if (rc) return rc;
-  for (int i = 0; i < nsv; ++i) {
-    StructuralVariantRecord const& sv = svs[i];
-    int32_t* o = sv_out + 13 * i;
-    o[0] = sv.svStart; o[1] = sv.svEnd; o[2] = sv.srSupport; o[3] = sv.mapq; o[4] = sv.srMapQuality; o[5] = sv.insLen; o[6] = sv.homLen; o[7] = sv.consBp;
-    o[8] = sv.precise ? 1 : 0; o[9] = sv.ciposlow; o[10] = sv.ciposhigh; o[11] = sv.ciendlow; o[12] = sv.ciendhigh;
-    srq[i] = sv.srAlignQuality;
-    cons_len[i] = (int32_t) sv.consensus.size();
-    memcpy(cons_out + (size_t) i * cons_stride, sv.consensus.data(), std::min<size_t>(sv.consensus.size(), cons_stride));
-    alleles_len[i] = (int32_t) sv.alleles.size();
-    memcpy(alleles_out + (size_t) i * alleles_stride, sv.alleles.data(), std::min<size_t>(sv.alleles.size(), alleles_stride));
-  }
+  put_assembled(svs, sv_out, srq, cons_out, cons_stride, cons_len, alleles_out, alleles_stride, alleles_len);
   return 0;
 }
 
@@ -455,14 +631,8 @@ int dh_scan_pe_sr(dgpu_ctx* ctx, const uint32_t* contig_len, int ncontig, const 
   c.maxReadSep = (uint32_t) maxReadSep; c.minCliqueSize = (uint16_t) minCliqueSize; c.graphPruning = (uint32_t) graphPruning; c.nchr = ncontig;
   LibraryInfo lib; lib.rs = lib5[0]; lib.median = lib5[1]; lib.mad = lib5[2]; lib.maxNormalISize = lib5[3]; lib.maxISizeCutoff = lib5[4];
   std::vector<uint32_t> tl(contig_len, contig_len + ncontig);
-  std::vector<SrRecord> recs(nrec);
-  for (int i = 0; i < nrec; ++i) {
-    const int32_t* r = rec12 + 12 * i;
-    recs[i].tid = r[0]; recs[i].pos = r[1]; recs[i].flag = (uint32_t) r[2]; recs[i].mapq = (uint8_t) r[3];
-    for (int k = 0; k < r[6]; ++k) recs[i].cigar.push_back(std::make_pair((uint8_t) (cigar[r[5] + k] & 0xf), cigar[r[5] + k] >> 4));
-    recs[i].lqseq = r[4]; recs[i].mtid = r[8]; recs[i].mpos = r[9]; recs[i].isize = r[10]; recs[i].name = (uint64_t) r[11];
-    recs[i].seed = (std::size_t) seeds[i]; recs[i].nameHash32 = name_hash[i];
-  }
+  std::vector<SrRecord> recs;
+  for (int i = 0; i < nrec; ++i) recs.push_back(sr_record(rec12 + 12 * i, cigar, nullptr, seeds, name_hash, i));
   std::vector<StructuralVariantRecord> svs, srSVs;
   std::vector<TPosReadSV> srStore;
   int rc = scanPEandSRBatch(ctx, c, lib, tl, recs, svs, srSVs, srStore);
@@ -513,7 +683,6 @@ int dh_merge_sort(const int32_t* pe20, int npe, const int32_t* sr20, int nsr, in
   return (int) pe.size();
 }
 
-// dellySrCall — layout as oracle/ref_wrap5.cpp::ref_delly_sr_call
 // `-t`: SV types of the following chain hooks (bit svt = wanted; 0 = all), as oracle/ref_wrap5.cpp::ref_set_svtset
 static uint32_t g_svtmask = 0;
 void dh_set_svtset(uint32_t mask) { g_svtmask = mask; }
@@ -554,144 +723,106 @@ int dh_vcf_parse(int ncontig, const int32_t* site22, int nsite, const char* strs
   for (int i = 0; i < n; ++i) {
     StructuralVariantRecord const& v = svs[i];
     int32_t* o = sv_out + 22 * i;
-    o[0] = v.chr; o[1] = v.svStart; o[2] = v.chr2; o[3] = v.svEnd; o[4] = v.ciposlow; o[5] = v.ciposhigh; o[6] = v.ciendlow; o[7] = v.ciendhigh;
-    o[8] = v.peSupport; o[9] = v.srSupport; o[10] = v.peMapQuality; o[11] = v.srMapQuality; o[12] = v.mapq; o[13] = v.insLen; o[14] = v.homLen; o[15] = v.svt;
-    o[16] = v.precise ? 1 : 0; o[17] = v.consBp; o[18] = v.id; memcpy(o + 19, &v.srAlignQuality, 4); o[20] = v.alleleid; o[21] = v.nallele;
-    alen[i] = (int32_t) v.alleles.size(); memcpy(alleles_out + (size_t) i * astride, v.alleles.data(), std::min<size_t>(v.alleles.size(), astride));
-    clen[i] = (int32_t) v.consensus.size(); memcpy(cons_out + (size_t) i * cstride, v.consensus.data(), std::min<size_t>(v.consensus.size(), cstride));
+    put_sv(o, v); o[20] = v.alleleid; o[21] = v.nallele;
+    put_bytes(alleles_out, astride, alen, i, v.alleles);
+    put_bytes(cons_out, cstride, clen, i, v.consensus);
   }
   return n;
 }
 
-static int delly_sr_hook(dgpu_ctx* ctx, const char* contig_arena, const uint32_t* contig_off, const uint32_t* contig_len, int ncontig, const int32_t* rec12,
-                     const uint64_t* seeds, const uint32_t* name_hash, int nrec, const uint32_t* cigar, const char* reads, const int32_t* lib6, int32_t* sv_out,
-                     int cap, int32_t* fmt_out, float* gl_out, char* cons_out, int cons_stride, int32_t* cons_len, const int32_t* site22, int nsite,
-                     const char* strs, const uint32_t* str_off) {
-  Config c;   // short-read defaults (src/delly.h:212-232)
-  c.nchr = ncontig; c.maxThreads = 1;
-  apply_svtset(c);
-  LibraryInfo lib; lib.rs = lib6[0]; lib.median = lib6[1]; lib.mad = lib6[2]; lib.minNormalISize = lib6[3]; lib.maxNormalISize = lib6[4]; lib.maxISizeCutoff = lib6[5];
-  std::vector<uint32_t> tl; std::vector<std::string> names; std::vector<const char*> chr;
-  for (int k = 0; k < ncontig; ++k) { tl.push_back(contig_len[k]); names.push_back("chr" + std::to_string(k)); chr.push_back(contig_arena + contig_off[k]); }
-  std::vector<SrRecord> recs(nrec);
-  for (int i = 0; i < nrec; ++i) {
-    const int32_t* r = rec12 + 12 * i;
-    recs[i].tid = r[0]; recs[i].pos = r[1]; recs[i].flag = (uint32_t) r[2]; recs[i].mapq = (uint8_t) r[3];
-    for (int k = 0; k < r[6]; ++k) recs[i].cigar.push_back(std::make_pair((uint8_t) (cigar[r[5] + k] & 0xf), cigar[r[5] + k] >> 4));
-    recs[i].seq.assign(reads + r[7], (std::size_t) r[4]);
-    recs[i].lqseq = r[4]; recs[i].mtid = r[8]; recs[i].mpos = r[9]; recs[i].isize = r[10]; recs[i].name = (uint64_t) r[11];
-    recs[i].seed = (std::size_t) seeds[i]; recs[i].nameHash32 = name_hash[i];
+// The inputs of an sr chain hook. Records grouped by file: file_off[nfile + 1] (a single-sample hook is nfile = 1, file_off = {0, nrec});
+// site22 (NULL = discovery): the sites of genotyping mode, rows as dh_vcf_parse. geno_* (may be NULL): a second record set, the whole
+// contigs, for the genotyping pass when an exclude set restricts the first to the valid regions; valid_intervals (may be NULL = no exclude
+// set): per contig, the number of valid regions the exclude set leaves.
+struct SrInput {
+  const char* contig_arena; const uint32_t* contig_off; const uint32_t* contig_len; int ncontig;
+  const int32_t* rec12; const uint64_t* seeds; const uint32_t* name_hash; const uint32_t* file_off; int nfile;
+  const uint32_t* cigar; const char* reads; const int32_t* lib6;
+  const int32_t* site22; int nsite; const char* strs; const uint32_t* str_off;
+  const int32_t* geno_rec12 = nullptr; const uint64_t* geno_seeds = nullptr; const uint32_t* geno_name_hash = nullptr; const uint32_t* geno_file_off = nullptr;
+  const int32_t* valid_intervals = nullptr;
+};
+
+// What the sr entry points take, built from an SrInput. own (NULL = every row): keep only the rows of contigs [own[0], own[1]);
+// held[ncontig] (may be NULL) counts the records kept, both sets.
+struct SrRun {
+  Config c; Genome g; std::vector<LibraryInfo> libs; std::vector<VcfSite> sites;
+  std::vector<std::vector<SrRecord> > recs, geno; std::vector<std::vector<SrRecord> const*> samples, genoSamples;
+  SrRun(SrRun const&) = delete;
+  SrRun(SrInput const& in, const std::size_t* own, int64_t* held) : g(in.contig_arena, in.contig_off, in.contig_len, in.ncontig) {
+    c.nchr = in.ncontig; c.maxThreads = 1;   // short-read defaults (src/delly.h:212-232)
+    apply_svtset(c);
+    if (in.valid_intervals) {   // the genome-wide region lists of the binding (dummy intervals: what matters is which lists are empty)
+      std::vector<std::vector<int> > valid((size_t) in.ncontig);
+      for (int t = 0; t < in.ncontig; ++t) valid[t].assign((size_t) in.valid_intervals[t], 0);
+      c.contigExcluded = excludedContigs(valid);
+    }
+    if (in.site22) sites = sites_from_rows(in.site22, in.nsite, in.strs, in.str_off);
+    auto read = [&](const int32_t* rec12, const uint64_t* seeds, const uint32_t* nh, uint32_t b, uint32_t e, std::vector<SrRecord>& out) {
+      for (uint32_t i = b; i < e; ++i) {
+        const int32_t* r = rec12 + 12 * (size_t) i;
+        if (own && (r[0] < 0 || (std::size_t) r[0] < own[0] || (std::size_t) r[0] >= own[1])) continue;
+        out.push_back(sr_record(r, in.cigar, in.reads, seeds, nh, i));
+        if (held) ++held[r[0]];
+      }
+    };
+    const std::size_t F = (std::size_t) in.nfile;
+    libs.resize(F); recs.resize(F); geno.resize(in.geno_rec12 ? F : 0);
+    for (std::size_t f = 0; f < F; ++f) {
+      const int32_t* l = in.lib6 + 6 * f;
+      libs[f].rs = l[0]; libs[f].median = l[1]; libs[f].mad = l[2]; libs[f].minNormalISize = l[3]; libs[f].maxNormalISize = l[4]; libs[f].maxISizeCutoff = l[5];
+      read(in.rec12, in.seeds, in.name_hash, in.file_off[f], in.file_off[f + 1], recs[f]);
+      samples.push_back(&recs[f]);
+      if (in.geno_rec12) {
+        read(in.geno_rec12, in.geno_seeds, in.geno_name_hash, in.geno_file_off[f], in.geno_file_off[f + 1], geno[f]);
+        genoSamples.push_back(&geno[f]);
+      }
+    }
   }
+};
+
+// dellySrCall / dellySrGenotype (site22 != NULL) — layout as oracle/ref_wrap5.cpp::ref_delly_sr_call; genotyping sites as dh_vcf_parse
+int dh_delly_sr_genotype(dgpu_ctx* ctx, const char* contig_arena, const uint32_t* contig_off, const uint32_t* contig_len, int ncontig, const int32_t* rec12,
+                         const uint64_t* seeds, const uint32_t* name_hash, int nrec, const uint32_t* cigar, const char* reads, const int32_t* lib6, int32_t* sv_out,
+                         int cap, int32_t* fmt_out, float* gl_out, char* cons_out, int cons_stride, int32_t* cons_len, const int32_t* site22, int nsite,
+                         const char* strs, const uint32_t* str_off) {
+  const uint32_t file_off[2] = {0, (uint32_t) nrec};
+  const SrInput in{contig_arena, contig_off, contig_len, ncontig, rec12, seeds, name_hash, file_off, 1, cigar, reads, lib6, site22, nsite, strs, str_off};
+  SrRun s(in, nullptr, nullptr);
   SrCallSet cs;
-  int rc = site22 ? dellySrGenotype(ctx, c, lib, tl, names, chr, sites_from_rows(site22, nsite, strs, str_off), true, recs, cs)
-                  : dellySrCall(ctx, c, lib, tl, names, chr, recs, cs);
+  int rc = site22 ? dellySrGenotype(ctx, s.c, s.libs[0], s.g.tl, s.g.names, s.g.chr, s.sites, true, s.recs[0], cs)
+                  : dellySrCall(ctx, s.c, s.libs[0], s.g.tl, s.g.names, s.g.chr, s.recs[0], cs);
   if (rc) return rc - 1;
-  const int n = (int) cs.svs.size();
-  if (n > cap) return -1;
-  for (int i = 0; i < n; ++i) {
-    StructuralVariantRecord const& v = cs.svs[i];
-    int32_t* o = sv_out + 20 * i;
-    o[0] = v.chr; o[1] = v.svStart; o[2] = v.chr2; o[3] = v.svEnd; o[4] = v.ciposlow; o[5] = v.ciposhigh; o[6] = v.ciendlow; o[7] = v.ciendhigh;
-    o[8] = v.peSupport; o[9] = v.srSupport; o[10] = v.peMapQuality; o[11] = v.srMapQuality; o[12] = v.mapq; o[13] = v.insLen; o[14] = v.homLen; o[15] = v.svt;
-    o[16] = v.precise ? 1 : 0; o[17] = v.consBp; o[18] = v.id; o[19] = 0;
-    memcpy(o + 19, &v.srAlignQuality, 4);
-    SampleFormat const& f = cs.format[i];
-    int32_t* q = fmt_out + 14 * i;
-    q[0] = f.gt[0]; q[1] = f.gt[1]; q[2] = f.gq; q[3] = f.pl[0]; q[4] = f.pl[1]; q[5] = f.pl[2]; q[6] = f.rcn; q[7] = f.pass ? 1 : 0;
-    q[8] = (int32_t) cs.spanMap[i].ref.size(); q[9] = (int32_t) cs.spanMap[i].alt.size(); q[10] = (int32_t) cs.jctMap[i].ref.size(); q[11] = (int32_t) cs.jctMap[i].alt.size();
-    q[12] = cs.rcMap[i].rc; q[13] = cs.rcMap[i].leftRC + cs.rcMap[i].rightRC;
-    for (int k = 0; k < 3; ++k) gl_out[3 * i + k] = f.gl[k];
-    cons_len[i] = (int32_t) v.consensus.size();
-    memcpy(cons_out + (size_t) i * cons_stride, v.consensus.data(), std::min<size_t>(v.consensus.size(), cons_stride));
-  }
-  return n;
+  return write_calls(one_sample(cs), ChainOut{sv_out, cap, fmt_out, gl_out, cons_out, cons_stride, cons_len}, cols_spanning);
 }
 
 int dh_delly_sr_call(dgpu_ctx* ctx, const char* contig_arena, const uint32_t* contig_off, const uint32_t* contig_len, int ncontig, const int32_t* rec12,
                      const uint64_t* seeds, const uint32_t* name_hash, int nrec, const uint32_t* cigar, const char* reads, const int32_t* lib6, int32_t* sv_out,
                      int cap, int32_t* fmt_out, float* gl_out, char* cons_out, int cons_stride, int32_t* cons_len) {
-  return delly_sr_hook(ctx, contig_arena, contig_off, contig_len, ncontig, rec12, seeds, name_hash, nrec, cigar, reads, lib6, sv_out, cap, fmt_out, gl_out, cons_out,
-                       cons_stride, cons_len, nullptr, 0, nullptr, nullptr);
+  return dh_delly_sr_genotype(ctx, contig_arena, contig_off, contig_len, ncontig, rec12, seeds, name_hash, nrec, cigar, reads, lib6, sv_out, cap, fmt_out, gl_out,
+                              cons_out, cons_stride, cons_len, nullptr, 0, nullptr, nullptr);
 }
 
-// several samples in one call set — layout as oracle/ref_wrap5.cpp::ref_delly_sr_call_multi (records grouped by file, fmt_out / gl_out file-major)
-static int delly_sr_multi_hook(dgpu_ctx* ctx, const char* contig_arena, const uint32_t* contig_off, const uint32_t* contig_len, int ncontig, const int32_t* rec12,
-                           const uint64_t* seeds, const uint32_t* name_hash, const uint32_t* file_off, int nfile, const uint32_t* cigar, const char* reads,
-                           const int32_t* lib6, int32_t* sv_out, int cap, int32_t* fmt_out, float* gl_out, char* cons_out, int cons_stride, int32_t* cons_len,
-                           const int32_t* site22, int nsite, const char* strs, const uint32_t* str_off) {
-  Config c;
-  c.nchr = ncontig; c.maxThreads = 1;
-  apply_svtset(c);
-  std::vector<uint32_t> tl; std::vector<std::string> names; std::vector<const char*> chr;
-  for (int k = 0; k < ncontig; ++k) { tl.push_back(contig_len[k]); names.push_back("chr" + std::to_string(k)); chr.push_back(contig_arena + contig_off[k]); }
-  std::vector<LibraryInfo> libs((size_t) nfile);
-  std::vector<std::vector<SrRecord> > recs((size_t) nfile);
-  std::vector<std::vector<SrRecord> const*> samples;
-  for (int f = 0; f < nfile; ++f) {
-    const int32_t* l = lib6 + 6 * f;
-    libs[f].rs = l[0]; libs[f].median = l[1]; libs[f].mad = l[2]; libs[f].minNormalISize = l[3]; libs[f].maxNormalISize = l[4]; libs[f].maxISizeCutoff = l[5];
-    for (uint32_t i = file_off[f]; i < file_off[f + 1]; ++i) {
-      const int32_t* r = rec12 + 12 * (size_t) i;
-      SrRecord rec;
-      rec.tid = r[0]; rec.pos = r[1]; rec.flag = (uint32_t) r[2]; rec.mapq = (uint8_t) r[3];
-      for (int k = 0; k < r[6]; ++k) rec.cigar.push_back(std::make_pair((uint8_t) (cigar[r[5] + k] & 0xf), cigar[r[5] + k] >> 4));
-      rec.seq.assign(reads + r[7], (std::size_t) r[4]);
-      rec.lqseq = r[4]; rec.mtid = r[8]; rec.mpos = r[9]; rec.isize = r[10]; rec.name = (uint64_t) r[11];
-      rec.seed = (std::size_t) seeds[i]; rec.nameHash32 = name_hash[i];
-      recs[f].push_back(rec);
-    }
-  }
-  for (int f = 0; f < nfile; ++f) samples.push_back(&recs[f]);
+// several samples in one call set — layout as oracle/ref_wrap5.cpp::ref_delly_sr_call_multi (records grouped by file, fmt_out / gl_out
+// file-major); site22 != NULL = genotyping mode
+int dh_delly_sr_genotype_multi(dgpu_ctx* ctx, const char* contig_arena, const uint32_t* contig_off, const uint32_t* contig_len, int ncontig, const int32_t* rec12,
+                               const uint64_t* seeds, const uint32_t* name_hash, const uint32_t* file_off, int nfile, const uint32_t* cigar, const char* reads,
+                               const int32_t* lib6, int32_t* sv_out, int cap, int32_t* fmt_out, float* gl_out, char* cons_out, int cons_stride, int32_t* cons_len,
+                               const int32_t* site22, int nsite, const char* strs, const uint32_t* str_off) {
+  const SrInput in{contig_arena, contig_off, contig_len, ncontig, rec12, seeds, name_hash, file_off, nfile, cigar, reads, lib6, site22, nsite, strs, str_off};
+  SrRun s(in, nullptr, nullptr);
   SrMultiCallSet cs;
-  int rc = site22 ? dellySrGenotypeMulti(ctx, c, libs, tl, names, chr, sites_from_rows(site22, nsite, strs, str_off), true, samples, cs)
-                  : dellySrCallMulti(ctx, c, libs, tl, names, chr, samples, cs);
+  int rc = site22 ? dellySrGenotypeMulti(ctx, s.c, s.libs, s.g.tl, s.g.names, s.g.chr, s.sites, true, s.samples, cs)
+                  : dellySrCallMulti(ctx, s.c, s.libs, s.g.tl, s.g.names, s.g.chr, s.samples, cs);
   if (rc) return rc - 1;
-  const int n = (int) cs.svs.size();
-  if (n > cap) return -1;
-  for (int i = 0; i < n; ++i) {
-    StructuralVariantRecord const& v = cs.svs[i];
-    int32_t* o = sv_out + 20 * i;
-    o[0] = v.chr; o[1] = v.svStart; o[2] = v.chr2; o[3] = v.svEnd; o[4] = v.ciposlow; o[5] = v.ciposhigh; o[6] = v.ciendlow; o[7] = v.ciendhigh;
-    o[8] = v.peSupport; o[9] = v.srSupport; o[10] = v.peMapQuality; o[11] = v.srMapQuality; o[12] = v.mapq; o[13] = v.insLen; o[14] = v.homLen; o[15] = v.svt;
-    o[16] = v.precise ? 1 : 0; o[17] = v.consBp; o[18] = v.id; o[19] = 0;
-    memcpy(o + 19, &v.srAlignQuality, 4);
-    for (int f = 0; f < nfile; ++f) {
-      SrSampleCounts const& sc = cs.sample[f];
-      SampleFormat const& fm = sc.format[i];
-      int32_t* q = fmt_out + 14 * ((size_t) f * cap + i);
-      q[0] = fm.gt[0]; q[1] = fm.gt[1]; q[2] = fm.gq; q[3] = fm.pl[0]; q[4] = fm.pl[1]; q[5] = fm.pl[2]; q[6] = fm.rcn; q[7] = fm.pass ? 1 : 0;
-      q[8] = (int32_t) sc.spanMap[i].ref.size(); q[9] = (int32_t) sc.spanMap[i].alt.size(); q[10] = (int32_t) sc.jctMap[i].ref.size(); q[11] = (int32_t) sc.jctMap[i].alt.size();
-      q[12] = sc.rcMap[i].rc; q[13] = sc.rcMap[i].leftRC + sc.rcMap[i].rightRC;
-      for (int k = 0; k < 3; ++k) gl_out[3 * ((size_t) f * cap + i) + k] = fm.gl[k];
-    }
-    cons_len[i] = (int32_t) v.consensus.size();
-    memcpy(cons_out + (size_t) i * cons_stride, v.consensus.data(), std::min<size_t>(v.consensus.size(), cons_stride));
-  }
-  return n;
+  return write_calls(cs, ChainOut{sv_out, cap, fmt_out, gl_out, cons_out, cons_stride, cons_len, nfile}, cols_spanning);
 }
 
 int dh_delly_sr_call_multi(dgpu_ctx* ctx, const char* contig_arena, const uint32_t* contig_off, const uint32_t* contig_len, int ncontig, const int32_t* rec12,
                            const uint64_t* seeds, const uint32_t* name_hash, const uint32_t* file_off, int nfile, const uint32_t* cigar, const char* reads,
                            const int32_t* lib6, int32_t* sv_out, int cap, int32_t* fmt_out, float* gl_out, char* cons_out, int cons_stride, int32_t* cons_len) {
-  return delly_sr_multi_hook(ctx, contig_arena, contig_off, contig_len, ncontig, rec12, seeds, name_hash, file_off, nfile, cigar, reads, lib6, sv_out, cap, fmt_out, gl_out,
-                             cons_out, cons_stride, cons_len, nullptr, 0, nullptr, nullptr);
-}
-// genotyping mode over several samples (site rows as dh_vcf_parse)
-int dh_delly_sr_genotype_multi(dgpu_ctx* ctx, const char* contig_arena, const uint32_t* contig_off, const uint32_t* contig_len, int ncontig, const int32_t* rec12,
-                               const uint64_t* seeds, const uint32_t* name_hash, const uint32_t* file_off, int nfile, const uint32_t* cigar, const char* reads,
-                               const int32_t* lib6, int32_t* sv_out, int cap, int32_t* fmt_out, float* gl_out, char* cons_out, int cons_stride, int32_t* cons_len,
-                               const int32_t* site22, int nsite, const char* strs, const uint32_t* str_off) {
-  return delly_sr_multi_hook(ctx, contig_arena, contig_off, contig_len, ncontig, rec12, seeds, name_hash, file_off, nfile, cigar, reads, lib6, sv_out, cap, fmt_out, gl_out,
-                             cons_out, cons_stride, cons_len, site22, nsite, strs, str_off);
-}
-
-// genotyping mode: the same outputs for a given site list (rows as dh_vcf_parse) instead of discovery
-int dh_delly_sr_genotype(dgpu_ctx* ctx, const char* contig_arena, const uint32_t* contig_off, const uint32_t* contig_len, int ncontig, const int32_t* rec12,
-                         const uint64_t* seeds, const uint32_t* name_hash, int nrec, const uint32_t* cigar, const char* reads, const int32_t* lib6, int32_t* sv_out,
-                         int cap, int32_t* fmt_out, float* gl_out, char* cons_out, int cons_stride, int32_t* cons_len, const int32_t* site22, int nsite,
-                         const char* strs, const uint32_t* str_off) {
-  return delly_sr_hook(ctx, contig_arena, contig_off, contig_len, ncontig, rec12, seeds, name_hash, nrec, cigar, reads, lib6, sv_out, cap, fmt_out, gl_out, cons_out,
-                       cons_stride, cons_len, site22, nsite, strs, str_off);
+  return dh_delly_sr_genotype_multi(ctx, contig_arena, contig_off, contig_len, ncontig, rec12, seeds, name_hash, file_off, nfile, cigar, reads, lib6, sv_out, cap,
+                                    fmt_out, gl_out, cons_out, cons_stride, cons_len, nullptr, 0, nullptr, nullptr);
 }
 
 // assembleLRBatch — layout as oracle/ref_wrap5.cpp::ref_assemble_lr (read id = name id here)
@@ -701,16 +832,12 @@ int dh_assemble_lr(dgpu_ctx* ctx, const char* contig_arena, const uint32_t* cont
                    int32_t* cons_len, char* alleles_out, int alleles_stride, int32_t* alleles_len) {
   Config c; c.maxReadPerSV = (uint32_t) maxReadPerSV; c.minCliqueSize = (uint16_t) minCliqueSize;
   c.flankQuality = flankQuality; c.minimumFlankSize = minimumFlankSize; c.indelsize = indelsize; c.minConsWindow = minConsWindow;
-  std::vector<uint32_t> tl; std::vector<const char*> chr;
-  for (int k = 0; k < ncontig; ++k) { tl.push_back(contig_len[k]); chr.push_back(contig_arena + contig_off[k]); }
-  std::vector<LrRecord> recs(nrec);
-  std::vector<std::size_t> ids(nrec);
+  const Genome g(contig_arena, contig_off, contig_len, ncontig);
+  std::vector<LrRecord> recs;
+  std::vector<std::size_t> ids;
   for (int i = 0; i < nrec; ++i) {
-    const int32_t* r = rec12 + 12 * i;
-    recs[i].tid = r[0]; recs[i].pos = r[1]; recs[i].flag = (uint32_t) r[2]; recs[i].mapq = (uint8_t) r[3];
-    for (int k = 0; k < r[6]; ++k) recs[i].cigar.push_back(std::make_pair((uint8_t) (cigar[r[5] + k] & 0xf), cigar[r[5] + k] >> 4));
-    recs[i].seq.assign(reads + r[7], (std::size_t) r[4]);
-    ids[i] = (std::size_t) r[11];
+    recs.push_back(lr_record(rec12 + 12 * i, cigar, reads, false, LrTags(), i));
+    ids.push_back((std::size_t) rec12[12 * i + 11]);
   }
   std::vector<StructuralVariantRecord> svs(nsv);
   for (int i = 0; i < nsv; ++i) {
@@ -724,213 +851,129 @@ int dh_assemble_lr(dgpu_ctx* ctx, const char* contig_arena, const uint32_t* cont
     const int32_t* e = store6 + 6 * i;
     srStore[e[0]][std::make_pair(e[1], (std::size_t) e[2])].push_back(SeqSlice(e[3], e[4], e[5], 60));
   }
-  int rc = assembleLRBatch(ctx, c, tl, chr, svs, srStore, recs, ids);
+  int rc = assembleLRBatch(ctx, c, g.tl, g.chr, svs, srStore, recs, ids);
   if (rc) return rc;
-  for (int i = 0; i < nsv; ++i) {
-    StructuralVariantRecord const& sv = svs[i];
-    int32_t* o = sv_out + 13 * i;
-    o[0] = sv.svStart; o[1] = sv.svEnd; o[2] = sv.srSupport; o[3] = sv.mapq; o[4] = sv.srMapQuality; o[5] = sv.insLen; o[6] = sv.homLen; o[7] = sv.consBp;
-    o[8] = sv.precise ? 1 : 0; o[9] = sv.ciposlow; o[10] = sv.ciposhigh; o[11] = sv.ciendlow; o[12] = sv.ciendhigh;
-    srq[i] = sv.srAlignQuality;
-    cons_len[i] = (int32_t) sv.consensus.size();
-    memcpy(cons_out + (size_t) i * cons_stride, sv.consensus.data(), std::min<size_t>(sv.consensus.size(), cons_stride));
-    alleles_len[i] = (int32_t) sv.alleles.size();
-    memcpy(alleles_out + (size_t) i * alleles_stride, sv.alleles.data(), std::min<size_t>(sv.alleles.size(), alleles_stride));
-  }
+  put_assembled(svs, sv_out, srq, cons_out, cons_stride, cons_len, alleles_out, alleles_stride, alleles_len);
   return 0;
 }
 
-// dellyLrCall — layout as oracle/ref_wrap5.cpp::ref_delly_lr_call; seeds = the read ids (hash_lr of the query names)
-// set (per thread) by the sharded test hook: the chain then runs as one rank of a sharded run
-static thread_local Shard const* g_lr_shard = nullptr;
+// The inputs of an lr chain hook: contigs, records, file_off and sites as SrInput (seeds NULL = read ids 0); cfg12 = minMapQual, minClip,
+// minRefSep, maxReadSep, minCliqueSize, graphPruning, maxReadPerSV, minimumFlankSize, indelsize, minConsWindow, maxGenoReadCount, genoCap.
+// tags.flags NULL = no MM / ML tags (and no methylation); tpl_arena NULL = no MEI templates (tpl_off[8] as load_mei); hpps: rows [8] / [9]
+// are the HP / PS tags; valid (may be NULL = no exclude set): 1 for the records inside the valid regions of an exclude set (discovery
+// sees those, genotyping all).
+struct LrInput {
+  const char* contig_arena; const uint32_t* contig_off; const uint32_t* contig_len; int ncontig;
+  const int32_t* rec12; const uint64_t* seeds; const uint32_t* file_off; int nfile;
+  const uint32_t* cigar; const char* reads; const int32_t* cfg12; float flankQuality, indelExtension;
+  const int32_t* site22; int nsite; const char* strs; const uint32_t* str_off;
+  LrTags tags = LrTags(); int methylWindow = 0, methylProb = 0, minCpgDepth = 0;
+  const char* tpl_arena = nullptr; const uint32_t* tpl_off = nullptr; float meiMinFrac = 0.f, trMinFrac = 0.f;
+  bool hpps = false; const uint8_t* valid = nullptr;
+};
 
-static int delly_lr_call_hook(dgpu_ctx* ctx, const char* contig_arena, const uint32_t* contig_off, const uint32_t* contig_len, int ncontig, const int32_t* rec12,
-                     const uint64_t* seeds, int nrec, const uint32_t* cigar, const char* reads, const int32_t* cfg12, float flankQuality, float indelExtension,
-                     int32_t* sv_out, int cap, int32_t* fmt_out, float* gl_out, char* cons_out, int cons_stride, int32_t* cons_len, const uint8_t* tagflags,
-                     const char* mm_arena, const uint32_t* mm_off, const uint8_t* ml_arena, const uint32_t* ml_off, int methylWindow, int methylProb,
-                     int minCpgDepth, const char* tpl_arena, const uint32_t* tpl_off, float meiMinFrac, float trMinFrac, int32_t* anno_out, int32_t* methyl_out,
-                     char* alleles_out, int alleles_stride, int32_t* alleles_len) {
-  Config c;
-  c.minMapQual = (uint16_t) cfg12[0]; c.minClip = (uint32_t) cfg12[1]; c.minRefSep = (uint32_t) cfg12[2]; c.maxReadSep = (uint32_t) cfg12[3];
-  c.minCliqueSize = (uint16_t) cfg12[4]; c.graphPruning = (uint32_t) cfg12[5]; c.maxReadPerSV = (uint32_t) cfg12[6]; c.minimumFlankSize = cfg12[7];
-  c.indelsize = cfg12[8]; c.minConsWindow = cfg12[9]; c.maxGenoReadCount = (uint32_t) cfg12[10]; c.genoCap = cfg12[11];
-  c.flankQuality = flankQuality; c.nchr = ncontig;
-  apply_svtset(c);
-  std::vector<uint32_t> tl; std::vector<std::string> names; std::vector<const char*> chr;
-  for (int k = 0; k < ncontig; ++k) { tl.push_back(contig_len[k]); names.push_back("chr" + std::to_string(k)); chr.push_back(contig_arena + contig_off[k]); }
-  std::vector<LrRecord> recs(nrec);
-  std::vector<std::size_t> ids(nrec);
-  for (int i = 0; i < nrec; ++i) {
-    const int32_t* r = rec12 + 12 * i;
-    recs[i].tid = r[0]; recs[i].pos = r[1]; recs[i].flag = (uint32_t) r[2]; recs[i].mapq = (uint8_t) r[3];
-    for (int k = 0; k < r[6]; ++k) recs[i].cigar.push_back(std::make_pair((uint8_t) (cigar[r[5] + k] & 0xf), cigar[r[5] + k] >> 4));
-    recs[i].seq.assign(reads + r[7], (std::size_t) r[4]);
-    ids[i] = (std::size_t) seeds[i];
-    if (tagflags && (tagflags[i] & 1)) { recs[i].hasMM = true; recs[i].mm.assign(mm_arena + mm_off[i], mm_arena + mm_off[i + 1]); }
-    if (tagflags && (tagflags[i] & 2)) { recs[i].hasML = true; recs[i].ml.assign(ml_arena + ml_off[i], ml_arena + ml_off[i + 1]); }
+// What the lr entry points take, built from an LrInput; own and held as for SrRun (held counts a record of both lists twice)
+struct LrRun {
+  Config c; Genome g; std::vector<VcfSite> sites;
+  MeiTemplates mei; AnnoConfig acfg; MethylConfig mcfg;
+  MeiTemplates const* meiP; MethylConfig const* mcfgP;   // NULL without templates / tags
+  std::vector<std::vector<LrRecord> > recs, whole; std::vector<std::vector<std::size_t> > ids, wholeIds; std::vector<LrSample> samples, genoSamples;
+  LrRun(LrRun const&) = delete;
+  LrRun(LrInput const& in, const std::size_t* own, int64_t* held) : g(in.contig_arena, in.contig_off, in.contig_len, in.ncontig) {
+    const int32_t* k = in.cfg12;
+    c.minMapQual = (uint16_t) k[0]; c.minClip = (uint32_t) k[1]; c.minRefSep = (uint32_t) k[2]; c.maxReadSep = (uint32_t) k[3];
+    c.minCliqueSize = (uint16_t) k[4]; c.graphPruning = (uint32_t) k[5]; c.maxReadPerSV = (uint32_t) k[6]; c.minimumFlankSize = k[7];
+    c.indelsize = k[8]; c.minConsWindow = k[9]; c.maxGenoReadCount = (uint32_t) k[10]; c.genoCap = k[11];
+    c.flankQuality = in.flankQuality; c.nchr = in.ncontig;
+    apply_svtset(c);
+    if (in.site22) sites = sites_from_rows(in.site22, in.nsite, in.strs, in.str_off);
+    if (in.tpl_arena) load_mei(mei, in.tpl_arena, in.tpl_off);
+    acfg.meiMinFrac = in.meiMinFrac; acfg.trMinFrac = in.trMinFrac;
+    mcfg.methylWindow = in.methylWindow; mcfg.methylProb = (uint16_t) in.methylProb; mcfg.minCpgDepth = (uint32_t) in.minCpgDepth;
+    meiP = in.tpl_arena ? &mei : nullptr;
+    mcfgP = in.tags.flags ? &mcfg : nullptr;
+    const std::size_t F = (std::size_t) in.nfile;
+    recs.resize(F); ids.resize(F); whole.resize(in.valid ? F : 0); wholeIds.resize(in.valid ? F : 0);
+    for (std::size_t f = 0; f < F; ++f) {
+      for (uint32_t i = in.file_off[f]; i < in.file_off[f + 1]; ++i) {
+        const int32_t* r = in.rec12 + 12 * (size_t) i;
+        if (own && (r[0] < 0 || (std::size_t) r[0] < own[0] || (std::size_t) r[0] >= own[1])) continue;
+        const LrRecord rec = lr_record(r, in.cigar, in.reads, in.hpps, in.tags, i);
+        const std::size_t id = in.seeds ? (std::size_t) in.seeds[i] : 0;
+        if (!in.valid || in.valid[i]) { recs[f].push_back(rec); ids[f].push_back(id); if (held) ++held[r[0]]; }
+        if (in.valid) { whole[f].push_back(rec); wholeIds[f].push_back(id); if (held) ++held[r[0]]; }
+      }
+      samples.push_back(LrSample{&recs[f], &ids[f]});
+      if (in.valid) genoSamples.push_back(LrSample{&whole[f], &wholeIds[f]});
+    }
   }
-  LrCallSet cs;
-  MeiTemplates mei;
-  AnnoConfig acfg; acfg.meiMinFrac = meiMinFrac; acfg.trMinFrac = trMinFrac;
-  MethylConfig mcfg; mcfg.methylWindow = methylWindow; mcfg.methylProb = (uint16_t) methylProb; mcfg.minCpgDepth = (uint32_t) minCpgDepth;
-  if (tpl_arena) {
-    for (int t = 1; t <= 6; ++t) mei.seq[t].assign(tpl_arena + tpl_off[t - 1], tpl_arena + tpl_off[t]);
-    mei.polyA.assign(tpl_arena + tpl_off[6], tpl_arena + tpl_off[7]);
-  }
+};
+
+// dellyLrCall over one file, or dellyLrCallSharded as one rank of a sharded run (shard != NULL)
+static int delly_lr_call(dgpu_ctx* ctx, LrInput const& in, Shard const* shard, ChainOut const& o) {
+  LrRun s(in, nullptr, nullptr);
+  LrMultiCallSet cs;
   int rc;
-  if (g_lr_shard) {
-    LrMultiCallSet ms;
-    std::vector<LrSample> samples(1, LrSample{&recs, &ids});
-    rc = dellyLrCallSharded(ctx, c, indelExtension, tl, names, chr, samples, *g_lr_shard, ms, tpl_arena ? &mei : nullptr, acfg, tagflags ? &mcfg : nullptr);
-    if (!rc) { cs.svs.swap(ms.svs); cs.jctMap.swap(ms.sample[0].jctMap); cs.rcMap.swap(ms.sample[0].rcMap); cs.format.swap(ms.sample[0].format); cs.methyl.swap(ms.sample[0].methyl); }
-  } else rc = dellyLrCall(ctx, c, indelExtension, tl, names, chr, recs, ids, cs, tpl_arena ? &mei : nullptr, acfg, tagflags ? &mcfg : nullptr);
-  if (rc) return rc - 1;
-  const int n = (int) cs.svs.size();
-  if (n > cap) return -1;
-  for (int i = 0; i < n; ++i) {
-    StructuralVariantRecord const& v = cs.svs[i];
-    int32_t* o = sv_out + 20 * i;
-    o[0] = v.chr; o[1] = v.svStart; o[2] = v.chr2; o[3] = v.svEnd; o[4] = v.ciposlow; o[5] = v.ciposhigh; o[6] = v.ciendlow; o[7] = v.ciendhigh;
-    o[8] = v.peSupport; o[9] = v.srSupport; o[10] = v.peMapQuality; o[11] = v.srMapQuality; o[12] = v.mapq; o[13] = v.insLen; o[14] = v.homLen; o[15] = v.svt;
-    o[16] = v.precise ? 1 : 0; o[17] = v.consBp; o[18] = v.id; o[19] = 0;
-    memcpy(o + 19, &v.srAlignQuality, 4);
-    SampleFormat const& f = cs.format[i];
-    int32_t* q = fmt_out + 14 * i;
-    q[0] = f.gt[0]; q[1] = f.gt[1]; q[2] = f.gq; q[3] = f.pl[0]; q[4] = f.pl[1]; q[5] = f.pl[2]; q[6] = f.rcn; q[7] = f.pass ? 1 : 0;
-    q[8] = 0; q[9] = 0; q[10] = (int32_t) cs.jctMap[i].ref.size(); q[11] = (int32_t) cs.jctMap[i].alt.size();
-    q[12] = cs.rcMap[i].rc; q[13] = cs.rcMap[i].leftRC + cs.rcMap[i].rightRC;
-    for (int k = 0; k < 3; ++k) gl_out[3 * i + k] = f.gl[k];
-    cons_len[i] = (int32_t) v.consensus.size();
-    memcpy(cons_out + (size_t) i * cons_stride, v.consensus.data(), std::min<size_t>(v.consensus.size(), cons_stride));
-    if (anno_out) {
-      int32_t* a = anno_out + 5 * i;
-      a[0] = v.anno.isRC ? 1 : 0; a[1] = v.anno.seqType; a[2] = v.anno.homLen; a[3] = v.anno.trPeriod; memcpy(a + 4, &v.anno.trCopies, 4);
-    }
-    if (methyl_out && !cs.methyl.empty()) {
-      MethylInfo const& mi = cs.methyl[v.id];
-      memcpy(methyl_out + 16 * i, mi.alt, 16); memcpy(methyl_out + 16 * i + 4, mi.ref, 16); memcpy(methyl_out + 16 * i + 8, mi.mnc, 16); memcpy(methyl_out + 16 * i + 12, mi.mdp, 16);
-    }
-    if (alleles_out) {
-      alleles_len[i] = (int32_t) v.alleles.size();
-      memcpy(alleles_out + (size_t) i * alleles_stride, v.alleles.data(), std::min<size_t>(v.alleles.size(), alleles_stride));
-    }
+  if (shard) rc = dellyLrCallSharded(ctx, s.c, in.indelExtension, s.g.tl, s.g.names, s.g.chr, s.samples, *shard, cs, s.meiP, s.acfg, s.mcfgP);
+  else {
+    LrCallSet one;
+    rc = dellyLrCall(ctx, s.c, in.indelExtension, s.g.tl, s.g.names, s.g.chr, s.recs[0], s.ids[0], one, s.meiP, s.acfg, s.mcfgP);
+    cs = one_sample(one);
   }
+  if (rc) return rc - 1;
+  const int n = write_calls(cs, o, cols_zero);
+  if (n >= 0) write_lr_extras(cs, o);
   return n;
 }
 
-int dh_delly_lr_call(dgpu_ctx* ctx, const char* contig_arena, const uint32_t* contig_off, const uint32_t* contig_len, int ncontig, const int32_t* rec12,
-                     const uint64_t* seeds, int nrec, const uint32_t* cigar, const char* reads, const int32_t* cfg12, float flankQuality, float indelExtension,
-                     int32_t* sv_out, int cap, int32_t* fmt_out, float* gl_out, char* cons_out, int cons_stride, int32_t* cons_len) {
-  return delly_lr_call_hook(ctx, contig_arena, contig_off, contig_len, ncontig, rec12, seeds, nrec, cigar, reads, cfg12, flankQuality, indelExtension, sv_out, cap, fmt_out,
-                            gl_out, cons_out, cons_stride, cons_len, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 0, 0, nullptr, nullptr, 0.f, 0.f, nullptr, nullptr,
-                            nullptr, 0, nullptr);
-}
-
-// the complete long-read chain — layout as oracle/ref_wrap5.cpp::ref_delly_lr_call_ex plus the template sequences
+// the complete long-read chain — layout as oracle/ref_wrap5.cpp::ref_delly_lr_call_ex plus the template sequences; seeds = the read ids
+// (hash_lr of the query names)
 int dh_delly_lr_call_ex(dgpu_ctx* ctx, const char* contig_arena, const uint32_t* contig_off, const uint32_t* contig_len, int ncontig, const int32_t* rec12,
                         const uint64_t* seeds, int nrec, const uint32_t* cigar, const char* reads, const int32_t* cfg12, float flankQuality, float indelExtension,
                         int32_t* sv_out, int cap, int32_t* fmt_out, float* gl_out, char* cons_out, int cons_stride, int32_t* cons_len, const uint8_t* tagflags,
                         const char* mm_arena, const uint32_t* mm_off, const uint8_t* ml_arena, const uint32_t* ml_off, int methylWindow, int methylProb,
                         int minCpgDepth, const char* tpl_arena, const uint32_t* tpl_off, float meiMinFrac, float trMinFrac, int32_t* anno_out, int32_t* methyl_out,
                         char* alleles_out, int alleles_stride, int32_t* alleles_len) {
-  return delly_lr_call_hook(ctx, contig_arena, contig_off, contig_len, ncontig, rec12, seeds, nrec, cigar, reads, cfg12, flankQuality, indelExtension, sv_out, cap, fmt_out,
-                            gl_out, cons_out, cons_stride, cons_len, tagflags, mm_arena, mm_off, ml_arena, ml_off, methylWindow, methylProb, minCpgDepth, tpl_arena,
-                            tpl_off, meiMinFrac, trMinFrac, anno_out, methyl_out, alleles_out, alleles_stride, alleles_len);
+  const uint32_t file_off[2] = {0, (uint32_t) nrec};
+  const LrInput in{contig_arena, contig_off, contig_len, ncontig, rec12, seeds, file_off, 1, cigar, reads, cfg12, flankQuality, indelExtension, nullptr, 0, nullptr,
+                   nullptr, LrTags{tagflags, mm_arena, mm_off, ml_arena, ml_off}, methylWindow, methylProb, minCpgDepth, tpl_arena, tpl_off, meiMinFrac, trMinFrac};
+  return delly_lr_call(ctx, in, nullptr, ChainOut{sv_out, cap, fmt_out, gl_out, cons_out, cons_stride, cons_len, 1, anno_out, methyl_out, alleles_out, alleles_stride,
+                                                  alleles_len});
+}
+
+// dellyLrCall — layout as oracle/ref_wrap5.cpp::ref_delly_lr_call
+int dh_delly_lr_call(dgpu_ctx* ctx, const char* contig_arena, const uint32_t* contig_off, const uint32_t* contig_len, int ncontig, const int32_t* rec12,
+                     const uint64_t* seeds, int nrec, const uint32_t* cigar, const char* reads, const int32_t* cfg12, float flankQuality, float indelExtension,
+                     int32_t* sv_out, int cap, int32_t* fmt_out, float* gl_out, char* cons_out, int cons_stride, int32_t* cons_len) {
+  return dh_delly_lr_call_ex(ctx, contig_arena, contig_off, contig_len, ncontig, rec12, seeds, nrec, cigar, reads, cfg12, flankQuality, indelExtension, sv_out, cap,
+                             fmt_out, gl_out, cons_out, cons_stride, cons_len, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 0, 0, nullptr, nullptr, 0.f, 0.f,
+                             nullptr, nullptr, nullptr, 0, nullptr);
 }
 
 // several long-read samples — layout as oracle/ref_wrap5.cpp::ref_delly_lr_call_multi
 int dh_delly_lr_call_multi(dgpu_ctx* ctx, const char* contig_arena, const uint32_t* contig_off, const uint32_t* contig_len, int ncontig, const int32_t* rec12,
                            const uint64_t* seeds, const uint32_t* file_off, int nfile, const uint32_t* cigar, const char* reads, const int32_t* cfg12, float flankQuality,
                            float indelExtension, int32_t* sv_out, int cap, int32_t* fmt_out, float* gl_out, char* cons_out, int cons_stride, int32_t* cons_len) {
-  Config c;
-  c.minMapQual = (uint16_t) cfg12[0]; c.minClip = (uint32_t) cfg12[1]; c.minRefSep = (uint32_t) cfg12[2]; c.maxReadSep = (uint32_t) cfg12[3];
-  c.minCliqueSize = (uint16_t) cfg12[4]; c.graphPruning = (uint32_t) cfg12[5]; c.maxReadPerSV = (uint32_t) cfg12[6]; c.minimumFlankSize = cfg12[7];
-  c.indelsize = cfg12[8]; c.minConsWindow = cfg12[9]; c.maxGenoReadCount = (uint32_t) cfg12[10]; c.genoCap = cfg12[11];
-  c.flankQuality = flankQuality; c.nchr = ncontig;
-  apply_svtset(c);
-  std::vector<uint32_t> tl; std::vector<std::string> names; std::vector<const char*> chr;
-  for (int k = 0; k < ncontig; ++k) { tl.push_back(contig_len[k]); names.push_back("chr" + std::to_string(k)); chr.push_back(contig_arena + contig_off[k]); }
-  std::vector<std::vector<LrRecord> > recs((size_t) nfile);
-  std::vector<std::vector<std::size_t> > ids((size_t) nfile);
-  for (int f = 0; f < nfile; ++f)
-    for (uint32_t i = file_off[f]; i < file_off[f + 1]; ++i) {
-      const int32_t* r = rec12 + 12 * (size_t) i;
-      LrRecord rec;
-      rec.tid = r[0]; rec.pos = r[1]; rec.flag = (uint32_t) r[2]; rec.mapq = (uint8_t) r[3];
-      for (int k = 0; k < r[6]; ++k) rec.cigar.push_back(std::make_pair((uint8_t) (cigar[r[5] + k] & 0xf), cigar[r[5] + k] >> 4));
-      rec.seq.assign(reads + r[7], (std::size_t) r[4]);
-      recs[f].push_back(rec); ids[f].push_back((std::size_t) seeds[i]);
-    }
-  std::vector<LrSample> samples;
-  for (int f = 0; f < nfile; ++f) samples.push_back(LrSample{&recs[f], &ids[f]});
+  const LrInput in{contig_arena, contig_off, contig_len, ncontig, rec12, seeds, file_off, nfile, cigar, reads, cfg12, flankQuality, indelExtension, nullptr, 0,
+                   nullptr, nullptr};
+  LrRun s(in, nullptr, nullptr);
   LrMultiCallSet cs;
-  int rc = dellyLrCallMulti(ctx, c, indelExtension, tl, names, chr, samples, cs);
+  int rc = dellyLrCallMulti(ctx, s.c, indelExtension, s.g.tl, s.g.names, s.g.chr, s.samples, cs);
   if (rc) return rc - 1;
-  const int n = (int) cs.svs.size();
-  if (n > cap) return -1;
-  for (int i = 0; i < n; ++i) {
-    StructuralVariantRecord const& v = cs.svs[i];
-    int32_t* o = sv_out + 20 * i;
-    o[0] = v.chr; o[1] = v.svStart; o[2] = v.chr2; o[3] = v.svEnd; o[4] = v.ciposlow; o[5] = v.ciposhigh; o[6] = v.ciendlow; o[7] = v.ciendhigh;
-    o[8] = v.peSupport; o[9] = v.srSupport; o[10] = v.peMapQuality; o[11] = v.srMapQuality; o[12] = v.mapq; o[13] = v.insLen; o[14] = v.homLen; o[15] = v.svt;
-    o[16] = v.precise ? 1 : 0; o[17] = v.consBp; o[18] = v.id; o[19] = 0;
-    memcpy(o + 19, &v.srAlignQuality, 4);
-    for (int f = 0; f < nfile; ++f) {
-      LrSampleCounts const& sc = cs.sample[f];
-      SampleFormat const& fm = sc.format[i];
-      int32_t* q = fmt_out + 14 * ((size_t) f * cap + i);
-      q[0] = fm.gt[0]; q[1] = fm.gt[1]; q[2] = fm.gq; q[3] = fm.pl[0]; q[4] = fm.pl[1]; q[5] = fm.pl[2]; q[6] = fm.rcn; q[7] = fm.pass ? 1 : 0;
-      q[8] = 0; q[9] = 0; q[10] = (int32_t) sc.jctMap[i].ref.size(); q[11] = (int32_t) sc.jctMap[i].alt.size();
-      q[12] = sc.rcMap[i].rc; q[13] = sc.rcMap[i].leftRC + sc.rcMap[i].rightRC;
-      for (int k = 0; k < 3; ++k) gl_out[3 * ((size_t) f * cap + i) + k] = fm.gl[k];
-    }
-    cons_len[i] = (int32_t) v.consensus.size();
-    memcpy(cons_out + (size_t) i * cons_stride, v.consensus.data(), std::min<size_t>(v.consensus.size(), cons_stride));
-  }
-  return n;
+  return write_calls(cs, ChainOut{sv_out, cap, fmt_out, gl_out, cons_out, cons_stride, cons_len, nfile}, cols_zero);
 }
 
-// long-read genotyping mode: one sample, the outputs of dh_delly_lr_call for a given site list (rows as dh_vcf_parse)
+// long-read genotyping mode: one sample, the outputs of dh_delly_lr_call for a given site list (rows as dh_vcf_parse) except the consensus
 int dh_delly_lr_genotype(dgpu_ctx* ctx, const char* contig_arena, const uint32_t* contig_off, const uint32_t* contig_len, int ncontig, const int32_t* rec12, int nrec,
                          const uint32_t* cigar, const char* reads, const int32_t* cfg12, float flankQuality, const int32_t* site22, int nsite, const char* strs,
                          const uint32_t* str_off, int32_t* sv_out, int cap, int32_t* fmt_out, float* gl_out) {
-  Config c;
-  c.minMapQual = (uint16_t) cfg12[0]; c.minClip = (uint32_t) cfg12[1]; c.minRefSep = (uint32_t) cfg12[2]; c.maxReadSep = (uint32_t) cfg12[3];
-  c.minCliqueSize = (uint16_t) cfg12[4]; c.graphPruning = (uint32_t) cfg12[5]; c.maxReadPerSV = (uint32_t) cfg12[6]; c.minimumFlankSize = cfg12[7];
-  c.indelsize = cfg12[8]; c.minConsWindow = cfg12[9]; c.maxGenoReadCount = (uint32_t) cfg12[10]; c.genoCap = cfg12[11];
-  c.flankQuality = flankQuality; c.nchr = ncontig;
-  apply_svtset(c);
-  std::vector<uint32_t> tl; std::vector<std::string> names; std::vector<const char*> chr;
-  for (int k = 0; k < ncontig; ++k) { tl.push_back(contig_len[k]); names.push_back("chr" + std::to_string(k)); chr.push_back(contig_arena + contig_off[k]); }
-  std::vector<LrRecord> recs(nrec);
-  std::vector<std::size_t> ids(nrec, 0);
-  for (int i = 0; i < nrec; ++i) {
-    const int32_t* r = rec12 + 12 * i;
-    recs[i].tid = r[0]; recs[i].pos = r[1]; recs[i].flag = (uint32_t) r[2]; recs[i].mapq = (uint8_t) r[3];
-    for (int k = 0; k < r[6]; ++k) recs[i].cigar.push_back(std::make_pair((uint8_t) (cigar[r[5] + k] & 0xf), cigar[r[5] + k] >> 4));
-    recs[i].seq.assign(reads + r[7], (std::size_t) r[4]);
-  }
+  const uint32_t file_off[2] = {0, (uint32_t) nrec};
+  const LrInput in{contig_arena, contig_off, contig_len, ncontig, rec12, nullptr, file_off, 1, cigar, reads, cfg12, flankQuality, 0.f, site22, nsite, strs, str_off};
+  LrRun s(in, nullptr, nullptr);
   LrMultiCallSet cs;
-  int rc = dellyLrGenotype(ctx, c, tl, names, chr, sites_from_rows(site22, nsite, strs, str_off), true, std::vector<LrSample>(1, LrSample{&recs, &ids}), cs);
+  int rc = dellyLrGenotype(ctx, s.c, s.g.tl, s.g.names, s.g.chr, s.sites, true, s.samples, cs);
   if (rc) return rc - 1;
-  const int n = (int) cs.svs.size();
-  if (n > cap) return -1;
-  for (int i = 0; i < n; ++i) {
-    StructuralVariantRecord const& v = cs.svs[i];
-    int32_t* o = sv_out + 20 * i;
-    o[0] = v.chr; o[1] = v.svStart; o[2] = v.chr2; o[3] = v.svEnd; o[4] = v.ciposlow; o[5] = v.ciposhigh; o[6] = v.ciendlow; o[7] = v.ciendhigh;
-    o[8] = v.peSupport; o[9] = v.srSupport; o[10] = v.peMapQuality; o[11] = v.srMapQuality; o[12] = v.mapq; o[13] = v.insLen; o[14] = v.homLen; o[15] = v.svt;
-    o[16] = v.precise ? 1 : 0; o[17] = v.consBp; o[18] = v.id; o[19] = 0;
-    memcpy(o + 19, &v.srAlignQuality, 4);
-    LrSampleCounts const& sc = cs.sample[0];
-    SampleFormat const& fm = sc.format[i];
-    int32_t* q = fmt_out + 14 * i;
-    q[0] = fm.gt[0]; q[1] = fm.gt[1]; q[2] = fm.gq; q[3] = fm.pl[0]; q[4] = fm.pl[1]; q[5] = fm.pl[2]; q[6] = fm.rcn; q[7] = fm.pass ? 1 : 0;
-    q[8] = 0; q[9] = 0; q[10] = (int32_t) sc.jctMap[i].ref.size(); q[11] = (int32_t) sc.jctMap[i].alt.size();
-    q[12] = sc.rcMap[i].rc; q[13] = sc.rcMap[i].leftRC + sc.rcMap[i].rightRC;
-    for (int k = 0; k < 3; ++k) gl_out[3 * i + k] = fm.gl[k];
-  }
-  return n;
+  return write_calls(cs, ChainOut{sv_out, cap, fmt_out, gl_out, nullptr, 0, nullptr}, cols_zero);
 }
 
 // clusterSRReadsLR — layout as oracle/ref_wrap5.cpp::ref_cluster_sr_reads (ctx may be NULL: host pair scans)
@@ -940,14 +983,9 @@ int dh_cluster_sr_reads(dgpu_ctx* ctx, const uint32_t* contig_len, int ncontig, 
   c.minMapQual = (uint16_t) cfg12[0]; c.minClip = (uint32_t) cfg12[1]; c.minRefSep = (uint32_t) cfg12[2]; c.maxReadSep = (uint32_t) cfg12[3];
   c.minCliqueSize = (uint16_t) cfg12[4]; c.graphPruning = (uint32_t) cfg12[5]; c.nchr = ncontig;
   std::vector<uint32_t> tl(contig_len, contig_len + ncontig);
-  std::vector<LrRecord> recs(nrec);
-  std::vector<std::size_t> ids(nrec);
-  for (int i = 0; i < nrec; ++i) {
-    const int32_t* r = rec12 + 12 * i;
-    recs[i].tid = r[0]; recs[i].pos = r[1]; recs[i].flag = (uint32_t) r[2]; recs[i].mapq = (uint8_t) r[3];
-    for (int k = 0; k < r[6]; ++k) recs[i].cigar.push_back(std::make_pair((uint8_t) (cigar[r[5] + k] & 0xf), cigar[r[5] + k] >> 4));
-    ids[i] = (std::size_t) seeds[i];
-  }
+  std::vector<LrRecord> recs;
+  for (int i = 0; i < nrec; ++i) recs.push_back(lr_record(rec12 + 12 * i, cigar, nullptr, false, LrTags(), i));
+  std::vector<std::size_t> ids(seeds, seeds + nrec);
   std::vector<StructuralVariantRecord> svc;
   std::vector<TPosReadSlices> srStore;
   int rc = clusterSRReadsLR(ctx, c, tl, recs, ids, indelExtension, svc, srStore);
@@ -971,20 +1009,21 @@ int dh_cluster_sr_reads(dgpu_ctx* ctx, const uint32_t* contig_len, int ncontig, 
   return 0;
 }
 
-// getLibraryParams — layout as oracle/ref_wrap6.cpp::ref_get_library_params
+// LibraryInfo as 7 ints: rs, median, mad, minNormalISize, minISizeCutoff, maxNormalISize, maxISizeCutoff
+static void put_lib7(LibraryInfo const& l, int32_t* o) {
+  o[0] = l.rs; o[1] = l.median; o[2] = l.mad; o[3] = l.minNormalISize; o[4] = l.minISizeCutoff; o[5] = l.maxNormalISize; o[6] = l.maxISizeCutoff;
+}
+
+// getLibraryParams — layout as oracle/ref_wrap6.cpp::ref_get_library_params (the screen reads no CIGAR)
 int dh_get_library_params(const uint32_t* contig_len, int ncontig, const int32_t* rec12, int nrec, const uint32_t* cigar, int madCutoff, int madNormalCutoff,
                           int32_t* out7) {
   Config c; c.madCutoff = (uint16_t) madCutoff; c.madNormalCutoff = (uint16_t) madNormalCutoff;
   std::vector<uint32_t> tl(contig_len, contig_len + ncontig);
-  std::vector<SrRecord> recs(nrec);
-  for (int i = 0; i < nrec; ++i) {
-    const int32_t* r = rec12 + 12 * i;
-    recs[i].tid = r[0]; recs[i].pos = r[1]; recs[i].flag = (uint32_t) r[2]; recs[i].mapq = (uint8_t) r[3];
-    recs[i].lqseq = r[4]; recs[i].mtid = r[8]; recs[i].mpos = r[9]; recs[i].isize = r[10]; recs[i].name = (uint64_t) r[11];
-  }
+  std::vector<SrRecord> recs;
+  for (int i = 0; i < nrec; ++i) recs.push_back(sr_record(rec12 + 12 * i, nullptr, nullptr, nullptr, nullptr, i));
   LibraryInfo l;
   getLibraryParams(c, tl, recs, l);
-  out7[0] = l.rs; out7[1] = l.median; out7[2] = l.mad; out7[3] = l.minNormalISize; out7[4] = l.minISizeCutoff; out7[5] = l.maxNormalISize; out7[6] = l.maxISizeCutoff;
+  put_lib7(l, out7);
   return 0;
 }
 
@@ -1066,27 +1105,20 @@ int dh_vcf_output_multi(const uint32_t* contig_len, int ncontig, const int32_t* 
                          cap, anno_tr, methyl16, minCpgDepth, nfile);
 }
 
-// genotypeLRBatch — layout as oracle/ref_wrap4.cpp::ref_genotype_lr (contigs named "chr0", "chr1", ...)
-static int genotype_lr_hook(dgpu_ctx* ctx, const char* contig_arena, const uint32_t* contig_off, const uint32_t* contig_len, int ncontig, const int32_t* rec10, int nrec,
-                   const uint32_t* cigar, const char* reads, const int32_t* sv8, int nsv, const char* cons_arena, const uint32_t* cons_off,
-                   const uint32_t* cons_len, int minMapQual, int minimumFlankSize, int minConsWindow, int maxGenoReadCount, float flankQuality, int genoCap,
-                   uint8_t* qual_out, int qual_cap, uint32_t* ref_off, uint32_t* alt_off, int32_t* hp_out, int32_t* rc_out, const uint8_t* tagflags,
-                   const char* mm_arena, const uint32_t* mm_off, const uint8_t* ml_arena, const uint32_t* ml_off, int methylWindow, int methylProb,
-                   int minCpgDepth, int32_t* methyl_out) {
+// genotypeLRBatch with MM / ML tags (tagflags may be NULL) — layout as oracle/ref_wrap4.cpp::ref_genotype_lr_methyl (contigs named "chr0",
+// "chr1", ...; record rows of 10: [8] = HP, [9] = PS)
+int dh_genotype_lr_methyl(dgpu_ctx* ctx, const char* contig_arena, const uint32_t* contig_off, const uint32_t* contig_len, int ncontig, const int32_t* rec10,
+                          int nrec, const uint32_t* cigar, const char* reads, const int32_t* sv8, int nsv, const char* cons_arena, const uint32_t* cons_off,
+                          const uint32_t* cons_len, int minMapQual, int minimumFlankSize, int minConsWindow, int maxGenoReadCount, float flankQuality,
+                          int genoCap, uint8_t* qual_out, int qual_cap, uint32_t* ref_off, uint32_t* alt_off, int32_t* hp_out, int32_t* rc_out,
+                          const uint8_t* tagflags, const char* mm_arena, const uint32_t* mm_off, const uint8_t* ml_arena, const uint32_t* ml_off,
+                          int methylWindow, int methylProb, int minCpgDepth, int32_t* methyl_out) {
   Config c; c.minMapQual = (uint16_t) minMapQual; c.minimumFlankSize = minimumFlankSize; c.minConsWindow = minConsWindow;
   c.maxGenoReadCount = (uint32_t) maxGenoReadCount; c.flankQuality = flankQuality; c.genoCap = genoCap;
-  std::vector<uint32_t> tl; std::vector<std::string> names; std::vector<const char*> chr;
-  for (int k = 0; k < ncontig; ++k) { tl.push_back(contig_len[k]); names.push_back("chr" + std::to_string(k)); chr.push_back(contig_arena + contig_off[k]); }
-  std::vector<LrRecord> recs(nrec);
-  for (int i = 0; i < nrec; ++i) {
-    const int32_t* r = rec10 + 10 * i;
-    recs[i].tid = r[0]; recs[i].pos = r[1]; recs[i].flag = (uint32_t) r[2]; recs[i].mapq = (uint8_t) r[3];
-    for (int k = 0; k < r[6]; ++k) recs[i].cigar.push_back(std::make_pair((uint8_t) (cigar[r[5] + k] & 0xf), cigar[r[5] + k] >> 4));
-    recs[i].seq.assign(reads + r[7], (std::size_t) r[4]);
-    recs[i].hp = (uint8_t) (r[8] > 0 ? r[8] : 0); recs[i].ps = r[9];
-    if (tagflags && (tagflags[i] & 1)) { recs[i].hasMM = true; recs[i].mm.assign(mm_arena + mm_off[i], mm_arena + mm_off[i + 1]); }
-    if (tagflags && (tagflags[i] & 2)) { recs[i].hasML = true; recs[i].ml.assign(ml_arena + ml_off[i], ml_arena + ml_off[i + 1]); }
-  }
+  const Genome g(contig_arena, contig_off, contig_len, ncontig);
+  const LrTags tags{tagflags, mm_arena, mm_off, ml_arena, ml_off};
+  std::vector<LrRecord> recs;
+  for (int i = 0; i < nrec; ++i) recs.push_back(lr_record(rec10 + 10 * i, cigar, reads, true, tags, i));
   std::vector<StructuralVariantRecord> svs(nsv);
   for (int i = 0; i < nsv; ++i) {
     const int32_t* s = sv8 + 8 * i;
@@ -1097,24 +1129,11 @@ static int genotype_lr_hook(dgpu_ctx* ctx, const char* contig_arena, const uint3
   std::vector<JunctionCount> jct; std::vector<ReadCount> cov;
   MethylConfig mcfg; mcfg.methylWindow = methylWindow; mcfg.methylProb = (uint16_t) methylProb; mcfg.minCpgDepth = (uint32_t) minCpgDepth;
   std::vector<MethylInfo> methyl;
-  int rc = genotypeLRBatch(ctx, c, tl, names, chr, svs, recs, jct, cov, tagflags ? &mcfg : nullptr, tagflags ? &methyl : nullptr);
+  int rc = genotypeLRBatch(ctx, c, g.tl, g.names, g.chr, svs, recs, jct, cov, tagflags ? &mcfg : nullptr, tagflags ? &methyl : nullptr);
   if (rc) return rc - 1;
-  if (tagflags && methyl_out)
-    for (int i = 0; i < nsv; ++i) {
-      memcpy(methyl_out + 16 * i, methyl[i].alt, 16); memcpy(methyl_out + 16 * i + 4, methyl[i].ref, 16);
-      memcpy(methyl_out + 16 * i + 8, methyl[i].mnc, 16); memcpy(methyl_out + 16 * i + 12, methyl[i].mdp, 16);
-    }
-  int pos = 0;
-  for (int pass = 0; pass < 2; ++pass) {
-    uint32_t* off = pass ? alt_off : ref_off;
-    for (int i = 0; i < nsv; ++i) {
-      off[i] = (uint32_t) pos;
-      std::vector<uint8_t> const& v = pass ? jct[i].alt : jct[i].ref;
-      if (pos + (int) v.size() > qual_cap) return -1;
-      for (uint8_t q : v) qual_out[pos++] = q;
-    }
-    off[nsv] = (uint32_t) pos;
-  }
+  if (tagflags && methyl_out) for (int i = 0; i < nsv; ++i) put_methyl(methyl_out + 16 * i, methyl[i]);
+  const int pos = put_qual_lists(jct, nsv, qual_out, qual_cap, ref_off, alt_off);
+  if (pos < 0) return pos;
   for (int i = 0; i < nsv; ++i) {
     hp_out[5 * i] = (int32_t) jct[i].hp1ref.size(); hp_out[5 * i + 1] = (int32_t) jct[i].hp1alt.size(); hp_out[5 * i + 2] = (int32_t) jct[i].hp2ref.size();
     hp_out[5 * i + 3] = (int32_t) jct[i].hp2alt.size(); hp_out[5 * i + 4] = jct[i].ps;
@@ -1127,21 +1146,9 @@ int dh_genotype_lr(dgpu_ctx* ctx, const char* contig_arena, const uint32_t* cont
                    const uint32_t* cigar, const char* reads, const int32_t* sv8, int nsv, const char* cons_arena, const uint32_t* cons_off,
                    const uint32_t* cons_len, int minMapQual, int minimumFlankSize, int minConsWindow, int maxGenoReadCount, float flankQuality, int genoCap,
                    uint8_t* qual_out, int qual_cap, uint32_t* ref_off, uint32_t* alt_off, int32_t* hp_out, int32_t* rc_out) {
-  return genotype_lr_hook(ctx, contig_arena, contig_off, contig_len, ncontig, rec10, nrec, cigar, reads, sv8, nsv, cons_arena, cons_off, cons_len, minMapQual,
-                          minimumFlankSize, minConsWindow, maxGenoReadCount, flankQuality, genoCap, qual_out, qual_cap, ref_off, alt_off, hp_out, rc_out, nullptr,
-                          nullptr, nullptr, nullptr, nullptr, 0, 0, 0, nullptr);
-}
-
-// genotypeLRBatch with MM / ML tags — layout as oracle/ref_wrap4.cpp::ref_genotype_lr_methyl
-int dh_genotype_lr_methyl(dgpu_ctx* ctx, const char* contig_arena, const uint32_t* contig_off, const uint32_t* contig_len, int ncontig, const int32_t* rec10,
-                          int nrec, const uint32_t* cigar, const char* reads, const int32_t* sv8, int nsv, const char* cons_arena, const uint32_t* cons_off,
-                          const uint32_t* cons_len, int minMapQual, int minimumFlankSize, int minConsWindow, int maxGenoReadCount, float flankQuality,
-                          int genoCap, uint8_t* qual_out, int qual_cap, uint32_t* ref_off, uint32_t* alt_off, int32_t* hp_out, int32_t* rc_out,
-                          const uint8_t* tagflags, const char* mm_arena, const uint32_t* mm_off, const uint8_t* ml_arena, const uint32_t* ml_off,
-                          int methylWindow, int methylProb, int minCpgDepth, int32_t* methyl_out) {
-  return genotype_lr_hook(ctx, contig_arena, contig_off, contig_len, ncontig, rec10, nrec, cigar, reads, sv8, nsv, cons_arena, cons_off, cons_len, minMapQual,
-                          minimumFlankSize, minConsWindow, maxGenoReadCount, flankQuality, genoCap, qual_out, qual_cap, ref_off, alt_off, hp_out, rc_out, tagflags,
-                          mm_arena, mm_off, ml_arena, ml_off, methylWindow, methylProb, minCpgDepth, methyl_out);
+  return dh_genotype_lr_methyl(ctx, contig_arena, contig_off, contig_len, ncontig, rec10, nrec, cigar, reads, sv8, nsv, cons_arena, cons_off, cons_len, minMapQual,
+                               minimumFlankSize, minConsWindow, maxGenoReadCount, flankQuality, genoCap, qual_out, qual_cap, ref_off, alt_off, hp_out, rc_out,
+                               nullptr, nullptr, nullptr, nullptr, nullptr, 0, 0, 0, nullptr);
 }
 
 // _seqIdentity / _bestSeqIdentity / _minRotation (src/merge.h:187-243) for n pairs: sequences in one arena, (offset, length) per side
@@ -1274,10 +1281,7 @@ int dh_msa_wfa_batch(dgpu_ctx* ctx, const char* arena, const uint32_t* read_off,
 int dh_annotate_sv(dgpu_ctx* ctx, const char* tpl_arena, const uint32_t* tpl_off, const char* seq, int chrLen, const int32_t* sv3, int nsv,
                    const char* alleles, const uint32_t* al_off, float meiMinFrac, float trMinFrac, int32_t* out5) {
   MeiTemplates mei;
-  if (tpl_arena && tpl_off) {
-    for (int t = 1; t <= 6; ++t) mei.seq[t].assign(tpl_arena + tpl_off[t - 1], tpl_arena + tpl_off[t]);
-    mei.polyA.assign(tpl_arena + tpl_off[6], tpl_arena + tpl_off[7]);
-  }
+  if (tpl_arena && tpl_off) load_mei(mei, tpl_arena, tpl_off);
   AnnoConfig c; c.meiMinFrac = meiMinFrac; c.trMinFrac = trMinFrac;
   std::vector<StructuralVariantRecord> svs(nsv);
   std::vector<int32_t> which(nsv);

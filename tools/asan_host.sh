@@ -11,7 +11,8 @@ mkdir -p tests/standin/_build
 g++ -std=c++17 -O1 -g -fsanitize=address,undefined -fno-omit-frame-pointer -fPIC -shared -w -Wl,-Bsymbolic -o tests/standin/_build/libhost_standin.so \
   tests/standin/host_standin.cpp -Loracle/_ref -l:libdelly_ref.so -Ldelly_b200 -l:libdelly_b200.so -Wl,-rpath,"$PWD/oracle/_ref" -Wl,-rpath,"$PWD/delly_b200"
 LD_PRELOAD="$(gcc -print-file-name=libasan.so) $(gcc -print-file-name=libubsan.so)" ASAN_OPTIONS=detect_leaks=0:protect_shadow_gap=0 \
-  python -m pytest tests/test_host_cluster.py tests/test_host_genotype.py tests/test_host_split.py tests/test_svanno.py tests/test_methyl.py tests/test_lr_full_chain.py tests/test_genotype_mode.py tests/test_multi_sample.py tests/test_seq_identity.py tests/test_svtset.py tests/test_edlib_compat.py tests/test_example_data.py -x -q -m "not gpu" \
+  python -m pytest tests/test_host_cluster.py tests/test_host_genotype.py tests/test_host_split.py tests/test_svanno.py tests/test_methyl.py tests/test_lr_full_chain.py tests/test_genotype_mode.py tests/test_multi_sample.py tests/test_seq_identity.py tests/test_svtset.py tests/test_edlib_compat.py tests/test_example_data.py \
+  tests/test_sharded.py tests/test_contig_shard.py tests/test_lr_contig_shard.py -x -q -m "not gpu" \
   -p no:cacheprovider || true
 rm -f tests/standin/_build/libhost_standin.so
 touch delly_b200/host/capi.cpp
