@@ -120,6 +120,23 @@ class Context:
     def launches(self):
         return int(self._lib.dgpu_launch_count(self.h))
 
+    @property
+    def unsupported(self):
+        """dgpu_unsupported_count: jobs refused per item so far (reads the device counter of asynchronous longNeedle calls)."""
+        self._lib.dgpu_unsupported_count.restype = C.c_uint64
+        return int(self._lib.dgpu_unsupported_count(self.h))
+
+    def set_ln_async_bound(self, max_cons, max_ref):
+        """dgpu_set_ln_async_bound: no later longNeedle job exceeds max_cons x max_ref, so long_needle_dev reads nothing back and can be
+        captured into a CUDA graph; (0, 0) switches back."""
+        self.check(self._lib.dgpu_set_ln_async_bound(self.h, C.c_uint32(int(max_cons)), C.c_uint32(int(max_ref))), "dgpu_set_ln_async_bound")
+
+    def set_msa_async_bound(self, max_reads, max_read_len):
+        """dgpu_set_msa_async_bound: reserves the MSA workspace for clusters of up to max_reads reads, so msa_dev never grows it; (0, 0)
+        switches back."""
+        self.check(self._lib.dgpu_set_msa_async_bound(self.h, C.c_uint32(int(max_reads)), C.c_uint32(int(max_read_len))),
+                   "dgpu_set_msa_async_bound")
+
     # ------------------------------------------------------------------ edit distance
     def edit_distance(self, seqs, q_off, q_len, t_off, t_len, k, mode, want_end=False):
         """Host form (numpy or pinned torch CPU tensors in, numpy out)."""

@@ -30,6 +30,14 @@ struct dgpu_ctx {
   void* comm = nullptr;      // ncclComm_t when multi-GPU gather is initialised
   int rank = 0, world = 1;
   uint32_t async_bound = 0;  // dgpu_set_async_bound: > 0 = the caller guarantees no sequence is longer; device-form calls then never synchronise
+  // dgpu_set_ln_async_bound: > 0 = no longNeedle job exceeds ln_max_cons x ln_max_ref; the device forms then plan on the device inside a
+  // workspace pool of ln_pool bytes reserved by the setter, and count their refusals in ln_refused (device, cumulative; ln_refused_folded of
+  // them are already in `unsupported`)
+  uint32_t ln_max_cons = 0, ln_max_ref = 0;
+  size_t ln_pool = 0;
+  unsigned long long* ln_refused = nullptr;
+  unsigned long long ln_refused_folded = 0;
+  uint32_t msa_max_reads = 0;  // dgpu_set_msa_async_bound: > 0 = the MSA workspace slots are reserved for clusters of up to this many reads
   bool no_band = false;      // development switch (DGPU_ED_NO_BAND): long NW jobs straight to the full-matrix kernel
   uint64_t unsupported = 0;  // jobs refused per item because they exceed a device limit (dgpu_unsupported_count)
   std::vector<size_t> seg_room;  // seg_rows_exceed (edit_path.cu): the shared memory each seg_kernel class may opt in to, asked once per context
@@ -83,6 +91,8 @@ int dgpu_fork_init(dgpu_ctx* ctx);  // creates the fork/join pool on first use
 int dgpu_set_cuda_error(dgpu_ctx* ctx, cudaError_t e, const char* what);
 // Returns device pointer of at least `bytes` bytes in `slot` (contents NOT preserved on growth).
 int dgpu_reserve(dgpu_ctx* ctx, int slot, size_t bytes, void** out);
+// Adds the longNeedle refusals that asynchronous calls counted on the device to ctx->unsupported (synchronises the context stream).
+int dgpu_fold_refusals(dgpu_ctx* ctx);
 
 #define DGPU_CUDA(ctx, call)                                            \
   do {                                                                  \

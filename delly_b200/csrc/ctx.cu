@@ -51,6 +51,22 @@ int dgpu_smem_optin_raise(dgpu_ctx* ctx, const void* kernel, size_t smem, const 
   return DGPU_OK;
 }
 
+int dgpu_fold_refusals(dgpu_ctx* ctx) {
+  if (!ctx->ln_refused) return DGPU_OK;
+  unsigned long long v = 0;
+  DGPU_CUDA(ctx, cudaSetDevice(ctx->device));
+  DGPU_CUDA(ctx, cudaMemcpyAsync(&v, ctx->ln_refused, sizeof(v), cudaMemcpyDeviceToHost, ctx->stream));
+  DGPU_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  if (v > ctx->ln_refused_folded) {
+    const unsigned long long d = v - ctx->ln_refused_folded;
+    ctx->unsupported += d;
+    ctx->ln_refused_folded = v;
+    ctx->last_error = "dgpu_long_needle[_ex]_dev: " + std::to_string(d) + " job(s) beyond the asynchronous bound (" + std::to_string(ctx->ln_max_cons) +
+                      " x " + std::to_string(ctx->ln_max_ref) + ") or the device limits were not aligned (ok = 0)";
+  }
+  return DGPU_OK;
+}
+
 int dgpu_fork_init(dgpu_ctx* ctx) {
   while (ctx->fork_streams.size() < DGPU_FORK_STREAMS) {
     cudaStream_t s;
@@ -120,6 +136,7 @@ void dgpu_ctx_destroy(dgpu_ctx* ctx) {
   cudaStreamSynchronize(ctx->stream);
   for (auto& b : ctx->bufs)
     if (b.p) cudaFree(b.p);
+  if (ctx->ln_refused) cudaFree(ctx->ln_refused);
   if (ctx->ev0) { cudaEventDestroy(ctx->ev0); cudaEventDestroy(ctx->ev1); }
   for (auto e : ctx->pipe_events) cudaEventDestroy(e);
   for (auto e : ctx->fork_events) cudaEventDestroy(e);
@@ -133,14 +150,18 @@ void dgpu_ctx_destroy(dgpu_ctx* ctx) {
 int dgpu_ctx_sync(dgpu_ctx* ctx) {
   if (!ctx) return DGPU_ERR_ARG;
   DGPU_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  return DGPU_OK;
+  return dgpu_fold_refusals(ctx);
 }
 
 const char* dgpu_last_error(dgpu_ctx* ctx) { return ctx ? ctx->last_error.c_str() : ""; }
 
 uint64_t dgpu_launch_count(dgpu_ctx* ctx) { return ctx ? ctx->launches : 0; }
 
-uint64_t dgpu_unsupported_count(dgpu_ctx* ctx) { return ctx ? ctx->unsupported : 0; }
+uint64_t dgpu_unsupported_count(dgpu_ctx* ctx) {
+  if (!ctx) return 0;
+  dgpu_fold_refusals(ctx);   // a failed read leaves the count as it was and its text in last_error
+  return ctx->unsupported;
+}
 
 int dgpu_set_async_bound(dgpu_ctx* ctx, uint32_t max_seq_len) {
   if (!ctx) return DGPU_ERR_ARG;

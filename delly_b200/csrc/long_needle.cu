@@ -41,6 +41,13 @@ namespace {
 constexpr int LN_NCLS = 16;  // 0 trivial; 1..15 the rows of ln_geom
 constexpr int LN_GEN = 16;   // class + LN_GEN: the same geometry for jobs with a byte outside ACGTN (scalar engine, byte compares)
 
+// Workspace plan of one class, written on the device by ln_plan_kernel when the call runs under dgpu_set_ln_async_bound: the class's slabs
+// start at `base` inside the pool, and only the first `grid` CTAs of its launch take jobs.
+struct LnPlan {
+  unsigned long long base, work_stride, off_dirsR, off_dirsF, off_trace;
+  uint32_t grid;
+};
+
 struct LnArgs {
   const uint8_t* seqs;
   const uint32_t* c_off;
@@ -63,7 +70,19 @@ struct LnArgs {
   size_t off_dirsR, off_dirsF, off_trace;  // offsets inside a slab (reverse prefix maxima at 0)
   uint32_t max_ref;              // widest window the wide engine takes (0: none, the dgpu_long_needle forms)
   unsigned long long wide_budget;  // workspace bytes one wide job may take
+  uint32_t bound_cons, bound_ref;  // dgpu_set_ln_async_bound (0: none): jobs beyond it are refused
+  const LnPlan* plan;            // per class, under the bound (the PLAN kernels); else work / work_stride / off_* and the launch grid hold
 };
+
+// The workspace slab of this CTA and the CTAs that take jobs, from the plan (PLAN) or from the arguments and the launch. The class kernels
+// are compiled both ways, so that reading the plan costs the kernels of the synchronous forms no registers.
+struct LnCta { uint8_t* slab; size_t off_dirsR, off_dirsF, off_trace; uint32_t grid; };
+template <bool PLAN>
+__device__ __forceinline__ LnCta ln_cta(const LnArgs& a, int cls) {
+  if (!PLAN) return {a.work + (size_t) blockIdx.x * a.work_stride, a.off_dirsR, a.off_dirsF, a.off_trace, gridDim.x};
+  const LnPlan& p = a.plan[cls];
+  return {a.work + p.base + (size_t) blockIdx.x * p.work_stride, (size_t) p.off_dirsR, (size_t) p.off_dirsF, (size_t) p.off_trace, p.grid};
+}
 
 // Geometry of the wavefront job classes: a job whose n reference columns satisfy n + 7 <= cap (7 columns of slack for the aligned
 // forward blocks) and not the previous row's cap takes the row's class, C columns per lane and T threads per CTA (MULTI: T > 32).
@@ -119,8 +138,9 @@ __host__ __device__ inline LnParts ln_parts(int C, uint32_t m, uint32_t n) {
 }
 // Slab layout of a class from the maxima over its jobs: prefix maxima, reverse direction nibbles, forward direction nibbles, then the four
 // trace strings of m + n bytes.
-inline void ln_slab(LnArgs& a, unsigned long long rev, unsigned long long dirs, unsigned long long mn) {
-  auto al = [](size_t x) { return (x + 255) & ~(size_t) 255; };
+template <class S>   // LnArgs (host planning) or LnPlan (device planning)
+__host__ __device__ inline void ln_slab(S& a, unsigned long long rev, unsigned long long dirs, unsigned long long mn) {
+  auto al = [](unsigned long long x) { return (x + 255) & ~255ull; };
   a.off_dirsR = al(rev + 1024);
   a.off_dirsF = a.off_dirsR + al(dirs + 1024);
   a.off_trace = a.off_dirsF + al(dirs + 1024);
@@ -169,16 +189,17 @@ inline size_t lnw_smem(uint32_t max_ref, size_t mmax) {
 }
 
 // one WARP per job: class by shape, and whether every byte of both sequences is one of ACGTN (then the packed engine applies)
-__global__ void ln_count_kernel(LnArgs a, int* unsupported) {
+__global__ void ln_count_kernel(LnArgs a, unsigned long long* unsupported) {
   const uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (i >= a.n) return;
   const uint32_t m = a.c_len[i], n = a.r_len[i];
   int c = ln_class(m, n);
   if (c < 0 && n <= a.max_ref && m <= LNW_MAX_CONS && lnw_geom(m, n).bytes <= a.wide_budget) c = LN_WIDE;
+  if (a.bound_cons && (m > a.bound_cons || n > a.bound_ref)) c = -1;
   if (c < 0) {   // beyond the kernel's shapes: this ONE job is reported as not aligned (ok = 0, info[2] = -1) and counted; the batch goes on
     if (lane == 0) {
-      atomicAdd(unsupported, 1);
+      atomicAdd(unsupported, 1ull);
       a.jobcls[i] = 0; atomicAdd(&a.counts[0], 1u);
       a.ok[i] = 0; a.aln_len[i] = 0;
       if (a.info) { a.info[4 * i] = 0; a.info[4 * i + 1] = 0; a.info[4 * i + 2] = -1; a.info[4 * i + 3] = 0; }
@@ -220,6 +241,44 @@ __global__ void ln_scatter_kernel(LnArgs a) {
   const int c = a.jobcls[i];
   uint32_t p = atomicAdd(&a.counts[64 + c], 1u);
   a.perm[p] = i;
+}
+
+// Device-side planning under dgpu_set_ln_async_bound: what ln_dev's host planner does from the counts and maxima it reads back, done by one
+// thread from the same counts and maxima. gmax[c] = the CTAs class c is launched with (0: not launched); pool = workspace bytes. Every
+// launched non-empty class gets the slab of its largest job and min(count, gmax) CTAs. The wide class then takes what the ordinary classes
+// leave of the pool, keeping them up to half of it, and never less than one CTA each; if the ordinary classes still ask for more than the
+// rest, each keeps one CTA and the CTAs above that are cut by one factor. (The host planner shrinks whole grids by one factor and may
+// reserve more than its budget to give every class one CTA; a pool reserved once cannot grow, so the device planner cuts so that it fits:
+// the setter sized the pool for one bound-shaped CTA of every class the bound admits.)
+struct LnPlanIn { uint32_t gmax[2 * LN_NCLS]; unsigned long long pool; };
+__global__ void ln_plan_kernel(const uint32_t* __restrict__ counts, const unsigned long long* __restrict__ maxc, LnPlanIn in, LnPlan* plan) {
+  if (threadIdx.x != 0) return;
+  LnPlan pl[2 * LN_NCLS];
+  unsigned long long ord = 0, base = 0;   // ordinary classes: bytes asked for, bytes of one CTA each
+  for (int c = 0; c < 2 * LN_NCLS; ++c) {
+    LnPlan& p = pl[c];
+    p.base = p.work_stride = p.off_dirsR = p.off_dirsF = p.off_trace = 0;
+    p.grid = 0;
+    if (c == 0 || !in.gmax[c] || !counts[c]) continue;
+    if (c == LN_WIDE) p.work_stride = maxc[c];
+    else ln_slab(p, maxc[c], maxc[32 + c], maxc[64 + c]);
+    p.grid = min(counts[c], in.gmax[c]);
+    if (c != LN_WIDE) { ord += p.grid * p.work_stride; base += p.work_stride; }
+  }
+  const unsigned long long P = in.pool;
+  unsigned long long wide_total = 0;
+  LnPlan& w = pl[LN_WIDE];
+  if (w.grid) {
+    const unsigned long long cap = P - max(min(ord, P / 2), base);
+    w.grid = (uint32_t) max(1ull, min((unsigned long long) w.grid, cap / w.work_stride));
+    wide_total = w.grid * w.work_stride;
+  }
+  const unsigned long long rest = P - wide_total;
+  if (ord > rest)
+    for (int c = 1; c < 2 * LN_NCLS; ++c)
+      if (c != LN_WIDE && pl[c].grid) pl[c].grid = 1 + (uint32_t) ((pl[c].grid - 1ull) * (rest - base) / (ord - base));
+  unsigned long long off = 0;
+  for (int c = 0; c < 2 * LN_NCLS; ++c) { pl[c].base = off; off += pl[c].grid * pl[c].work_stride; plan[c] = pl[c]; }
 }
 
 // src/util.h:549-563 applied to position i of the output
@@ -320,7 +379,7 @@ __device__ __forceinline__ uint32_t ln_traceback_warp(const uint32_t* __restrict
 // (a register cap tight enough for more single-warp CTAs per SM would spill the DP state that lives in registers)
 // MAXT = threads per CTA the register allocation is sized for: a multi-warp CTA of 8 warps may use 255 registers per
 // thread (the DP state of C columns lives in registers), 16 warps would be capped at 128 and spill.
-template <int C, bool MULTI, int MAXT>
+template <int C, bool MULTI, int MAXT, bool PLAN>
 __global__ void __launch_bounds__(MAXT, 1) ln_kernel(LnArgs a, int cls) {
   extern __shared__ uint8_t sm_dyn[];
   constexpr int UPS = ln_ups(C, MAXT) ? MAXT : 0;   // wide column blocks: previous-row state in shared memory (wavefront.cuh)
@@ -334,14 +393,15 @@ __global__ void __launch_bounds__(MAXT, 1) ln_kernel(LnArgs a, int cls) {
   const int T = blockDim.x;
   const int lane = tid & 31;
   const uint32_t cnt = a.counts[cls], start = a.counts[32 + cls];
-  uint8_t* slab = a.work + (size_t) blockIdx.x * a.work_stride;
-  int16_t* brev = (int16_t*) slab;
-  uint32_t* dirsR = (uint32_t*) (slab + a.off_dirsR);
-  uint32_t* dirsF = (uint32_t*) (slab + a.off_dirsF);
-  uint8_t* trace = slab + a.off_trace;
+  const LnCta cta = ln_cta<PLAN>(a, cls);
+  if (PLAN && blockIdx.x >= cta.grid) return;
+  int16_t* brev = (int16_t*) cta.slab;
+  uint32_t* dirsR = (uint32_t*) (cta.slab + cta.off_dirsR);
+  uint32_t* dirsF = (uint32_t*) (cta.slab + cta.off_dirsF);
+  uint8_t* trace = cta.slab + cta.off_trace;
   const wf::Scoring sc = {1, -1, true, true};  // DnaScore(1,-1,-1,-1), AlignConfig<true,false> (src/split.h:541-542)
 
-  for (uint32_t idx = blockIdx.x; idx < cnt; idx += gridDim.x) {
+  for (uint32_t idx = blockIdx.x; idx < cnt; idx += cta.grid) {
     const uint32_t job = a.perm[start + idx];
     const uint32_t m = a.c_len[job], n = a.r_len[job];
     const uint8_t* s1 = a.seqs + a.c_off[job];
@@ -524,7 +584,7 @@ __device__ __forceinline__ uint32_t ln_traceback_warp2(const uint32_t* __restric
   return k + (uint32_t) cc + (uint32_t) rr;
 }
 
-template <int C, bool MULTI, int MAXT>
+template <int C, bool MULTI, int MAXT, bool PLAN>
 __global__ void __launch_bounds__(MAXT, ln2_occ(MAXT)) ln_kernel2(LnArgs a, int cls) {
   extern __shared__ uint8_t sm_dyn[];
   const int tid = threadIdx.x;
@@ -540,13 +600,14 @@ __global__ void __launch_bounds__(MAXT, ln2_occ(MAXT)) ln_kernel2(LnArgs a, int 
   __shared__ wf::Best sm_best[16];
   __shared__ int sm_scan[16];
   const uint32_t cnt = a.counts[cls], start = a.counts[32 + cls];
-  uint8_t* slab = a.work + (size_t) blockIdx.x * a.work_stride;
-  uint4* brev4 = (uint4*) slab;                       // step-major workspace (wavefront2.cuh)
-  uint32_t* dirsR = (uint32_t*) (slab + a.off_dirsR);
-  uint32_t* dirsF = (uint32_t*) (slab + a.off_dirsF);
-  uint8_t* trace = slab + a.off_trace;
+  const LnCta cta = ln_cta<PLAN>(a, cls);
+  if (PLAN && blockIdx.x >= cta.grid) return;
+  uint4* brev4 = (uint4*) cta.slab;                     // step-major workspace (wavefront2.cuh)
+  uint32_t* dirsR = (uint32_t*) (cta.slab + cta.off_dirsR);
+  uint32_t* dirsF = (uint32_t*) (cta.slab + cta.off_dirsF);
+  uint8_t* trace = cta.slab + cta.off_trace;
 
-  for (uint32_t idx = blockIdx.x; idx < cnt; idx += gridDim.x) {
+  for (uint32_t idx = blockIdx.x; idx < cnt; idx += cta.grid) {
     const uint32_t job = a.perm[start + idx];
     const uint32_t m = a.c_len[job], n = a.r_len[job];
     const uint8_t* s1 = a.seqs + a.c_off[job];
@@ -829,6 +890,7 @@ __device__ __forceinline__ void lnw_pass(const uint8_t* sm_rows, const uint8_t* 
 
 // One CTA per wide job: reverse pass, forward pass with the join, refRight, the two warp tracebacks and the stitched output, with the
 // semantics of ln_kernel (see the head of this file).
+template <bool PLAN>
 __global__ void __launch_bounds__(LNW_THREADS, 1) lnw_kernel(LnArgs a) {
   extern __shared__ uint8_t sm_dyn[];
   const uint32_t nqmax = (a.max_ref + 6) / 8 + 1;
@@ -842,9 +904,11 @@ __global__ void __launch_bounds__(LNW_THREADS, 1) lnw_kernel(LnArgs a) {
   const int tid = threadIdx.x;
   const int lane = tid & 31;
   const uint32_t cnt = a.counts[LN_WIDE], start = a.counts[32 + LN_WIDE];
-  uint8_t* slab = a.work + (size_t) blockIdx.x * a.work_stride;
+  const LnCta cta = ln_cta<PLAN>(a, LN_WIDE);   // (the slab's layout is per job: lnw_geom)
+  if (PLAN && blockIdx.x >= cta.grid) return;
+  uint8_t* slab = cta.slab;
 
-  for (uint32_t idx = blockIdx.x; idx < cnt; idx += gridDim.x) {
+  for (uint32_t idx = blockIdx.x; idx < cnt; idx += cta.grid) {
     const uint32_t job = a.perm[start + idx];
     const uint32_t m = a.c_len[job], n = a.r_len[job];
     const uint8_t* s1 = a.seqs + a.c_off[job];
@@ -963,19 +1027,74 @@ __global__ void __launch_bounds__(LNW_THREADS, 1) lnw_kernel(LnArgs a) {
 }
 
 // The wavefront kernel of each job class, its template arguments read from ln_geom: classes 1..15 on the packed engine, 17..31 the same
-// geometries on the scalar engine.
+// geometries on the scalar engine; the PLAN kernels for calls under dgpu_set_ln_async_bound.
 using LnKernel = void (*)(LnArgs, int);
-template <size_t... G>
+template <bool PLAN, size_t... G>
 constexpr std::array<LnKernel, 2 * LN_NCLS> ln_kernels(std::index_sequence<G...>) {
-  return {{nullptr, ln_kernel2<ln_geom(G + 1).C, (ln_geom(G + 1).T > 32), ln_geom(G + 1).T>..., nullptr,
-           ln_kernel<ln_geom(G + 1).C, (ln_geom(G + 1).T > 32), ln_geom(G + 1).T>...}};
+  return {{nullptr, ln_kernel2<ln_geom(G + 1).C, (ln_geom(G + 1).T > 32), ln_geom(G + 1).T, PLAN>..., nullptr,
+           ln_kernel<ln_geom(G + 1).C, (ln_geom(G + 1).T > 32), ln_geom(G + 1).T, PLAN>...}};
 }
-constexpr std::array<LnKernel, 2 * LN_NCLS> LN_KERNELS = ln_kernels(std::make_index_sequence<LN_NCLS - 1>());
+constexpr std::array<LnKernel, 2 * LN_NCLS> LN_KERNELS[2] = {ln_kernels<false>(std::make_index_sequence<LN_NCLS - 1>()),
+                                                             ln_kernels<true>(std::make_index_sequence<LN_NCLS - 1>())};
 
 int check_max_ref(dgpu_ctx* ctx, uint32_t max_ref) {
   if (max_ref >= 1 && max_ref <= DGPU_LN_MAX_REF) return DGPU_OK;
   ctx->last_error = "dgpu_long_needle_ex: max_ref must be 1 .. " + std::to_string(DGPU_LN_MAX_REF);
   return DGPU_ERR_ARG;
+}
+
+// Launch shape of class c for consensus strings up to mmax bytes (wide class: windows up to max_ref): threads, dynamic shared memory and
+// the CTAs per SM its grid is capped at.
+struct LnShape { unsigned threads; size_t smem; int per_sm; };
+LnShape ln_shape(int c, size_t mmax, uint32_t max_ref) {
+  if (c == LN_WIDE) return {(unsigned) LNW_THREADS, lnw_smem(max_ref, mmax), 1};   // one 512-thread CTA per SM
+  const LnGeom g = ln_geom(c & (LN_GEN - 1));
+  if (c < LN_GEN) {
+    const size_t smem = ln2_smem(g.C, g.T).bytes(mmax);
+    return {(unsigned) g.T, smem, std::max(1, std::min<int>(ln2_occ(g.T), (int) ((200 * 1024) / (smem + 2048))))};
+  }
+  return {(unsigned) g.T, ln_smem_ups(g.C, g.T) + ((mmax + 15) & ~(size_t) 15), ln_per_sm(g.T)};
+}
+
+int ln_optin(dgpu_ctx* ctx, int c, bool plan, size_t smem) {
+  if (c == LN_WIDE) return dgpu_smem_optin(ctx, plan ? lnw_kernel<true> : lnw_kernel<false>, smem, "cudaFuncSetAttribute(lnw_kernel)");
+  return dgpu_smem_optin(ctx, LN_KERNELS[plan][c], smem, c < LN_GEN ? "cudaFuncSetAttribute(ln_kernel2)" : "cudaFuncSetAttribute(ln_kernel)");
+}
+
+int ln_launch(dgpu_ctx* ctx, int c, const LnArgs& a, unsigned grid, const LnShape& s, cudaStream_t cs) {
+  const bool plan = a.plan != nullptr;
+  int rc;
+  if ((rc = ln_optin(ctx, c, plan, s.smem))) return rc;
+  if (c == LN_WIDE) {
+    (plan ? lnw_kernel<true> : lnw_kernel<false>)<<<grid, s.threads, s.smem, cs>>>(a);
+    DGPU_LAUNCH_CHECK(ctx, "lnw_kernel");
+  } else {
+    LN_KERNELS[plan][c]<<<grid, s.threads, s.smem, cs>>>(a, c);
+    DGPU_LAUNCH_CHECK(ctx, c < LN_GEN ? "ln_kernel2" : "ln_kernel");
+  }
+  return DGPU_OK;
+}
+
+// The classes a bound of max_cons x max_ref admits, each with its launch shape at the bound and the slab bytes of a bound-shaped job of
+// the class: the wavefront classes whose narrowest window fits max_ref (both engines), and the wide class when the bound exceeds the
+// wavefront shapes. The shapes are the same for both forms; dgpu_long_needle_dev takes only bounds without the wide class.
+struct LnBoundClass { int c; LnShape s; unsigned long long slab; };
+std::vector<LnBoundClass> ln_bound_classes(uint32_t max_cons, uint32_t max_ref) {
+  std::vector<LnBoundClass> v;
+  for (int c = 1; c < LN_NCLS; ++c) {
+    const uint32_t nlo = c == 1 ? 1 : ln_geom(c - 1).cap - 6;   // the narrowest window of the class: n + 7 > the previous row's cap
+    if (nlo > max_ref || nlo >= 32000) continue;
+    const LnGeom g = ln_geom(c);
+    const uint32_t n = std::min(max_ref, g.cap - 7), m = std::min(max_cons, 32000 - nlo);
+    for (int e : {c, c + LN_GEN}) {
+      const LnParts p = e < LN_GEN ? ln2_parts(g.C, g.T, m) : ln_parts(g.C, m, n);
+      LnPlan pl;
+      ln_slab(pl, p.rev, p.dirs, (unsigned long long) m + n);
+      v.push_back({e, ln_shape(e, max_cons, max_ref), pl.work_stride});
+    }
+  }
+  if (ln_class(max_cons, max_ref) < 0) v.push_back({LN_WIDE, ln_shape(LN_WIDE, max_cons, max_ref), lnw_geom(max_cons, max_ref).bytes});
+  return v;
 }
 
 // the device form of both entry points; max_ref = 0: no wide engine (dgpu_long_needle_dev)
@@ -985,26 +1104,38 @@ int ln_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes, const uint32
   if (n == 0) return DGPU_OK;
   if (n >= (1ull << 31) || seqs_bytes >= (1ull << 32)) return DGPU_ERR_ARG;
   if (!seqs || !c_off || !c_len || !r_off || !r_len || !aln || !aln_off || !aln_len || !ok) return DGPU_ERR_ARG;
+  const bool bound = ctx->ln_max_cons != 0;   // dgpu_set_ln_async_bound: plan on the device, no readback
+  if (bound && !max_ref && ln_class(ctx->ln_max_cons, ctx->ln_max_ref) < 0) {
+    ctx->last_error = "dgpu_long_needle_dev: the asynchronous bound exceeds the wavefront shapes (|ref| <= 16377, |cons| + |ref| <= 32000); "
+                      "use dgpu_long_needle_ex_dev";
+    return DGPU_ERR_ARG;
+  }
   DGPU_CUDA(ctx, cudaSetDevice(ctx->device));
   cudaStream_t st = stream ? (cudaStream_t) stream : ctx->stream;
-  LnArgs a;
+  LnArgs a{};
   a.seqs = seqs;
   a.c_off = c_off; a.c_len = c_len; a.r_off = r_off; a.r_len = r_len; a.n = (uint32_t) n;
   a.aln = aln; a.aln_off = aln_off; a.aln_len = aln_len; a.ok = ok; a.info = info;
   a.max_ref = max_ref; a.wide_budget = 0;
+  a.bound_cons = ctx->ln_max_cons; a.bound_ref = ctx->ln_max_ref;
+  a.plan = nullptr;
   void* p;
   int rc;
-  if (max_ref) {   // a wide job may take half of the workspace budget below; one that needs more is refused alone
+  if (bound) {   // every wide job inside the bound fits the pool (the setter sized it so)
+    a.max_ref = std::min(max_ref, ctx->ln_max_ref);
+    if (max_ref) a.wide_budget = lnw_geom(ctx->ln_max_cons, ctx->ln_max_ref).bytes;
+  } else if (max_ref) {   // a wide job may take half of the workspace budget below; one that needs more is refused alone
     size_t free0 = 0, total0 = 0;
     cudaMemGetInfo(&free0, &total0);
     a.wide_budget = dgpu_workspace_budget(ctx, SLOT_WAVEFRONT, free0) / 2;
   }
   if ((rc = dgpu_reserve(ctx, SLOT_JOB_PERM, n * sizeof(uint32_t), &p))) return rc;
   a.perm = (uint32_t*) p;
-  if ((rc = dgpu_reserve(ctx, SLOT_COUNTS, 2048, &p))) return rc;
+  if ((rc = dgpu_reserve(ctx, SLOT_COUNTS, 2048 + 2 * LN_NCLS * sizeof(LnPlan), &p))) return rc;
   a.counts = (uint32_t*) p;                                   // 96 uint32 = 384 B
   a.maxcells = (unsigned long long*) ((uint8_t*) p + 512);     // 128 uint64 = 1024 B
-  int* d_unsupported = (int*) ((uint8_t*) p + 1536);
+  unsigned long long* d_unsupported = bound ? ctx->ln_refused : (unsigned long long*) ((uint8_t*) p + 1536);
+  LnPlan* d_plan = (LnPlan*) ((uint8_t*) p + 2048);
   DGPU_CUDA(ctx, cudaMemsetAsync(p, 0, 2048, st));
   void* pc;
   if ((rc = dgpu_reserve(ctx, SLOT_LN_JOBCLS, n + 64, &pc))) return rc;
@@ -1016,11 +1147,32 @@ int ln_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes, const uint32
   DGPU_LAUNCH_CHECK(ctx, "ln_offsets");
   ln_scatter_kernel<<<cb, 256, 0, st>>>(a);
   DGPU_LAUNCH_CHECK(ctx, "ln_scatter");
-  struct { uint32_t counts[128]; unsigned long long maxc[128]; int unsupported; } h;
+  if (bound) {
+    // Launch every class the bound admits with its grid cap and the shared memory of the bound; ln_plan_kernel gives each its slabs and
+    // its active CTAs in the pool, and the CTAs above them (all of an empty class's) return at once.
+    std::vector<LnBoundClass> cls = ln_bound_classes(ctx->ln_max_cons, ctx->ln_max_ref);
+    if (!max_ref && !cls.empty() && cls.back().c == LN_WIDE) cls.pop_back();
+    LnPlanIn in{};
+    for (const LnBoundClass& k : cls) in.gmax[k.c] = (uint32_t) ctx->num_sms * k.s.per_sm;
+    in.pool = ctx->ln_pool;
+    if ((rc = dgpu_reserve(ctx, SLOT_WAVEFRONT, ctx->ln_pool, &p))) return rc;
+    a.work = (uint8_t*) p;
+    ln_plan_kernel<<<1, 32, 0, st>>>(a.counts, a.maxcells, in, d_plan);
+    DGPU_LAUNCH_CHECK(ctx, "ln_plan");
+    a.plan = d_plan;
+    DgpuFork fork(ctx, st, cls.size());
+    if ((rc = fork.begin())) return rc;
+    for (const LnBoundClass& k : cls) {
+      cudaStream_t cs;
+      if ((rc = fork.next(cs)) || (rc = ln_launch(ctx, k.c, a, in.gmax[k.c], k.s, cs))) return rc;
+    }
+    return fork.end();
+  }
+  struct { uint32_t counts[128]; unsigned long long maxc[128]; unsigned long long unsupported; } h;
   DGPU_CUDA(ctx, cudaMemcpyAsync(&h, p, sizeof(h), cudaMemcpyDeviceToHost, st));
   DGPU_CUDA(ctx, cudaStreamSynchronize(st));
   if (h.unsupported) {   // per-item refusal: those jobs come back with ok = 0 (and info[2] = -1); never a silent approximation, never a failed batch
-    ctx->unsupported += (uint64_t) h.unsupported;
+    ctx->unsupported += h.unsupported;
     ctx->last_error = max_ref
         ? "dgpu_long_needle_ex: " + std::to_string(h.unsupported) + " job(s) with |ref| > max_ref (" + std::to_string(max_ref) + "), |cons| > " +
               std::to_string(LNW_MAX_CONS) + " or a workspace beyond the device budget were not aligned (ok = 0)"
@@ -1032,33 +1184,17 @@ int ln_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes, const uint32
   // streams forked from `st` (each class has its own region of the workspace): a batch of a few hundred SVs spread over
   // several classes would otherwise run as a sequence of under-filled launches.
   // Classes 1..15: jobs over ACGTN only -> packed two-row engine (ln_kernel2); 17..31: the same geometries for jobs with other bytes -> scalar engine.
-  struct Plan { int c; LnArgs a; size_t grid; unsigned threads; size_t smem; };
+  struct Plan { int c; LnArgs a; size_t grid; LnShape s; };
   std::vector<Plan> plans;
   size_t total = 0;
   for (int c = 1; c < 2 * LN_NCLS; ++c) {
     if (!h.counts[c]) continue;
     Plan pl;
     pl.c = c; pl.a = a;
-    const size_t mmax = (size_t) h.maxc[96 + c];
-    int per_sm;
-    if (c == LN_WIDE) {   // one 512-thread CTA per SM; the slab is the largest job's (lnw_geom), laid out per job by the kernel
-      pl.a.work_stride = (size_t) h.maxc[c];
-      pl.threads = LNW_THREADS;
-      pl.smem = lnw_smem(max_ref, mmax);
-      per_sm = 1;
-    } else {
-      const LnGeom g = ln_geom(c & (LN_GEN - 1));
-      ln_slab(pl.a, h.maxc[c], h.maxc[32 + c], h.maxc[64 + c]);
-      pl.threads = (unsigned) g.T;
-      if (c < LN_GEN) {
-        pl.smem = ln2_smem(g.C, g.T).bytes(mmax);
-        per_sm = std::max(1, std::min<int>(ln2_occ(g.T), (int) ((200 * 1024) / (pl.smem + 2048))));
-      } else {
-        pl.smem = ln_smem_ups(g.C, g.T) + ((mmax + 15) & ~(size_t) 15);
-        per_sm = ln_per_sm(g.T);
-      }
-    }
-    pl.grid = std::min<size_t>(h.counts[c], (size_t) ctx->num_sms * per_sm);
+    pl.s = ln_shape(c, (size_t) h.maxc[96 + c], max_ref);
+    if (c == LN_WIDE) pl.a.work_stride = (size_t) h.maxc[c];   // the slab is the largest job's (lnw_geom), laid out per job by the kernel
+    else ln_slab(pl.a, h.maxc[c], h.maxc[32 + c], h.maxc[64 + c]);
+    pl.grid = std::min<size_t>(h.counts[c], (size_t) ctx->num_sms * pl.s.per_sm);
     total += pl.grid * pl.a.work_stride;
     plans.push_back(pl);
   }
@@ -1086,21 +1222,8 @@ int ln_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes, const uint32
   DgpuFork fork(ctx, st, plans.size());
   if ((rc = fork.begin())) return rc;
   for (Plan& pl : plans) {
-    const int c = pl.c;
     cudaStream_t cs;
-    if ((rc = fork.next(cs))) return rc;
-    const unsigned grid = (unsigned) pl.grid, threads = pl.threads;
-    const size_t smem = pl.smem;
-    if (c == LN_WIDE) {
-      if ((rc = dgpu_smem_optin(ctx, lnw_kernel, smem, "cudaFuncSetAttribute(lnw_kernel)"))) return rc;
-      lnw_kernel<<<grid, threads, smem, cs>>>(pl.a);
-      DGPU_LAUNCH_CHECK(ctx, "lnw_kernel");
-    } else {
-      const LnKernel k = LN_KERNELS[c];
-      if ((rc = dgpu_smem_optin(ctx, k, smem, c < LN_GEN ? "cudaFuncSetAttribute(ln_kernel2)" : "cudaFuncSetAttribute(ln_kernel)"))) return rc;
-      k<<<grid, threads, smem, cs>>>(pl.a, c);
-      DGPU_LAUNCH_CHECK(ctx, c < LN_GEN ? "ln_kernel2" : "ln_kernel");
-    }
+    if ((rc = fork.next(cs)) || (rc = ln_launch(ctx, pl.c, pl.a, (unsigned) pl.grid, pl.s, cs))) return rc;
   }
   return fork.end();
 }
@@ -1133,6 +1256,40 @@ int ln_host(dgpu_ctx* ctx, const char* name, const uint8_t* seqs, uint64_t seqs_
 }  // namespace
 
 extern "C" {
+
+int dgpu_set_ln_async_bound(dgpu_ctx* ctx, uint32_t max_cons, uint32_t max_ref) {
+  if (!ctx) return DGPU_ERR_ARG;
+  if (!max_cons && !max_ref) { ctx->ln_max_cons = ctx->ln_max_ref = 0; ctx->ln_pool = 0; return DGPU_OK; }
+  if (!max_cons || !max_ref || max_cons > LNW_MAX_CONS || max_ref > DGPU_LN_MAX_REF) {
+    ctx->last_error = "dgpu_set_ln_async_bound: max_cons must be 1 .. " + std::to_string(LNW_MAX_CONS) + " and max_ref 1 .. " +
+                      std::to_string(DGPU_LN_MAX_REF) + " (or both 0)";
+    return DGPU_ERR_ARG;
+  }
+  DGPU_CUDA(ctx, cudaSetDevice(ctx->device));
+  // The pool: every admitted class at its grid cap with bound-shaped slabs, within the workspace budget, but never less than one
+  // bound-shaped slab per class (ln_plan_kernel relies on that).
+  unsigned long long one = 0, all = 0;
+  int rc;
+  for (const LnBoundClass& k : ln_bound_classes(max_cons, max_ref)) {
+    if ((rc = ln_optin(ctx, k.c, true, k.s.smem))) return rc;
+    one += k.slab;
+    all += (unsigned long long) ctx->num_sms * k.s.per_sm * k.slab;
+  }
+  size_t free_b = 0, total_b = 0;
+  DGPU_CUDA(ctx, cudaMemGetInfo(&free_b, &total_b));
+  const size_t pool = std::max<size_t>(one, std::min<size_t>(all, dgpu_workspace_budget(ctx, SLOT_WAVEFRONT, free_b)));
+  void* p;
+  if ((rc = dgpu_reserve(ctx, SLOT_WAVEFRONT, pool, &p)) || (rc = dgpu_reserve(ctx, SLOT_COUNTS, 2048 + 2 * LN_NCLS * sizeof(LnPlan), &p)) ||
+      (rc = dgpu_fork_init(ctx)))
+    return rc;
+  if (!ctx->ln_refused) {
+    DGPU_CUDA(ctx, cudaMalloc(&ctx->ln_refused, sizeof(unsigned long long)));
+    DGPU_CUDA(ctx, cudaMemsetAsync(ctx->ln_refused, 0, sizeof(unsigned long long), ctx->stream));
+    DGPU_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  }
+  ctx->ln_max_cons = max_cons; ctx->ln_max_ref = max_ref; ctx->ln_pool = pool;
+  return DGPU_OK;
+}
 
 int dgpu_long_needle_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
                          const uint32_t* c_off, const uint32_t* c_len, const uint32_t* r_off, const uint32_t* r_len,

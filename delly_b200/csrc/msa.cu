@@ -1043,9 +1043,74 @@ int check_max_reads(dgpu_ctx* ctx, uint32_t max_reads) {
   return DGPU_ERR_ARG;
 }
 
+constexpr size_t MSA_B_TRACE = ((size_t) (MSA_LCAP + 1) * ((MSA_LCAP + 8) / 8) * 4 + 255) & ~(size_t) 255;   // traceback bits of one alignment
+
+// Slab layout of msa_kernel's warps (fixed: sized for MSA_MAXR reads and MSA_LCAP columns).
+void msa_warp_layout(MsaArgs& A) {
+  auto al = [](size_t x) { return (x + 255) & ~(size_t) 255; };
+  // node alignments of one cluster, never freed: a node takes R x L bytes rounded up to 16, at most R x (MSA_LCAP + 1). The R of all
+  // nodes sum to the leaves' depths, at most 2 + 3 + .. + MSA_MAXR for a chain-shaped guide tree.
+  A.aln_cap = al((size_t) (MSA_MAXR * (MSA_MAXR + 1) / 2 - 1) * (MSA_LCAP + 1));
+  A.off_prof = A.aln_cap;
+  const size_t b_prof = al((size_t) (MSA_LCAP + 1) * 5);  // gapped consensus + the two column-kind arrays
+  A.off_trace = A.off_prof + b_prof;
+  A.off_lcs = A.off_trace + MSA_B_TRACE;
+  A.off_keys = A.off_lcs + al((size_t) 32 * (MSA_LCAP + 2) * sizeof(int) + MSA_TRI);
+  A.off_src = A.off_keys + al((size_t) (MSA_LCAP + 1) * 16);
+  A.off_bnd = A.off_src + al((size_t) (2 * MSA_LCAP + 4) * 4);
+  A.off_tab = A.off_bnd + al((size_t) 2 * (MSA_LCAP + 1) * 8);
+  A.off_spans = A.off_tab + al((size_t) MSA_LCAP * MSA_LCAP);
+  A.work_stride = A.off_spans + al((size_t) MSA_N * 2 * MSA_MAXR * 2);
+}
+
+// Slab layout of one msa_large_kernel CTA for clusters of up to max_reads reads.
+MsaLargeWork msa_large_layout(size_t max_reads) {
+  auto al = [](size_t x) { return (x + 255) & ~(size_t) 255; };
+  MsaLargeWork W{};
+  const size_t nmax = max_reads, nn = 2 * nmax + 1;
+  W.off_peq = al(nn * (nn - 1) / 2);
+  W.off_rows = W.off_peq + al(nmax * 5 * LCS_W * 4);
+  W.off_gapped = W.off_rows + al(nmax * 2 * (MSA_LCAP + 1));
+  W.off_warps = W.off_gapped + al(MSA_LCAP + 1);
+  W.w_tab = std::max(MSA_B_TRACE, al((size_t) 32 * (MSA_LCAP + 2) * sizeof(int)));  // the trace, or the LCS phase's DP rows
+  W.w_keys = W.w_tab + al((size_t) MSA_LCAP * MSA_LCAP);
+  W.w_ids = W.w_keys + al((size_t) (MSA_LCAP + 1) * 16);
+  W.w_src = W.w_ids + al((size_t) (MSA_LCAP + 1) * 4);
+  W.w_bnd = W.w_src + al((size_t) (2 * MSA_LCAP + 4) * 4);
+  W.w_rows = W.w_bnd + al((size_t) 2 * (MSA_LCAP + 1) * 8);
+  W.warp_stride = W.w_rows + al((size_t) 6 * (MSA_LCAP + 1) * 2);
+  W.cta_stride = W.off_warps + MSA_LWARPS * W.warp_stride;
+  return W;
+}
+
 }  // namespace
 
 extern "C" {
+
+int dgpu_set_msa_async_bound(dgpu_ctx* ctx, uint32_t max_reads, uint32_t max_read_len) {
+  if (!ctx) return DGPU_ERR_ARG;
+  if (!max_reads && !max_read_len) { ctx->msa_max_reads = 0; return DGPU_OK; }
+  if (!max_reads || !max_read_len || max_reads > (uint32_t) MSA_LARGE_MAXR || max_read_len > (uint32_t) MSA_LCAP) {
+    ctx->last_error = "dgpu_set_msa_async_bound: max_reads must be 1 .. " + std::to_string(MSA_LARGE_MAXR) + " and max_read_len 1 .. " +
+                      std::to_string(MSA_LCAP) + " (or both 0)";
+    return DGPU_ERR_ARG;
+  }
+  DGPU_CUDA(ctx, cudaSetDevice(ctx->device));
+  // the slots of the largest grids dgpu_msa_ex_dev launches (their slabs are sized for MSA_LCAP columns whatever the read length)
+  MsaArgs A;
+  msa_warp_layout(A);
+  void* p;
+  int rc;
+  if ((rc = dgpu_smem_optin(ctx, msa_kernel, sizeof(WarpSm) * MSA_WARPS, "cudaFuncSetAttribute(msa_kernel)")) ||
+      (rc = dgpu_reserve(ctx, SLOT_MSA_SEGJOBS, (size_t) ctx->num_sms * MSA_PER_SM * MSA_WARPS * A.work_stride, &p)))
+    return rc;
+  if (max_reads > (uint32_t) MSA_MAXR &&
+      ((rc = dgpu_smem_optin(ctx, msa_large_kernel, sizeof(LargeSm), "cudaFuncSetAttribute(msa_large_kernel)")) ||
+       (rc = dgpu_reserve(ctx, SLOT_MSA_LARGE, (size_t) ctx->num_sms * msa_large_layout(max_reads).cta_stride, &p))))
+    return rc;
+  ctx->msa_max_reads = max_reads;
+  return DGPU_OK;
+}
 
 int dgpu_msa_ex_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
                     const uint32_t* read_off, const uint32_t* read_len, const uint32_t* cluster_off, uint32_t nclusters,
@@ -1061,26 +1126,13 @@ int dgpu_msa_ex_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
   if (match > 127 || match < -127 || mismatch > 127 || mismatch < -127) return DGPU_ERR_UNSUPPORTED;  // the score table is int8
   DGPU_CUDA(ctx, cudaSetDevice(ctx->device));
   cudaStream_t st = stream ? (cudaStream_t) stream : ctx->stream;
+  if (ctx->msa_max_reads) max_reads = std::min(max_reads, ctx->msa_max_reads);   // inside the slots dgpu_set_msa_async_bound reserved
   MsaArgs A;
   A.seqs = seqs; A.read_off = read_off; A.read_len = read_len; A.cluster_off = cluster_off; A.nclusters = nclusters;
   A.match = match; A.mismatch = mismatch; A.go = go; A.ge = ge; A.min_clique = min_clique; A.max_reads = (int) max_reads;
   A.cons = cons; A.cons_off = cons_off; A.cons_len = cons_len; A.n_rows = n_rows; A.status = status;
   A.aln = aln; A.aln_off = aln_off; A.aln_cols = aln_cols;
-  auto al = [](size_t x) { return (x + 255) & ~(size_t) 255; };
-  // node alignments of one cluster, never freed: a node takes R x L bytes rounded up to 16, at most R x (MSA_LCAP + 1). The R of all
-  // nodes sum to the leaves' depths, at most 2 + 3 + .. + MSA_MAXR for a chain-shaped guide tree.
-  A.aln_cap = al((size_t) (MSA_MAXR * (MSA_MAXR + 1) / 2 - 1) * (MSA_LCAP + 1));
-  A.off_prof = A.aln_cap;
-  const size_t b_prof = al((size_t) (MSA_LCAP + 1) * 5);  // gapped consensus + the two column-kind arrays
-  A.off_trace = A.off_prof + b_prof;
-  const size_t b_trace = al((size_t) (MSA_LCAP + 1) * ((MSA_LCAP + 8) / 8) * 4);
-  A.off_lcs = A.off_trace + b_trace;
-  A.off_keys = A.off_lcs + al((size_t) 32 * (MSA_LCAP + 2) * sizeof(int) + MSA_TRI);
-  A.off_src = A.off_keys + al((size_t) (MSA_LCAP + 1) * 16);
-  A.off_bnd = A.off_src + al((size_t) (2 * MSA_LCAP + 4) * 4);
-  A.off_tab = A.off_bnd + al((size_t) 2 * (MSA_LCAP + 1) * 8);
-  A.off_spans = A.off_tab + al((size_t) MSA_LCAP * MSA_LCAP);
-  A.work_stride = A.off_spans + al((size_t) MSA_N * 2 * MSA_MAXR * 2);
+  msa_warp_layout(A);
   const int per_sm = MSA_PER_SM;  // CTAs of four independent warps
   const size_t smem = sizeof(WarpSm) * MSA_WARPS;
   if ((rc = dgpu_smem_optin(ctx, msa_kernel, smem, "cudaFuncSetAttribute(msa_kernel)"))) return rc;   // per device: set on the first call
@@ -1092,19 +1144,7 @@ int dgpu_msa_ex_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
   MsaLargeWork W{};
   size_t lgrid = 0, lsmem = sizeof(LargeSm);
   if (max_reads > (uint32_t) MSA_MAXR) {
-    const size_t nmax = max_reads, nn = 2 * nmax + 1;
-    W.off_peq = al(nn * (nn - 1) / 2);
-    W.off_rows = W.off_peq + al(nmax * 5 * LCS_W * 4);
-    W.off_gapped = W.off_rows + al(nmax * 2 * (MSA_LCAP + 1));
-    W.off_warps = W.off_gapped + al(MSA_LCAP + 1);
-    W.w_tab = std::max(b_trace, al((size_t) 32 * (MSA_LCAP + 2) * sizeof(int)));  // the trace, or the LCS phase's DP rows
-    W.w_keys = W.w_tab + al((size_t) MSA_LCAP * MSA_LCAP);
-    W.w_ids = W.w_keys + al((size_t) (MSA_LCAP + 1) * 16);
-    W.w_src = W.w_ids + al((size_t) (MSA_LCAP + 1) * 4);
-    W.w_bnd = W.w_src + al((size_t) (2 * MSA_LCAP + 4) * 4);
-    W.w_rows = W.w_bnd + al((size_t) 2 * (MSA_LCAP + 1) * 8);
-    W.warp_stride = W.w_rows + al((size_t) 6 * (MSA_LCAP + 1) * 2);
-    W.cta_stride = W.off_warps + MSA_LWARPS * W.warp_stride;
+    W = msa_large_layout(max_reads);
     lgrid = std::min<size_t>(nclusters, (size_t) ctx->num_sms);
     if ((rc = dgpu_smem_optin(ctx, msa_large_kernel, lsmem, "cudaFuncSetAttribute(msa_large_kernel)"))) return rc;
     if ((rc = dgpu_reserve(ctx, SLOT_MSA_LARGE, lgrid * W.cta_stride, &p))) return rc;

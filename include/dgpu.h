@@ -68,15 +68,36 @@ int dgpu_version(void);
 int dgpu_device_count(void);
 /* Number of kernel launches issued through this context so far (bench accounting). */
 uint64_t dgpu_launch_count(dgpu_ctx* ctx);
-/* jobs refused PER ITEM so far because they exceed a device limit (the call still succeeds; the item comes back flagged: ok = 0 / status != 0) */
+/* jobs refused PER ITEM so far because they exceed a device limit (the call still succeeds; the item comes back flagged: ok = 0 / status != 0).
+ * Refusals of longNeedle calls under dgpu_set_ln_async_bound are read from the device here (a synchronisation of the context stream):
+ * synchronise the stream such a call was enqueued on first. */
 uint64_t dgpu_unsupported_count(dgpu_ctx* ctx);
 /* Stream-asynchronous device forms. By default dgpu_edit_distance_dev reads its job-class counts back once per call (one small D2H + stream
  * synchronisation) so that it launches exactly the kernels the batch needs. With max_seq_len > 0 the caller guarantees that no query or target of
  * later calls is longer; the call then enqueues everything on `stream` and returns without any host synchronisation (scratch buffers are sized from
  * the bound and grown only between calls; it can be followed by further work on the stream, overlapped with copies on other streams, or captured
- * into a CUDA graph once the scratch exists). 0 switches back. dgpu_long_needle_dev / dgpu_msa_dev / dgpu_edit_path_dev always synchronise once:
- * their workspace depends on the shapes in the batch. */
+ * into a CUDA graph once the scratch exists). 0 switches back. dgpu_long_needle[_ex]_dev and dgpu_msa[_ex]_dev have bounds of their own,
+ * below; dgpu_edit_path[_ex|_wide]_dev always synchronise: they plan each Hirschberg level on the host between device rounds. */
 int dgpu_set_async_bound(dgpu_ctx* ctx, uint32_t max_seq_len);
+/* The same for longNeedle. With (max_cons, max_ref) set, the caller guarantees that no job of a later dgpu_long_needle[_ex][_dev] call has
+ * c_len > max_cons or r_len > max_ref. The device forms then read nothing back: one small kernel plans the workspace on the device from the
+ * batch's per-class counts and largest shapes, and every job class the bound admits is launched with the grid and shared memory of the
+ * bound (CTAs a class does not need return at once). The setter opts every such kernel in to its shared memory and reserves the workspace
+ * pool: each admitted class at its full grid with bound-shaped slabs, within the workspace budget (0.6 x free memory), but at least one
+ * bound-shaped slab per class. The per-job scratch grows with the number of jobs, so a call may be captured into a CUDA graph after one call
+ * with at least as many jobs. Rules: max_cons <= 16383, max_ref <= DGPU_LN_MAX_REF, both > 0, else DGPU_ERR_ARG; (0, 0) switches back.
+ * The bound applies to every longNeedle call of the context. dgpu_long_needle[_dev] (no wide engine) returns DGPU_ERR_ARG under a bound
+ * its wavefront kernels cannot take, max_ref > 16377 or max_cons + max_ref > 32000; the _ex forms take any bound, and their max_ref
+ * argument still limits the wide engine. A job beyond the bound or the limits below is refused alone (ok = 0, aln_len = 0, info[2] = -1).
+ * The device forms count such refusals on the device: dgpu_unsupported_count and dgpu_ctx_sync add them to the count (and set
+ * dgpu_last_error) once the work that made them has finished, not when the call returns. */
+int dgpu_set_ln_async_bound(dgpu_ctx* ctx, uint32_t max_cons, uint32_t max_ref);
+/* The same for the MSA. dgpu_msa[_ex]_dev read nothing back, but grow their workspace slots (which synchronises the device) the first time
+ * a call needs more. With (max_reads, max_read_len) set, the setter reserves the slots of the largest grids for clusters of up to
+ * max_reads reads, and later calls never grow them; a call's max_reads above the bound is lowered to it, so a larger cluster gets status 1.
+ * Reads longer than 1023 bases get status 2 as always; the slots are sized for 1023-column alignments whatever max_read_len is.
+ * Rules: max_reads <= DGPU_MSA_LARGE_MAXR, max_read_len <= 1023, both > 0, else DGPU_ERR_ARG; (0, 0) switches back. */
+int dgpu_set_msa_async_bound(dgpu_ctx* ctx, uint32_t max_reads, uint32_t max_read_len);
 /* Measurement hooks (bench.py): when profiling is on, every batch call brackets its dominant
  * kernels (not the staging copies or the binning pre-pass) with CUDA events on the launching
  * stream; dgpu_last_kernel_ms waits for and returns that span for the most recent call. */
