@@ -122,7 +122,7 @@ class Context:
 
     @property
     def unsupported(self):
-        """dgpu_unsupported_count: jobs refused per item so far (reads the device counter of asynchronous longNeedle calls)."""
+        """dgpu_unsupported_count: jobs refused per item so far (reads the device counters of asynchronous longNeedle and edit-path calls)."""
         self._lib.dgpu_unsupported_count.restype = C.c_uint64
         return int(self._lib.dgpu_unsupported_count(self.h))
 
@@ -136,6 +136,11 @@ class Context:
         switches back."""
         self.check(self._lib.dgpu_set_msa_async_bound(self.h, C.c_uint32(int(max_reads)), C.c_uint32(int(max_read_len))),
                    "dgpu_set_msa_async_bound")
+
+    def set_ep_async_bound(self, max_query, max_target):
+        """dgpu_set_ep_async_bound: no later edit-path job exceeds max_query x max_target, so edit_path_dev plans its Hirschberg levels on
+        the device, reads nothing back and can be captured into a CUDA graph; (0, 0) switches back."""
+        self.check(self._lib.dgpu_set_ep_async_bound(self.h, C.c_uint32(int(max_query)), C.c_uint32(int(max_target))), "dgpu_set_ep_async_bound")
 
     # ------------------------------------------------------------------ edit distance
     def edit_distance(self, seqs, q_off, q_len, t_off, t_len, k, mode, want_end=False):

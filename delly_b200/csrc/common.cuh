@@ -37,10 +37,15 @@ struct dgpu_ctx {
   size_t ln_pool = 0;
   unsigned long long* ln_refused = nullptr;
   unsigned long long ln_refused_folded = 0;
+  // dgpu_set_ep_async_bound: > 0 = no edit-path job exceeds ep_max_query x ep_max_target; the device forms then plan every Hirschberg level
+  // on the device and count their refusals in ep_refused (device, cumulative; ep_refused_folded of them are already in `unsupported`)
+  uint32_t ep_max_query = 0, ep_max_target = 0;
+  unsigned long long* ep_refused = nullptr;
+  unsigned long long ep_refused_folded = 0;
   uint32_t msa_max_reads = 0;  // dgpu_set_msa_async_bound: > 0 = the MSA workspace slots are reserved for clusters of up to this many reads
   bool no_band = false;      // development switch (DGPU_ED_NO_BAND): long NW jobs straight to the full-matrix kernel
   uint64_t unsupported = 0;  // jobs refused per item because they exceed a device limit (dgpu_unsupported_count)
-  std::vector<size_t> seg_room;  // seg_rows_exceed (edit_path.cu): the shared memory each seg_kernel class may opt in to, asked once per context
+  std::vector<size_t> seg_room;  // seg_rooms (edit_path.cu): the shared memory each seg_kernel class may opt in to, [eq][class], asked once per context
   // optional CUDA-event timing of the dominant kernels of the last batch call
   bool profiling = false;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
@@ -83,6 +88,7 @@ enum {
   SLOT_EP_BOUNDS,    // edit path: HW-start bounds and reverse end locations (edit_path.cu)
   SLOT_EP_EQTAB,     // edit path: generalised-equality tables (edit_path.cu)
   SLOT_EP_HROW,      // edit path: per-warp scratch rows of the half columns wider than the wavefront classes (edit_path.cu)
+  SLOT_EP_PLAN,      // edit path under dgpu_set_ep_async_bound: the per-job, per-segment and per-level planning arrays (edit_path.cu)
   SLOT_COUNT
 };
 
@@ -91,7 +97,8 @@ int dgpu_fork_init(dgpu_ctx* ctx);  // creates the fork/join pool on first use
 int dgpu_set_cuda_error(dgpu_ctx* ctx, cudaError_t e, const char* what);
 // Returns device pointer of at least `bytes` bytes in `slot` (contents NOT preserved on growth).
 int dgpu_reserve(dgpu_ctx* ctx, int slot, size_t bytes, void** out);
-// Adds the longNeedle refusals that asynchronous calls counted on the device to ctx->unsupported (synchronises the context stream).
+// Adds the longNeedle and edit-path refusals that asynchronous calls counted on the device to ctx->unsupported (synchronises the context
+// stream).
 int dgpu_fold_refusals(dgpu_ctx* ctx);
 
 #define DGPU_CUDA(ctx, call)                                            \

@@ -1102,12 +1102,13 @@ int launch_mode(dgpu_ctx* ctx, EdArgs& a, const uint32_t* hc, cudaStream_t st) {
 
 }  // namespace
 
-// Internal entry shared with edit_path.cu: last_pos selects the last optimal end position.
+// Internal entry shared with edit_path.cu: last_pos selects the last optimal end position; async_bound > 0 launches without reading the class
+// counts back, with the stripe scratch sized for sequences of up to that length (dgpu_set_async_bound).
 int dgpu_edit_distance_impl(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
                             const uint32_t* q_off, const uint32_t* q_len,
                             const uint32_t* t_off, const uint32_t* t_len,
                             const int32_t* k, int mode, uint64_t n,
-                            int32_t* dist, int32_t* end_loc, void* stream, int last_pos, const uint32_t* eq_tabs);
+                            int32_t* dist, int32_t* end_loc, void* stream, int last_pos, const uint32_t* eq_tabs, uint32_t async_bound);
 
 extern "C" {
 
@@ -1116,7 +1117,7 @@ int dgpu_edit_distance_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_byt
                            const uint32_t* t_off, const uint32_t* t_len,
                            const int32_t* k, int mode, uint64_t n,
                            int32_t* dist, int32_t* end_loc, void* stream) {
-  return dgpu_edit_distance_impl(ctx, seqs, seqs_bytes, q_off, q_len, t_off, t_len, k, mode, n, dist, end_loc, stream, 0, nullptr);
+  return dgpu_edit_distance_impl(ctx, seqs, seqs_bytes, q_off, q_len, t_off, t_len, k, mode, n, dist, end_loc, stream, 0, nullptr, ctx ? ctx->async_bound : 0);
 }
 
 }  // extern "C"
@@ -1125,7 +1126,7 @@ int dgpu_edit_distance_impl(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_by
                             const uint32_t* q_off, const uint32_t* q_len,
                             const uint32_t* t_off, const uint32_t* t_len,
                             const int32_t* k, int mode, uint64_t n,
-                            int32_t* dist, int32_t* end_loc, void* stream, int last_pos, const uint32_t* eq_tabs) {
+                            int32_t* dist, int32_t* end_loc, void* stream, int last_pos, const uint32_t* eq_tabs, uint32_t async_bound) {
   if (!ctx) return DGPU_ERR_ARG;
   if (mode != DGPU_MODE_NW && mode != DGPU_MODE_SHW && mode != DGPU_MODE_HW) return DGPU_ERR_ARG;
   if (n == 0) return DGPU_OK;
@@ -1177,11 +1178,11 @@ int dgpu_edit_distance_impl(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_by
   ed_scatter_kernel<<<cb, ED_BIN_THREADS, 0, st>>>(a);
   DGPU_LAUNCH_CHECK(ctx, "ed_scatter");
   uint32_t hc[ED_TMAX + 1];
-  if (ctx->async_bound) {
-    // Asynchronous form (dgpu_set_async_bound): no host round trip. Every class is launched with a grid sized from the job count (the kernels
+  if (async_bound) {
+    // Asynchronous form (dgpu_set_async_bound, or the edit path's bound): no host round trip. Every class is launched with a grid sized from the job count (the kernels
     // read their own class counts on the device and an empty class returns at once), the stripe scratch of long targets from the caller's bound.
     for (uint32_t& c : hc) c = 0;
-    const uint32_t bound = ctx->async_bound;
+    const uint32_t bound = async_bound;
     hc[1] = hc[2] = (uint32_t) n;
     if (bound > 64) hc[3] = (uint32_t) n;
     if (bound > 96) hc[4] = (uint32_t) n;

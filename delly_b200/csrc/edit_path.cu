@@ -25,7 +25,7 @@
 
 int dgpu_edit_distance_impl(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes, const uint32_t* q_off, const uint32_t* q_len,
                             const uint32_t* t_off, const uint32_t* t_len, const int32_t* k, int mode, uint64_t n, int32_t* dist,
-                            int32_t* end_loc, void* stream, int last_pos, const uint32_t* eq_tabs);
+                            int32_t* end_loc, void* stream, int last_pos, const uint32_t* eq_tabs, uint32_t async_bound);
 
 #include <vector>
 
@@ -87,7 +87,12 @@ struct SegJobs {
   const uint32_t* plan_m;  // rows / columns of the problem whose band the segment lives in: its own for a leaf, the parent's for a half column
   const uint32_t* plan_n;
   const uint8_t* eq_cls;   // class table of the generalised equality (null: byte equality)
+  const uint32_t* plan_count;  // PLAN kernels (asynchronous form): the number of jobs in `list`, on the device; `count` is not read
 };
+
+// the job count of a class kernel: a.count, or the count the device planned (PLAN)
+template <bool PLAN>
+__device__ __forceinline__ uint32_t seg_count(const SegJobs& a) { return PLAN ? *a.plan_count : a.count; }
 
 // Geometry of the seg_kernel classes: a segment of n target columns takes the first row with n <= cap (class 0: n = 0), with C columns
 // per lane, T threads per CTA (MULTI: T > 32) and a grid of at most per_sm CTAs per SM.
@@ -98,13 +103,18 @@ constexpr SegGeom SEG_GEOM[SEG_NCLS] = {{0, 0, 0, 0},
                                         {1280, 40, 32, 16}, {1536, 48, 32, 16}, {1792, 56, 32, 16}, {2048, 64, 32, 16},
                                         {4096, 32, 128, 4}, {8192, 32, 256, 2}, {16384, 32, 512, 1}};
 __host__ __device__ inline uint32_t seg_dstride(uint32_t n, uint32_t C) { return ((n + C - 1) / C + 1) * (C / 8); }
-inline int seg_class(uint32_t n) {
-  for (int c = 0; c < SEG_NCLS; ++c)
-    if (n <= SEG_GEOM[c].cap) return c;
-  return -1;
+// the first row of SEG_GEOM whose cap holds n; -1: none (written out for device code, checked against the table below)
+__host__ __device__ constexpr int seg_class(uint32_t n) {
+  return n <= 2048 ? (int) ((n + 255) / 256) : n <= 4096 ? 9 : n <= 8192 ? 10 : n <= 16384 ? 11 : -1;
 }
+constexpr bool seg_class_matches_geom() {
+  for (int c = 1; c < SEG_NCLS; ++c)
+    if (seg_class(SEG_GEOM[c].cap) != c || seg_class(SEG_GEOM[c - 1].cap + 1) != c) return false;
+  return seg_class(0) == 0 && seg_class(SEG_GEOM[SEG_NCLS - 1].cap + 1) == -1;
+}
+static_assert(seg_class_matches_geom(), "seg_class and SEG_GEOM disagree");
 
-template <int C, bool MULTI, bool EQ>
+template <int C, bool MULTI, bool EQ, bool PLAN = false>
 __global__ void __launch_bounds__(MULTI ? 512 : 32) seg_kernel(SegJobs a) {
   extern __shared__ uint8_t sm_rows[];
   __shared__ int sm_x[wf::WF_SMX];
@@ -114,7 +124,8 @@ __global__ void __launch_bounds__(MULTI ? 512 : 32) seg_kernel(SegJobs a) {
   uint32_t* dirs = (uint32_t*) slab;
   uint8_t* trace = slab + a.off_trace;
   const wf::Scoring sc = {0, -1, false, false};
-  for (uint32_t idx = blockIdx.x; idx < a.count; idx += gridDim.x) {
+  const uint32_t count = seg_count<PLAN>(a);
+  for (uint32_t idx = blockIdx.x; idx < count; idx += gridDim.x) {
     const uint32_t job = a.list[idx];
     const uint32_t m = a.q_len[job], n = a.t_len[job];
     const uint8_t* q = a.seqs + a.q_off[job];
@@ -182,7 +193,7 @@ __global__ void __launch_bounds__(MULTI ? 512 : 32) seg_kernel(SegJobs a) {
 //     many); the host shifts the leaf offset.
 constexpr int SEGB_WARPS = 2;
 
-template <int G, bool EQ>
+template <int G, bool EQ, bool PLAN = false>
 __global__ void __launch_bounds__(SEGB_WARPS * 32) seg_band_kernel(SegJobs a) {
   constexpr int JPW = 32 / G;
   constexpr int PEQ_JOB = EDB_PEQ_WORDS / JPW;
@@ -199,8 +210,8 @@ __global__ void __launch_bounds__(SEGB_WARPS * 32) seg_band_kernel(SegJobs a) {
   uint4* store = (uint4*) (a.work + ((size_t) gwarp * JPW + grp) * a.work_stride);
   const EqTabs tabs = {a.eq.f, a.eq.s, a.eq_cls};
 
-  for (uint32_t base = gwarp * JPW; base < a.count; base += nwarps * JPW) {
-    const bool have = base + grp < a.count;
+  for (uint32_t base = gwarp * JPW; base < seg_count<PLAN>(a); base += nwarps * JPW) {   // the count is read where it is used, as a.count was
+    const bool have = base + grp < seg_count<PLAN>(a);
     const uint32_t job = have ? a.list[base + grp] : 0;
     const int m = have ? (int) a.q_len[job] : 0, n = have ? (int) a.t_len[job] : 0;
     const uint8_t* q = a.seqs + (have ? a.q_off[job] : 0);
@@ -266,14 +277,15 @@ constexpr int EPL_WCOLS = 32;    // traceback window, columns
 // parked in the warp's scratch row (n bytes). NW top boundary (D[0][j] = j), rows / columns read back to front when rev. After each
 // stripe the lanes' final Pv / Mv are the vertical deltas of column n, which give colbuf[out_off + i] = -D[i][n] for every row of the
 // stripe, run on from the stripe above; the column is exact on every row.
-template <bool EQ>
+template <bool EQ, bool PLAN = false>
 __global__ void __launch_bounds__(EPW_WARPS * 32) seg_half_wide_kernel(SegJobs a, size_t hrow_stride) {
   __shared__ uint64_t peq_s[EPW_WARPS][5][32];
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
   const uint32_t gwarp = blockIdx.x * EPW_WARPS + wib, nwarps = gridDim.x * EPW_WARPS;
   volatile int8_t* hrow = (volatile int8_t*) (a.work + (size_t) gwarp * hrow_stride);
   const EqTabs tabs = {a.eq.f, a.eq.s, a.eq_cls};
-  for (uint32_t idx = gwarp; idx < a.count; idx += nwarps) {
+  const uint32_t count = seg_count<PLAN>(a);
+  for (uint32_t idx = gwarp; idx < count; idx += nwarps) {
     const uint32_t job = a.list[idx];
     const uint32_t m = a.q_len[job], n = a.t_len[job];
     const uint8_t* q = a.seqs + a.q_off[job];
@@ -306,7 +318,7 @@ __global__ void __launch_bounds__(EPW_WARPS * 32) seg_half_wide_kernel(SegJobs a
 // Leaf (kind 0) of at most two 64-row blocks and any width: EPL_G = 2 lanes per leaf, 16 leaves per warp. Lane p holds block p over the
 // whole column (lane 1 one step behind lane 0, its horizontal delta arriving by shuffle) and stores (Pv after the column, Ph into the
 // column) for every column, 16 B per lane-column. The traceback is seg_band_kernel's (leaf_trace, a window of EPL_WCOLS columns).
-template <bool EQ>
+template <bool EQ, bool PLAN = false>
 __global__ void __launch_bounds__(EPL_WARPS * 32) seg_leaf_wide_kernel(SegJobs a) {
   constexpr int G = EPL_G, JPW = 32 / G;
   __shared__ uint64_t peq_s[EPL_WARPS][JPW * G * EDB_BLOCK_WORDS];
@@ -319,8 +331,9 @@ __global__ void __launch_bounds__(EPL_WARPS * 32) seg_leaf_wide_kernel(SegJobs a
   uint4* store = (uint4*) (a.work + ((size_t) gwarp * JPW + grp) * a.work_stride);
   const EqTabs tabs = {a.eq.f, a.eq.s, a.eq_cls};
 
-  for (uint32_t base = gwarp * JPW; base < a.count; base += nwarps * JPW) {
-    const bool have = base + grp < a.count;
+  const uint32_t count = seg_count<PLAN>(a);
+  for (uint32_t base = gwarp * JPW; base < count; base += nwarps * JPW) {
+    const bool have = base + grp < count;
     const uint32_t job = have ? a.list[base + grp] : 0;
     const int m = have ? (int) a.q_len[job] : 0, n = have ? (int) a.t_len[job] : 0;
     const uint8_t* q = a.seqs + (have ? a.q_off[job] : 0);
@@ -367,11 +380,13 @@ __global__ void __launch_bounds__(EPL_WARPS * 32) seg_leaf_wide_kernel(SegJobs a
 }
 
 // Hirschberg split row (src/edlib.cpp:1303-1338): F = forward half column (F[i] = -fcol[i]), B = reverse half column
-// (B[i] = -bcol[m-i]); interior rows i = 1..m-1 ascending, then i = 0, then i = m. One warp per segment.
+// (B[i] = -bcol[m-i]); interior rows i = 1..m-1 ascending, then i = 0, then i = m. One warp per segment. PLAN: the segment count is
+// *plan_nseg, on the device.
+template <bool PLAN = false>
 __global__ void hb_select_kernel(const int* colbuf, const uint64_t* f_off, const uint64_t* b_off, const uint32_t* m_arr, const uint32_t* h_arr,
-                                 const uint32_t* n_arr, const int32_t* best_arr, uint32_t nseg, int32_t* out3) {
+                                 const uint32_t* n_arr, const int32_t* best_arr, uint32_t nseg, const uint32_t* plan_nseg, int32_t* out3) {
   const uint32_t w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (w >= nseg) return;
+  if (w >= (PLAN ? *plan_nseg : nseg)) return;
   const int* F = colbuf + f_off[w];
   const int* B = colbuf + b_off[w];
   const int m = (int) m_arr[w], h = (int) h_arr[w], n = (int) n_arr[w], best = best_arr[w];
@@ -447,27 +462,36 @@ struct SegRunner {
 
 // seg_kernel of each class, [0] without and [1] with equality tables, its template arguments read from SEG_GEOM
 using SegKernel = void (*)(SegJobs);
-template <bool EQ, size_t... G>
+template <bool EQ, bool PLAN, size_t... G>
 constexpr std::array<SegKernel, SEG_NCLS> seg_kernels(std::index_sequence<G...>) {
-  return {{nullptr, seg_kernel<SEG_GEOM[G + 1].C, (SEG_GEOM[G + 1].T > 32), EQ>...}};
+  return {{nullptr, seg_kernel<SEG_GEOM[G + 1].C, (SEG_GEOM[G + 1].T > 32), EQ, PLAN>...}};
 }
-constexpr std::array<SegKernel, SEG_NCLS> SEG_KERNELS[2] = {seg_kernels<false>(std::make_index_sequence<SEG_NCLS - 1>()),
-                                                            seg_kernels<true>(std::make_index_sequence<SEG_NCLS - 1>())};
+// [PLAN][eq]: the PLAN copies serve the asynchronous form
+constexpr std::array<SegKernel, SEG_NCLS> SEG_KERNELS_P[2][2] = {
+    {seg_kernels<false, false>(std::make_index_sequence<SEG_NCLS - 1>()), seg_kernels<true, false>(std::make_index_sequence<SEG_NCLS - 1>())},
+    {seg_kernels<false, true>(std::make_index_sequence<SEG_NCLS - 1>()), seg_kernels<true, true>(std::make_index_sequence<SEG_NCLS - 1>())}};
+constexpr const std::array<SegKernel, SEG_NCLS>* SEG_KERNELS = SEG_KERNELS_P[0];
 
 // seg_band_kernel of each band class (G = edb_lanes), [0] without and [1] with equality tables
-template <bool EQ, size_t... C>
+template <bool EQ, bool PLAN, size_t... C>
 constexpr std::array<SegKernel, EDB_CLASSES> segb_kernels(std::index_sequence<C...>) {
-  return {{seg_band_kernel<edb_lanes(C), EQ>...}};
+  return {{seg_band_kernel<edb_lanes(C), EQ, PLAN>...}};
 }
-constexpr std::array<SegKernel, EDB_CLASSES> SEGB_KERNELS[2] = {segb_kernels<false>(std::make_index_sequence<EDB_CLASSES>()),
-                                                                segb_kernels<true>(std::make_index_sequence<EDB_CLASSES>())};
-// the segments wider than the wavefront classes, [eq]
+constexpr std::array<SegKernel, EDB_CLASSES> SEGB_KERNELS_P[2][2] = {
+    {segb_kernels<false, false>(std::make_index_sequence<EDB_CLASSES>()), segb_kernels<true, false>(std::make_index_sequence<EDB_CLASSES>())},
+    {segb_kernels<false, true>(std::make_index_sequence<EDB_CLASSES>()), segb_kernels<true, true>(std::make_index_sequence<EDB_CLASSES>())}};
+constexpr const std::array<SegKernel, EDB_CLASSES>* SEGB_KERNELS = SEGB_KERNELS_P[0];
+// the segments wider than the wavefront classes, [PLAN][eq]
 using SegHalfKernel = void (*)(SegJobs, size_t);
-constexpr SegHalfKernel SEG_HALF_WIDE_KERNELS[2] = {seg_half_wide_kernel<false>, seg_half_wide_kernel<true>};
-constexpr SegKernel SEG_LEAF_WIDE_KERNELS[2] = {seg_leaf_wide_kernel<false>, seg_leaf_wide_kernel<true>};
+constexpr SegHalfKernel SEG_HALF_WIDE_KERNELS_P[2][2] = {{seg_half_wide_kernel<false>, seg_half_wide_kernel<true>},
+                                                         {seg_half_wide_kernel<false, true>, seg_half_wide_kernel<true, true>}};
+constexpr SegKernel SEG_LEAF_WIDE_KERNELS_P[2][2] = {{seg_leaf_wide_kernel<false>, seg_leaf_wide_kernel<true>},
+                                                     {seg_leaf_wide_kernel<false, true>, seg_leaf_wide_kernel<true, true>}};
+constexpr const SegHalfKernel* SEG_HALF_WIDE_KERNELS = SEG_HALF_WIDE_KERNELS_P[0];
+constexpr const SegKernel* SEG_LEAF_WIDE_KERNELS = SEG_LEAF_WIDE_KERNELS_P[0];
 
 // narrowest band class that holds the segment's rows and certifies the optimum `k` of the problem (pm x pn) it belongs to; -1: none
-inline int seg_band_class(uint32_t m, uint32_t pm, uint32_t pn, int32_t k) {
+__host__ __device__ inline int seg_band_class(uint32_t m, uint32_t pm, uint32_t pn, int32_t k) {
   if (k < 0) return -1;
   const int nblk = (int) ((m + 63) >> 6);
   for (int c = 0; c < EDB_CLASSES; ++c) {
@@ -477,21 +501,49 @@ inline int seg_band_class(uint32_t m, uint32_t pm, uint32_t pn, int32_t k) {
   return -1;
 }
 
-// Whether seg_kernel cannot stage m query rows in shared memory: the launch's opt-in of (m + 15) & ~15 dynamic bytes would exceed the
-// device's per-block maximum less the kernel's static shared memory, and the whole call would fail. Such half columns (Hirschberg over a
-// query of more than ~230 kb) run on seg_half_wide_kernel instead; every segment seg_kernel can launch still runs there.
-bool seg_rows_exceed(dgpu_ctx* ctx, uint32_t m, int cls, bool eq) {
-  if (ctx->seg_room.empty()) ctx->seg_room.assign(SEG_NCLS * 2, 0);
-  size_t& r = ctx->seg_room[cls * 2 + eq];   // [class][eq]: dynamic shared memory the class's seg_kernel may opt in to
-  if (!r) {
+// The dynamic shared memory each seg_kernel class may opt in to ([class], class 0 unused): the device's per-block maximum less the kernel's
+// static shared memory, asked once per context.
+const size_t* seg_rooms(dgpu_ctx* ctx, bool eq) {
+  if (ctx->seg_room.empty()) {
+    ctx->seg_room.assign(2 * SEG_NCLS, 0);
     int optin = 0;
     cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device);
-    cudaFuncAttributes fa{};
-    cudaFuncGetAttributes(&fa, (const void*) SEG_KERNELS[eq][cls]);
-    r = (size_t) optin - fa.sharedSizeBytes;
+    for (int e = 0; e < 2; ++e)
+      for (int c = 1; c < SEG_NCLS; ++c) {
+        cudaFuncAttributes fa{};
+        cudaFuncGetAttributes(&fa, (const void*) SEG_KERNELS[e][c]);
+        ctx->seg_room[e * SEG_NCLS + c] = (size_t) optin - fa.sharedSizeBytes;
+      }
   }
+  return ctx->seg_room.data() + (eq ? SEG_NCLS : 0);
+}
+
+// Whether seg_kernel cannot stage m query rows in shared memory: the launch's opt-in of (m + 15) & ~15 dynamic bytes would exceed the
+// device's per-block maximum less the kernel's static shared memory (`room`), and the whole call would fail. Such half columns (Hirschberg
+// over a query of more than ~230 kb) run on seg_half_wide_kernel instead; every segment seg_kernel can launch still runs there.
+__host__ __device__ inline bool seg_rows_exceed(uint32_t m, size_t room) {
   const size_t smem = ((size_t) m + 15) & ~(size_t) 15;
-  return smem > 48 * 1024 && smem > r;
+  return smem > 48 * 1024 && smem > room;
+}
+
+// The kernel a segment runs on: a band class that certifies its optimum (0 .. EDB_CLASSES - 1), else the wavefront class c of its width
+// (EPK_SEG + c) unless a half column's rows do not fit its shared memory, else seg_half_wide_kernel (EPK_HALF) or seg_leaf_wide_kernel
+// (EPK_LEAF); -1: a leaf of more than two row blocks and more than 16384 columns, which Hirschberg's split rule never leaves.
+constexpr int EPK_HALF = EDB_CLASSES, EPK_LEAF = EDB_CLASSES + 1, EPK_SEG = EDB_CLASSES + 1, EPK_N = EPK_SEG + SEG_NCLS;
+__host__ __device__ inline int seg_kind(uint32_t qlen, uint32_t tlen, int kind, uint32_t pm, uint32_t pn, int32_t bound, bool no_band,
+                                        const size_t* room) {
+  const int bc = no_band ? -1 : seg_band_class(qlen, pm, pn, bound);
+  if (bc >= 0) return bc;
+  const int c = seg_class(tlen);
+  if (c > 0 && !(kind == 1 && seg_rows_exceed(qlen, room[c]))) return EPK_SEG + c;
+  if (kind == 1) return EPK_HALF;
+  return qlen > 64 * EPL_G ? -1 : EPK_LEAF;
+}
+
+// development switch: no band classes (wavefront and wide kernels only)
+inline bool ep_no_band() {
+  static const bool no_band = getenv("DGPU_EP_NO_BAND") != nullptr;
+  return no_band;
 }
 
 int SegRunner::run(uint8_t* tmp_ops, int* colbuf) {
@@ -526,16 +578,15 @@ int SegRunner::run(uint8_t* tmp_ops, int* colbuf) {
   std::vector<std::vector<uint32_t> > lists(SEG_NCLS + EDB_CLASSES);
   std::vector<uint32_t> wide_half, wide_leaf;
   tail_ops.assign(N, 0);
-  static const bool no_band = getenv("DGPU_EP_NO_BAND") != nullptr;   // development switch: no band classes (wavefront and wide kernels only)
+  const bool no_band = ep_no_band();
+  const size_t* room = seg_rooms(ctx, use_eq);
   for (size_t i = 0; i < N; ++i) {
-    const int bc = no_band ? -1 : seg_band_class(qlen[i], plan_m[i], plan_n[i], bound[i]);
-    if (bc >= 0) { lists[SEG_NCLS + bc].push_back((uint32_t) i); tail_ops[i] = 1; continue; }
-    const int c = seg_class(tlen[i]);
-    if (c > 0 && !(kind[i] == 1 && seg_rows_exceed(ctx, qlen[i], c, use_eq))) { lists[c].push_back((uint32_t) i); continue; }
-    if (kind[i] == 1) { wide_half.push_back((uint32_t) i); continue; }
-    if (qlen[i] > 64 * EPL_G) return DGPU_ERR_UNSUPPORTED;   // Hirschberg's split rule leaves no such leaf
-    wide_leaf.push_back((uint32_t) i);
-    tail_ops[i] = 1;
+    const int kd = seg_kind(qlen[i], tlen[i], kind[i], plan_m[i], plan_n[i], bound[i], no_band, room);
+    if (kd < 0) return DGPU_ERR_UNSUPPORTED;
+    if (kd < EDB_CLASSES) { lists[SEG_NCLS + kd].push_back((uint32_t) i); tail_ops[i] = 1; }
+    else if (kd == EPK_HALF) wide_half.push_back((uint32_t) i);
+    else if (kd == EPK_LEAF) { wide_leaf.push_back((uint32_t) i); tail_ops[i] = 1; }
+    else lists[kd - EPK_SEG].push_back((uint32_t) i);
   }
   std::vector<uint32_t> flat;
   std::vector<size_t> lo(SEG_NCLS + 1 + EDB_CLASSES, 0);
@@ -549,7 +600,7 @@ int SegRunner::run(uint8_t* tmp_ops, int* colbuf) {
   SegJobs a;
   a.seqs = seqs; a.q_off = d_qoff; a.q_len = d_qlen; a.t_off = d_toff; a.t_len = d_tlen; a.rev = d_rev; a.kind = d_kind; a.out_off = d_oo;
   a.out_len = d_out_len; a.corner = d_corner; a.tmp_ops = tmp_ops; a.colbuf = colbuf; a.eq = eq;
-  a.plan_m = d_pm; a.plan_n = d_pn; a.eq_cls = eq_cls;
+  a.plan_m = d_pm; a.plan_n = d_pn; a.eq_cls = eq_cls; a.plan_count = nullptr;
   // One launch per kind of segment, in turn on st: band classes G = 2 .. 32, wide half columns, wide leaves, seg_kernel classes. A kind's CTA
   // takes `per_cta` jobs, each with `stride` bytes of workspace in `slot` (a wide half column's scratch row, a leaf's trace storage, a
   // seg_kernel job's directions and, from off_trace on, its trace); the grid is at most per_sm CTAs per SM, shrunk to the workspace budget.
@@ -618,7 +669,7 @@ int SegRunner::run(uint8_t* tmp_ops, int* colbuf) {
   return DGPU_OK;
 }
 
-inline bool seg_needs_split(uint32_t m, uint32_t n) {  // src/edlib.cpp:1189-1191
+__host__ __device__ inline bool seg_needs_split(uint32_t m, uint32_t n) {  // src/edlib.cpp:1189-1191
   const long long est = 20ll * ((m + 63) / 64) * n + 8ll * n;
   return est >= 1024 * 1024;
 }
@@ -641,7 +692,8 @@ int ep_locate(dgpu_ctx* ctx, cudaStream_t st, const uint8_t* seqs, uint64_t seqs
   int rc;
   const uint32_t nb = (uint32_t) ((n + 255) / 256);
   // 1. distance + first end location (k = -1 at every PATH call site of the reference); generalised equalities ride along as tables
-  if ((rc = dgpu_edit_distance_impl(ctx, seqs, seqs_bytes, q_off, q_len, t_off, t_len, nullptr, mode, n, dist, end_loc, st, 0, d_eqtabs))) return rc;
+  if ((rc = dgpu_edit_distance_impl(ctx, seqs, seqs_bytes, q_off, q_len, t_off, t_len, nullptr, mode, n, dist, end_loc, st, 0, d_eqtabs,
+                                    ctx->async_bound))) return rc;
   void* d_rev = nullptr;
   // mirror layout of the HW start pass: job i's reversed query at mq[i], its reversed target right after it, jobs back to back in runs
   // of at most EP_MIRROR_RUN bytes; each run is mirrored and searched in one SHW pass (offsets relative to the run)
@@ -685,7 +737,7 @@ int ep_locate(dgpu_ctx* ctx, cudaStream_t st, const uint8_t* seqs, uint64_t seqs
       DGPU_LAUNCH_CHECK(ctx, "ep_mirror(t)");
       if ((rc = dgpu_edit_distance_impl(ctx, (const uint8_t*) d_mirror, run_bytes[r], d_mq + j0, q_len + j0, (const uint32_t*) d_t2off + j0,
                                         (const uint32_t*) d_t2len + j0, (const int32_t*) d_k2 + j0, DGPU_MODE_SHW, cnt, start_loc + j0,
-                                        (int32_t*) d_rev + j0, st, 1, d_eqtabs))) return rc;
+                                        (int32_t*) d_rev + j0, st, 1, d_eqtabs, ctx->async_bound))) return rc;
     }
   }
   ep_start_kernel<<<nb, 256, 0, st>>>(mode, q_len, t_len, dist, end_loc, (const int32_t*) d_rev, (uint32_t) n, start_loc);
@@ -752,7 +804,8 @@ int ep_split(dgpu_ctx* ctx, cudaStream_t st, SegRunner& R, uint64_t n, std::vect
     DGPU_CUDA(ctx, cudaMemcpyAsync(d_h, sh_.data(), S * 4, cudaMemcpyHostToDevice, st));
     DGPU_CUDA(ctx, cudaMemcpyAsync(d_n, sn_.data(), S * 4, cudaMemcpyHostToDevice, st));
     DGPU_CUDA(ctx, cudaMemcpyAsync(d_best, sbest.data(), S * 4, cudaMemcpyHostToDevice, st));
-    hb_select_kernel<<<(unsigned) ((S * 32 + 255) / 256), 256, 0, st>>>((const int*) d_col, d_foff, d_boff, d_m, d_h, d_n, d_best, (uint32_t) S, d_out3);
+    hb_select_kernel<<<(unsigned) ((S * 32 + 255) / 256), 256, 0, st>>>((const int*) d_col, d_foff, d_boff, d_m, d_h, d_n, d_best, (uint32_t) S, nullptr,
+                                                                        d_out3);
     DGPU_LAUNCH_CHECK(ctx, "hb_select");
     std::vector<int32_t> out3(3 * S);
     DGPU_CUDA(ctx, cudaMemcpyAsync(out3.data(), d_out3, S * 12, cudaMemcpyDeviceToHost, st));
@@ -848,6 +901,473 @@ int ep_leaves(dgpu_ctx* ctx, cudaStream_t st, SegRunner& R, uint64_t n, std::vec
   return DGPU_OK;
 }
 
+// ---- asynchronous form (dgpu_set_ep_async_bound) --------------------------------------------------------------------------------------
+// Under a bound (max_query x max_target) the device form reads nothing back. Everything ep_locate / ep_split / ep_leaves decide on the host
+// from copied-back values is decided here by kernels, in arrays whose sizes follow from n and the bound alone:
+//   * a job's segments live in slots j << l .. (j << l) + cnt[j] - 1 at level l (a level at most doubles them), so no segment list is
+//     compacted across jobs; the number of levels is the largest any admitted slice can need (ep_bound_levels);
+//   * ep_plan_kernel (one CTA) compacts the segments that still need a split, in job order, into hb_select_kernel's inputs and two half
+//     columns each, and appends every half column to the list of the kernel that runs it (seg_kind), in that order;
+//   * the half columns of a job's segment k start at 2 ((qoff_k - q_off[j]) + k) in the job's colbuf region, a traced leaf's ops at
+//     (qoff_k - q_off[j]) + (toff_k - t_off[j]) in its tmp-ops region: the segments of a job partition its query and its slice in order;
+//   * every kind the bound can reach at a level is launched with the grid of the bound (the PLAN copies read their job count from the plan,
+//     and CTAs beyond it find no work).
+// job status while planning: 0, 2 (slice wider than max_slice), 3 (no split row / leaf distance reproduces the optimum), 4 (refused)
+struct EpBound {
+  uint32_t mq, mt;   // the bound
+  uint32_t w;        // widest slice a call traces: min(max_target, max_slice)
+  int levels;        // Hirschberg levels any admitted slice can need
+};
+
+// the number of Hirschberg levels after which no segment of at most mq rows and w columns needs a split
+inline int ep_bound_levels(uint32_t mq, uint32_t w) {
+  int l = 0;
+  while (seg_needs_split(mq, (uint32_t) ((w + (1ull << l) - 1) >> l))) ++l;
+  return l;
+}
+// the widest segment of nblk row blocks that needs no split
+inline uint32_t leaf_nmax(uint32_t nblk) { return (uint32_t) ((1024u * 1024u - 1) / (20u * nblk + 8)); }
+
+// Launch geometry of kind `id` under a bound (the largest stride any segment of that kind can need), for half columns or for leaves.
+struct BoundKind {
+  size_t per_cta; int per_sm, slot; size_t stride, off_trace; unsigned threads; size_t smem;
+  SegKernel k; SegHalfKernel half; const char* name;
+};
+BoundKind bound_kind(int id, bool leaves, bool eq, uint32_t mq, uint32_t w, const size_t* room) {
+  auto al = [](size_t x) { return (x + 255) & ~(size_t) 255; };
+  if (id < EDB_CLASSES) {   // a leaf's trace storage: one uint4 per lane and step; half columns store none
+    const int G = edb_lanes(id);
+    const size_t N = std::min(w, leaf_nmax(1));
+    const size_t steps = leaves ? 65 * ((N - 1) >> 6) + ((N - 1) & 63) + G : 0;
+    return {(size_t) (32 / G) * SEGB_WARPS, 8, SLOT_WAVEFRONT, steps * G * sizeof(uint4), 0, SEGB_WARPS * 32, 0, SEGB_KERNELS_P[1][eq][id], nullptr,
+            "seg_band_kernel"};
+  }
+  if (id == EPK_HALF)
+    return {EPW_WARPS, 4, SLOT_EP_HROW, al((w + 1) / 2), 0, EPW_WARPS * 32, 0, nullptr, SEG_HALF_WIDE_KERNELS_P[1][eq], "seg_half_wide_kernel"};
+  if (id == EPK_LEAF) {
+    const size_t cells = std::max<size_t>(std::min(w, leaf_nmax(1)), 2 * (size_t) std::min(w, leaf_nmax(2)));
+    return {(size_t) (32 / EPL_G) * EPL_WARPS, 8, SLOT_WAVEFRONT, cells * sizeof(uint4), 0, EPL_WARPS * 32, 0, SEG_LEAF_WIDE_KERNELS_P[1][eq], nullptr,
+            "seg_leaf_wide_kernel"};
+  }
+  const int c = id - EPK_SEG;
+  const SegGeom& g = SEG_GEOM[c];
+  const uint32_t N = std::min(g.cap, w);
+  size_t maxwords = 0;   // a leaf's directions: its rows and columns are bounded by mq, N and the split rule
+  for (uint32_t nb = 1; leaves && nb <= (mq + 63) / 64; ++nb)
+    maxwords = std::max(maxwords, (size_t) (std::min(mq, 64 * nb) + 1) * seg_dstride(std::min(N, leaf_nmax(nb)), g.C));
+  const size_t off_trace = al(maxwords * 4 + 1024);
+  size_t rows = ((size_t) mq + 15) & ~(size_t) 15;   // shared memory: the most rows a segment of this class stages
+  if (seg_rows_exceed(mq, room[c])) rows = room[c] & ~(size_t) 15;
+  return {1, g.per_sm, SLOT_WAVEFRONT, off_trace + al((size_t) mq + N + 64), off_trace, (unsigned) g.T, rows, SEG_KERNELS_P[1][eq][c], nullptr,
+          "seg_kernel"};
+}
+
+// The kinds the segments of a level (leaves: the leaves) can reach under the bound.
+std::vector<int> bound_kinds(EpBound const& b, int level, bool leaves, const size_t* room) {
+  std::vector<int> ids;
+  if (!ep_no_band())
+    for (int bc = 0; bc < EDB_CLASSES; ++bc) ids.push_back(bc);
+  uint32_t lo = 0, hi;   // widths of the segments
+  if (leaves) hi = std::min(b.w, leaf_nmax(1));
+  else {
+    uint32_t nmin = 1;   // narrowest segment of at most mq rows that needs a split; its half columns are at least half as wide
+    while (!seg_needs_split(b.mq, nmin)) ++nmin;
+    lo = nmin / 2;
+    hi = (uint32_t) ((b.w + (2ull << level) - 1) >> (level + 1));
+  }
+  bool wide = hi > SEG_GEOM[SEG_NCLS - 1].cap;
+  for (int c = 1; c < SEG_NCLS; ++c)
+    if (SEG_GEOM[c].cap >= lo && SEG_GEOM[c - 1].cap < hi) {
+      ids.push_back(EPK_SEG + c);
+      if (!leaves && seg_rows_exceed(b.mq, room[c])) wide = true;
+    }
+  if (wide) ids.push_back(leaves ? EPK_LEAF : EPK_HALF);
+  return ids;
+}
+
+struct EpPlan {
+  uint64_t n;
+  const uint32_t *q_off, *q_len, *t_off, *t_len;   // q_len / t_len: 0 for a refused job
+  uint32_t* jst;                                    // job status
+  // segments of the level (in) and of the next one (out), slot (j << shift) + k
+  uint32_t shift;
+  const uint32_t* cnt; const uint32_t *sq, *sql, *st, *stl; const int32_t* ssc;
+  uint32_t* cnt2; uint32_t *oq, *oql, *ot, *otl; int32_t* osc;
+  uint32_t* pre;                                    // splits before each slot, in job order (n << shift) + 1
+  // the jobs of the class kernels (half columns or leaves) and their per-kind lists
+  uint32_t *jq, *jql, *jt, *jtl, *jpm, *jpn; int32_t* jbound; uint8_t *jrev, *jkind, *jtail; uint64_t* joff;
+  uint32_t* out_len; int32_t* corner;
+  uint32_t* lists; uint64_t list_cap; uint32_t* counts;   // counts[EPK_N]: the splits of the level
+  // hb_select_kernel's inputs and outputs
+  uint64_t *f_off, *b_off; uint32_t *sm, *sh, *sn; int32_t *sbest, *out3;
+  uint64_t col_stride, tmp_stride;   // ints of colbuf, bytes of tmp ops per job
+  // leaves
+  uint32_t* leaf_lo; uint32_t* leaf_kind; uint64_t* leaf_off; uint32_t* leaf_len;
+  size_t room[SEG_NCLS]; bool no_band;
+};
+
+constexpr int EPP_THREADS = 1024;
+struct EpPlanShared { uint32_t scan[32], wc[32][EPK_N], run[EPK_N]; };
+
+// exclusive prefix of v over the CTA (EPP_THREADS threads); total: the sum
+__device__ uint32_t cta_exscan(uint32_t v, EpPlanShared& sh, uint32_t& total) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  uint32_t x = v;
+  for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
+  if (lane == 31) sh.scan[w] = x;
+  __syncthreads();
+  if (w == 0) {
+    uint32_t s = sh.scan[lane];
+    for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, s, o); if (lane >= o) s += y; }
+    sh.scan[lane] = s;
+  }
+  __syncthreads();
+  const uint32_t ex = x - v + (w ? sh.scan[w - 1] : 0);
+  total = sh.scan[31];
+  __syncthreads();
+  return ex;
+}
+
+// appends item `it` to the list of kind k (-1: none), in thread order; every thread of the CTA calls it
+__device__ void plan_append(EpPlan const& p, EpPlanShared& sh, int k, uint32_t it) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const unsigned peers = __match_any_sync(0xffffffffu, k);
+  const uint32_t rank = __popc(peers & ((1u << lane) - 1));
+  if (k >= 0 && rank == 0) sh.wc[w][k] = __popc(peers);
+  __syncthreads();
+  if (threadIdx.x < EPK_N) {
+    uint32_t s = sh.run[threadIdx.x];
+    for (int x = 0; x < 32; ++x) { const uint32_t c = sh.wc[x][threadIdx.x]; sh.wc[x][threadIdx.x] = s; s += c; }
+    sh.run[threadIdx.x] = s;
+  }
+  __syncthreads();
+  if (k >= 0) p.lists[k * p.list_cap + sh.wc[w][k] + rank] = it;
+  __syncthreads();
+  for (int i = threadIdx.x; i < 32 * EPK_N; i += EPP_THREADS) (&sh.wc[0][0])[i] = 0;
+  __syncthreads();
+}
+
+// One level of Hirschberg's recursion planned (leaves = false) or the leaves planned (leaves = true). One CTA.
+template <bool LEAVES>
+__global__ void __launch_bounds__(EPP_THREADS) ep_plan_kernel(EpPlan p) {
+  __shared__ EpPlanShared sh;
+  for (int i = threadIdx.x; i < 32 * EPK_N; i += EPP_THREADS) (&sh.wc[0][0])[i] = 0;
+  if (threadIdx.x < EPK_N) sh.run[threadIdx.x] = 0;
+  __syncthreads();
+  const uint64_t nslots = p.n << p.shift;
+  const uint32_t kmask = (1u << p.shift) - 1;
+  if (LEAVES) {
+    // every slot gets a leaf entry (an unused one an empty run), so that hb_concat_kernel finds a job's leaves at j << shift
+    for (uint64_t j = threadIdx.x; j <= p.n; j += EPP_THREADS) p.leaf_lo[j] = (uint32_t) (j << p.shift);
+    for (uint64_t b = 0; b < nslots; b += EPP_THREADS) {
+      const uint64_t i = b + threadIdx.x;
+      int kd = -1;
+      if (i < nslots) {
+        const uint32_t j = (uint32_t) (i >> p.shift), k = (uint32_t) i & kmask;
+        uint32_t lk = 1, len = 0;
+        if (k < p.cnt[j] && !p.jst[j]) {
+          const uint32_t m = p.sql[i], n = p.stl[i];
+          if (m == 0 || n == 0) { lk = m == 0 ? 2 : 1; len = m + n; }   // src/edlib.cpp:1169-1176
+          else {
+            const int32_t sc = p.ssc[i];
+            kd = seg_kind(m, n, 0, m, n, sc, p.no_band, p.room);
+            if (kd > EPK_SEG && seg_rows_exceed(m, p.room[kd - EPK_SEG])) kd = -1;   // the synchronous form fails such a launch
+            if (kd < 0) p.jst[j] = 3;   // Hirschberg's split rule leaves no such leaf
+            else {
+              lk = 0;
+              const uint64_t off = j * p.tmp_stride + (p.sq[i] - p.q_off[j]) + (p.st[i] - p.t_off[j]);
+              p.leaf_off[i] = off;
+              p.jq[i] = p.sq[i]; p.jql[i] = m; p.jt[i] = p.st[i]; p.jtl[i] = n; p.jrev[i] = 0; p.jkind[i] = 0; p.joff[i] = off;
+              p.jpm[i] = m; p.jpn[i] = n; p.jbound[i] = sc; p.jtail[i] = kd < EDB_CLASSES || kd == EPK_LEAF;
+            }
+          }
+        }
+        p.leaf_kind[i] = lk;
+        if (lk) { p.leaf_len[i] = len; p.leaf_off[i] = 0; }
+      }
+      plan_append(p, sh, kd, (uint32_t) i);
+    }
+  } else {
+    // the segments that need a split, in job order: hb_select_kernel's inputs and the two half columns of each
+    uint32_t nsplit = 0;
+    for (uint64_t b = 0; b < nslots; b += EPP_THREADS) {
+      const uint64_t i = b + threadIdx.x;
+      uint32_t need = 0, j = 0, k = 0;
+      if (i < nslots) {
+        j = (uint32_t) (i >> p.shift); k = (uint32_t) i & kmask;
+        if (k < p.cnt[j] && !p.jst[j]) { const uint32_t m = p.sql[i], n = p.stl[i]; need = m && n && seg_needs_split(m, n); }
+      }
+      uint32_t total;
+      const uint32_t s = nsplit + cta_exscan(need, sh, total);
+      if (i < nslots) p.pre[i] = s;
+      if (need) {
+        const uint32_t qo = p.sq[i], m = p.sql[i], to = p.st[i], n = p.stl[i], h = n / 2;
+        const int32_t sc = p.ssc[i];
+        const uint64_t f = j * p.col_stride + 2 * ((uint64_t) (qo - p.q_off[j]) + k), bo = f + m + 1;
+        p.f_off[s] = f; p.b_off[s] = bo; p.sm[s] = m; p.sh[s] = h; p.sn[s] = n; p.sbest[s] = sc;
+        for (int r = 0; r < 2; ++r) {
+          const uint32_t x = 2 * s + r;
+          p.jq[x] = qo; p.jql[x] = m; p.jt[x] = r ? to + h : to; p.jtl[x] = r ? n - h : h; p.jrev[x] = (uint8_t) r; p.jkind[x] = 1;
+          p.joff[x] = r ? bo : f; p.jpm[x] = m; p.jpn[x] = n; p.jbound[x] = sc;
+        }
+      }
+      nsplit += total;
+    }
+    if (threadIdx.x == 0) { p.pre[nslots] = nsplit; p.counts[EPK_N] = nsplit; }
+    __syncthreads();
+    for (uint32_t b = 0; b < 2 * nsplit; b += EPP_THREADS) {
+      const uint32_t x = b + threadIdx.x;
+      const int kd = x < 2 * nsplit ? seg_kind(p.jql[x], p.jtl[x], 1, p.jpm[x], p.jpn[x], p.jbound[x], p.no_band, p.room) : -1;
+      plan_append(p, sh, kd, x);
+    }
+  }
+  if (threadIdx.x < EPK_N) p.counts[threadIdx.x] = sh.run[threadIdx.x];
+}
+
+// every split segment replaced by its two children (hb_select_kernel's row and distances), the others copied: the next level's slots
+__global__ void ep_split_kernel(EpPlan p) {
+  const uint64_t i = (uint64_t) blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (p.n << p.shift)) return;
+  const uint32_t j = (uint32_t) (i >> p.shift), k = (uint32_t) i & ((1u << p.shift) - 1), cnt = p.cnt[j];
+  if (k == 0 && cnt == 0) p.cnt2[j] = 0;
+  if (k >= cnt) return;
+  const uint32_t pre0 = p.pre[(uint64_t) j << p.shift], s = p.pre[i], split = p.pre[i + 1] - s;
+  const uint64_t o = ((uint64_t) j << (p.shift + 1)) + k + (s - pre0);
+  const uint32_t qo = p.sq[i], m = p.sql[i], to = p.st[i], n = p.stl[i];
+  if (!split) { p.oq[o] = qo; p.oql[o] = m; p.ot[o] = to; p.otl[o] = n; p.osc[o] = p.ssc[i]; }
+  else {
+    const int32_t row = p.out3[3 * s];
+    if (row < 0) p.jst[j] = 3;   // no split row reproduces the optimum: internal error
+    else {
+      const uint32_t h = n / 2, r = (uint32_t) row;
+      p.oq[o] = qo; p.oql[o] = r; p.ot[o] = to; p.otl[o] = h; p.osc[o] = p.out3[3 * s + 1];
+      p.oq[o + 1] = qo + r; p.oql[o + 1] = m - r; p.ot[o + 1] = to + h; p.otl[o + 1] = n - h; p.osc[o + 1] = p.out3[3 * s + 2];
+    }
+  }
+  if (k == cnt - 1) p.cnt2[j] = cnt + (s + split - pre0);
+}
+
+// a traced leaf's length, the check that it reproduces the distance Hirschberg assigned to it, and the offset of ops written from the end
+// of the slot (seg_band_kernel, seg_leaf_wide_kernel)
+__global__ void ep_leaf_done_kernel(EpPlan p) {
+  const uint64_t i = (uint64_t) blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (p.n << p.shift) || p.leaf_kind[i] != 0) return;
+  const uint32_t L = p.out_len[i];
+  if (-p.corner[i] != p.jbound[i]) p.jst[i >> p.shift] = 3;
+  else if (p.jtail[i]) p.leaf_off[i] += (uint64_t) p.jql[i] + p.jtl[i] - L;
+  p.leaf_len[i] = L;
+}
+
+// refusals, the lengths every later pass reads (0 for a refused job) and the HW start-pass mirror offsets: job j at (j % run_jobs) x
+// (max_query + max_target) of its run
+__global__ void ep_async_jobs_kernel(const uint32_t* q_len, const uint32_t* t_len, uint64_t n, uint32_t mq, uint32_t mt, uint32_t run_jobs,
+                                     uint32_t* ql2, uint32_t* tl2, uint32_t* mq_off, uint32_t* mt_off, uint32_t* jst, unsigned long long* refused) {
+  const uint64_t j = (uint64_t) blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  const bool out = q_len[j] > mq || t_len[j] > mt;
+  if (out) atomicAdd(refused, 1ull);
+  ql2[j] = out ? 0 : q_len[j];
+  tl2[j] = out ? 0 : t_len[j];
+  jst[j] = out ? 4 : 0;
+  mq_off[j] = (uint32_t) (j % run_jobs) * (mq + mt);
+  mt_off[j] = mq_off[j] + mq;
+}
+
+// level 0: each job's aligned slice as its one segment (ep_split's first loop)
+__global__ void ep_seg_init_kernel(EpPlan p, const int32_t* dist, const int32_t* start_loc, const int32_t* end_loc, uint32_t max_slice) {
+  const uint64_t j = (uint64_t) blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= p.n) return;
+  uint32_t c = 0;
+  if (!p.jst[j] && p.q_len[j] && p.t_len[j] && dist[j] >= 0) {
+    const int s = start_loc[j], e = end_loc[j];
+    const uint32_t w = (uint32_t) (e - s + 1);
+    if (w > max_slice) p.jst[j] = 2;
+    else { p.oq[j] = p.q_off[j]; p.oql[j] = p.q_len[j]; p.ot[j] = p.t_off[j] + (uint32_t) s; p.otl[j] = w; p.osc[j] = dist[j]; c = 1; }
+  }
+  p.cnt2[j] = c;
+}
+
+__global__ void ep_status_kernel(const uint32_t* jst, uint64_t n, uint32_t* status, int32_t* dist, int32_t* start_loc, int32_t* end_loc, uint32_t* ops_len) {
+  const uint64_t j = (uint64_t) blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  status[j] = jst[j];
+  if (jst[j] == 4) { dist[j] = start_loc[j] = end_loc[j] = -1; ops_len[j] = 0; }
+}
+
+// the generalised-equality tables of ep_dev (f[256], s[256], cls[256 bytes]) from pairs passed by value. 256 threads.
+struct EqPairs { uint8_t p[64]; uint32_t n; };
+__global__ void ep_eqtab_kernel(EqPairs e, uint32_t* tab) {
+  const uint32_t b = threadIdx.x;
+  auto fs = [&](uint32_t x, int side) { uint32_t v = 0; for (uint32_t i = 0; i < e.n; ++i) v |= (uint32_t) (e.p[2 * i + side] == x) << i; return v; };
+  const uint32_t f = fs(b, 0), s = fs(b, 1);
+  tab[b] = f; tab[256 + b] = s;
+  const uint8_t sym[5] = {'A', 'C', 'G', 'T', 'N'};
+  uint8_t cls = 0;
+  for (int sy = 0; sy < 5; ++sy)
+    if (b == sym[sy] || (f & fs(sym[sy], 1)) || (s & fs(sym[sy], 0))) cls |= (uint8_t) (1u << sy);
+  ((uint8_t*) (tab + 512))[b] = cls;
+}
+constexpr size_t EP_EQTAB_BYTES = (512 + 64) * 4;
+
+// The kinds in `ids` on st, with the lists and counts the plan wrote. Each grid is the largest the workspace the setter reserved holds.
+int run_bound(dgpu_ctx* ctx, cudaStream_t st, SegJobs a, std::vector<int> const& ids, bool leaves, bool eq, EpBound const& b, const size_t* room,
+              const uint32_t* lists, uint64_t list_cap, const uint32_t* counts) {
+  int rc;
+  for (int id : ids) {
+    const BoundKind k = bound_kind(id, leaves, eq, b.mq, b.w, room);
+    const size_t per_block = k.per_cta * k.stride;
+    size_t grid = (size_t) ctx->num_sms * k.per_sm;
+    if (per_block) grid = std::max<size_t>(1, std::min(grid, ctx->bufs[k.slot].cap / per_block));
+    void* w;
+    if ((rc = dgpu_reserve(ctx, k.slot, std::max<size_t>(grid * per_block, 256), &w))) return rc;
+    a.work = (uint8_t*) w;
+    a.list = lists + id * list_cap;
+    a.plan_count = counts + id;
+    a.count = 0;
+    a.work_stride = k.stride;
+    a.off_trace = k.off_trace;
+    if (k.half) k.half<<<(unsigned) grid, k.threads, 0, st>>>(a, k.stride);
+    else k.k<<<(unsigned) grid, k.threads, k.smem, st>>>(a);
+    DGPU_LAUNCH_CHECK(ctx, k.name);
+  }
+  return DGPU_OK;
+}
+
+int ep_dev_async(dgpu_ctx* ctx, cudaStream_t st, const uint8_t* seqs, uint64_t seqs_bytes, const uint32_t* q_off, const uint32_t* q_len,
+                 const uint32_t* t_off, const uint32_t* t_len, int mode, const uint8_t* eq_pairs, uint32_t n_eq, uint64_t n, int32_t* dist,
+                 int32_t* start_loc, int32_t* end_loc, uint8_t* ops, const uint64_t* ops_off, uint32_t* ops_len, uint32_t* status, uint32_t max_slice) {
+  int rc;
+  EpBound b;
+  b.mq = ctx->ep_max_query; b.mt = ctx->ep_max_target; b.w = std::min(b.mt, max_slice);
+  b.levels = ep_bound_levels(b.mq, b.w);
+  const bool eq = n_eq > 0;
+  const size_t* room = seg_rooms(ctx, eq);
+  const uint64_t S = 1ull << b.levels, NS = n * S;   // segment slots per job and in all
+  const uint64_t qt = (uint64_t) b.mq + b.mt;
+  const uint32_t run_jobs = (uint32_t) std::min<uint64_t>(EP_MIRROR_RUN / qt, n);
+  const unsigned nb = (unsigned) ((n + 255) / 256), sb = (unsigned) ((NS + 255) / 256);
+
+  // the per-call arrays, all sized from n and the bound
+  void* base;
+  const size_t plan_bytes = n * 4 * 12 + NS * (4 * 10 + 4 * 19 + 8 * 3 + 3 + 4 * EPK_N) + 4 * (EPK_N + 1) + 64 * 32;
+  if ((rc = dgpu_reserve(ctx, SLOT_EP_PLAN, plan_bytes, &base))) return rc;
+  uint8_t* cur = (uint8_t*) base;
+  auto carve = [&](size_t nbytes) { uint8_t* r = cur; cur += (nbytes + 15) & ~(size_t) 15; return (void*) r; };
+  uint32_t *ql2 = (uint32_t*) carve(n * 4), *tl2 = (uint32_t*) carve(n * 4), *mq_off = (uint32_t*) carve(n * 4), *mt_off = (uint32_t*) carve(n * 4);
+  uint32_t *t2off = (uint32_t*) carve(n * 4), *t2len = (uint32_t*) carve(n * 4);
+  int32_t *k2 = (int32_t*) carve(n * 4), *rev_pos = (int32_t*) carve(n * 4);
+  uint32_t* cnt[2] = {(uint32_t*) carve(n * 4), (uint32_t*) carve(n * 4)};
+  EpPlan p;
+  p.n = n; p.q_off = q_off; p.q_len = ql2; p.t_off = t_off; p.t_len = tl2;
+  p.jst = (uint32_t*) carve(n * 4);
+  p.leaf_lo = (uint32_t*) carve((n + 1) * 4);
+  uint32_t* sq[2]; uint32_t* sql[2]; uint32_t* sto[2]; uint32_t* stl[2]; int32_t* ssc[2];
+  for (int x = 0; x < 2; ++x) {
+    sq[x] = (uint32_t*) carve(NS * 4); sql[x] = (uint32_t*) carve(NS * 4); sto[x] = (uint32_t*) carve(NS * 4); stl[x] = (uint32_t*) carve(NS * 4);
+    ssc[x] = (int32_t*) carve(NS * 4);
+  }
+  p.pre = (uint32_t*) carve((NS + 1) * 4);
+  p.jq = (uint32_t*) carve(NS * 4); p.jql = (uint32_t*) carve(NS * 4); p.jt = (uint32_t*) carve(NS * 4); p.jtl = (uint32_t*) carve(NS * 4);
+  p.jpm = (uint32_t*) carve(NS * 4); p.jpn = (uint32_t*) carve(NS * 4); p.jbound = (int32_t*) carve(NS * 4);
+  p.out_len = (uint32_t*) carve(NS * 4); p.corner = (int32_t*) carve(NS * 4);
+  p.sm = (uint32_t*) carve(NS * 4); p.sh = (uint32_t*) carve(NS * 4); p.sn = (uint32_t*) carve(NS * 4); p.sbest = (int32_t*) carve(NS * 4);
+  p.leaf_kind = (uint32_t*) carve(NS * 4); p.leaf_len = (uint32_t*) carve(NS * 4);
+  p.out3 = (int32_t*) carve(NS * 12);
+  p.joff = (uint64_t*) carve(NS * 8); p.f_off = (uint64_t*) carve(NS * 8); p.b_off = (uint64_t*) carve(NS * 8);
+  p.leaf_off = p.f_off;   // the leaves come after the last split
+  p.jrev = (uint8_t*) carve(NS); p.jkind = (uint8_t*) carve(NS); p.jtail = (uint8_t*) carve(NS);
+  p.list_cap = NS;
+  p.lists = (uint32_t*) carve(NS * 4 * EPK_N);
+  p.counts = (uint32_t*) carve(4 * (EPK_N + 1));
+  p.col_stride = 2 * ((uint64_t) b.mq + S / 2);
+  p.tmp_stride = qt;
+  for (int c = 0; c < SEG_NCLS; ++c) p.room[c] = room[c];
+  p.no_band = ep_no_band();
+  void *d_col = nullptr, *d_mirror;
+  if (b.levels && (rc = dgpu_reserve(ctx, SLOT_EP_COLS, (n * p.col_stride + 16) * sizeof(int), &d_col))) return rc;
+  if ((rc = dgpu_reserve(ctx, SLOT_EP_MIRROR, n * qt + 64, &d_mirror))) return rc;   // the HW mirror, then the traced leaves' ops
+
+  SegJobs a;
+  a.seqs = seqs; a.q_off = p.jq; a.q_len = p.jql; a.t_off = p.jt; a.t_len = p.jtl; a.rev = p.jrev; a.kind = p.jkind; a.out_off = p.joff;
+  a.out_len = p.out_len; a.corner = p.corner; a.tmp_ops = nullptr; a.colbuf = (int*) d_col; a.plan_m = p.jpm; a.plan_n = p.jpn;
+  a.eq.f = nullptr; a.eq.s = nullptr; a.eq_cls = nullptr;
+  const uint32_t* d_eqtabs = nullptr;
+  if (eq) {
+    EqPairs e;
+    for (uint32_t i = 0; i < 2 * n_eq; ++i) e.p[i] = eq_pairs[i];
+    e.n = n_eq;
+    void* d_tab;
+    if ((rc = dgpu_reserve(ctx, SLOT_EP_EQTAB, EP_EQTAB_BYTES, &d_tab))) return rc;
+    ep_eqtab_kernel<<<1, 256, 0, st>>>(e, (uint32_t*) d_tab);
+    DGPU_LAUNCH_CHECK(ctx, "ep_eqtab");
+    d_eqtabs = (const uint32_t*) d_tab;
+    a.eq.f = d_eqtabs; a.eq.s = d_eqtabs + 256; a.eq_cls = (const uint8_t*) (d_eqtabs + 512);
+  }
+
+  // distance, end and start locations (ep_locate), on the lengths with refused jobs emptied
+  ep_async_jobs_kernel<<<nb, 256, 0, st>>>(q_len, t_len, n, b.mq, b.mt, run_jobs, ql2, tl2, mq_off, mt_off, p.jst, ctx->ep_refused);
+  DGPU_LAUNCH_CHECK(ctx, "ep_async_jobs");
+  const uint32_t ed_bound = std::max(b.mq, b.mt);
+  if ((rc = dgpu_edit_distance_impl(ctx, seqs, seqs_bytes, q_off, ql2, t_off, tl2, nullptr, mode, n, dist, end_loc, st, 0, d_eqtabs, ed_bound))) return rc;
+  if (mode == DGPU_MODE_HW) {
+    ep_hwstart_jobs_kernel<<<nb, 256, 0, st>>>(mt_off, tl2, dist, end_loc, (uint32_t) n, t2off, t2len, k2);
+    DGPU_LAUNCH_CHECK(ctx, "ep_hwstart_jobs");
+    for (uint64_t j0 = 0; j0 < n; j0 += run_jobs) {   // a run reuses the mirror after the previous run's pass on the same stream
+      const uint64_t c = std::min<uint64_t>(run_jobs, n - j0);
+      const uint32_t wb = (uint32_t) ((c * 32 + 255) / 256);
+      ep_mirror_kernel<<<wb, 256, 0, st>>>(seqs, (uint8_t*) d_mirror, q_off + j0, ql2 + j0, mq_off + j0, (uint32_t) c);
+      DGPU_LAUNCH_CHECK(ctx, "ep_mirror(q)");
+      ep_mirror_kernel<<<wb, 256, 0, st>>>(seqs, (uint8_t*) d_mirror, t_off + j0, tl2 + j0, mt_off + j0, (uint32_t) c);
+      DGPU_LAUNCH_CHECK(ctx, "ep_mirror(t)");
+      if ((rc = dgpu_edit_distance_impl(ctx, (const uint8_t*) d_mirror, c * qt, mq_off + j0, ql2 + j0, t2off + j0, t2len + j0, k2 + j0, DGPU_MODE_SHW, c,
+                                        start_loc + j0, rev_pos + j0, st, 1, d_eqtabs, ed_bound))) return rc;
+    }
+  }
+  ep_start_kernel<<<nb, 256, 0, st>>>(mode, ql2, tl2, dist, end_loc, rev_pos, (uint32_t) n, start_loc);
+  DGPU_LAUNCH_CHECK(ctx, "ep_start");
+
+  // Hirschberg's levels (ep_split)
+  p.shift = 0; p.cnt2 = cnt[0]; p.oq = sq[0]; p.oql = sql[0]; p.ot = sto[0]; p.otl = stl[0]; p.osc = ssc[0];
+  ep_seg_init_kernel<<<nb, 256, 0, st>>>(p, dist, start_loc, end_loc, max_slice);
+  DGPU_LAUNCH_CHECK(ctx, "ep_seg_init");
+  int in = 0;
+  for (int l = 0; l < b.levels; ++l, in ^= 1) {
+    p.shift = (uint32_t) l;
+    p.cnt = cnt[in]; p.sq = sq[in]; p.sql = sql[in]; p.st = sto[in]; p.stl = stl[in]; p.ssc = ssc[in];
+    p.cnt2 = cnt[in ^ 1]; p.oq = sq[in ^ 1]; p.oql = sql[in ^ 1]; p.ot = sto[in ^ 1]; p.otl = stl[in ^ 1]; p.osc = ssc[in ^ 1];
+    const uint64_t slots = n << l;
+    ep_plan_kernel<false><<<1, EPP_THREADS, 0, st>>>(p);
+    DGPU_LAUNCH_CHECK(ctx, "ep_plan");
+    const std::vector<int> ids = bound_kinds(b, l, false, room);
+    if ((rc = run_bound(ctx, st, a, ids, false, eq, b, room, p.lists, p.list_cap, p.counts))) return rc;
+    hb_select_kernel<true><<<(unsigned) ((slots * 32 + 255) / 256), 256, 0, st>>>((const int*) d_col, p.f_off, p.b_off, p.sm, p.sh, p.sn, p.sbest, 0,
+                                                                               p.counts + EPK_N, p.out3);
+    DGPU_LAUNCH_CHECK(ctx, "hb_select");
+    ep_split_kernel<<<(unsigned) ((slots + 255) / 256), 256, 0, st>>>(p);
+    DGPU_LAUNCH_CHECK(ctx, "ep_split");
+  }
+
+  // the leaves (ep_leaves)
+  p.shift = (uint32_t) b.levels;
+  p.cnt = cnt[in]; p.sq = sq[in]; p.sql = sql[in]; p.st = sto[in]; p.stl = stl[in]; p.ssc = ssc[in];
+  ep_plan_kernel<true><<<1, EPP_THREADS, 0, st>>>(p);
+  DGPU_LAUNCH_CHECK(ctx, "ep_plan");
+  a.tmp_ops = (uint8_t*) d_mirror;
+  a.colbuf = nullptr;
+  dgpu_prof_begin(ctx, st);
+  const std::vector<int> leaf_ids = bound_kinds(b, 0, true, room);
+  if ((rc = run_bound(ctx, st, a, leaf_ids, true, eq, b, room, p.lists, p.list_cap, p.counts))) return rc;
+  dgpu_prof_end(ctx, st);
+  ep_leaf_done_kernel<<<sb, 256, 0, st>>>(p);
+  DGPU_LAUNCH_CHECK(ctx, "ep_leaf_done");
+  hb_concat_kernel<<<(unsigned) ((n * 32 + 255) / 256), 256, 0, st>>>((const uint8_t*) d_mirror, p.leaf_lo, p.leaf_kind, p.leaf_off, p.leaf_len,
+                                                                      (uint32_t) n, ops, ops_off, ops_len);
+  DGPU_LAUNCH_CHECK(ctx, "hb_concat");
+  ep_status_kernel<<<nb, 256, 0, st>>>(p.jst, n, status, dist, start_loc, end_loc, ops_len);
+  DGPU_LAUNCH_CHECK(ctx, "ep_status");
+  return DGPU_OK;
+}
+
 // The device form of every entry point: a job whose aligned target slice is wider than max_slice gets status 2 alone.
 int ep_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
            const uint32_t* q_off, const uint32_t* q_len, const uint32_t* t_off, const uint32_t* t_len,
@@ -861,6 +1381,9 @@ int ep_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
   if (n_eq > 32 || (n_eq && !eq_pairs)) return DGPU_ERR_ARG;
   DGPU_CUDA(ctx, cudaSetDevice(ctx->device));
   cudaStream_t st = stream ? (cudaStream_t) stream : ctx->stream;
+  if (ctx->ep_max_query)
+    return ep_dev_async(ctx, st, seqs, seqs_bytes, q_off, q_len, t_off, t_len, mode, eq_pairs, n_eq, n, dist, start_loc, end_loc, ops, ops_off, ops_len,
+                        status, max_slice);
   int rc;
   // host copies of the job geometry
   std::vector<uint32_t> h_qoff(n), h_qlen(n), h_toff(n), h_tlen(n);
@@ -927,6 +1450,50 @@ int ep_host(dgpu_ctx* ctx, const char* name, const uint8_t* seqs, uint64_t seqs_
 }  // namespace
 
 extern "C" {
+
+int dgpu_set_ep_async_bound(dgpu_ctx* ctx, uint32_t max_query, uint32_t max_target) {
+  if (!ctx) return DGPU_ERR_ARG;
+  if (!max_query && !max_target) { ctx->ep_max_query = ctx->ep_max_target = 0; return DGPU_OK; }
+  if (max_query < 1 || max_target < 1 || max_query > DGPU_EP_MAX_SLICE || max_target > DGPU_EP_MAX_SLICE) {
+    ctx->last_error = "dgpu_set_ep_async_bound: max_query and max_target must be 1 .. " + std::to_string(DGPU_EP_MAX_SLICE) + ", or both 0";
+    return DGPU_ERR_ARG;
+  }
+  DGPU_CUDA(ctx, cudaSetDevice(ctx->device));
+  if (!ctx->ep_refused) {
+    DGPU_CUDA(ctx, cudaMalloc(&ctx->ep_refused, sizeof(unsigned long long)));
+    DGPU_CUDA(ctx, cudaMemset(ctx->ep_refused, 0, sizeof(unsigned long long)));
+  }
+  // every kind any level or the leaves can reach, with or without equalities: its shared-memory opt-in and its workspace at the full grid
+  // within the budget, at least one bound-shaped slab
+  EpBound b;
+  b.mq = max_query; b.mt = b.w = max_target; b.levels = ep_bound_levels(b.mq, b.w);
+  size_t free_b = 0, total_b = 0;
+  DGPU_CUDA(ctx, cudaMemGetInfo(&free_b, &total_b));
+  std::vector<size_t> need(SLOT_COUNT, 0);
+  int rc;
+  for (int eq = 0; eq < 2; ++eq) {
+    const size_t* room = seg_rooms(ctx, eq);
+    for (int l = 0; l <= b.levels; ++l) {
+      const bool leaves = l == b.levels;
+      for (int id : bound_kinds(b, leaves ? 0 : l, leaves, room)) {
+        const BoundKind k = bound_kind(id, leaves, eq, b.mq, b.w, room);
+        const size_t per_block = k.per_cta * k.stride;
+        size_t grid = (size_t) ctx->num_sms * k.per_sm;
+        if (per_block) grid = std::max<size_t>(1, std::min(grid, dgpu_workspace_budget(ctx, k.slot, free_b) / per_block));
+        need[k.slot] = std::max(need[k.slot], std::max<size_t>(grid * per_block, 256));
+        if (!k.half && (rc = dgpu_smem_optin(ctx, k.k, k.smem, "cudaFuncSetAttribute(seg_kernel)"))) return rc;
+      }
+    }
+  }
+  need[SLOT_EP_EQTAB] = EP_EQTAB_BYTES;
+  for (int slot = 0; slot < SLOT_COUNT; ++slot) {
+    void* w;
+    if (need[slot] && (rc = dgpu_reserve(ctx, slot, need[slot], &w))) return rc;
+  }
+  ctx->ep_max_query = max_query;
+  ctx->ep_max_target = max_target;
+  return DGPU_OK;
+}
 
 int dgpu_edit_path_wide_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
                             const uint32_t* q_off, const uint32_t* q_len, const uint32_t* t_off, const uint32_t* t_len,

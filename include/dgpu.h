@@ -69,7 +69,7 @@ int dgpu_device_count(void);
 /* Number of kernel launches issued through this context so far (bench accounting). */
 uint64_t dgpu_launch_count(dgpu_ctx* ctx);
 /* jobs refused PER ITEM so far because they exceed a device limit (the call still succeeds; the item comes back flagged: ok = 0 / status != 0).
- * Refusals of longNeedle calls under dgpu_set_ln_async_bound are read from the device here (a synchronisation of the context stream):
+ * Refusals of longNeedle and edit-path calls under dgpu_set_ln_async_bound / dgpu_set_ep_async_bound are read from the device here (a synchronisation of the context stream):
  * synchronise the stream such a call was enqueued on first. */
 uint64_t dgpu_unsupported_count(dgpu_ctx* ctx);
 /* Stream-asynchronous device forms. By default dgpu_edit_distance_dev reads its job-class counts back once per call (one small D2H + stream
@@ -77,8 +77,20 @@ uint64_t dgpu_unsupported_count(dgpu_ctx* ctx);
  * later calls is longer; the call then enqueues everything on `stream` and returns without any host synchronisation (scratch buffers are sized from
  * the bound and grown only between calls; it can be followed by further work on the stream, overlapped with copies on other streams, or captured
  * into a CUDA graph once the scratch exists). 0 switches back. dgpu_long_needle[_ex]_dev and dgpu_msa[_ex]_dev have bounds of their own,
- * below; dgpu_edit_path[_ex|_wide]_dev always synchronise: they plan each Hirschberg level on the host between device rounds. */
+ * below, and so has dgpu_edit_path[_ex|_wide]_dev (dgpu_set_ep_async_bound). */
 int dgpu_set_async_bound(dgpu_ctx* ctx, uint32_t max_seq_len);
+/* The same for the edit paths. With (max_query, max_target) set, the caller guarantees that no job of a later dgpu_edit_path[_ex|_wide][_dev]
+ * call has q_len > max_query or t_len > max_target. The device forms then enqueue everything on `stream` and return without any host
+ * synchronisation, read-back or copy from host memory: the distance passes run their asynchronous branch sized from max(max_query,
+ * max_target), and every Hirschberg level is planned on the device, as many levels as the bound can need, each launching the half-column
+ * kernels the bound can reach at that level with the grid and shared memory of the bound. The setter opts those kernels in to their shared
+ * memory and reserves their workspace (within the workspace budget, at least one bound-shaped slab per kernel). The per-job scratch grows with
+ * the number of jobs, so a call may be captured into a CUDA graph after one call with at least as many jobs. A job beyond the bound is refused
+ * alone: status 4, dist = start = end = -1, ops_len = 0; the device forms count such refusals on the device, and dgpu_unsupported_count and
+ * dgpu_ctx_sync add them once the work that made them has finished. The host forms take the same path and return the same bytes. Rules:
+ * 1 <= max_query, max_target <= DGPU_EP_MAX_SLICE, else DGPU_ERR_ARG; (0, 0) switches back to the synchronous forms. The bound applies to
+ * every edit-path call of the context and leaves dgpu_set_async_bound's meaning for dgpu_edit_distance* unchanged. */
+int dgpu_set_ep_async_bound(dgpu_ctx* ctx, uint32_t max_query, uint32_t max_target);
 /* The same for longNeedle. With (max_cons, max_ref) set, the caller guarantees that no job of a later dgpu_long_needle[_ex][_dev] call has
  * c_len > max_cons or r_len > max_ref. The device forms then read nothing back: one small kernel plans the workspace on the device from the
  * batch's per-class counts and largest shapes, and every job class the bound admits is launched with the grid and shared memory of the
@@ -142,7 +154,8 @@ int dgpu_edit_distance_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_byt
  * (reserve q_len + t_len bytes), ops_len (alignmentLength). Problems above edlib's 1 MiB switch are split with
  * Hirschberg's recursion exactly like the reference (src/edlib.cpp:1189-1212, :1232-1397), so paths are identical
  * at every size. status: 0 ok; 2 = aligned target slice t[start..end] wider than DGPU_EP_CLASSIC_SLICE = 16384 columns (_wide forms: wider than
- * max_slice); the job keeps the reference's distance and locations, its path is NOT produced; 3 = internal consistency failure.
+ * max_slice); the job keeps the reference's distance and locations, its path is NOT produced; 3 = internal consistency failure;
+ * 4 = refused under dgpu_set_ep_async_bound (q_len or t_len beyond the bound): dist = start = end = -1, ops_len = 0.
  * The _ex forms take edlib's additionalEqualities (src/edlib.h:100-106) as 2*n_eq bytes (first,second pairs,
  * n_eq <= 32) in every mode — the reference's call sites are src/assemble.h:425-447 (NW, msaEdlib) and
  * src/assemble.h:663-693 (HW, msaWfa).
