@@ -31,17 +31,16 @@ struct dgpu_ctx {
   int rank = 0, world = 1;
   uint32_t async_bound = 0;  // dgpu_set_async_bound: > 0 = the caller guarantees no sequence is longer; device-form calls then never synchronise
   // dgpu_set_ln_async_bound: > 0 = no longNeedle job exceeds ln_max_cons x ln_max_ref; the device forms then plan on the device inside a
-  // workspace pool of ln_pool bytes reserved by the setter, and count their refusals in ln_refused (device, cumulative; ln_refused_folded of
-  // them are already in `unsupported`)
+  // workspace pool of ln_pool bytes reserved by the setter, and count their refusals in refused[DGPU_REFUSED_LN]
   uint32_t ln_max_cons = 0, ln_max_ref = 0;
   size_t ln_pool = 0;
-  unsigned long long* ln_refused = nullptr;
-  unsigned long long ln_refused_folded = 0;
   // dgpu_set_ep_async_bound: > 0 = no edit-path job exceeds ep_max_query x ep_max_target; the device forms then plan every Hirschberg level
-  // on the device and count their refusals in ep_refused (device, cumulative; ep_refused_folded of them are already in `unsupported`)
+  // on the device and count their refusals in refused[DGPU_REFUSED_EP]
   uint32_t ep_max_query = 0, ep_max_target = 0;
-  unsigned long long* ep_refused = nullptr;
-  unsigned long long ep_refused_folded = 0;
+  // the refusals of the bounded forms per family (device, cumulative, allocated by dgpu_refusals_init); refused_folded[f] of them are
+  // already in `unsupported`
+  unsigned long long* refused = nullptr;
+  unsigned long long refused_folded[2] = {0, 0};
   uint32_t msa_max_reads = 0;  // dgpu_set_msa_async_bound: > 0 = the MSA workspace slots are reserved for clusters of up to this many reads
   bool no_band = false;      // development switch (DGPU_ED_NO_BAND): long NW jobs straight to the full-matrix kernel
   uint64_t unsupported = 0;  // jobs refused per item because they exceed a device limit (dgpu_unsupported_count)
@@ -97,6 +96,10 @@ int dgpu_fork_init(dgpu_ctx* ctx);  // creates the fork/join pool on first use
 int dgpu_set_cuda_error(dgpu_ctx* ctx, cudaError_t e, const char* what);
 // Returns device pointer of at least `bytes` bytes in `slot` (contents NOT preserved on growth).
 int dgpu_reserve(dgpu_ctx* ctx, int slot, size_t bytes, void** out);
+// The families whose bounded forms count refusals on the device: ctx->refused[f].
+enum { DGPU_REFUSED_LN = 0, DGPU_REFUSED_EP = 1 };
+// Allocates and zeroes ctx->refused on first use (synchronises the context stream).
+int dgpu_refusals_init(dgpu_ctx* ctx);
 // Adds the longNeedle and edit-path refusals that asynchronous calls counted on the device to ctx->unsupported (synchronises the context
 // stream).
 int dgpu_fold_refusals(dgpu_ctx* ctx);

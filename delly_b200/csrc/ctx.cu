@@ -51,26 +51,31 @@ int dgpu_smem_optin_raise(dgpu_ctx* ctx, const void* kernel, size_t smem, const 
   return DGPU_OK;
 }
 
-int dgpu_fold_refusals(dgpu_ctx* ctx) {
-  if (!ctx->ln_refused && !ctx->ep_refused) return DGPU_OK;
-  unsigned long long v[2] = {0, 0};
-  DGPU_CUDA(ctx, cudaSetDevice(ctx->device));
-  if (ctx->ln_refused) DGPU_CUDA(ctx, cudaMemcpyAsync(&v[0], ctx->ln_refused, sizeof(v[0]), cudaMemcpyDeviceToHost, ctx->stream));
-  if (ctx->ep_refused) DGPU_CUDA(ctx, cudaMemcpyAsync(&v[1], ctx->ep_refused, sizeof(v[1]), cudaMemcpyDeviceToHost, ctx->stream));
+int dgpu_refusals_init(dgpu_ctx* ctx) {
+  if (ctx->refused) return DGPU_OK;
+  DGPU_CUDA(ctx, cudaMalloc(&ctx->refused, 2 * sizeof(unsigned long long)));
+  DGPU_CUDA(ctx, cudaMemsetAsync(ctx->refused, 0, 2 * sizeof(unsigned long long), ctx->stream));
   DGPU_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  if (v[0] > ctx->ln_refused_folded) {
-    const unsigned long long d = v[0] - ctx->ln_refused_folded;
+  return DGPU_OK;
+}
+
+int dgpu_fold_refusals(dgpu_ctx* ctx) {
+  if (!ctx->refused) return DGPU_OK;
+  unsigned long long v[2];
+  DGPU_CUDA(ctx, cudaSetDevice(ctx->device));
+  DGPU_CUDA(ctx, cudaMemcpyAsync(v, ctx->refused, sizeof(v), cudaMemcpyDeviceToHost, ctx->stream));
+  DGPU_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  for (int f = 0; f < 2; ++f) {
+    if (v[f] <= ctx->refused_folded[f]) continue;
+    const unsigned long long d = v[f] - ctx->refused_folded[f];
     ctx->unsupported += d;
-    ctx->ln_refused_folded = v[0];
-    ctx->last_error = "dgpu_long_needle[_ex]_dev: " + std::to_string(d) + " job(s) beyond the asynchronous bound (" + std::to_string(ctx->ln_max_cons) +
-                      " x " + std::to_string(ctx->ln_max_ref) + ") or the device limits were not aligned (ok = 0)";
-  }
-  if (v[1] > ctx->ep_refused_folded) {
-    const unsigned long long d = v[1] - ctx->ep_refused_folded;
-    ctx->unsupported += d;
-    ctx->ep_refused_folded = v[1];
-    ctx->last_error = "dgpu_edit_path[_ex|_wide]_dev: " + std::to_string(d) + " job(s) beyond the asynchronous bound (" +
-                      std::to_string(ctx->ep_max_query) + " x " + std::to_string(ctx->ep_max_target) + ") were not aligned (status 4)";
+    ctx->refused_folded[f] = v[f];
+    if (f == DGPU_REFUSED_LN)
+      ctx->last_error = "dgpu_long_needle[_ex]_dev: " + std::to_string(d) + " job(s) beyond the asynchronous bound (" + std::to_string(ctx->ln_max_cons) +
+                        " x " + std::to_string(ctx->ln_max_ref) + ") or the device limits were not aligned (ok = 0)";
+    else
+      ctx->last_error = "dgpu_edit_path[_ex|_wide]_dev: " + std::to_string(d) + " job(s) beyond the asynchronous bound (" +
+                        std::to_string(ctx->ep_max_query) + " x " + std::to_string(ctx->ep_max_target) + ") were not aligned (status 4)";
   }
   return DGPU_OK;
 }
@@ -144,8 +149,7 @@ void dgpu_ctx_destroy(dgpu_ctx* ctx) {
   cudaStreamSynchronize(ctx->stream);
   for (auto& b : ctx->bufs)
     if (b.p) cudaFree(b.p);
-  if (ctx->ln_refused) cudaFree(ctx->ln_refused);
-  if (ctx->ep_refused) cudaFree(ctx->ep_refused);
+  if (ctx->refused) cudaFree(ctx->refused);
   if (ctx->ev0) { cudaEventDestroy(ctx->ev0); cudaEventDestroy(ctx->ev1); }
   for (auto e : ctx->pipe_events) cudaEventDestroy(e);
   for (auto e : ctx->fork_events) cudaEventDestroy(e);

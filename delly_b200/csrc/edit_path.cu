@@ -470,7 +470,6 @@ constexpr std::array<SegKernel, SEG_NCLS> seg_kernels(std::index_sequence<G...>)
 constexpr std::array<SegKernel, SEG_NCLS> SEG_KERNELS_P[2][2] = {
     {seg_kernels<false, false>(std::make_index_sequence<SEG_NCLS - 1>()), seg_kernels<true, false>(std::make_index_sequence<SEG_NCLS - 1>())},
     {seg_kernels<false, true>(std::make_index_sequence<SEG_NCLS - 1>()), seg_kernels<true, true>(std::make_index_sequence<SEG_NCLS - 1>())}};
-constexpr const std::array<SegKernel, SEG_NCLS>* SEG_KERNELS = SEG_KERNELS_P[0];
 
 // seg_band_kernel of each band class (G = edb_lanes), [0] without and [1] with equality tables
 template <bool EQ, bool PLAN, size_t... C>
@@ -480,15 +479,12 @@ constexpr std::array<SegKernel, EDB_CLASSES> segb_kernels(std::index_sequence<C.
 constexpr std::array<SegKernel, EDB_CLASSES> SEGB_KERNELS_P[2][2] = {
     {segb_kernels<false, false>(std::make_index_sequence<EDB_CLASSES>()), segb_kernels<true, false>(std::make_index_sequence<EDB_CLASSES>())},
     {segb_kernels<false, true>(std::make_index_sequence<EDB_CLASSES>()), segb_kernels<true, true>(std::make_index_sequence<EDB_CLASSES>())}};
-constexpr const std::array<SegKernel, EDB_CLASSES>* SEGB_KERNELS = SEGB_KERNELS_P[0];
 // the segments wider than the wavefront classes, [PLAN][eq]
 using SegHalfKernel = void (*)(SegJobs, size_t);
 constexpr SegHalfKernel SEG_HALF_WIDE_KERNELS_P[2][2] = {{seg_half_wide_kernel<false>, seg_half_wide_kernel<true>},
                                                          {seg_half_wide_kernel<false, true>, seg_half_wide_kernel<true, true>}};
 constexpr SegKernel SEG_LEAF_WIDE_KERNELS_P[2][2] = {{seg_leaf_wide_kernel<false>, seg_leaf_wide_kernel<true>},
                                                      {seg_leaf_wide_kernel<false, true>, seg_leaf_wide_kernel<true, true>}};
-constexpr const SegHalfKernel* SEG_HALF_WIDE_KERNELS = SEG_HALF_WIDE_KERNELS_P[0];
-constexpr const SegKernel* SEG_LEAF_WIDE_KERNELS = SEG_LEAF_WIDE_KERNELS_P[0];
 
 // narrowest band class that holds the segment's rows and certifies the optimum `k` of the problem (pm x pn) it belongs to; -1: none
 __host__ __device__ inline int seg_band_class(uint32_t m, uint32_t pm, uint32_t pn, int32_t k) {
@@ -511,7 +507,7 @@ const size_t* seg_rooms(dgpu_ctx* ctx, bool eq) {
     for (int e = 0; e < 2; ++e)
       for (int c = 1; c < SEG_NCLS; ++c) {
         cudaFuncAttributes fa{};
-        cudaFuncGetAttributes(&fa, (const void*) SEG_KERNELS[e][c]);
+        cudaFuncGetAttributes(&fa, (const void*) SEG_KERNELS_P[0][e][c]);
         ctx->seg_room[e * SEG_NCLS + c] = (size_t) optin - fa.sharedSizeBytes;
       }
   }
@@ -538,6 +534,68 @@ __host__ __device__ inline int seg_kind(uint32_t qlen, uint32_t tlen, int kind, 
   if (c > 0 && !(kind == 1 && seg_rows_exceed(qlen, room[c]))) return EPK_SEG + c;
   if (kind == 1) return EPK_HALF;
   return qlen > 64 * EPL_G ? -1 : EPK_LEAF;
+}
+// whether kind k writes a traced leaf's ops from the end of its slot (seg_band_kernel, seg_leaf_wide_kernel)
+__host__ __device__ inline bool seg_kind_tail(int k) { return k < EDB_CLASSES || k == EPK_LEAF; }
+
+// The largest extents the jobs of one kind can have (0 where its jobs need none: half columns store no trace and no directions): a traced
+// leaf's columns (band classes), a leaf's trace cells of one uint4 per row block and column (seg_leaf_wide_kernel), a half column's width
+// (seg_half_wide_kernel), a leaf's direction words, the rows staged in shared memory and m + n (seg_kernel).
+struct SegExtent { size_t cols, cells, half, words, rows, mn; };
+
+// Launch geometry of kind `id`: a CTA takes `per_cta` jobs, each with `stride` bytes of workspace in `slot` (a wide half column's scratch
+// row, a leaf's trace storage, a seg_kernel job's directions and, from off_trace on, its trace); the grid is at most per_sm CTAs per SM.
+struct SegKindGeom {
+  size_t per_cta; int per_sm, slot; size_t stride, off_trace; unsigned threads; size_t smem;
+  SegKernel k; SegHalfKernel half;   // seg_half_wide_kernel (half) takes the stride as its row stride
+  const char* name;
+};
+SegKindGeom seg_kind_geom(int id, bool eq, bool plan, SegExtent const& x) {
+  auto al = [](size_t v) { return (v + 255) & ~(size_t) 255; };
+  if (id < EDB_CLASSES) {   // a leaf's trace storage: one uint4 per lane and step
+    const int G = edb_lanes(id);
+    const size_t steps = x.cols ? 65 * ((x.cols - 1) >> 6) + ((x.cols - 1) & 63) + G : 0;
+    return {(size_t) (32 / G) * SEGB_WARPS, 8, SLOT_WAVEFRONT, steps * G * sizeof(uint4), 0, SEGB_WARPS * 32, 0, SEGB_KERNELS_P[plan][eq][id], nullptr,
+            "seg_band_kernel"};
+  }
+  if (id == EPK_HALF)   // one warp per half column, a scratch row of n bytes per warp
+    return {EPW_WARPS, 4, SLOT_EP_HROW, al(x.half), 0, EPW_WARPS * 32, 0, nullptr, SEG_HALF_WIDE_KERNELS_P[plan][eq], "seg_half_wide_kernel"};
+  if (id == EPK_LEAF)
+    return {(size_t) (32 / EPL_G) * EPL_WARPS, 8, SLOT_WAVEFRONT, x.cells * sizeof(uint4), 0, EPL_WARPS * 32, 0, SEG_LEAF_WIDE_KERNELS_P[plan][eq], nullptr,
+            "seg_leaf_wide_kernel"};
+  const SegGeom& g = SEG_GEOM[id - EPK_SEG];
+  const size_t off_trace = al(x.words * 4 + 1024);
+  return {1, g.per_sm, SLOT_WAVEFRONT, off_trace + al(x.mn + 64), off_trace, (unsigned) g.T, (x.rows + 15) & ~(size_t) 15,
+          SEG_KERNELS_P[plan][eq][id - EPK_SEG], nullptr, "seg_kernel"};
+}
+
+// The grid of kind k: at most `ctas` CTAs and per_sm per SM, cut to the CTAs whose workspace `avail` bytes of its slot hold (at least one).
+size_t seg_grid(const dgpu_ctx* ctx, SegKindGeom const& k, size_t ctas, size_t avail) {
+  size_t grid = std::min(ctas, (size_t) ctx->num_sms * k.per_sm);
+  const size_t per_block = k.per_cta * k.stride;
+  if (per_block) grid = std::max<size_t>(1, std::min(grid, avail / per_block));
+  return grid;
+}
+
+// Kind k on st over `list`, with seg_grid's grid and its workspace reserved: `count` jobs, or the PLAN copies the count the plan wrote at
+// plan_count.
+int seg_launch(dgpu_ctx* ctx, cudaStream_t st, SegJobs a, SegKindGeom const& k, size_t ctas, size_t avail, const uint32_t* list, uint32_t count,
+               const uint32_t* plan_count) {
+  int rc;
+  const size_t grid = seg_grid(ctx, k, ctas, avail);
+  void* w;   // at least 256 bytes: a band class of half columns alone stores no trace (the other kinds always take more)
+  if ((rc = dgpu_reserve(ctx, k.slot, std::max<size_t>(grid * k.per_cta * k.stride, 256), &w))) return rc;
+  a.work = (uint8_t*) w;
+  a.list = list;
+  a.count = count;
+  a.plan_count = plan_count;
+  a.work_stride = k.stride;
+  a.off_trace = k.off_trace;
+  if (!k.half && (rc = dgpu_smem_optin(ctx, k.k, k.smem, "cudaFuncSetAttribute(seg_kernel)"))) return rc;
+  if (k.half) k.half<<<(unsigned) grid, k.threads, 0, st>>>(a, k.stride);
+  else k.k<<<(unsigned) grid, k.threads, k.smem, st>>>(a);
+  DGPU_LAUNCH_CHECK(ctx, k.name);
+  return DGPU_OK;
 }
 
 // development switch: no band classes (wavefront and wide kernels only)
@@ -572,99 +630,47 @@ int SegRunner::run(uint8_t* tmp_ops, int* colbuf) {
   DGPU_CUDA(ctx, cudaMemcpyAsync(d_oo, out_off.data(), N * 8, cudaMemcpyHostToDevice, st));
   DGPU_CUDA(ctx, cudaMemcpyAsync(d_rev, rev.data(), N, cudaMemcpyHostToDevice, st));
   DGPU_CUDA(ctx, cudaMemcpyAsync(d_kind, kind.data(), N, cudaMemcpyHostToDevice, st));
-  // class lists
-  // lists[1..11]: wavefront classes by target length (SEG_GEOM); lists[12..16]: band classes G = 2, 4, 8, 16, 32
-  // wide_half / wide_leaf: unbanded segments wider than the wavefront classes (seg_half_wide_kernel, seg_leaf_wide_kernel)
-  std::vector<std::vector<uint32_t> > lists(SEG_NCLS + EDB_CLASSES);
-  std::vector<uint32_t> wide_half, wide_leaf;
+  // the jobs of each kind (seg_kind), listed back to back in d_list in kind order
+  std::vector<std::vector<uint32_t> > lists(EPK_N);
   tail_ops.assign(N, 0);
   const bool no_band = ep_no_band();
   const size_t* room = seg_rooms(ctx, use_eq);
   for (size_t i = 0; i < N; ++i) {
     const int kd = seg_kind(qlen[i], tlen[i], kind[i], plan_m[i], plan_n[i], bound[i], no_band, room);
     if (kd < 0) return DGPU_ERR_UNSUPPORTED;
-    if (kd < EDB_CLASSES) { lists[SEG_NCLS + kd].push_back((uint32_t) i); tail_ops[i] = 1; }
-    else if (kd == EPK_HALF) wide_half.push_back((uint32_t) i);
-    else if (kd == EPK_LEAF) { wide_leaf.push_back((uint32_t) i); tail_ops[i] = 1; }
-    else lists[kd - EPK_SEG].push_back((uint32_t) i);
+    lists[kd].push_back((uint32_t) i);
+    tail_ops[i] = seg_kind_tail(kd);
   }
   std::vector<uint32_t> flat;
-  std::vector<size_t> lo(SEG_NCLS + 1 + EDB_CLASSES, 0);
-  for (int c = 1; c < SEG_NCLS + EDB_CLASSES; ++c) { lo[c] = flat.size(); flat.insert(flat.end(), lists[c].begin(), lists[c].end()); }
-  lo[SEG_NCLS + EDB_CLASSES] = flat.size();
-  const size_t lo_half = flat.size();
-  flat.insert(flat.end(), wide_half.begin(), wide_half.end());
-  const size_t lo_leaf = flat.size();
-  flat.insert(flat.end(), wide_leaf.begin(), wide_leaf.end());
+  for (std::vector<uint32_t> const& L : lists) flat.insert(flat.end(), L.begin(), L.end());
   DGPU_CUDA(ctx, cudaMemcpyAsync(d_list, flat.data(), flat.size() * 4, cudaMemcpyHostToDevice, st));
   SegJobs a;
   a.seqs = seqs; a.q_off = d_qoff; a.q_len = d_qlen; a.t_off = d_toff; a.t_len = d_tlen; a.rev = d_rev; a.kind = d_kind; a.out_off = d_oo;
   a.out_len = d_out_len; a.corner = d_corner; a.tmp_ops = tmp_ops; a.colbuf = colbuf; a.eq = eq;
-  a.plan_m = d_pm; a.plan_n = d_pn; a.eq_cls = eq_cls; a.plan_count = nullptr;
-  // One launch per kind of segment, in turn on st: band classes G = 2 .. 32, wide half columns, wide leaves, seg_kernel classes. A kind's CTA
-  // takes `per_cta` jobs, each with `stride` bytes of workspace in `slot` (a wide half column's scratch row, a leaf's trace storage, a
-  // seg_kernel job's directions and, from off_trace on, its trace); the grid is at most per_sm CTAs per SM, shrunk to the workspace budget.
-  struct Kind {
-    const std::vector<uint32_t>* jobs; size_t lo;   // the jobs and their offset in d_list
-    size_t per_cta; int per_sm, slot; size_t stride, off_trace; unsigned threads; size_t smem;
-    SegKernel k; SegHalfKernel half;                 // seg_half_wide_kernel (half) takes the stride as its row stride
-    const char* name;
-  };
-  std::vector<Kind> kinds;
-  for (int bc = 0; bc < EDB_CLASSES; ++bc) {
-    std::vector<uint32_t> const& L = lists[SEG_NCLS + bc];
-    if (L.empty()) continue;
-    const int G = edb_lanes(bc), jpw = 32 / G;
-    size_t maxsteps = 0;   // trace storage of a leaf: one uint4 per lane and step
-    for (uint32_t i : L)
-      if (kind[i] == 0) maxsteps = std::max<size_t>(maxsteps, 65 * (size_t) ((tlen[i] - 1) >> 6) + ((tlen[i] - 1) & 63) + G);
-    kinds.push_back({&L, lo[SEG_NCLS + bc], (size_t) jpw * SEGB_WARPS, 8, SLOT_WAVEFRONT, maxsteps * G * sizeof(uint4), 0, SEGB_WARPS * 32, 0,
-                     SEGB_KERNELS[use_eq][bc], nullptr, "seg_band_kernel"});
-  }
-  if (!wide_half.empty()) {   // one warp per half column, a scratch row of n bytes per warp
-    size_t nmax = 0;
-    for (uint32_t i : wide_half) nmax = std::max<size_t>(nmax, tlen[i]);
-    kinds.push_back({&wide_half, lo_half, EPW_WARPS, 4, SLOT_EP_HROW, (nmax + 255) & ~(size_t) 255, 0, EPW_WARPS * 32, 0, nullptr,
-                     SEG_HALF_WIDE_KERNELS[use_eq], "seg_half_wide_kernel"});
-  }
-  if (!wide_leaf.empty()) {   // trace storage of a leaf: one uint4 per block and column
-    size_t maxcells = 0;
-    for (uint32_t i : wide_leaf) maxcells = std::max<size_t>(maxcells, (size_t) tlen[i] * ((qlen[i] + 63) >> 6));
-    kinds.push_back({&wide_leaf, lo_leaf, (size_t) (32 / EPL_G) * EPL_WARPS, 8, SLOT_WAVEFRONT, maxcells * sizeof(uint4), 0, EPL_WARPS * 32, 0,
-                     SEG_LEAF_WIDE_KERNELS[use_eq], nullptr, "seg_leaf_wide_kernel"});
-  }
-  for (int c = 1; c < SEG_NCLS; ++c) {
-    if (lists[c].empty()) continue;
-    const SegGeom& g = SEG_GEOM[c];
-    size_t maxwords = 0, mmax = 0, mnmax = 0;
-    for (uint32_t i : lists[c]) {
-      if (kind[i] == 0) maxwords = std::max(maxwords, (size_t) (qlen[i] + 1) * seg_dstride(tlen[i], g.C));   // half columns store no directions
-      mmax = std::max<size_t>(mmax, qlen[i]);
-      mnmax = std::max<size_t>(mnmax, (size_t) qlen[i] + tlen[i]);
-    }
-    auto al = [](size_t x) { return (x + 255) & ~(size_t) 255; };
-    const size_t off_trace = al(maxwords * 4 + 1024);
-    kinds.push_back({&lists[c], lo[c], 1, g.per_sm, SLOT_WAVEFRONT, off_trace + al(mnmax + 64), off_trace, (unsigned) g.T, (mmax + 15) & ~(size_t) 15,
-                     SEG_KERNELS[use_eq][c], nullptr, "seg_kernel"});
-  }
+  a.plan_m = d_pm; a.plan_n = d_pn; a.eq_cls = eq_cls;
+  // One launch per non-empty kind, in turn on st: band classes G = 2 .. 32, wide half columns, wide leaves, seg_kernel classes; the geometry
+  // of the largest extents its jobs have, the grid shrunk to the workspace budget.
   size_t free_b = 0, total_b = 0;
   cudaMemGetInfo(&free_b, &total_b);
-  for (Kind const& k : kinds) {
-    size_t grid = std::min<size_t>((k.jobs->size() + k.per_cta - 1) / k.per_cta, (size_t) ctx->num_sms * k.per_sm);
-    const size_t per_block = k.per_cta * k.stride;
-    const size_t budget = dgpu_workspace_budget(ctx, k.slot, free_b);
-    if (per_block && grid * per_block > budget) grid = std::max<size_t>(1, budget / per_block);
-    void* w;   // at least 256 bytes: a band class of half columns alone stores no trace (the other kinds always take more)
-    if ((rc = dgpu_reserve(ctx, k.slot, std::max<size_t>(grid * per_block, 256), &w))) return rc;
-    a.work = (uint8_t*) w;
-    a.list = d_list + k.lo;
-    a.count = (uint32_t) k.jobs->size();
-    a.work_stride = k.stride;
-    a.off_trace = k.off_trace;
-    if (!k.half && (rc = dgpu_smem_optin(ctx, k.k, k.smem, "cudaFuncSetAttribute(seg_kernel)"))) return rc;
-    if (k.half) k.half<<<(unsigned) grid, k.threads, 0, st>>>(a, k.stride);
-    else k.k<<<(unsigned) grid, k.threads, k.smem, st>>>(a);
-    DGPU_LAUNCH_CHECK(ctx, k.name);
+  size_t lo = 0;
+  for (int id = 0; id < EPK_N; lo += lists[id].size(), ++id) {
+    std::vector<uint32_t> const& L = lists[id];
+    if (L.empty()) continue;
+    SegExtent x{};
+    for (uint32_t i : L) {
+      if (kind[i] == 0) {   // leaves
+        x.cols = std::max<size_t>(x.cols, tlen[i]);
+        x.cells = std::max<size_t>(x.cells, (size_t) tlen[i] * ((qlen[i] + 63) >> 6));
+        if (id > EPK_SEG) x.words = std::max(x.words, (size_t) (qlen[i] + 1) * seg_dstride(tlen[i], SEG_GEOM[id - EPK_SEG].C));
+      }
+      x.half = std::max<size_t>(x.half, tlen[i]);
+      x.rows = std::max<size_t>(x.rows, qlen[i]);
+      x.mn = std::max<size_t>(x.mn, (size_t) qlen[i] + tlen[i]);
+    }
+    const SegKindGeom k = seg_kind_geom(id, use_eq, false, x);
+    if ((rc = seg_launch(ctx, st, a, k, (L.size() + k.per_cta - 1) / k.per_cta, dgpu_workspace_budget(ctx, k.slot, free_b), d_list + lo,
+                         (uint32_t) L.size(), nullptr)))
+      return rc;
   }
   return DGPU_OK;
 }
@@ -928,38 +934,23 @@ inline int ep_bound_levels(uint32_t mq, uint32_t w) {
 // the widest segment of nblk row blocks that needs no split
 inline uint32_t leaf_nmax(uint32_t nblk) { return (uint32_t) ((1024u * 1024u - 1) / (20u * nblk + 8)); }
 
-// Launch geometry of kind `id` under a bound (the largest stride any segment of that kind can need), for half columns or for leaves.
-struct BoundKind {
-  size_t per_cta; int per_sm, slot; size_t stride, off_trace; unsigned threads; size_t smem;
-  SegKernel k; SegHalfKernel half; const char* name;
-};
-BoundKind bound_kind(int id, bool leaves, bool eq, uint32_t mq, uint32_t w, const size_t* room) {
-  auto al = [](size_t x) { return (x + 255) & ~(size_t) 255; };
-  if (id < EDB_CLASSES) {   // a leaf's trace storage: one uint4 per lane and step; half columns store none
-    const int G = edb_lanes(id);
-    const size_t N = std::min(w, leaf_nmax(1));
-    const size_t steps = leaves ? 65 * ((N - 1) >> 6) + ((N - 1) & 63) + G : 0;
-    return {(size_t) (32 / G) * SEGB_WARPS, 8, SLOT_WAVEFRONT, steps * G * sizeof(uint4), 0, SEGB_WARPS * 32, 0, SEGB_KERNELS_P[1][eq][id], nullptr,
-            "seg_band_kernel"};
+// Launch geometry (PLAN copies) of kind `id` under a bound: the largest extents any segment of that kind can have, for half columns or for
+// leaves.
+SegKindGeom bound_kind(int id, bool leaves, bool eq, uint32_t mq, uint32_t w, const size_t* room) {
+  SegExtent x{};
+  if (id < EDB_CLASSES) x.cols = leaves ? std::min(w, leaf_nmax(1)) : 0;
+  else if (id == EPK_HALF) x.half = (w + 1) / 2;
+  else if (id == EPK_LEAF) x.cells = std::max<size_t>(std::min(w, leaf_nmax(1)), 2 * (size_t) std::min(w, leaf_nmax(2)));
+  else {
+    const int c = id - EPK_SEG;
+    const SegGeom& g = SEG_GEOM[c];
+    const uint32_t N = std::min(g.cap, w);
+    for (uint32_t nb = 1; leaves && nb <= (mq + 63) / 64; ++nb)   // a leaf's rows and columns are bounded by mq, N and the split rule
+      x.words = std::max(x.words, (size_t) (std::min(mq, 64 * nb) + 1) * seg_dstride(std::min(N, leaf_nmax(nb)), g.C));
+    x.rows = seg_rows_exceed(mq, room[c]) ? room[c] & ~(size_t) 15 : mq;   // the most rows a segment of this class stages
+    x.mn = (size_t) mq + N;
   }
-  if (id == EPK_HALF)
-    return {EPW_WARPS, 4, SLOT_EP_HROW, al((w + 1) / 2), 0, EPW_WARPS * 32, 0, nullptr, SEG_HALF_WIDE_KERNELS_P[1][eq], "seg_half_wide_kernel"};
-  if (id == EPK_LEAF) {
-    const size_t cells = std::max<size_t>(std::min(w, leaf_nmax(1)), 2 * (size_t) std::min(w, leaf_nmax(2)));
-    return {(size_t) (32 / EPL_G) * EPL_WARPS, 8, SLOT_WAVEFRONT, cells * sizeof(uint4), 0, EPL_WARPS * 32, 0, SEG_LEAF_WIDE_KERNELS_P[1][eq], nullptr,
-            "seg_leaf_wide_kernel"};
-  }
-  const int c = id - EPK_SEG;
-  const SegGeom& g = SEG_GEOM[c];
-  const uint32_t N = std::min(g.cap, w);
-  size_t maxwords = 0;   // a leaf's directions: its rows and columns are bounded by mq, N and the split rule
-  for (uint32_t nb = 1; leaves && nb <= (mq + 63) / 64; ++nb)
-    maxwords = std::max(maxwords, (size_t) (std::min(mq, 64 * nb) + 1) * seg_dstride(std::min(N, leaf_nmax(nb)), g.C));
-  const size_t off_trace = al(maxwords * 4 + 1024);
-  size_t rows = ((size_t) mq + 15) & ~(size_t) 15;   // shared memory: the most rows a segment of this class stages
-  if (seg_rows_exceed(mq, room[c])) rows = room[c] & ~(size_t) 15;
-  return {1, g.per_sm, SLOT_WAVEFRONT, off_trace + al((size_t) mq + N + 64), off_trace, (unsigned) g.T, rows, SEG_KERNELS_P[1][eq][c], nullptr,
-          "seg_kernel"};
+  return seg_kind_geom(id, eq, true, x);
 }
 
 // The kinds the segments of a level (leaves: the leaves) can reach under the bound.
@@ -1078,7 +1069,7 @@ __global__ void __launch_bounds__(EPP_THREADS) ep_plan_kernel(EpPlan p) {
               const uint64_t off = j * p.tmp_stride + (p.sq[i] - p.q_off[j]) + (p.st[i] - p.t_off[j]);
               p.leaf_off[i] = off;
               p.jq[i] = p.sq[i]; p.jql[i] = m; p.jt[i] = p.st[i]; p.jtl[i] = n; p.jrev[i] = 0; p.jkind[i] = 0; p.joff[i] = off;
-              p.jpm[i] = m; p.jpn[i] = n; p.jbound[i] = sc; p.jtail[i] = kd < EDB_CLASSES || kd == EPK_LEAF;
+              p.jpm[i] = m; p.jpn[i] = n; p.jbound[i] = sc; p.jtail[i] = seg_kind_tail(kd);
             }
           }
         }
@@ -1209,26 +1200,27 @@ __global__ void ep_eqtab_kernel(EqPairs e, uint32_t* tab) {
 }
 constexpr size_t EP_EQTAB_BYTES = (512 + 64) * 4;
 
+// The equality tables of n_eq > 0 pairs, built on st into SLOT_EP_EQTAB; *tab: f[256], s[256], cls[256 bytes].
+int ep_eqtabs(dgpu_ctx* ctx, cudaStream_t st, const uint8_t* eq_pairs, uint32_t n_eq, const uint32_t** tab) {
+  EqPairs e;
+  for (uint32_t i = 0; i < 2 * n_eq; ++i) e.p[i] = eq_pairs[i];
+  e.n = n_eq;
+  void* d_tab;
+  int rc;
+  if ((rc = dgpu_reserve(ctx, SLOT_EP_EQTAB, EP_EQTAB_BYTES, &d_tab))) return rc;
+  ep_eqtab_kernel<<<1, 256, 0, st>>>(e, (uint32_t*) d_tab);
+  DGPU_LAUNCH_CHECK(ctx, "ep_eqtab");
+  *tab = (const uint32_t*) d_tab;
+  return DGPU_OK;
+}
+
 // The kinds in `ids` on st, with the lists and counts the plan wrote. Each grid is the largest the workspace the setter reserved holds.
 int run_bound(dgpu_ctx* ctx, cudaStream_t st, SegJobs a, std::vector<int> const& ids, bool leaves, bool eq, EpBound const& b, const size_t* room,
               const uint32_t* lists, uint64_t list_cap, const uint32_t* counts) {
   int rc;
   for (int id : ids) {
-    const BoundKind k = bound_kind(id, leaves, eq, b.mq, b.w, room);
-    const size_t per_block = k.per_cta * k.stride;
-    size_t grid = (size_t) ctx->num_sms * k.per_sm;
-    if (per_block) grid = std::max<size_t>(1, std::min(grid, ctx->bufs[k.slot].cap / per_block));
-    void* w;
-    if ((rc = dgpu_reserve(ctx, k.slot, std::max<size_t>(grid * per_block, 256), &w))) return rc;
-    a.work = (uint8_t*) w;
-    a.list = lists + id * list_cap;
-    a.plan_count = counts + id;
-    a.count = 0;
-    a.work_stride = k.stride;
-    a.off_trace = k.off_trace;
-    if (k.half) k.half<<<(unsigned) grid, k.threads, 0, st>>>(a, k.stride);
-    else k.k<<<(unsigned) grid, k.threads, k.smem, st>>>(a);
-    DGPU_LAUNCH_CHECK(ctx, k.name);
+    const SegKindGeom k = bound_kind(id, leaves, eq, b.mq, b.w, room);
+    if ((rc = seg_launch(ctx, st, a, k, SIZE_MAX, ctx->bufs[k.slot].cap, lists + id * list_cap, 0, counts + id))) return rc;
   }
   return DGPU_OK;
 }
@@ -1293,19 +1285,12 @@ int ep_dev_async(dgpu_ctx* ctx, cudaStream_t st, const uint8_t* seqs, uint64_t s
   a.eq.f = nullptr; a.eq.s = nullptr; a.eq_cls = nullptr;
   const uint32_t* d_eqtabs = nullptr;
   if (eq) {
-    EqPairs e;
-    for (uint32_t i = 0; i < 2 * n_eq; ++i) e.p[i] = eq_pairs[i];
-    e.n = n_eq;
-    void* d_tab;
-    if ((rc = dgpu_reserve(ctx, SLOT_EP_EQTAB, EP_EQTAB_BYTES, &d_tab))) return rc;
-    ep_eqtab_kernel<<<1, 256, 0, st>>>(e, (uint32_t*) d_tab);
-    DGPU_LAUNCH_CHECK(ctx, "ep_eqtab");
-    d_eqtabs = (const uint32_t*) d_tab;
+    if ((rc = ep_eqtabs(ctx, st, eq_pairs, n_eq, &d_eqtabs))) return rc;
     a.eq.f = d_eqtabs; a.eq.s = d_eqtabs + 256; a.eq_cls = (const uint8_t*) (d_eqtabs + 512);
   }
 
   // distance, end and start locations (ep_locate), on the lengths with refused jobs emptied
-  ep_async_jobs_kernel<<<nb, 256, 0, st>>>(q_len, t_len, n, b.mq, b.mt, run_jobs, ql2, tl2, mq_off, mt_off, p.jst, ctx->ep_refused);
+  ep_async_jobs_kernel<<<nb, 256, 0, st>>>(q_len, t_len, n, b.mq, b.mt, run_jobs, ql2, tl2, mq_off, mt_off, p.jst, ctx->refused + DGPU_REFUSED_EP);
   DGPU_LAUNCH_CHECK(ctx, "ep_async_jobs");
   const uint32_t ed_bound = std::max(b.mq, b.mt);
   if ((rc = dgpu_edit_distance_impl(ctx, seqs, seqs_bytes, q_off, ql2, t_off, tl2, nullptr, mode, n, dist, end_loc, st, 0, d_eqtabs, ed_bound))) return rc;
@@ -1395,21 +1380,10 @@ int ep_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes,
   DGPU_CUDA(ctx, cudaMemcpyAsync(h_opsoff.data(), ops_off, n * 8, cudaMemcpyDeviceToHost, st));
   SegRunner R;
   R.ctx = ctx; R.st = st; R.seqs = seqs; R.use_eq = n_eq > 0; R.eq.f = nullptr; R.eq.s = nullptr;
-  const uint32_t* d_eqtabs = nullptr;  // f[256], s[256], cls[256 bytes]
+  const uint32_t* d_eqtabs = nullptr;
   if (n_eq) {
-    uint32_t tab[512 + 64] = {0};
-    for (uint32_t p = 0; p < n_eq; ++p) { tab[eq_pairs[2 * p]] |= 1u << p; tab[256 + eq_pairs[2 * p + 1]] |= 1u << p; }
-    uint8_t* cls = (uint8_t*) (tab + 512);
-    static const uint8_t sym[5] = {'A', 'C', 'G', 'T', 'N'};
-    for (uint32_t b = 0; b < 256; ++b)
-      for (int sy = 0; sy < 5; ++sy)
-        if (b == sym[sy] || (tab[b] & tab[256 + sym[sy]]) || (tab[256 + b] & tab[sym[sy]])) cls[b] |= (uint8_t) (1u << sy);
-    void* d_tab;
-    if ((rc = dgpu_reserve(ctx, SLOT_EP_EQTAB, sizeof(tab), &d_tab))) return rc;
-    DGPU_CUDA(ctx, cudaMemcpyAsync(d_tab, tab, sizeof(tab), cudaMemcpyHostToDevice, st));
-    DGPU_CUDA(ctx, cudaStreamSynchronize(st));  // tab is a stack array
-    R.eq.f = (const uint32_t*) d_tab; R.eq.s = (const uint32_t*) d_tab + 256; R.eq_cls = (const uint8_t*) ((const uint32_t*) d_tab + 512);
-    d_eqtabs = (const uint32_t*) d_tab;
+    if ((rc = ep_eqtabs(ctx, st, eq_pairs, n_eq, &d_eqtabs))) return rc;
+    R.eq.f = d_eqtabs; R.eq.s = d_eqtabs + 256; R.eq_cls = (const uint8_t*) (d_eqtabs + 512);
   }
   std::vector<int32_t> h_dist(n), h_start(n), h_end(n);
   if ((rc = ep_locate(ctx, st, seqs, seqs_bytes, q_off, q_len, t_off, t_len, mode, d_eqtabs, n, h_qlen, h_tlen, dist, start_loc, end_loc, h_dist,
@@ -1459,10 +1433,8 @@ int dgpu_set_ep_async_bound(dgpu_ctx* ctx, uint32_t max_query, uint32_t max_targ
     return DGPU_ERR_ARG;
   }
   DGPU_CUDA(ctx, cudaSetDevice(ctx->device));
-  if (!ctx->ep_refused) {
-    DGPU_CUDA(ctx, cudaMalloc(&ctx->ep_refused, sizeof(unsigned long long)));
-    DGPU_CUDA(ctx, cudaMemset(ctx->ep_refused, 0, sizeof(unsigned long long)));
-  }
+  int rc;
+  if ((rc = dgpu_refusals_init(ctx))) return rc;
   // every kind any level or the leaves can reach, with or without equalities: its shared-memory opt-in and its workspace at the full grid
   // within the budget, at least one bound-shaped slab
   EpBound b;
@@ -1470,17 +1442,14 @@ int dgpu_set_ep_async_bound(dgpu_ctx* ctx, uint32_t max_query, uint32_t max_targ
   size_t free_b = 0, total_b = 0;
   DGPU_CUDA(ctx, cudaMemGetInfo(&free_b, &total_b));
   std::vector<size_t> need(SLOT_COUNT, 0);
-  int rc;
   for (int eq = 0; eq < 2; ++eq) {
     const size_t* room = seg_rooms(ctx, eq);
     for (int l = 0; l <= b.levels; ++l) {
       const bool leaves = l == b.levels;
       for (int id : bound_kinds(b, leaves ? 0 : l, leaves, room)) {
-        const BoundKind k = bound_kind(id, leaves, eq, b.mq, b.w, room);
-        const size_t per_block = k.per_cta * k.stride;
-        size_t grid = (size_t) ctx->num_sms * k.per_sm;
-        if (per_block) grid = std::max<size_t>(1, std::min(grid, dgpu_workspace_budget(ctx, k.slot, free_b) / per_block));
-        need[k.slot] = std::max(need[k.slot], std::max<size_t>(grid * per_block, 256));
+        const SegKindGeom k = bound_kind(id, leaves, eq, b.mq, b.w, room);
+        const size_t grid = seg_grid(ctx, k, SIZE_MAX, dgpu_workspace_budget(ctx, k.slot, free_b));
+        need[k.slot] = std::max(need[k.slot], std::max<size_t>(grid * k.per_cta * k.stride, 256));
         if (!k.half && (rc = dgpu_smem_optin(ctx, k.k, k.smem, "cudaFuncSetAttribute(seg_kernel)"))) return rc;
       }
     }

@@ -41,8 +41,8 @@ namespace {
 constexpr int LN_NCLS = 16;  // 0 trivial; 1..15 the rows of ln_geom
 constexpr int LN_GEN = 16;   // class + LN_GEN: the same geometry for jobs with a byte outside ACGTN (scalar engine, byte compares)
 
-// Workspace plan of one class, written on the device by ln_plan_kernel when the call runs under dgpu_set_ln_async_bound: the class's slabs
-// start at `base` inside the pool, and only the first `grid` CTAs of its launch take jobs.
+// Workspace plan of one class (ln_fit): the class's slabs start at `base` inside the workspace, and only the first `grid` CTAs of its launch
+// take jobs.
 struct LnPlan {
   unsigned long long base, work_stride, off_dirsR, off_dirsF, off_trace;
   uint32_t grid;
@@ -138,8 +138,7 @@ __host__ __device__ inline LnParts ln_parts(int C, uint32_t m, uint32_t n) {
 }
 // Slab layout of a class from the maxima over its jobs: prefix maxima, reverse direction nibbles, forward direction nibbles, then the four
 // trace strings of m + n bytes.
-template <class S>   // LnArgs (host planning) or LnPlan (device planning)
-__host__ __device__ inline void ln_slab(S& a, unsigned long long rev, unsigned long long dirs, unsigned long long mn) {
+__host__ __device__ inline void ln_slab(LnPlan& a, unsigned long long rev, unsigned long long dirs, unsigned long long mn) {
   auto al = [](unsigned long long x) { return (x + 255) & ~255ull; };
   a.off_dirsR = al(rev + 1024);
   a.off_dirsF = a.off_dirsR + al(dirs + 1024);
@@ -243,42 +242,51 @@ __global__ void ln_scatter_kernel(LnArgs a) {
   a.perm[p] = i;
 }
 
-// Device-side planning under dgpu_set_ln_async_bound: what ln_dev's host planner does from the counts and maxima it reads back, done by one
-// thread from the same counts and maxima. gmax[c] = the CTAs class c is launched with (0: not launched); pool = workspace bytes. Every
-// launched non-empty class gets the slab of its largest job and min(count, gmax) CTAs. The wide class then takes what the ordinary classes
-// leave of the pool, keeping them up to half of it, and never less than one CTA each; if the ordinary classes still ask for more than the
-// rest, each keeps one CTA and the CTAs above that are cut by one factor. (The host planner shrinks whole grids by one factor and may
-// reserve more than its budget to give every class one CTA; a pool reserved once cannot grow, so the device planner cuts so that it fits:
-// the setter sized the pool for one bound-shaped CTA of every class the bound admits.)
-struct LnPlanIn { uint32_t gmax[2 * LN_NCLS]; unsigned long long pool; };
-__global__ void ln_plan_kernel(const uint32_t* __restrict__ counts, const unsigned long long* __restrict__ maxc, LnPlanIn in, LnPlan* plan) {
-  if (threadIdx.x != 0) return;
-  LnPlan pl[2 * LN_NCLS];
-  unsigned long long ord = 0, base = 0;   // ordinary classes: bytes asked for, bytes of one CTA each
+// The workspace plan pl[2 * LN_NCLS] of both forms from the class counts and the maxima over each class's jobs (ln_count_kernel's layout),
+// within `limit` bytes; cap[c] = the most CTAs class c may take (0: not launched). Returns the bytes the plan takes. Every launched non-empty
+// class gets the slab of its largest job and min(count, cap) CTAs. The wide class's slabs are hundreds of MB, so it takes what the ordinary
+// classes leave, keeping them up to half of the limit and never less than one CTA each; if the ordinary classes still ask for more than the
+// rest, each keeps one CTA and the CTAs above that are cut by one factor, so that the plan fits. A limit that cannot hold one CTA of every
+// class leaves each class one CTA, and the plan takes more than the limit.
+__host__ __device__ inline unsigned long long ln_fit(const uint32_t* counts, const unsigned long long* maxc, const uint32_t* cap, unsigned long long limit,
+                                                     LnPlan* pl) {
+  typedef unsigned long long u64;
+  auto sub = [](u64 a, u64 b) { return a > b ? a - b : 0ull; };   // saturating
+  auto lo = [](u64 a, u64 b) { return a < b ? a : b; };
+  u64 ord = 0, base = 0;   // ordinary classes: bytes asked for, bytes of one CTA each
   for (int c = 0; c < 2 * LN_NCLS; ++c) {
     LnPlan& p = pl[c];
     p.base = p.work_stride = p.off_dirsR = p.off_dirsF = p.off_trace = 0;
     p.grid = 0;
-    if (c == 0 || !in.gmax[c] || !counts[c]) continue;
-    if (c == LN_WIDE) p.work_stride = maxc[c];
+    if (c == 0 || !cap[c] || !counts[c]) continue;
+    if (c == LN_WIDE) p.work_stride = maxc[c];   // the slab is the largest job's (lnw_geom), laid out per job by the kernel
     else ln_slab(p, maxc[c], maxc[32 + c], maxc[64 + c]);
-    p.grid = min(counts[c], in.gmax[c]);
+    p.grid = (uint32_t) lo(counts[c], cap[c]);
     if (c != LN_WIDE) { ord += p.grid * p.work_stride; base += p.work_stride; }
   }
-  const unsigned long long P = in.pool;
-  unsigned long long wide_total = 0;
+  u64 wide_total = 0;
   LnPlan& w = pl[LN_WIDE];
   if (w.grid) {
-    const unsigned long long cap = P - max(min(ord, P / 2), base);
-    w.grid = (uint32_t) max(1ull, min((unsigned long long) w.grid, cap / w.work_stride));
+    const u64 keep = lo(ord, limit / 2);
+    w.grid = (uint32_t) lo(w.grid, sub(limit, keep > base ? keep : base) / w.work_stride);
+    if (!w.grid) w.grid = 1;
     wide_total = w.grid * w.work_stride;
   }
-  const unsigned long long rest = P - wide_total;
+  const u64 rest = sub(limit, wide_total);
   if (ord > rest)
     for (int c = 1; c < 2 * LN_NCLS; ++c)
-      if (c != LN_WIDE && pl[c].grid) pl[c].grid = 1 + (uint32_t) ((pl[c].grid - 1ull) * (rest - base) / (ord - base));
-  unsigned long long off = 0;
-  for (int c = 0; c < 2 * LN_NCLS; ++c) { pl[c].base = off; off += pl[c].grid * pl[c].work_stride; plan[c] = pl[c]; }
+      if (c != LN_WIDE && pl[c].grid) pl[c].grid = 1 + (uint32_t) (rest > base ? (pl[c].grid - 1ull) * (rest - base) / (ord - base) : 0);
+  u64 off = 0;
+  for (int c = 0; c < 2 * LN_NCLS; ++c) { pl[c].base = off; off += pl[c].grid * pl[c].work_stride; }
+  return off;
+}
+
+// Device-side planning under dgpu_set_ln_async_bound: ln_fit by one thread, from the counts and maxima the synchronous form reads back.
+// gmax[c] = the CTAs class c is launched with (0: not launched); pool = the workspace the setter reserved, sized for one bound-shaped CTA of
+// every class the bound admits, so the plan fits it.
+struct LnPlanIn { uint32_t gmax[2 * LN_NCLS]; unsigned long long pool; };
+__global__ void ln_plan_kernel(const uint32_t* __restrict__ counts, const unsigned long long* __restrict__ maxc, LnPlanIn in, LnPlan* plan) {
+  if (threadIdx.x == 0) ln_fit(counts, maxc, in.gmax, in.pool, plan);
 }
 
 // src/util.h:549-563 applied to position i of the output
@@ -1134,7 +1142,7 @@ int ln_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes, const uint32
   if ((rc = dgpu_reserve(ctx, SLOT_COUNTS, 2048 + 2 * LN_NCLS * sizeof(LnPlan), &p))) return rc;
   a.counts = (uint32_t*) p;                                   // 96 uint32 = 384 B
   a.maxcells = (unsigned long long*) ((uint8_t*) p + 512);     // 128 uint64 = 1024 B
-  unsigned long long* d_unsupported = bound ? ctx->ln_refused : (unsigned long long*) ((uint8_t*) p + 1536);
+  unsigned long long* d_unsupported = bound ? ctx->refused + DGPU_REFUSED_LN : (unsigned long long*) ((uint8_t*) p + 1536);
   LnPlan* d_plan = (LnPlan*) ((uint8_t*) p + 2048);
   DGPU_CUDA(ctx, cudaMemsetAsync(p, 0, 2048, st));
   void* pc;
@@ -1180,50 +1188,31 @@ int ln_dev(dgpu_ctx* ctx, const uint8_t* seqs, uint64_t seqs_bytes, const uint32
   }
   size_t free_b = 0, total_b = 0;
   cudaMemGetInfo(&free_b, &total_b);
-  // Plan every non-empty class first: workspace geometry and grid. The classes then run CONCURRENTLY on a small pool of
+  // Plan every non-empty class first (ln_fit within the workspace budget). The classes then run CONCURRENTLY on a small pool of
   // streams forked from `st` (each class has its own region of the workspace): a batch of a few hundred SVs spread over
   // several classes would otherwise run as a sequence of under-filled launches.
   // Classes 1..15: jobs over ACGTN only -> packed two-row engine (ln_kernel2); 17..31: the same geometries for jobs with other bytes -> scalar engine.
-  struct Plan { int c; LnArgs a; size_t grid; LnShape s; };
-  std::vector<Plan> plans;
-  size_t total = 0;
-  for (int c = 1; c < 2 * LN_NCLS; ++c) {
-    if (!h.counts[c]) continue;
-    Plan pl;
-    pl.c = c; pl.a = a;
-    pl.s = ln_shape(c, (size_t) h.maxc[96 + c], max_ref);
-    if (c == LN_WIDE) pl.a.work_stride = (size_t) h.maxc[c];   // the slab is the largest job's (lnw_geom), laid out per job by the kernel
-    else ln_slab(pl.a, h.maxc[c], h.maxc[32 + c], h.maxc[64 + c]);
-    pl.grid = std::min<size_t>(h.counts[c], (size_t) ctx->num_sms * pl.s.per_sm);
-    total += pl.grid * pl.a.work_stride;
-    plans.push_back(pl);
-  }
-  const size_t budget = dgpu_workspace_budget(ctx, SLOT_WAVEFRONT, free_b);
-  // The wide class's slabs are hundreds of MB: left in the common shrink, a few wide jobs would cut the grids of every ordinary class. So
-  // the ordinary classes keep what they ask for, up to half of the budget, and the wide class is sized within the rest (all of it when
-  // the batch has only wide jobs).
-  size_t wide_total = 0;
-  for (auto& pl : plans)
-    if (pl.c == LN_WIDE) {
-      total -= pl.grid * pl.a.work_stride;
-      const size_t wide_cap = budget - std::min(total, budget / 2);
-      pl.grid = std::max<size_t>(1, std::min<size_t>(pl.grid, wide_cap / pl.a.work_stride));
-      wide_total = pl.grid * pl.a.work_stride;
+  LnShape shape[2 * LN_NCLS];
+  uint32_t cap[2 * LN_NCLS] = {};
+  size_t nplans = 0;
+  for (int c = 1; c < 2 * LN_NCLS; ++c)
+    if (h.counts[c]) {
+      shape[c] = ln_shape(c, (size_t) h.maxc[96 + c], max_ref);
+      cap[c] = (uint32_t) ctx->num_sms * shape[c].per_sm;
+      ++nplans;
     }
-  if (total + wide_total > budget) {  // shrink every ordinary class's grid by the same factor (at least one CTA each)
-    const double f = (double) (budget > wide_total ? budget - wide_total : 0) / (double) total;
-    total = 0;
-    for (auto& pl : plans)
-      if (pl.c != LN_WIDE) { pl.grid = std::max<size_t>(1, (size_t) ((double) pl.grid * f)); total += pl.grid * pl.a.work_stride; }
-  }
-  total += wide_total;
+  LnPlan pl[2 * LN_NCLS];
+  const size_t total = ln_fit(h.counts, h.maxc, cap, dgpu_workspace_budget(ctx, SLOT_WAVEFRONT, free_b), pl);
   if ((rc = dgpu_reserve(ctx, SLOT_WAVEFRONT, total, &p))) return rc;
-  { size_t off = 0; for (auto& pl : plans) { pl.a.work = (uint8_t*) p + off; off += pl.grid * pl.a.work_stride; } }
-  DgpuFork fork(ctx, st, plans.size());
+  DgpuFork fork(ctx, st, nplans);
   if ((rc = fork.begin())) return rc;
-  for (Plan& pl : plans) {
+  for (int c = 1; c < 2 * LN_NCLS; ++c) {
+    if (!pl[c].grid) continue;
+    LnArgs ac = a;
+    ac.work = (uint8_t*) p + pl[c].base;
+    ac.work_stride = pl[c].work_stride; ac.off_dirsR = pl[c].off_dirsR; ac.off_dirsF = pl[c].off_dirsF; ac.off_trace = pl[c].off_trace;
     cudaStream_t cs;
-    if ((rc = fork.next(cs)) || (rc = ln_launch(ctx, pl.c, pl.a, (unsigned) pl.grid, pl.s, cs))) return rc;
+    if ((rc = fork.next(cs)) || (rc = ln_launch(ctx, c, ac, pl[c].grid, shape[c], cs))) return rc;
   }
   return fork.end();
 }
@@ -1280,13 +1269,8 @@ int dgpu_set_ln_async_bound(dgpu_ctx* ctx, uint32_t max_cons, uint32_t max_ref) 
   const size_t pool = std::max<size_t>(one, std::min<size_t>(all, dgpu_workspace_budget(ctx, SLOT_WAVEFRONT, free_b)));
   void* p;
   if ((rc = dgpu_reserve(ctx, SLOT_WAVEFRONT, pool, &p)) || (rc = dgpu_reserve(ctx, SLOT_COUNTS, 2048 + 2 * LN_NCLS * sizeof(LnPlan), &p)) ||
-      (rc = dgpu_fork_init(ctx)))
+      (rc = dgpu_fork_init(ctx)) || (rc = dgpu_refusals_init(ctx)))
     return rc;
-  if (!ctx->ln_refused) {
-    DGPU_CUDA(ctx, cudaMalloc(&ctx->ln_refused, sizeof(unsigned long long)));
-    DGPU_CUDA(ctx, cudaMemsetAsync(ctx->ln_refused, 0, sizeof(unsigned long long), ctx->stream));
-    DGPU_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  }
   ctx->ln_max_cons = max_cons; ctx->ln_max_ref = max_ref; ctx->ln_pool = pool;
   return DGPU_OK;
 }
